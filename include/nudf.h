@@ -324,6 +324,43 @@ int nudf_gen_rays(const float* intrinsics_inv, const float* pose, const int64_t*
 int nudf_gen_rays_grid(const float* intrinsics_inv, const float* pose, int32_t W, int32_t H, int32_t Wl, int32_t Hl, float* rays_o,
                        float* rays_d, float* near, float* far, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * MeshUDF marching cubes (replaces custom_mc's udf_mc_lewiner; neuraludf_b200/mesh.py drives the stages)
+ * ------------------------------------------------------------------------------------------------------------
+ * df: DEVICE fp32 lattice [n0, n1, n2] (axis 0 slowest).  Cells are named by the flat index of their lower corner; every cell
+ * list is sorted ascending.  Normals are unit vectors towards the surface: dense [n0*n1*n2, 3] (idx = NULL) or the sparse
+ * rows of the sorted flat indices idx[n_idx] (grid.near_surface_cells); a corner without a row counts as the zero vector.
+ * All buffers are caller-provided; nothing is allocated. */
+/* flags[t] = 1 when cell cand[t] (cand = NULL: cell t of the whole lattice) is active: mean corner udf < avg_t and max <= max_t */
+int nudf_mc_active(const float* df, int32_t n0, int32_t n1, int32_t n2, const int64_t* cand, int64_t n_cand, float avg_t,
+                   float max_t, uint8_t* flags, void* stream);
+/* mask[t] bit c = corner c of cells[t] on the other pseudo-side than the cell's largest-udf corner (c = 4 a0 + 2 a1 + a2) */
+int nudf_mc_cell_signs(const float* df, int32_t n0, int32_t n1, int32_t n2, const int64_t* cells, int64_t n_cells,
+                       const int64_t* idx, int64_t n_idx, const float* normals, uint8_t* mask, void* stream);
+/* links[t*3+axis] = 2 * (position of the + axis neighbour in cells) + (1 when the shared corners with udf > 0 all disagree,
+ * 0 when they all agree), or -1 (no active neighbour, mixed or no evidence) */
+int nudf_mc_links(const float* df, int32_t n0, int32_t n1, int32_t n2, const int64_t* cells, int64_t n_cells,
+                  const uint8_t* mask, int64_t* links, void* stream);
+/* one polarity per linked component (deterministic union-find with parity; the root cell's corner 0 ends positive):
+ * mask_out = mask_in, complemented where the cell flips.  Workspace: parent_ws, hook_ws [n_cells] int64, flag_ws [1] int32.
+ * Synchronises the stream (one host read of flag_ws per pass).  stats (HOST int32[2], may be NULL): hooking rounds,
+ * pointer-jumping passes.  At most n_cells - 1 hooking rounds; a handful in practice. */
+int nudf_mc_polarity(const int64_t* links, int64_t n_cells, const uint8_t* mask_in, int64_t* parent_ws, int64_t* hook_ws,
+                     int32_t* flag_ws, uint8_t* mask_out, int32_t* stats, void* stream);
+/* triangles per cell (<= 12): each crossing loop is triangulated with no chord lying in a cube face (every edge of a
+ * closed surface is shared by exactly two triangles); a loop that admits no such triangulation is fanned around a centre
+ * vertex of its own */
+int nudf_mc_count(const float* df, int32_t n0, int32_t n1, int32_t n2, const int64_t* cells, int64_t n_cells,
+                  const uint8_t* mask, int32_t* counts, void* stream);
+/* keys[3 * (offsets[t] + i) + k] = key of vertex k of triangle i of cells[t]: 3 * corner + axis for a lattice-edge point,
+ * 3 * n0 * n1 * n2 + 4 * t + l for the centre vertex of the cell's loop l; offsets = exclusive scan of the counts */
+int nudf_mc_emit(const float* df, int32_t n0, int32_t n1, int32_t n2, const int64_t* cells, int64_t n_cells,
+                 const uint8_t* mask, const int64_t* offsets, int64_t* keys, void* stream);
+/* verts[n_keys, 3]: lattice-index coordinates of the vertices of the keys: edge points at t = u_a / (u_a + u_b) from the
+ * lower corner, loop centres at the mean of their edge points (cells / mask: those given to nudf_mc_emit) */
+int nudf_mc_vertices(const float* df, int32_t n0, int32_t n1, int32_t n2, const int64_t* cells, int64_t n_cells,
+                     const uint8_t* mask, const int64_t* keys, int64_t n_keys, float* verts, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

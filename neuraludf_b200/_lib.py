@@ -153,6 +153,18 @@ _SIGNATURES = {
     "nudf_gen_rays_grid": (ctypes.c_int, [c_void_p] * 2 + [ctypes.c_int32] * 4 + [c_void_p] * 5),
     "nudf_outside_points": (ctypes.c_int, [c_void_p, c_void_p, c_void_p, ctypes.c_int32, ctypes.c_int32, ctypes.c_int32,
                                            ctypes.c_float, c_void_p, c_void_p, c_void_p]),
+    "nudf_mc_active": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [c_void_p, ctypes.c_int64, ctypes.c_float,
+                                                                          ctypes.c_float, c_void_p, c_void_p]),
+    "nudf_mc_cell_signs": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [c_void_p, ctypes.c_int64, c_void_p,
+                                                                              ctypes.c_int64, c_void_p, c_void_p, c_void_p]),
+    "nudf_mc_links": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [c_void_p, ctypes.c_int64, c_void_p, c_void_p,
+                                                                         c_void_p]),
+    "nudf_mc_polarity": (ctypes.c_int, [c_void_p, ctypes.c_int64] + [c_void_p] * 7),
+    "nudf_mc_count": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [c_void_p, ctypes.c_int64, c_void_p, c_void_p,
+                                                                         c_void_p]),
+    "nudf_mc_emit": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [c_void_p, ctypes.c_int64] + [c_void_p] * 4),
+    "nudf_mc_vertices": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [c_void_p, ctypes.c_int64, c_void_p, c_void_p,
+                                                                            ctypes.c_int64, c_void_p, c_void_p]),
 }
 
 

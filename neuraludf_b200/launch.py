@@ -4,9 +4,12 @@
 
 `models.fields`, `models.embedder`, `models.udf_renderer_blending` and `models.patch_projector` are bound to the nudf
 mirrors before the runner is executed from the reference root; everything else the runner imports (`dataset`, `loss`, ...)
-still resolves from the reference checkout (its `models/` directory is a namespace package).
+still resolves from the reference checkout (its `models/` directory is a namespace package).  `custom_mc` (the Cython
+MeshUDF marching cubes that extract_mesh.py imports) is bound to neuraludf_b200.mesh when the reference's own build cannot
+be imported by the running interpreter.
 """
 import importlib
+import importlib.machinery
 import os
 import runpy
 import sys
@@ -29,7 +32,37 @@ def install_shadow_modules(reference_root=None):
                       ("patch_projector", patch_projector)):
         sys.modules["models." + name] = mod
         setattr(pkg, name, mod)
+    _install_custom_mc(reference_root)
     return pkg
+
+
+def _native_custom_mc(reference_root):
+    """True when `<root>/custom_mc` holds a `_marching_cubes_lewiner_cy` extension this interpreter can import (the
+    reference ships one built for CPython 3.6 only)."""
+    if reference_root is None:
+        return False
+    d = os.path.join(reference_root, "custom_mc")
+    return any(os.path.isfile(os.path.join(d, "_marching_cubes_lewiner_cy" + s))
+               for s in importlib.machinery.EXTENSION_SUFFIXES)
+
+
+def _install_custom_mc(reference_root):
+    """Serves `custom_mc._marching_cubes_lewiner.udf_mc_lewiner` (imported at module level by the runner's
+    extract_mesh.py) from neuraludf_b200.mesh, unless the name is already bound or the reference's own Cython build can
+    serve this interpreter."""
+    if "custom_mc._marching_cubes_lewiner" in sys.modules or _native_custom_mc(reference_root):
+        return
+    from neuraludf_b200 import mesh
+    pkg = sys.modules.get("custom_mc")
+    if pkg is None:
+        pkg = types.ModuleType("custom_mc")
+        pkg.__path__ = []
+        sys.modules["custom_mc"] = pkg
+    mod = types.ModuleType("custom_mc._marching_cubes_lewiner")
+    mod.__doc__ = "MeshUDF marching cubes on the nudf CUDA kernels (neuraludf_b200.mesh)"
+    mod.udf_mc_lewiner = mesh.udf_mc_lewiner
+    sys.modules["custom_mc._marching_cubes_lewiner"] = mod
+    pkg._marching_cubes_lewiner = mod
 
 
 def main(argv=None):
