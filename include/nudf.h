@@ -361,6 +361,44 @@ int nudf_mc_emit(const float* df, int32_t n0, int32_t n1, int32_t n2, const int6
 int nudf_mc_vertices(const float* df, int32_t n0, int32_t n1, int32_t n2, const int64_t* cells, int64_t n_cells,
                      const uint8_t* mask, const int64_t* keys, int64_t n_keys, float* verts, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * Point-cloud evaluation (the DTU / DeepFashion3D Chamfer protocols; neuraludf_b200/evaluate.py drives the stages)
+ * ------------------------------------------------------------------------------------------------------------
+ * Points are DEVICE fp64 [n, 3]; all buffers are caller-provided, nothing is allocated.  Host arrays are marked HOST. */
+/* counts[f] = samples of triangle f of the scripts' surface sampling (0 when area2 == 0) */
+int nudf_pc_sample_count(const double* verts, int64_t n_verts, const int64_t* faces, int64_t n_faces, double density,
+                         int64_t* counts, void* stream);
+/* points[offsets[f] + s] = sample s of triangle f (row-major over i, j); offsets = exclusive scan of the counts */
+int nudf_pc_sample_emit(const double* verts, int64_t n_verts, const int64_t* faces, int64_t n_faces, double density,
+                        const int64_t* offsets, double* points, void* stream);
+/* keys[t] = (cx * dims[1] + cy) * dims[2] + cz, c = floor((p - lo) / cell) clamped to [0, dims - 1] (lo, dims: HOST [3]) */
+int nudf_pc_cell_keys(const double* points, int64_t n, const double* lo, double cell, const int64_t* dims, int64_t* keys,
+                      void* stream);
+/* radius graph over n points of rank 0..n-1 sorted by cell: sorted_points[s] = point of rank order[s], sorted_keys[s] its key;
+ * cells[n_cells] the distinct keys ascending, cell_start[n_cells + 1] their first sorted positions.  Neighbours of rank v:
+ * ranks u < v with (dx^2 + dy^2) + dz^2 <= radius * radius; cell must be > radius (adjacent cells only are scanned).
+ * counts[v] = their number; nbr[offsets[v] ...] = their ranks (offsets [n + 1]: exclusive scan of the counts) */
+int nudf_pc_radius_count(const double* sorted_points, const int64_t* order, const int64_t* sorted_keys, int64_t n,
+                         const int64_t* cells, const int64_t* cell_start, int64_t n_cells, const double* lo, double cell,
+                         const int64_t* dims, double radius, int32_t* counts, void* stream);
+int nudf_pc_radius_emit(const double* sorted_points, const int64_t* order, const int64_t* sorted_keys, int64_t n,
+                        const int64_t* cells, const int64_t* cell_start, int64_t n_cells, const double* lo, double cell,
+                        const int64_t* dims, double radius, const int64_t* offsets, int32_t* nbr, void* stream);
+/* the scripts' greedy downsampling: state[v] = 1 (kept) / 2 (dropped) -- the lexicographically-first maximal independent set
+ * in rank order, in parallel rounds.  Workspace flag_ws [1] int32.  Synchronises the stream (one host read per round).
+ * rounds (HOST int32, may be NULL): the number of rounds */
+int nudf_pc_greedy_mis(const int64_t* offsets, const int32_t* nbr, int64_t n, uint8_t* state, int32_t* flag_ws,
+                       int32_t* rounds, void* stream);
+/* codes[t] = 63-bit Morton code of floor((p - lo) * scale) clamped to [0, 2^21 - 1] per axis (lo: HOST [3]) */
+int nudf_pc_morton(const double* points, int64_t n, const double* lo, double scale, int64_t* codes, void* stream);
+/* AABBs of the implicit complete binary tree over 32-point leaves of the sorted targets: boxes [2 n_leaves - 1, 6]
+ * (lo xyz, hi xyz; node i has children 2i+1, 2i+2; leaf l is node n_leaves - 1 + l); n_leaves a power of two >= n / 32 */
+int nudf_pc_bvh_build(const double* sorted_targets, int64_t n, int64_t n_leaves, double* boxes, void* stream);
+/* dist[q] = exact nearest distance sqrt((dx^2 + dy^2) + dz^2) from queries[q] to the targets when it is < max_dist, else +inf
+ * (max_dist = +inf: unbounded).  query_order (may be NULL) = the processing order of the queries (Morton order for coherence) */
+int nudf_pc_nearest(const double* queries, int64_t n_queries, const int64_t* query_order, const double* sorted_targets,
+                    int64_t n_targets, const double* boxes, int64_t n_leaves, double max_dist, double* dist, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -165,6 +165,22 @@ _SIGNATURES = {
     "nudf_mc_emit": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [c_void_p, ctypes.c_int64] + [c_void_p] * 4),
     "nudf_mc_vertices": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [c_void_p, ctypes.c_int64, c_void_p, c_void_p,
                                                                             ctypes.c_int64, c_void_p, c_void_p]),
+    "nudf_pc_sample_count": (ctypes.c_int, [c_void_p, ctypes.c_int64, c_void_p, ctypes.c_int64, ctypes.c_double, c_void_p,
+                                            c_void_p]),
+    "nudf_pc_sample_emit": (ctypes.c_int, [c_void_p, ctypes.c_int64, c_void_p, ctypes.c_int64, ctypes.c_double, c_void_p,
+                                           c_void_p, c_void_p]),
+    "nudf_pc_cell_keys": (ctypes.c_int, [c_void_p, ctypes.c_int64, c_void_p, ctypes.c_double, c_void_p, c_void_p, c_void_p]),
+    "nudf_pc_radius_count": (ctypes.c_int, [c_void_p] * 3 + [ctypes.c_int64] + [c_void_p] * 2 + [ctypes.c_int64, c_void_p,
+                                                                                                  ctypes.c_double, c_void_p,
+                                                                                                  ctypes.c_double] + [c_void_p] * 2),
+    "nudf_pc_radius_emit": (ctypes.c_int, [c_void_p] * 3 + [ctypes.c_int64] + [c_void_p] * 2 + [ctypes.c_int64, c_void_p,
+                                                                                                 ctypes.c_double, c_void_p,
+                                                                                                 ctypes.c_double] + [c_void_p] * 3),
+    "nudf_pc_greedy_mis": (ctypes.c_int, [c_void_p, c_void_p, ctypes.c_int64] + [c_void_p] * 4),
+    "nudf_pc_morton": (ctypes.c_int, [c_void_p, ctypes.c_int64, c_void_p, ctypes.c_double, c_void_p, c_void_p]),
+    "nudf_pc_bvh_build": (ctypes.c_int, [c_void_p, ctypes.c_int64, ctypes.c_int64, c_void_p, c_void_p]),
+    "nudf_pc_nearest": (ctypes.c_int, [c_void_p, ctypes.c_int64, c_void_p, c_void_p, ctypes.c_int64, c_void_p, ctypes.c_int64,
+                                       ctypes.c_double, c_void_p, c_void_p]),
 }
 
 

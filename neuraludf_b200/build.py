@@ -7,7 +7,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libnudf.so")
 SOURCES = ["capi.cu", "udf_net.cu", "mlp_nets.cu", "ray_kernels.cu", "sampling.cu", "gemm_tc.cu", "blend.cu", "raygen.cu",
-           "mesh_udf.cu"]
+           "mesh_udf.cu", "eval_pc.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
