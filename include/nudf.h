@@ -399,6 +399,24 @@ int nudf_pc_bvh_build(const double* sorted_targets, int64_t n, int64_t n_leaves,
 int nudf_pc_nearest(const double* queries, int64_t n_queries, const int64_t* query_order, const double* sorted_targets,
                     int64_t n_targets, const double* boxes, int64_t n_leaves, double max_dist, double* dist, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * DTU mesh cleaning by masks and visual hull (evaluation/clean_dtu_mesh.py; neuraludf_b200/clean.py drives the stages)
+ * ------------------------------------------------------------------------------------------------------------
+ * Caller-provided buffers only; host arrays are marked HOST. */
+/* packed[v, y, w] bit b = (D(v, y, 32 w + b) > 128), or < 128 when below != 0, for columns < width (other bits 0), where
+ * D = the grayscale dilation of masks [n_views, height, width] uint8 by the element whose row i covers columns
+ * [row_lo[i], row_hi[i]) (HOST [kh]; empty when row_hi <= row_lo): D(y, x) = max of masks(y + i - anchor_y, x + j - anchor_x)
+ * over the element, pixels outside the image not contributing.  packed: [n_views, height, ceil(width / 32)] uint32.
+ * kh, kw <= 255. */
+int nudf_cl_dilate(const uint8_t* masks, int32_t n_views, int32_t height, int32_t width, const int32_t* row_lo,
+                   const int32_t* row_hi, int32_t kh, int32_t kw, int32_t anchor_x, int32_t anchor_y, int32_t below,
+                   uint32_t* packed, void* stream);
+/* counts[t] = number of views v (mats: DEVICE fp64 [n_views, 3, 4], n_views <= 512) in which points[t] projects to
+ * u = rint(s0 / s2) + 1, v = rint(s1 / s2) + 1 (s = ((m0 x + m1 y) + m2 z) + m3 per row, fp64, half to even) with
+ * border <= u <= width - border, border <= v <= height - border and the packed mask, padded by a ring of ones, set at (v, u) */
+int nudf_cl_vote(const double* points, int64_t n, const double* mats, int32_t n_views, const uint32_t* packed,
+                 int32_t height, int32_t width, int32_t border, int32_t* counts, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -181,6 +181,10 @@ _SIGNATURES = {
     "nudf_pc_bvh_build": (ctypes.c_int, [c_void_p, ctypes.c_int64, ctypes.c_int64, c_void_p, c_void_p]),
     "nudf_pc_nearest": (ctypes.c_int, [c_void_p, ctypes.c_int64, c_void_p, c_void_p, ctypes.c_int64, c_void_p, ctypes.c_int64,
                                        ctypes.c_double, c_void_p, c_void_p]),
+    "nudf_cl_dilate": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [c_void_p] * 2 + [ctypes.c_int32] * 5
+                       + [c_void_p] * 2),
+    "nudf_cl_vote": (ctypes.c_int, [c_void_p, ctypes.c_int64, c_void_p, ctypes.c_int32, c_void_p] + [ctypes.c_int32] * 3
+                     + [c_void_p] * 2),
 }
 
 

@@ -449,6 +449,22 @@ def write_ply_points(path, points, colors=None, ascii=False):
             f.write(a.tobytes())
 
 
+def write_ply_mesh(path, verts, faces):
+    """A triangle mesh as binary little-endian PLY: double x / y / z and faces as `list uchar int vertex_indices`."""
+    v = np.ascontiguousarray(torch.as_tensor(verts).detach().cpu().numpy(), dtype="<f8").reshape(-1, 3)
+    f = np.asarray(torch.as_tensor(faces).detach().cpu().numpy()).reshape(-1, 3)
+    if f.size and (f.min() < 0 or f.max() >= len(v)):
+        raise ValueError("face index out of range")
+    head = ["ply", "format binary_little_endian 1.0", "element vertex %d" % len(v), "property double x", "property double y",
+            "property double z", "element face %d" % len(f), "property list uchar int vertex_indices", "end_header"]
+    fd = np.empty(len(f), dtype=[("n", "u1"), ("i", "<i4", (3,))])
+    fd["n"], fd["i"] = 3, f
+    with open(path, "wb") as fh:
+        fh.write(("\n".join(head) + "\n").encode("ascii"))
+        fh.write(v.tobytes())
+        fh.write(fd.tobytes())
+
+
 def read_ply_colors(path):
     """The red / green / blue vertex properties of a PLY point cloud as uint8 [V,3] (None when absent)."""
     with open(path, "rb") as f:
