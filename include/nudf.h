@@ -417,6 +417,30 @@ int nudf_cl_dilate(const uint8_t* masks, int32_t n_views, int32_t height, int32_
 int nudf_cl_vote(const double* points, int64_t n, const double* mats, int32_t n_views, const uint32_t* packed,
                  int32_t height, int32_t width, int32_t border, int32_t* counts, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * Narrow-band lattice evaluation, coarse to fine (neuraludf_b200/grid.py udf_band drives the levels)
+ * ------------------------------------------------------------------------------------------------------------
+ * The N^3 lattice on [-1,1]^3, flat index (i * N + j) * N + k, voxel = 2 / (N - 1).  The stride-s lattice holds the
+ * coordinates 0, s, 2 s, ... and N - 1 per axis; a block of stride s is the box [a, min(a + s, N - 1)] per axis (a a multiple
+ * of s below N - 1), nb = ceil((N - 1) / s) per axis, numbered (bx * nb + by) * nb + bz.  Coordinates are fp32
+ * fl(fl(i * fl32(voxel)) - 1), as grid.lattice_points makes them.  Caller-provided buffers only. */
+/* idx / pts [m^3] (m = ceil((N - 1) / s) + 1): the stride-s lattice in (x, y, z) lexicographic order */
+int nudf_nb_sublattice(int32_t n, int32_t s, double voxel, int64_t* idx, float* pts, void* stream);
+/* flags[nb^3] (may be NULL) = 1 for the kept blocks of stride s: candidates (every block when parent_flags is NULL, else the
+ * blocks inside a kept block of stride parent_s) with a NaN corner or min(corner df) - lipschitz r < tau in fp64, r = half
+ * the box diagonal, with slack (r + 1e-6 relative + 1e-6, tau + 1e-6 relative) against rounding.  Candidates' corners must
+ * have been evaluated.  max_slope (DEVICE uint32[1], fp32 bits, zeroed by the caller) is raised to the largest
+ * |du| / (edge length) over the candidates' box edges with finite ends */
+int nudf_nb_block_test(const float* df, int32_t n, int32_t s, const uint8_t* parent_flags, int32_t parent_s, double voxel,
+                       double lipschitz, double tau, uint8_t* flags, uint32_t* max_slope, void* stream);
+/* counts[i] = the points block kept[i] of stride s emits: the stride-t lattice (t divides s) in its closed box, less the
+ * stride-s lattice, less the points that a lower-numbered kept block (flags) also holds.  kept: ascending block numbers */
+int nudf_nb_count(const uint8_t* flags, int32_t n, int32_t s, int32_t t, const int64_t* kept, int64_t n_kept,
+                  int32_t* counts, void* stream);
+/* idx / pts[offsets[i] ...] = those points of block kept[i] in (x, y, z) lexicographic order; offsets = exclusive scan */
+int nudf_nb_emit(const uint8_t* flags, int32_t n, int32_t s, int32_t t, const int64_t* kept, int64_t n_kept,
+                 const int64_t* offsets, double voxel, int64_t* idx, float* pts, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

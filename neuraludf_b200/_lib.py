@@ -185,6 +185,12 @@ _SIGNATURES = {
                        + [c_void_p] * 2),
     "nudf_cl_vote": (ctypes.c_int, [c_void_p, ctypes.c_int64, c_void_p, ctypes.c_int32, c_void_p] + [ctypes.c_int32] * 3
                      + [c_void_p] * 2),
+    "nudf_nb_sublattice": (ctypes.c_int, [ctypes.c_int32] * 2 + [ctypes.c_double] + [c_void_p] * 3),
+    "nudf_nb_block_test": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 2 + [c_void_p, ctypes.c_int32] + [ctypes.c_double] * 3
+                           + [c_void_p] * 3),
+    "nudf_nb_count": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [c_void_p, ctypes.c_int64] + [c_void_p] * 2),
+    "nudf_nb_emit": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [c_void_p, ctypes.c_int64, c_void_p, ctypes.c_double]
+                     + [c_void_p] * 3),
 }
 
 

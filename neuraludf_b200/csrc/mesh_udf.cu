@@ -15,6 +15,10 @@
 //   5. welding        vertices are keyed by lattice edge (3 * corner + axis) and placed at t = u_a / (u_a + u_b); the few
 //                     loops that need a centre vertex key it after all edges (3 * n_points + 4 * cell + loop).
 // Deviation from Lewiner: interior ambiguities (case 13 tunnels) are not resolved -- each loop is fanned on its own.
+// Reads of df: stage 1 reads the 8 corners of each candidate cell; every later stage reads only the corners of active cells
+// (k_signs, k_links and cell_loops read cell g's own corners, edge_point an edge of an active cell).  So, for the same
+// candidates and normals, a lattice whose values equal the dense ones wherever those are <= max_t and are > max_t elsewhere
+// (+inf included: max <= max_t fails) meshes exactly like the dense one -- what grid.udf_band's narrow band relies on.
 // tests/proto/udf_mc.py restates every stage in NumPy with the same float32 operation order.
 #include <algorithm>
 

@@ -1,7 +1,8 @@
 """MeshUDF marching cubes on the device: the last stage of a run, UDF -> triangle mesh.
 
 `udf_mesh` is the device-resident pipeline (grid.udf_grid -> grid.near_surface_cells -> CUDA MC -> the reference's vertex
-filter, extract_mesh.py:205-214); `udf_marching_cubes` is the MC alone; `udf_mc_lewiner` is a NumPy-in / NumPy-out drop-in
+filter, extract_mesh.py:205-214); `udf_mesh_band` is the same with the lattice evaluated narrow-band (grid.udf_band);
+`python -m neuraludf_b200.mesh` meshes a runner checkpoint to PLY; `udf_marching_cubes` is the MC alone; `udf_mc_lewiner` is a NumPy-in / NumPy-out drop-in
 for the reference's `custom_mc._marching_cubes_lewiner.udf_mc_lewiner`, served to the unmodified runner by
 `launch.install_shadow_modules` when the reference's Cython build cannot be imported.  The kernels are in
 csrc/mesh_udf.cu (stages and deviations documented there); tests/proto/udf_mc.py is their NumPy restatement.
@@ -117,9 +118,15 @@ def udf_mesh(udf_network, N, dist_threshold_ratio=1.0, lo=0, hi=None, max_batch=
     hi = N ** 3 if hi is None else hi
     if lo % (N * N) or hi % (N * N) or not 0 <= lo < hi <= N ** 3:
         raise ValueError("lo / hi must select whole x-planes of the N^3 lattice")
-    planes = (hi - lo) // (N * N)
-    voxel = 2.0 / (N - 1)
     df = grid.udf_grid(udf_network, N, max_batch=max_batch, lo=lo, hi=hi)
+    return _mesh_lattice(udf_network, N, df, dist_threshold_ratio, lo, max_batch)
+
+
+def _mesh_lattice(udf_network, N, df, dist_threshold_ratio, lo, max_batch):
+    """near-surface normals -> MC -> vertex filter of the lattice values df (whole x-planes from flat index lo)"""
+    from neuraludf_b200 import grid
+    planes = df.numel() // (N * N)
+    voxel = 2.0 / (N - 1)
     idx, normals = grid.near_surface_cells(udf_network, N, df, max_batch=max(max_batch // 2, 1), lo=lo)
     verts, faces, _ = marching_cubes_index(df, (planes, N, N), normals, idx - lo)
     verts = verts * voxel - 1.0
@@ -129,6 +136,20 @@ def udf_mesh(udf_network, N, dist_threshold_ratio=1.0, lo=0, hi=None, max_batch=
     vd = udf_network.udf_values(verts).reshape(-1)
     keep = vd[faces].max(dim=1).values < voxel * dist_threshold_ratio
     return _compact(verts, faces[keep])
+
+
+@torch.no_grad()
+def udf_mesh_band(udf_network, N, dist_threshold_ratio=1.0, lipschitz=2.0, strides=None, max_batch=1 << 21):
+    """`udf_mesh` with the lattice evaluated narrow-band (grid.udf_band) instead of densely: the same (verts, faces).
+
+    Exact when the field is `lipschitz`-Lipschitz and `udf_values` / `gradient` give the same bits for a point in any batch:
+    udf_band's df then equals the dense one below 2 voxels and is >= 2 voxels (+inf) elsewhere, so near_surface_cells picks
+    the same points and normals, an unevaluated (+inf) corner fails the MC's active-cell test (max <= 1.74 voxel) exactly
+    as its dense value >= 2 voxels does, and the later MC stages read df only at the corners of active cells
+    (csrc/mesh_udf.cu).  grid.udf_band warns when the lattice shows a slope above `lipschitz`."""
+    from neuraludf_b200 import grid
+    df, _ = grid.udf_band(udf_network, N, lipschitz=lipschitz, strides=strides, max_batch=max_batch)
+    return _mesh_lattice(udf_network, N, df, dist_threshold_ratio, 0, max_batch)
 
 
 def udf_mc_lewiner(volume, grads, spacing=(1., 1., 1.), gradient_direction='descent', step_size=1, allow_degenerate=True,
@@ -189,3 +210,62 @@ def udf_mc_lewiner(volume, grads, spacing=(1., 1., 1.), gradient_direction='desc
     if not np.array_equal(spacing, (1, 1, 1)):
         vertices = vertices * np.r_[spacing]
     return vertices, faces.to(torch.int32).cpu().numpy(), nrm.cpu().numpy(), values.cpu().numpy()
+
+
+def udf_network_from_state(sd, scale=1.0):
+    """A UDFNetwork holding the state dict `sd` (the runner's `udf_network_fine`), its n_layers, d_hidden, d_out, skip_in and
+    multires read off the weight shapes: lin0 is [d_hidden, 3 + 6 multires], a layer feeding the skip is
+    [d_hidden - (3 + 6 multires), d_hidden], the last one [d_out, d_hidden].  `scale` is not stored in the weights (every
+    shipped conf uses 1.0)."""
+    from neuraludf_b200.models.fields import UDFNetwork
+    n_lin = 0
+    while "lin%d.weight_v" % n_lin in sd:
+        n_lin += 1
+    if n_lin < 2:
+        raise ValueError("not a UDFNetwork state dict (no lin0 / lin1 .weight_v)")
+    d_hidden, input_ch = (int(x) for x in sd["lin0.weight_v"].shape)
+    if (input_ch - 3) % 6:
+        raise ValueError("lin0 takes %d inputs: not 3 + 6 multires" % input_ch)
+    skip_in = tuple(l + 1 for l in range(n_lin - 2) if int(sd["lin%d.weight_v" % l].shape[0]) == d_hidden - input_ch)
+    net = UDFNetwork(d_in=3, d_out=int(sd["lin%d.weight_v" % (n_lin - 1)].shape[0]), d_hidden=d_hidden, n_layers=n_lin - 1,
+                     skip_in=skip_in, multires=(input_ch - 3) // 6, scale=scale, geometric_init=False, weight_norm=True,
+                     udf_type="abs")
+    net.load_state_dict(sd)
+    return net
+
+
+def main(argv=None):
+    """python -m neuraludf_b200.mesh: a runner checkpoint's UDF network -> PLY mesh (see INTEGRATION.md)"""
+    import argparse
+    from neuraludf_b200.evaluate import write_ply_mesh
+    ap = argparse.ArgumentParser(prog="python -m neuraludf_b200.mesh",
+                                 description="Mesh the UDF network of a runner checkpoint (the mesh before the runner's trimesh "
+                                             "post-processing, as udf_mesh makes it).")
+    ap.add_argument("--ckpt", required=True, help="checkpoint written by the runner (its udf_network_fine state dict is used)")
+    ap.add_argument("--resolution", type=int, default=512, help="lattice points per axis")
+    ap.add_argument("--cameras", default=None, help="cameras_sphere.npz: map the mesh to world space with its scale_mat_0")
+    ap.add_argument("--dist_threshold_ratio", type=float, default=1.0)
+    ap.add_argument("--lipschitz", type=float, default=2.0, help="Lipschitz bound of the band's culling test")
+    ap.add_argument("--scale", type=float, default=1.0, help="the conf's udf_network.scale")
+    ap.add_argument("--dense", action="store_true", help="evaluate the whole lattice (udf_mesh) instead of the narrow band")
+    ap.add_argument("--out", required=True, help="output PLY")
+    a = ap.parse_args(argv)
+    if not torch.cuda.is_available():
+        raise SystemExit("meshing runs on a CUDA device")
+    ck = torch.load(a.ckpt, map_location="cpu", weights_only=True)
+    net = udf_network_from_state(ck["udf_network_fine"] if "udf_network_fine" in ck else ck, a.scale).cuda()
+    if a.dense:
+        verts, faces = udf_mesh(net, a.resolution, a.dist_threshold_ratio)
+    else:
+        verts, faces = udf_mesh_band(net, a.resolution, a.dist_threshold_ratio, a.lipschitz)
+    v = verts.double().cpu().numpy()
+    if a.cameras is not None:                     # exp_runner_blending.py:792-794, with the dataset's fp32 scale_mat_0
+        sm = np.load(a.cameras)["scale_mat_0"].astype(np.float32)
+        v = v * sm[0, 0] + sm[:3, 3][None]
+    write_ply_mesh(a.out, v, faces)
+    print("%s: %d vertices, %d faces" % (a.out, v.shape[0], faces.shape[0]))
+    return v, faces.cpu().numpy()
+
+
+if __name__ == "__main__":
+    main()
