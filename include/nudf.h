@@ -441,6 +441,32 @@ int nudf_nb_count(const uint8_t* flags, int32_t n, int32_t s, int32_t t, const i
 int nudf_nb_emit(const uint8_t* flags, int32_t n, int32_t s, int32_t t, const int64_t* kept, int64_t n_kept,
                  const int64_t* offsets, double voxel, int64_t* idx, float* pts, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * Mesh post-processing (neuraludf_b200/mesh_post.py drives the steps; sorting, unique and compaction in torch)
+ * ------------------------------------------------------------------------------------------------------------
+ * verts: fp64 [V,3]; faces and edges: int64 rows.  All fp64 arithmetic is correctly rounded per operation with no
+ * contraction.  Caller-provided buffers only. */
+/* per face i: out_faces[i] = remap[faces[i]] (faces[i] when remap is NULL), sorted_faces[i] = its ascending triple,
+ * edge_codes[3 i + k] = (lo * V + hi) * 2 + (1 when the face runs hi -> lo) of its edge (k, k + 1 mod 3), and
+ * nondegenerate[i] = 1 when |a|, |b|, |a x b| / |a| and |a x b| / |b| all exceed 1e-8 (a = v1 - v0, b = v2 - v0, in the
+ * remapped vertices).  V < 2^30 */
+int nudf_mp_faces(const double* verts, int64_t n_verts, const int64_t* faces, int64_t n_faces, const int64_t* remap,
+                  int64_t* out_faces, int64_t* sorted_faces, int64_t* edge_codes, uint8_t* nondegenerate, void* stream);
+/* boundary edges [B,2] (u < v, ascending) with the CSR (rowptr [V+1], cols ascending per row) of boundary neighbours:
+ * counts[i] = the faces edge i emits: 1 or 2 when it is the smallest edge of a boundary component that is a simple cycle of 3
+ * or 4 vertices, else 0 */
+int nudf_mp_hole_count(const int64_t* edges, int64_t n_edges, const int64_t* rowptr, const int64_t* cols, int64_t n_verts,
+                       int32_t* counts, void* stream);
+/* faces[offsets[i] ...] = those faces (offsets = exclusive scan of counts): they traverse edge i against its direction in its
+ * face (dirs[i] = 1: the face runs v -> u); a quad is split along its shorter diagonal (squared fp64 length), a tie along the
+ * diagonal through the smallest vertex */
+int nudf_mp_hole_emit(const double* verts, const int64_t* edges, const uint8_t* dirs, int64_t n_edges, const int64_t* rowptr,
+                      const int64_t* cols, int64_t n_verts, const int64_t* offsets, int64_t* faces, void* stream);
+/* one Jacobi step of border smoothing: for each vertex b in border, verts_out[b] = v + lambda (s / count - v), v =
+ * verts_in[b], s = its CSR neighbours' verts_in summed in ascending order.  Other rows of verts_out are not written */
+int nudf_mp_smooth_step(const double* verts_in, double* verts_out, const int64_t* border, int64_t n_border,
+                        const int64_t* rowptr, const int64_t* cols, double lambda, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

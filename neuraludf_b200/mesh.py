@@ -2,6 +2,7 @@
 
 `udf_mesh` is the device-resident pipeline (grid.udf_grid -> grid.near_surface_cells -> CUDA MC -> the reference's vertex
 filter, extract_mesh.py:205-214); `udf_mesh_band` is the same with the lattice evaluated narrow-band (grid.udf_band);
+`udf_mesh_post` adds the runner's post-processing (mesh_post.py) and returns the mesh `Runner.extract_udf_mesh` exports;
 `python -m neuraludf_b200.mesh` meshes a runner checkpoint to PLY; `udf_marching_cubes` is the MC alone; `udf_mc_lewiner` is a NumPy-in / NumPy-out drop-in
 for the reference's `custom_mc._marching_cubes_lewiner.udf_mc_lewiner`, served to the unmodified runner by
 `launch.install_shadow_modules` when the reference's Cython build cannot be imported.  The kernels are in
@@ -122,13 +123,20 @@ def udf_mesh(udf_network, N, dist_threshold_ratio=1.0, lo=0, hi=None, max_batch=
     return _mesh_lattice(udf_network, N, df, dist_threshold_ratio, lo, max_batch)
 
 
-def _mesh_lattice(udf_network, N, df, dist_threshold_ratio, lo, max_batch):
-    """near-surface normals -> MC -> vertex filter of the lattice values df (whole x-planes from flat index lo)"""
+def _mc_lattice(udf_network, N, df, lo, max_batch):
+    """near-surface normals -> MC of the lattice values df (whole x-planes from flat index lo): (verts [V,3] fp32 in the
+    slab's lattice-index units, faces [F,3] int64)"""
     from neuraludf_b200 import grid
     planes = df.numel() // (N * N)
-    voxel = 2.0 / (N - 1)
     idx, normals = grid.near_surface_cells(udf_network, N, df, max_batch=max(max_batch // 2, 1), lo=lo)
     verts, faces, _ = marching_cubes_index(df, (planes, N, N), normals, idx - lo)
+    return verts, faces
+
+
+def _mesh_lattice(udf_network, N, df, dist_threshold_ratio, lo, max_batch):
+    """near-surface normals -> MC -> vertex filter of the lattice values df (whole x-planes from flat index lo)"""
+    voxel = 2.0 / (N - 1)
+    verts, faces = _mc_lattice(udf_network, N, df, lo, max_batch)
     verts = verts * voxel - 1.0
     verts[:, 0] += (lo // (N * N)) * voxel
     if faces.shape[0] == 0:
@@ -150,6 +158,35 @@ def udf_mesh_band(udf_network, N, dist_threshold_ratio=1.0, lipschitz=2.0, strid
     from neuraludf_b200 import grid
     df, _ = grid.udf_band(udf_network, N, lipschitz=lipschitz, strides=strides, max_batch=max_batch)
     return _mesh_lattice(udf_network, N, df, dist_threshold_ratio, 0, max_batch)
+
+
+@torch.no_grad()
+def udf_mesh_post(udf_network, N, dist_threshold_ratio=5.0, dense=False, lipschitz=2.0, strides=None, smooth_borders=True,
+                  max_batch=1 << 21):
+    """The mesh `Runner.extract_udf_mesh` exports, before its world transform and final merge: (fp64 verts [V,3], int64
+    faces [F,3], info) on the device.
+
+    The lattice is evaluated narrow-band (`udf_mesh_band`'s, `lipschitz` / `strides`) or, with `dense`, whole (`udf_mesh`'s);
+    the normals and MC are theirs.  The vertices are then formed as the reference holds them, fp64(fp32 MC vertex) *
+    fp64(voxel) - 1 in fp64, the vertex filter of extract_mesh.py:205-214 evaluates the udf at their fp32 rounding, and
+    `mesh_post.postprocess` does the rest of get_mesh_udf_fast (extract_mesh.py:215-265; the runner passes
+    `dist_threshold_ratio` 5 and `smooth_borders` True).  info: postprocess's, plus `mc` ((V, F) of the raw MC) and
+    `filtered` (faces after the vertex filter)."""
+    from neuraludf_b200 import grid, mesh_post
+    voxel = 2.0 / (N - 1)
+    if dense:
+        df = grid.udf_grid(udf_network, N, max_batch=max_batch)
+    else:
+        df, _ = grid.udf_band(udf_network, N, lipschitz=lipschitz, strides=strides, max_batch=max_batch)
+    verts, faces = _mc_lattice(udf_network, N, df, 0, max_batch)
+    v64 = verts.double() * voxel - 1.0
+    n_mc = faces.shape[0]
+    if n_mc:
+        vd = udf_network.udf_values(v64.float()).reshape(-1)
+        faces = faces[vd[faces].max(dim=1).values < voxel * dist_threshold_ratio]
+    v, f, info = mesh_post.postprocess(v64, faces, smooth_borders=smooth_borders)
+    info["mc"], info["filtered"] = (verts.shape[0], n_mc), int(faces.shape[0])
+    return v, f, info
 
 
 def udf_mc_lewiner(volume, grads, spacing=(1., 1., 1.), gradient_direction='descent', step_size=1, allow_degenerate=True,
@@ -239,8 +276,8 @@ def main(argv=None):
     import argparse
     from neuraludf_b200.evaluate import write_ply_mesh
     ap = argparse.ArgumentParser(prog="python -m neuraludf_b200.mesh",
-                                 description="Mesh the UDF network of a runner checkpoint (the mesh before the runner's trimesh "
-                                             "post-processing, as udf_mesh makes it).")
+                                 description="Mesh the UDF network of a runner checkpoint: the mesh as udf_mesh makes it, or with "
+                                             "--postprocess the mesh the runner's extract_udf_mesh exports.")
     ap.add_argument("--ckpt", required=True, help="checkpoint written by the runner (its udf_network_fine state dict is used)")
     ap.add_argument("--resolution", type=int, default=512, help="lattice points per axis")
     ap.add_argument("--cameras", default=None, help="cameras_sphere.npz: map the mesh to world space with its scale_mat_0")
@@ -248,13 +285,19 @@ def main(argv=None):
     ap.add_argument("--lipschitz", type=float, default=2.0, help="Lipschitz bound of the band's culling test")
     ap.add_argument("--scale", type=float, default=1.0, help="the conf's udf_network.scale")
     ap.add_argument("--dense", action="store_true", help="evaluate the whole lattice (udf_mesh) instead of the narrow band")
+    ap.add_argument("--postprocess", action="store_true",
+                    help="apply the runner's post-processing (merge, duplicate and degenerate faces, hole filling, border "
+                         "smoothing, the final merge after --cameras): the mesh Runner.extract_udf_mesh writes; the runner "
+                         "passes --dist_threshold_ratio 5")
     ap.add_argument("--out", required=True, help="output PLY")
     a = ap.parse_args(argv)
     if not torch.cuda.is_available():
         raise SystemExit("meshing runs on a CUDA device")
     ck = torch.load(a.ckpt, map_location="cpu", weights_only=True)
     net = udf_network_from_state(ck["udf_network_fine"] if "udf_network_fine" in ck else ck, a.scale).cuda()
-    if a.dense:
+    if a.postprocess:
+        verts, faces, _ = udf_mesh_post(net, a.resolution, a.dist_threshold_ratio, dense=a.dense, lipschitz=a.lipschitz)
+    elif a.dense:
         verts, faces = udf_mesh(net, a.resolution, a.dist_threshold_ratio)
     else:
         verts, faces = udf_mesh_band(net, a.resolution, a.dist_threshold_ratio, a.lipschitz)
@@ -262,6 +305,10 @@ def main(argv=None):
     if a.cameras is not None:                     # exp_runner_blending.py:792-794, with the dataset's fp32 scale_mat_0
         sm = np.load(a.cameras)["scale_mat_0"].astype(np.float32)
         v = v * sm[0, 0] + sm[:3, 3][None]
+    if a.postprocess:                             # exp_runner_blending.py:796: Trimesh(...) merges once more
+        from neuraludf_b200.mesh_post import export_merge
+        vt, faces = export_merge(torch.from_numpy(v).to(verts.device), faces)
+        v = vt.cpu().numpy()
     write_ply_mesh(a.out, v, faces)
     print("%s: %d vertices, %d faces" % (a.out, v.shape[0], faces.shape[0]))
     return v, faces.cpu().numpy()
