@@ -20,7 +20,7 @@ extern "C" {
 #endif
 
 #define NUDF_MAX_LAYERS 16
-#define NUDF_ABI_VERSION 3
+#define NUDF_ABI_VERSION 4
 /* bits of the device-side status word (nudf_render_out.status, `status` of the sampling entry points): set by the kernels,
  * never cleared by the library; the caller reads it at a host synchronisation point of its choice */
 #define NUDF_STATUS_NONFINITE_SAMPLES 1   /* sample_pdf / up_sample produced a non-finite sample position (:97-101, 265-269) */
@@ -38,11 +38,6 @@ int nudf_get_engine(void);
 int nudf_set_tc_mask(int mask);
 int nudf_get_tc_mask(void);
 int nudf_default_tc_mask(void);   /* the mask the library ships (what bench.py times and the parity suite pins) */
-/* Plane-fed reverse-sweep / tangent chains (engine 1 only): intermediate tensors of those chains are kept as split-bf16
- * plane tensors (see nudf_pack_planes) and fetched with cp.async.bulk.  Default 0 (env NUDF_PLANES).  Like the engine
- * and the mask it must not change between a forward call and its backward (the ctx layout depends on it). */
-int nudf_set_chain_planes(int on);
-int nudf_get_chain_planes(void);
 /* --- tensor engine building blocks (unit-tested on their own) ---
  * weight image: bf16 hi/lo split of B(n,k) in UMMA shared-memory order; `transposed` selects B(n,k) = W[k*ldw+n]. */
 /* planes: 2 = hi/lo (3 products, ~4e-6 vs fp64), 3 = hi/mid/lo (6 products, fp32-grade; used by the value chain) */
@@ -55,21 +50,6 @@ int nudf_dense_forward_tc(const float* X, int64_t ldx, const uint16_t* img, int3
 int nudf_wgrad(const float* dZ, int64_t ldz, const float* X, int64_t ldx, int32_t n_out, int32_t n_in, int64_t P,
                float* dW, int64_t ldw, int32_t engine, void* stream);
 
-/* Split-bf16 plane tensors (csrc/gemm_pl.cuh): a fp32 matrix [rows x cols] stored as hi = bf16(x), lo = bf16(x - hi) in
- * 64 x 64 blocks, [row block][col block][plane][64 rows x 128 B SWIZZLE_128B]; 1024-byte aligned; pad rows are zero.
- * The tcgen05 kernels fetch these blocks with cp.async.bulk and use them as K-major (layer chains) or MN-major
- * (weight gradients) operands without conversion.  nudf_planes_elems: uint16 elements to allocate. */
-int64_t nudf_planes_elems(int64_t rows, int32_t cols);
-int nudf_pack_planes(const float* X, int64_t ldx, int64_t rows, int32_t cols, uint16_t* planes, void* stream);
-int nudf_unpack_planes(const uint16_t* planes, int64_t rows, int32_t cols, float* X, int64_t ldx, void* stream);
-/* Y = act(X W^T + b), X given as a plane tensor allocated for round_up(M, 128) rows, W as a 2-plane weight image
- * (nudf_tc_prepare_weights, transposed = 0), K <= 256: the plane-fed weights-resident chain kernel on one layer. */
-int nudf_dense_forward_planes(const uint16_t* X_planes, const uint16_t* img, const float* bias, float* Y, int64_t ldy, int64_t M,
-                              int32_t N, int32_t K, int32_t act, void* stream);
-/* dW[n_out, n_in] += dZ[P, n_out]^T X[P, n_in], both operands plane tensors (replaces the autograd weight gradient of one
- * nn.Linear, models/fields.py:185; tensor engine only). */
-int nudf_wgrad_planes(const uint16_t* dZ_planes, const uint16_t* X_planes, int32_t n_out, int32_t n_in, int64_t P, float* dW,
-                      int64_t ldw, void* stream);
 /* number of CUDA kernels this library has launched in this process (bench.py reports it as gpu_launches) */
 int64_t nudf_launch_count(void);
 /* Per-kernel-family device times for the benchmark's roofline table: while enabled, the library brackets its launches with

@@ -92,15 +92,6 @@ _SIGNATURES = {
                                   ctypes.c_int64, c_void_p, ctypes.c_int64, ctypes.c_int32, c_void_p]),
     "nudf_blend_forward": (ctypes.c_int, [c_void_p] * 7 + [ctypes.c_int64] + [c_void_p] * 4),
     "nudf_blend_backward": (ctypes.c_int, [c_void_p] * 7 + [ctypes.c_int64] + [c_void_p] * 4),
-    "nudf_set_chain_planes": (ctypes.c_int, [ctypes.c_int]),
-    "nudf_get_chain_planes": (ctypes.c_int, []),
-    "nudf_planes_elems": (ctypes.c_int64, [ctypes.c_int64, ctypes.c_int32]),
-    "nudf_pack_planes": (ctypes.c_int, [c_void_p, ctypes.c_int64, ctypes.c_int64, ctypes.c_int32, c_void_p, c_void_p]),
-    "nudf_unpack_planes": (ctypes.c_int, [c_void_p, ctypes.c_int64, ctypes.c_int32, c_void_p, ctypes.c_int64, c_void_p]),
-    "nudf_dense_forward_planes": (ctypes.c_int, [c_void_p, c_void_p, c_void_p, c_void_p, ctypes.c_int64, ctypes.c_int64,
-                                                 ctypes.c_int32, ctypes.c_int32, ctypes.c_int32, c_void_p]),
-    "nudf_wgrad_planes": (ctypes.c_int, [c_void_p, c_void_p, ctypes.c_int32, ctypes.c_int32, ctypes.c_int64, c_void_p,
-                                         ctypes.c_int64, c_void_p]),
     "nudf_dense_forward": (ctypes.c_int, [c_void_p, ctypes.c_int64, c_void_p, ctypes.c_int64, c_void_p, c_void_p,
                                           ctypes.c_int64, ctypes.c_int64, ctypes.c_int32, ctypes.c_int32, ctypes.c_int32,
                                           c_void_p]),
@@ -216,7 +207,7 @@ def lib():
             fn = getattr(L, name)
             fn.restype = res
             fn.argtypes = args
-        if L.nudf_abi_version() != 3:
+        if L.nudf_abi_version() != 4:
             raise RuntimeError("libnudf.so ABI version mismatch")
         _lib = L
     return _lib

@@ -58,16 +58,6 @@ int tc_mask() {
   return g_tc_mask;
 }
 
-// NUDF_PLANES / nudf_set_chain_planes: plane-fed reverse-sweep and tangent chains (gemm_engine.cuh)
-static int g_chain_planes = -1;
-int chain_planes_flag() {
-  if (g_chain_planes < 0) {
-    const char* e = getenv("NUDF_PLANES");
-    g_chain_planes = (e && atoi(e) != 0) ? 1 : 0;
-  }
-  return g_chain_planes;
-}
-
 // Workspace of the deterministic split-K reductions (common.cuh): one per device, kept for the life of the process.
 float* split_workspace(cudaStream_t st) {
   static float* ws[64] = {};
@@ -117,8 +107,6 @@ int nudf_get_engine(void) { return nudf::get_engine(); }
 int nudf_set_tc_mask(int mask) { nudf::g_tc_mask = mask & 255; return 0; }
 int nudf_get_tc_mask(void) { return nudf::tc_mask(); }
 int nudf_default_tc_mask(void) { return nudf::kDefaultTcMask; }
-int nudf_set_chain_planes(int on) { nudf::g_chain_planes = on ? 1 : 0; return 0; }
-int nudf_get_chain_planes(void) { return nudf::chain_planes_flag(); }
 int64_t nudf_launch_count(void) { return (int64_t)__atomic_load_n(&nudf::g_launches, __ATOMIC_RELAXED); }
 
 int nudf_launch_family_count(void) { return nudf::FAM_COUNT; }

@@ -7,8 +7,6 @@
 #pragma once
 #include <stdlib.h>
 #include "gemm_tc.cuh"
-#include "gemm_pl.cuh"
-#include "epi_planes.cuh"
 
 namespace nudf {
 
@@ -39,27 +37,6 @@ static inline int gemm_nn(const float* A, int64_t lda, const float* W, int64_t l
 }
 // C[M x N] += A[K x M]^T B[K x N]   (contraction over points)
 int colsum(const float* X, int64_t ldx, const float* w, float wscale, int64_t P, int N, float* out, cudaStream_t st);
-
-// ---- plane-fed chains (gemm_pl.cuh) -------------------------------------------------------------------------------
-// Optional mode (nudf_set_chain_planes(1) / NUDF_PLANES=1): the reverse-sweep and tangent chains of the UDF network carry
-// D[l] / Adot[l] between kernels as split-bf16 plane tensors -- operands fetched by cp.async.bulk, weight gradients on the
-// MN-major plane kernel.  Parity-tested; off by default (its speed on H100 is not measured).
-int chain_planes_flag();
-static inline bool chain_planes_on() { return chain_planes_flag() == 1 && tc_on(TC_REV) && tc_on(TC_TAN) && tc_on(TC_WGRAD); }
-static inline int64_t plane_rows(int64_t P) { return round_up(P, 128); }     // gemm_wrp reads whole 128-row tiles
-template <class Epi>
-static inline int gemm_tn_planes(const tc::Planes& X, int M, const tc::Planes& Y, int N, int64_t P, const Epi& epi, cudaStream_t st) {
-  return tc::gemm_tn_pl(X, M, Y, N, P, epi, st, tc::tn_splits(M, N, P, 64));
-}
-// dst planes[:, col0 + c] = src[:, c] * scale  for c < ncols (skip-concatenated columns of the tangent chain)
-static __global__ void copy_cols_planes_kernel(const float* __restrict__ src, int64_t lds, tc::Planes dst, int col0, int ncols, int64_t P,
-                                               float scale) {
-  int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  int64_t row = idx / ncols;
-  int c = (int)(idx - row * ncols);
-  if (row >= P) return;
-  tc::pl_store1(dst, row, col0 + c, src[row * lds + c] * scale);
-}
 
 // colsum_a (optional): colsum_a[m] += sum_k A[k, m] -- the bias gradient that goes with a weight gradient; fused into the
 // tensor-engine kernel's operand staging, a separate reduction kernel on the FFMA path.

@@ -3,7 +3,6 @@
 #include "../../include/nudf.h"
 #include "common.cuh"
 #include "gemm_engine.cuh"
-#include "gemm_pl.cuh"
 
 using namespace nudf;
 
@@ -43,65 +42,6 @@ int nudf_wgrad(const float* dZ, int64_t ldz, const float* X, int64_t ldx, int32_
     return tc::gemm_tn(dZ, ldz, X, ldx, n_out, n_in, P, e, (cudaStream_t)stream, splits);
   }
   return gemm_simt<false, false, EpiAtomicAdd>(dZ, ldz, X, ldx, n_out, n_in, P, e, (cudaStream_t)stream, (int)cdiv(P, 2048));
-}
-
-// ---- split-bf16 plane tensors (gemm_pl.cuh) ----
-int64_t nudf_planes_elems(int64_t rows, int32_t cols) { return rows < 0 || cols < 0 ? -1 : tc::planes_elems(rows, cols); }
-
-int nudf_pack_planes(const float* X, int64_t ldx, int64_t rows, int32_t cols, uint16_t* planes, void* stream) {
-  if (rows <= 0 || cols <= 0) return 0;
-  NUDF_REQUIRE(X && planes, "null pointer");
-  NUDF_REQUIRE((reinterpret_cast<uintptr_t>(planes) & 1023) == 0, "plane tensors must be 1024-byte aligned");
-  return tc::pack_planes(X, ldx, rows, cols, tc::Planes{planes, (cols + 63) / 64}, (cudaStream_t)stream);
-}
-
-static __global__ void unpack_planes_kernel(tc::Planes in, int64_t rows, int cols, float* __restrict__ X, int64_t ldx) {
-  const int groups = in.cb * 16;
-  const int64_t total = rows * groups;
-  for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
-    const int64_t row = idx / groups;
-    const int col = (int)(idx - row * groups) * 4;
-    float v[4];
-    tc::pl_load4(in, row, col, v);
-    for (int j = 0; j < 4; ++j)
-      if (col + j < cols) X[row * ldx + col + j] = v[j];
-  }
-}
-int nudf_unpack_planes(const uint16_t* planes, int64_t rows, int32_t cols, float* X, int64_t ldx, void* stream) {
-  if (rows <= 0 || cols <= 0) return 0;
-  NUDF_REQUIRE(X && planes, "null pointer");
-  const int64_t total = rows * ((cols + 63) / 64) * 16;
-  int64_t blocks = (total + 255) / 256;
-  if (blocks > 8192) blocks = 8192;
-  unpack_planes_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(tc::Planes{const_cast<uint16_t*>(planes), (cols + 63) / 64}, rows,
-                                                                           cols, X, ldx);
-  NUDF_LAUNCH_OK();
-  return 0;
-}
-
-// Y = act(X W^T + b) with X a plane tensor of round_up(M, 128) rows (weights-resident plane-fed kernel, K <= 256)
-int nudf_dense_forward_planes(const uint16_t* Xp, const uint16_t* img, const float* bias, float* Y, int64_t ldy, int64_t M, int32_t N,
-                              int32_t K, int32_t act, void* stream) {
-  if (M <= 0 || N <= 0) return 0;
-  NUDF_REQUIRE(Xp && img && Y, "null pointer");
-  NUDF_REQUIRE((reinterpret_cast<uintptr_t>(Xp) & 1023) == 0, "plane tensors must be 1024-byte aligned");
-  NUDF_REQUIRE(act >= 0 && act <= 3, "bad act");
-  EpiAct e{Y, ldy, bias, act, 1.0f};
-  return tc::gemm_wrp(tc::Planes{const_cast<uint16_t*>(Xp), (K + 63) / 64}, M, N, K, img, e, (cudaStream_t)stream);
-}
-
-// dW[n_out, n_in] += dZ^T X with both operands given as plane tensors of P rows (pad rows zero)
-int nudf_wgrad_planes(const uint16_t* dZp, const uint16_t* Xp, int32_t n_out, int32_t n_in, int64_t P, float* dW, int64_t ldw,
-                      void* stream) {
-  if (P <= 0 || n_out <= 0 || n_in <= 0) return 0;
-  NUDF_REQUIRE(dZp && Xp && dW, "null pointer");
-  NUDF_REQUIRE(((reinterpret_cast<uintptr_t>(dZp) | reinterpret_cast<uintptr_t>(Xp)) & 1023) == 0, "plane tensors must be 1024-byte aligned");
-  EpiAtomicAdd e{dW, ldw};
-  const int tiles = (int)(cdiv(n_out, 128) * cdiv(n_in, 256));
-  int splits = tc::sm_count() / tiles;
-  if (splits < 1) splits = 1;
-  return tc::gemm_tn_pl(tc::Planes{const_cast<uint16_t*>(dZp), (n_out + 63) / 64}, n_out, tc::Planes{const_cast<uint16_t*>(Xp), (n_in + 63) / 64},
-                        n_in, P, e, (cudaStream_t)stream, splits);
 }
 
 }  // extern "C"

@@ -10,7 +10,6 @@
 #include <cuda_fp16.h>
 
 #include "gemm_simt.cuh"
-#include "planes.cuh"
 
 namespace nudf {
 namespace tc {
@@ -22,10 +21,34 @@ constexpr int THREADS = 256;   // 2 warpgroups: MMA issue, operand staging and e
 constexpr int A_HALF_BYTES = BM * BK * 2;   // 16 KB: one plane of a [128 x 64] operand slice
 constexpr int B_HALF_BYTES = BN * BK * 2;
 constexpr int ACC_LD = BN + 4;              // floats per row of the accumulator tile in shared memory
-constexpr int WR_MAX_SLICES = 4;            // K <= 256 for the plane-fed layer kernel
 
 __host__ __device__ inline int pad16(int n) { return (n + 15) & ~15; }
 __host__ __device__ inline int pad64(int k) { return (k + 63) & ~63; }
+
+// byte offset of element (row, k) inside a [rows x 64] bf16 K-major SWIZZLE_128B tile (tile base 1024-aligned)
+__host__ __device__ inline uint32_t sw128(uint32_t row, uint32_t k) {
+  return (row >> 3) * 1024u + (row & 7u) * 128u + ((((k >> 3) ^ (row & 7u)) & 7u) << 4) + ((k & 7u) << 1);
+}
+
+__device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
+  __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
+  return *reinterpret_cast<uint32_t*>(&v);
+}
+// split 4 consecutive values into NP bf16 planes (packed pairs)
+template <int NP>
+__device__ __forceinline__ void split4(const float x[4], uint2 planes[NP]) {
+  float r[4] = {x[0], x[1], x[2], x[3]};
+#pragma unroll
+  for (int p = 0; p < NP; ++p) {
+    float h[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      h[j] = __bfloat162float(__float2bfloat16_rn(r[j]));
+      r[j] -= h[j];
+    }
+    planes[p] = make_uint2(pack_bf16(h[0], h[1]), pack_bf16(h[2], h[3]));
+  }
+}
 // ---- weight image --------------------------------------------------------------------------------------------------
 // For operand B(n, k), n < N, k < K: n-tiles of NT rows (NT = 256 with 2 planes, 128 with 3 planes; the last tile is
 // padded to a multiple of 16), k-slices of 64.  NP planes per element: p0 = bf16(x), p1 = bf16(x - p0),
@@ -114,19 +137,16 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, u
                : "memory");
 }
 
-// wgmma smem descriptors: start, LBO, SBO (16-byte units), bits 62-63 = 1 (SWIZZLE_128B).  K-major: SBO = 1024 B (8-row
-// atoms).  MN-major: SBO = 1024 B between 8-row K groups, LBO = bytes between 64-element MN groups.
+// wgmma smem descriptor of a K-major operand: start, LBO, SBO (16-byte units), bits 62-63 = 1 (SWIZZLE_128B); SBO = 1024 B
+// (8-row atoms)
 __device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
   return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 62);
-}
-__device__ __forceinline__ uint64_t make_desc_mn(uint32_t smem_addr, uint32_t lbo_bytes) {
-  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | (64ull << 32) | (1ull << 62);
 }
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
 
-// D[64 x 128] (+)= A[64 x 16] B[128 x 16]^T from shared memory, bf16 or (F16) fp16 operands; TRANS = 1: both MN-major
+// D[64 x 128] (+)= A[64 x 16] B[128 x 16]^T from shared memory (both K-major), bf16 or (F16) fp16 operands
 #define NUDF_WGMMA_M64N128K16(TYPE) \
   asm volatile( \
       "{\n" \
@@ -135,7 +155,7 @@ __device__ __forceinline__ void wg_wait_all() { asm volatile("wgmma.wait_group.s
       "wgmma.mma_async.sync.aligned.m64n128k16.f32." TYPE "." TYPE " " \
       "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, " \
       "%26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, " \
-      "%50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %67;\n" \
+      "%50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n" \
       "}\n" \
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), \
         "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), \
@@ -144,39 +164,36 @@ __device__ __forceinline__ void wg_wait_all() { asm volatile("wgmma.wait_group.s
         "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), \
         "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), \
         "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]) \
-      : "l"(da), "l"(db), "r"(accumulate), "n"(TRANS))
-template <int TRANS, bool F16 = false>
+      : "l"(da), "l"(db), "r"(accumulate))
+template <bool F16 = false>
 __device__ __forceinline__ void wgmma_128(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
   if constexpr (F16) NUDF_WGMMA_M64N128K16("f16");
   else NUDF_WGMMA_M64N128K16("bf16");
 }
 
-// The wgmma group of one 64-wide K slice, smallest products first; plane p at +p * stride.  K-major operands advance 32 B
-// per 16-wide K step, MN-major ones two 1024-byte atoms.
-template <int NP, int TRANS>
-__device__ __forceinline__ void mma_slice(float (&d)[64], uint32_t a, uint32_t a_stride, uint32_t b, uint32_t b_stride, uint32_t lbo_b,
-                                          bool zero_first) {
+// The wgmma group of one 64-wide K slice, smallest products first; plane p at +p * stride, 32 B per 16-wide K step.
+template <int NP>
+__device__ __forceinline__ void mma_slice(float (&d)[64], uint32_t a, uint32_t a_stride, uint32_t b, uint32_t b_stride, bool zero_first) {
 #pragma unroll
   for (int j = 0; j < BK / 16; ++j) {
     uint64_t da[NP], db[NP];
-    const uint32_t kstep = TRANS ? 2048u * j : 32u * j;
 #pragma unroll
     for (int p = 0; p < NP; ++p) {
-      da[p] = TRANS ? make_desc_mn(a + p * a_stride + kstep, 0u) : make_desc(a + p * a_stride + kstep);
-      db[p] = TRANS ? make_desc_mn(b + p * b_stride + kstep, lbo_b) : make_desc(b + p * b_stride + kstep);
+      da[p] = make_desc(a + p * a_stride + 32u * j);
+      db[p] = make_desc(b + p * b_stride + 32u * j);
     }
     const uint32_t acc0 = (zero_first && j == 0) ? 0u : 1u;
     if (NP == 2) {
-      wgmma_128<TRANS>(d, da[1], db[0], acc0);
-      wgmma_128<TRANS>(d, da[0], db[1], 1u);
-      wgmma_128<TRANS>(d, da[0], db[0], 1u);
+      wgmma_128(d, da[1], db[0], acc0);
+      wgmma_128(d, da[0], db[1], 1u);
+      wgmma_128(d, da[0], db[0], 1u);
     } else {
-      wgmma_128<TRANS>(d, da[NP - 1], db[0], acc0);        // lo * hi
-      wgmma_128<TRANS>(d, da[0], db[NP - 1], 1u);          // hi * lo
-      wgmma_128<TRANS>(d, da[1], db[1], 1u);               // mid * mid
-      wgmma_128<TRANS>(d, da[1], db[0], 1u);               // mid * hi
-      wgmma_128<TRANS>(d, da[0], db[1], 1u);               // hi * mid
-      wgmma_128<TRANS>(d, da[0], db[0], 1u);               // hi * hi
+      wgmma_128(d, da[NP - 1], db[0], acc0);        // lo * hi
+      wgmma_128(d, da[0], db[NP - 1], 1u);          // hi * lo
+      wgmma_128(d, da[1], db[1], 1u);               // mid * mid
+      wgmma_128(d, da[1], db[0], 1u);               // mid * hi
+      wgmma_128(d, da[0], db[1], 1u);               // hi * mid
+      wgmma_128(d, da[0], db[0], 1u);               // hi * hi
     }
   }
 }
@@ -321,12 +338,10 @@ __device__ __forceinline__ void stage_block_t(const float* __restrict__ X, int64
 
 // ---------------------------------------------------------------------------------------------------------------
 // C[M x N] = epi( A[M x K] * B^T ),  B given as a pre-split NP-plane weight image.  grid = (ceil(M/128), ceil(N/128)).
-// APL: A is a 2-plane tensor (planes.cuh) of whole 128-row tiles, fetched with cp.async.bulk instead of staged.
 // ---------------------------------------------------------------------------------------------------------------
-template <int NP, bool APL, class Epi>
+template <int NP, class Epi>
 __global__ void __launch_bounds__(THREADS, 1)
-gemm_w_kernel(const float* __restrict__ A, int64_t lda, Planes Ap, int64_t M, int N, int K, const uint16_t* __restrict__ img, Epi epi) {
-  static_assert(!APL || NP == 2, "plane tensors have two planes");
+gemm_w_kernel(const float* __restrict__ A, int64_t lda, int64_t M, int N, int K, const uint16_t* __restrict__ img, Epi epi) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = align1024(smem_raw);
   const int tid = threadIdx.x, wg = tid >> 7;
@@ -340,16 +355,13 @@ gemm_w_kernel(const float* __restrict__ A, int64_t lda, Planes Ap, int64_t M, in
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + 2 * stage_bytes);
   const int64_t m0 = (int64_t)blockIdx.x * BM;
   const uint16_t* img_t = img + tile_offset(N, K, t, NP) + (int64_t)row_in_tile * 64;
-  const bool vec_ok = !APL && ((lda & 3) == 0) && aligned16(A);
+  const bool vec_ok = ((lda & 3) == 0) && aligned16(A);
 
-  auto issue_copies = [&](int ks) {                         // one thread: weight slice ks (+ plane-fed A slice)
+  auto issue_copies = [&](int ks) {                         // one thread: weight slice ks
     uint8_t* st = smem + (ks & 1) * stage_bytes;
     const uint32_t wb = (uint32_t)rows_h * 128u;
-    mbar_arrive_expect_tx(&full[ks & 1], NP * wb + (APL ? 2u * A_HALF_BYTES : 0u));
+    mbar_arrive_expect_tx(&full[ks & 1], NP * wb);
     for (int p = 0; p < NP; ++p) bulk_g2s(st + a_bytes + p * B_HALF_BYTES, img_t + ((int64_t)ks * NP + p) * rows_t * 64, wb, &full[ks & 1]);
-    if (APL)
-      for (int p = 0; p < 2; ++p)
-        for (int h = 0; h < 2; ++h) bulk_g2s(st + p * A_HALF_BYTES + h * PL_PLANE_BYTES, pl_block(Ap, 2 * blockIdx.x + h, ks, p), PL_PLANE_BYTES, &full[ks & 1]);
   };
   if (tid == 0) {
     mbar_init(&full[0], 1);
@@ -359,10 +371,8 @@ gemm_w_kernel(const float* __restrict__ A, int64_t lda, Planes Ap, int64_t M, in
   __syncthreads();
   if (n_slices > 0) {
     if (tid == 0) issue_copies(0);
-    if (!APL) {
-      stage_a_direct<NP, THREADS>(A, lda, m0, M, 0, K, smem, tid, vec_ok);
-      fence_proxy_async();
-    }
+    stage_a_direct<NP, THREADS>(A, lda, m0, M, 0, K, smem, tid, vec_ok);
+    fence_proxy_async();
   }
   __syncthreads();
   // 3 planes: each K slice in fresh registers, added to the running sum in fp32 (short truncating accumulation chains)
@@ -377,9 +387,9 @@ gemm_w_kernel(const float* __restrict__ A, int64_t lda, Planes Ap, int64_t M, in
     mbar_wait(&full[s], (uint32_t)((ks >> 1) & 1));
     const uint32_t st = smem_u32(smem + s * stage_bytes);
     wg_fence();
-    mma_slice<NP, 0>(acc, st + wg * (64 * 128), A_HALF_BYTES, st + a_bytes, B_HALF_BYTES, 0u, NP == 3 || ks == 0);
+    mma_slice<NP>(acc, st + wg * (64 * 128), A_HALF_BYTES, st + a_bytes, B_HALF_BYTES, NP == 3 || ks == 0);
     wg_commit();
-    if (!APL && ks + 1 < n_slices) stage_a_direct<NP, THREADS>(A, lda, m0, M, (ks + 1) * BK, K, smem + (s ^ 1) * stage_bytes, tid, vec_ok);
+    if (ks + 1 < n_slices) stage_a_direct<NP, THREADS>(A, lda, m0, M, (ks + 1) * BK, K, smem + (s ^ 1) * stage_bytes, tid, vec_ok);
     wg_wait_all();
     if constexpr (NP == 3) {
 #pragma unroll
@@ -441,7 +451,7 @@ gemm_tn_kernel(const float* __restrict__ A, int64_t lda, const float* __restrict
     const int s = i & 1;
     const uint32_t st = smem_u32(smem + s * stage_bytes);
     wg_fence();
-    mma_slice<2, 0>(acc, st + wg * (64 * 128), A_HALF_BYTES, st + 2 * A_HALF_BYTES, B_HALF_BYTES, 0u, i == 0);
+    mma_slice<2>(acc, st + wg * (64 * 128), A_HALF_BYTES, st + 2 * A_HALF_BYTES, B_HALF_BYTES, i == 0);
     wg_commit();
     if (i + 1 < n_sl) stage(i + 1, smem + (s ^ 1) * stage_bytes);
     wg_wait_all();
@@ -572,11 +582,11 @@ gemm_wx_kernel(const float* __restrict__ A, int64_t lda, int64_t M, int N, int K
     for (int j = 0; j < BK / 16; ++j) {
       const uint64_t a0 = make_desc(a + 32 * j), a1 = make_desc(a + A_HALF_BYTES + 32 * j);
       const uint64_t w0 = make_desc(b + 32 * j), w1 = make_desc(b + B_HALF_BYTES + 32 * j), w2 = make_desc(b + 2 * B_HALF_BYTES + 32 * j);
-      wgmma_128<0, true>(accm, a0, w0, (ks == 0 && j == 0) ? 0u : 1u);
-      wgmma_128<0, true>(accc, a1, w1, j == 0 ? 0u : 1u);
-      wgmma_128<0, true>(accc, a1, w0, 1u);
-      wgmma_128<0, true>(accc, a0, w2, 1u);
-      wgmma_128<0, true>(accc, a0, w1, 1u);
+      wgmma_128<true>(accm, a0, w0, (ks == 0 && j == 0) ? 0u : 1u);
+      wgmma_128<true>(accc, a1, w1, j == 0 ? 0u : 1u);
+      wgmma_128<true>(accc, a1, w0, 1u);
+      wgmma_128<true>(accc, a0, w2, 1u);
+      wgmma_128<true>(accc, a0, w1, 1u);
     }
     wg_commit();
     if (ks + 1 < n_slices) stage_a(ks + 1, smem + (s ^ 1) * stage_bytes);
@@ -610,26 +620,20 @@ static inline int sm_count() {
 inline size_t w_smem_bytes(int np) { return 2 * (size_t)np * (A_HALF_BYTES + B_HALF_BYTES) + 2 * sizeof(uint64_t) + 1024; }
 constexpr size_t TN_SMEM = 2 * (size_t)(2 * A_HALF_BYTES + 2 * B_HALF_BYTES) + 2 * sizeof(uint64_t) + 1024;
 
-template <int NP, bool APL, class Epi>
-static inline int launch_w(const float* A, int64_t lda, const Planes& Ap, int64_t M, int N, int K, const uint16_t* img, const Epi& epi,
-                           cudaStream_t st) {
+template <int NP, class Epi>
+static inline int gemm_w(const float* A, int64_t lda, int64_t M, int N, int K, const uint16_t* img, const Epi& epi, cudaStream_t st) {
+  if (M <= 0 || N <= 0) return 0;
   const size_t smem = w_smem_bytes(NP);
   static bool attr_set = false;   // per template instantiation
   if (!attr_set) {
-    NUDF_CUDA_OK(cudaFuncSetAttribute(gemm_w_kernel<NP, APL, Epi>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    NUDF_CUDA_OK(cudaFuncSetAttribute(gemm_w_kernel<NP, Epi>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr_set = true;
   }
   dim3 grid((unsigned)cdiv(M, BM), (unsigned)cdiv(N, BN));
   LaunchTimer lt_(epi_family<Epi>::value, st);
-  gemm_w_kernel<NP, APL, Epi><<<grid, THREADS, smem, st>>>(A, lda, Ap, M, N, K, img, epi);
+  gemm_w_kernel<NP, Epi><<<grid, THREADS, smem, st>>>(A, lda, M, N, K, img, epi);
   NUDF_LAUNCH_OK();
   return 0;
-}
-
-template <int NP, class Epi>
-static inline int gemm_w(const float* A, int64_t lda, int64_t M, int N, int K, const uint16_t* img, const Epi& epi, cudaStream_t st) {
-  if (M <= 0 || N <= 0) return 0;
-  return launch_w<NP, false>(A, lda, Planes{nullptr, 0}, M, N, K, img, epi, st);
 }
 
 // exact fp16-slice layer (gemm_wx_kernel); img / meta from chain::run_prep_jobs (udf_chain.cuh)

@@ -301,52 +301,6 @@ static void color_scratch_layout(const ColorPlan& p, int64_t P, ColorScratch* s)
   s->total = off;
 }
 
-__global__ void fold_kernel2(const float* __restrict__ g, const float* __restrict__ v, int out, int in, int64_t ld,
-                             float* __restrict__ w) {
-  int row = blockIdx.x;
-  if (row >= out) return;
-  const float* vr = v + (int64_t)row * in;
-  float ss = 0.f;
-  for (int k = threadIdx.x; k < in; k += blockDim.x) ss += vr[k] * vr[k];
-  __shared__ float red[32];
-  for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = ss;
-  __syncthreads();
-  if (threadIdx.x < 32) {
-    float t = threadIdx.x < (blockDim.x >> 5) ? red[threadIdx.x] : 0.f;
-    for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
-    if (threadIdx.x == 0) red[0] = t;
-  }
-  __syncthreads();
-  float s = g[row] / sqrtf(red[0]);
-  for (int k = threadIdx.x; k < ld; k += blockDim.x) w[(int64_t)row * ld + k] = k < in ? vr[k] * s : 0.f;
-}
-__global__ void unfold_kernel2(const float* __restrict__ g, const float* __restrict__ v, const float* __restrict__ dw,
-                               int out, int in, int64_t ld, float* __restrict__ dg, float* __restrict__ dv) {
-  int row = blockIdx.x;
-  if (row >= out) return;
-  const float* vr = v + (int64_t)row * in;
-  const float* dr = dw + (int64_t)row * ld;
-  float ss = 0.f, dot = 0.f;
-  for (int k = threadIdx.x; k < in; k += blockDim.x) { ss += vr[k] * vr[k]; dot += vr[k] * dr[k]; }
-  __shared__ float red[2][32];
-  for (int o = 16; o > 0; o >>= 1) { ss += __shfl_xor_sync(0xffffffffu, ss, o); dot += __shfl_xor_sync(0xffffffffu, dot, o); }
-  if ((threadIdx.x & 31) == 0) { red[0][threadIdx.x >> 5] = ss; red[1][threadIdx.x >> 5] = dot; }
-  __syncthreads();
-  if (threadIdx.x < 32) {
-    float t0 = threadIdx.x < (blockDim.x >> 5) ? red[0][threadIdx.x] : 0.f;
-    float t1 = threadIdx.x < (blockDim.x >> 5) ? red[1][threadIdx.x] : 0.f;
-    for (int o = 16; o > 0; o >>= 1) { t0 += __shfl_xor_sync(0xffffffffu, t0, o); t1 += __shfl_xor_sync(0xffffffffu, t1, o); }
-    if (threadIdx.x == 0) { red[0][0] = t0; red[1][0] = t1; }
-  }
-  __syncthreads();
-  float n = sqrtf(red[0][0]);
-  float dgv = red[1][0] / n;
-  if (threadIdx.x == 0) dg[row] = dgv;
-  float gn = g[row] / n;
-  for (int k = threadIdx.x; k < in; k += blockDim.x) dv[(int64_t)row * in + k] = gn * (dr[k] - dgv * vr[k] / n);
-}
-
 }  // namespace nudf
 
 using namespace nudf;

@@ -4,6 +4,7 @@
 // tests/proto/udf_pipeline.py (the torch prototype of exactly this sequence, checked against autograd).
 #include "../../include/nudf.h"
 #include "common.cuh"
+#include "ew_kernels.cuh"
 #include "gemm_engine.cuh"
 #include "udf_chain.cuh"
 #include <string.h>
@@ -77,14 +78,7 @@ static int make_plan(const nudf_udf_desc* d, UdfPlan* p) {
 // ---- context / scratch layout (all offsets in floats; every block starts 16B-aligned) -------------------------
 struct UdfCtx {
   int64_t e0, a[NUDF_MAX_LAYERS], y, sgn, d[NUDF_MAX_LAYERS], gpe, ge, total;
-  // plane mode (chain_planes_on()): D[l] lives only as a split-bf16 plane tensor.  pl_off: float offset of the plane
-  // area (aligned to 1024 B at run time), dpl[l]: uint16 offsets inside it.
-  int64_t pl_off, dpl[NUDF_MAX_LAYERS];
 };
-static inline uint16_t* plane_area(float* base, int64_t off) {
-  return reinterpret_cast<uint16_t*>((reinterpret_cast<uintptr_t>(base + off) + 1023) & ~(uintptr_t)1023);
-}
-static inline int cb_of(int cols) { return (cols + 63) / 64; }
 static void ctx_layout(const UdfPlan& p, int64_t P, int with_grad, UdfCtx* c) {
   int64_t off = 0;
   auto take = [&](int64_t n) { int64_t o = off; off += round_up(n, 4); return o; };
@@ -92,15 +86,8 @@ static void ctx_layout(const UdfPlan& p, int64_t P, int with_grad, UdfCtx* c) {
   for (int l = 1; l < p.n_lin; ++l) c->a[l] = take(P * p.a_ld[l]);
   c->y = take(P * p.y_ld);
   c->sgn = take(P);
-  c->pl_off = 0;
   if (with_grad) {
-    if (chain_planes_on()) {
-      int64_t e = 0;
-      for (int l = 0; l < p.n_lin - 1; ++l) { c->d[l] = 0; c->dpl[l] = e; e += tc::planes_elems(plane_rows(P), p.out_dim[l]); }
-      c->pl_off = take(e / 2 + 256);
-    } else {
-      for (int l = 0; l < p.n_lin - 1; ++l) c->d[l] = take(P * p.o_ld[l]);
-    }
+    for (int l = 0; l < p.n_lin - 1; ++l) c->d[l] = take(P * p.o_ld[l]);
     c->gpe = take(P * p.pe_ld);
     c->ge = take(P * p.pe_ld);
   }
@@ -108,7 +95,6 @@ static void ctx_layout(const UdfPlan& p, int64_t P, int with_grad, UdfCtx* c) {
 }
 struct UdfScratch {
   int64_t edot, adot[2], q[NUDF_MAX_LAYERS], zlast, total;
-  int64_t pl_off, adpl[NUDF_MAX_LAYERS];     // plane mode: Adot[l] (input of layer l of the tangent chain)
 };
 static void scratch_layout(const UdfPlan& p, int64_t P, UdfScratch* s) {
   int64_t off = 0;
@@ -118,65 +104,10 @@ static void scratch_layout(const UdfPlan& p, int64_t P, UdfScratch* s) {
   s->adot[1] = take(P * p.max_ld);
   for (int l = 0; l < p.n_lin - 1; ++l) s->q[l] = take(P * p.o_ld[l]);
   s->zlast = take(P * p.y_ld);
-  s->pl_off = 0;
-  if (chain_planes_on()) {
-    int64_t e = 0;
-    for (int l = 0; l < p.n_lin; ++l) { s->adpl[l] = e; e += tc::planes_elems(plane_rows(P), p.in_dim[l]); }
-    s->pl_off = take(e / 2 + 256);
-  }
   s->total = off;
 }
 
 // ---- element-wise kernels ---------------------------------------------------------------------------------------
-
-// W = g * v / ||v||  per output row (legacy weight_norm, dim=0); rows padded with zeros up to ld.
-__global__ void fold_kernel(const float* __restrict__ g, const float* __restrict__ v, int out, int in, int64_t ld,
-                            float* __restrict__ w) {
-  int row = blockIdx.x;
-  if (row >= out) return;
-  const float* vr = v + (int64_t)row * in;
-  float ss = 0.f;
-  for (int k = threadIdx.x; k < in; k += blockDim.x) ss += vr[k] * vr[k];
-  __shared__ float red[32];
-  for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = ss;
-  __syncthreads();
-  if (threadIdx.x < 32) {
-    float t = threadIdx.x < (blockDim.x >> 5) ? red[threadIdx.x] : 0.f;
-    for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
-    if (threadIdx.x == 0) red[0] = t;
-  }
-  __syncthreads();
-  float s = g[row] / sqrtf(red[0]);
-  for (int k = threadIdx.x; k < ld; k += blockDim.x) w[(int64_t)row * ld + k] = k < in ? vr[k] * s : 0.f;
-}
-
-// dW -> dg = <dW, v>/||v|| ; dv = g/||v|| (dW - dg v/||v||)
-__global__ void unfold_kernel(const float* __restrict__ g, const float* __restrict__ v, const float* __restrict__ dw,
-                              int out, int in, int64_t ld, float* __restrict__ dg, float* __restrict__ dv) {
-  int row = blockIdx.x;
-  if (row >= out) return;
-  const float* vr = v + (int64_t)row * in;
-  const float* dr = dw + (int64_t)row * ld;
-  float ss = 0.f, dot = 0.f;
-  for (int k = threadIdx.x; k < in; k += blockDim.x) { ss += vr[k] * vr[k]; dot += vr[k] * dr[k]; }
-  __shared__ float red[2][32];
-  for (int o = 16; o > 0; o >>= 1) { ss += __shfl_xor_sync(0xffffffffu, ss, o); dot += __shfl_xor_sync(0xffffffffu, dot, o); }
-  if ((threadIdx.x & 31) == 0) { red[0][threadIdx.x >> 5] = ss; red[1][threadIdx.x >> 5] = dot; }
-  __syncthreads();
-  if (threadIdx.x < 32) {
-    float t0 = threadIdx.x < (blockDim.x >> 5) ? red[0][threadIdx.x] : 0.f;
-    float t1 = threadIdx.x < (blockDim.x >> 5) ? red[1][threadIdx.x] : 0.f;
-    for (int o = 16; o > 0; o >>= 1) { t0 += __shfl_xor_sync(0xffffffffu, t0, o); t1 += __shfl_xor_sync(0xffffffffu, t1, o); }
-    if (threadIdx.x == 0) { red[0][0] = t0; red[1][0] = t1; }
-  }
-  __syncthreads();
-  float n = sqrtf(red[0][0]);
-  float dgv = red[1][0] / n;          // <dW, v/||v||>
-  if (threadIdx.x == 0) dg[row] = dgv;
-  float gn = g[row] / n;
-  for (int k = threadIdx.x; k < in; k += blockDim.x) dv[(int64_t)row * in + k] = gn * (dr[k] - dgv * vr[k] / n);
-}
 
 // E0 = PE(x*scale) [P, pe_ld]; optionally also E0/sqrt2 into the skip columns of A[skip].
 __global__ void pe_forward_kernel(const float* __restrict__ pts, int64_t P, int L, float scale, float* __restrict__ e0,
@@ -289,16 +220,6 @@ __global__ void pe_jvp_kernel(const float* __restrict__ pts, const float* __rest
     f *= 2.0f;
   }
   for (int c = d_pe; c < pe_ld; ++c) e[c] = 0.f;
-}
-
-// dst[:, col0 + c] = src[:, c] * scale   for c < ncols
-__global__ void copy_cols_kernel(const float* __restrict__ src, int64_t lds, float* __restrict__ dst, int64_t ldd, int col0,
-                                 int ncols, int64_t P, float scale) {
-  int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  int64_t row = idx / ncols;
-  int c = (int)(idx - row * ncols);
-  if (row >= P) return;
-  dst[row * ldd + col0 + c] = src[row * lds + c] * scale;
 }
 
 // out[c] (+)= sum_rows w[row] * X[row, c]   (w may be null = 1).  grid: (col tiles of 32, row chunks).  With several row
@@ -436,45 +357,8 @@ static int value_chain(const UdfPlan& p, const nudf_udf_desc* d, const float* wf
   return 0;
 }
 
-// Reverse sweep with D[l] carried as plane tensors: every GEMM fetches its A operand with cp.async.bulk (gemm_wrp_kernel).
-static int reverse_chain_planes(const UdfPlan& p, const float* wfold, const float* pts, int64_t P, float* ctx, const UdfCtx& c,
-                                float* grad, cudaStream_t st) {
-  const int last = p.n_lin - 1;
-  uint16_t* pla = plane_area(ctx, c.pl_off);
-  auto dpl = [&](int l) { return tc::Planes{pla + c.dpl[l], cb_of(p.out_dim[l])}; };
-  auto make_rev = [&](int l) {
-    EpiRevP e;
-    e.n_main = p.out_dim[l - 1];
-    e.post_scale = (l == p.skip) ? NUDF_SQRT1_2 : 1.0f;
-    e.Anext = ctx + c.a[l]; e.lda = p.a_ld[l]; e.a_unscale = (l == p.skip) ? 1.41421356237309504880f : 1.0f;
-    e.dpl = dpl(l - 1);
-    e.Gpe = (l == p.skip) ? ctx + c.gpe : nullptr; e.ldg = p.pe_ld;
-    return e;
-  };
-  for (int l = 0; l < last; ++l)                      // rows [P, round_up(P, 64)) are part of the weight-gradient contraction
-    if (int rc = tc::zero_pad_rows(P, dpl(l), st)) return rc;
-  {
-    EpiRevP e = make_rev(last);
-    int cols4 = (p.in_dim[last] + 3) / 4;
-    rev_init_kernel<EpiRevP><<<nblk(P * cols4, 256), 256, 0, st>>>(ctx + c.sgn, wfold + p.w_off[last], p.in_dim[last], 1.0f / p.scale, P, e);
-    NUDF_LAUNCH_OK();
-  }
-  for (int l = last - 1; l >= 1; --l) {
-    EpiRevP e = make_rev(l);
-    if (int rc = tc::gemm_wrp(dpl(l), P, p.in_dim[l], p.out_dim[l], img_base(p, wfold) + p.img_nn[l], e, st)) return rc;
-  }
-  {
-    EpiRevFinal e{ctx + c.ge, p.pe_ld, p.skip >= 1 ? ctx + c.gpe : nullptr, p.pe_ld};
-    if (int rc = tc::gemm_wrp(dpl(0), P, p.in_dim[0], p.out_dim[0], img_base(p, wfold) + p.img_nn[0], e, st)) return rc;
-  }
-  pe_vjp_kernel<<<nblk(P, 128), 128, 0, st>>>(pts, ctx + c.ge, p.pe_ld, P, p.L, p.scale, grad);
-  NUDF_LAUNCH_OK();
-  return 0;
-}
-
 static int reverse_chain(const UdfPlan& p, const float* wfold, const float* pts, int64_t P, float* ctx, const UdfCtx& c,
                          float* grad, cudaStream_t st) {
-  if (chain_planes_on()) return reverse_chain_planes(p, wfold, pts, P, ctx, c, grad, st);
   const int last = p.n_lin - 1;
   auto make_rev = [&](int l) {  // epilogue that turns G (wrt A[l]) into D[l-1]
     EpiRev e;
@@ -634,38 +518,7 @@ static int udf_backward_impl(const nudf_udf_desc* d, const float* wfold, const f
   const int split = (int)cdiv(P, 2048);
 
   // ---- tangent chain (second-order terms) ----
-  if (grad_bar && chain_planes_on()) {
-    // plane mode: D[l] (ctx) and Adot[l] (scratch) are split-bf16 plane tensors; the chain kernels and the weight gradients
-    // fetch them with cp.async.bulk.  (A ctx filled without its gradient part never gets here: grad_bar is null then.)
-    uint16_t* cpl = plane_area(ctx, c.pl_off);
-    uint16_t* spl = plane_area(scratch, s.pl_off);
-    auto dpl = [&](int l) { return tc::Planes{cpl + c.dpl[l], cb_of(p.out_dim[l])}; };
-    auto adpl = [&](int l) { return tc::Planes{spl + s.adpl[l], cb_of(p.in_dim[l])}; };
-    float* edot = scratch + s.edot;
-    pe_jvp_kernel<<<nblk(P, 128), 128, 0, st>>>(pts, grad_bar, P, p.L, p.scale, edot, p.pe_ld);
-    NUDF_LAUNCH_OK();
-    if (int rc = tc::pack_planes(edot, p.pe_ld, P, p.d_pe, adpl(0), st)) return rc;
-    for (int l = 1; l <= last; ++l)
-      if (int rc = tc::zero_pad_rows(P, adpl(l), st)) return rc;
-    float* adot_last = scratch + s.adot[0];                     // fp32 copy of Adot[last] for the weighted column sum
-    for (int l = 0; l < last; ++l) {
-      EpiAtomicAdd ew{dwfold + p.w_off[l], p.w_ld[l]};          // dW_l += D_l^T Adot_l
-      if (int rc = gemm_tn_planes(dpl(l), p.out_dim[l], adpl(l), p.in_dim[l], P, ew, st)) return rc;
-      EpiTanP et;
-      et.Anext = ctx + c.a[l + 1]; et.lda = p.a_ld[l + 1];
-      et.a_unscale = (l + 1 == p.skip) ? 1.41421356237309504880f : 1.0f;
-      et.D = dpl(l);
-      et.Q = scratch + s.q[l]; et.ldq = p.o_ld[l];
-      et.npl = adpl(l + 1); et.post_scale = (l + 1 == p.skip) ? NUDF_SQRT1_2 : 1.0f;
-      et.AdotNext = (l + 1 == last) ? adot_last : nullptr; et.ldn = p.a_ld[l + 1];
-      if (int rc = tc::gemm_wrp(adpl(l), P, p.out_dim[l], p.in_dim[l], img_base(p, wfold) + p.img_nt[l], et, st)) return rc;
-      if (l + 1 == p.skip) {
-        copy_cols_planes_kernel<<<nblk(P * p.d_pe, 256), 256, 0, st>>>(edot, p.pe_ld, adpl(l + 1), p.out_dim[l], p.d_pe, P, NUDF_SQRT1_2);
-        NUDF_LAUNCH_OK();
-      }
-    }
-    if (int rc = colsum(adot_last, p.a_ld[last], ctx + c.sgn, 1.0f / p.scale, P, p.in_dim[last], dwfold + p.w_off[last], st)) return rc;
-  } else if (grad_bar) {
+  if (grad_bar) {
     float* edot = scratch + s.edot;
     pe_jvp_kernel<<<nblk(P, 128), 128, 0, st>>>(pts, grad_bar, P, p.L, p.scale, edot, p.pe_ld);
     NUDF_LAUNCH_OK();
@@ -687,8 +540,8 @@ static int udf_backward_impl(const nudf_udf_desc* d, const float* wfold, const f
                            img_base(p, wfold) + p.img_nt[l], TC_TAN))
         return rc;
       if (l + 1 == p.skip) {
-        copy_cols_kernel<<<nblk(P * p.d_pe, 256), 256, 0, st>>>(edot, p.pe_ld, nxt, ld_nxt, p.out_dim[l], p.d_pe, P,
-                                                                 NUDF_SQRT1_2);
+        ew_copy_cols_kernel<<<nblk(P * p.d_pe, 256), 256, 0, st>>>(edot, p.pe_ld, nxt, ld_nxt, p.out_dim[l], p.d_pe, P,
+                                                                    NUDF_SQRT1_2);
         NUDF_LAUNCH_OK();
       }
       adot = nxt; ld_adot = ld_nxt;
@@ -704,10 +557,10 @@ static int udf_backward_impl(const nudf_udf_desc* d, const float* wfold, const f
       NUDF_CUDA_OK(cudaMemsetAsync(scratch + s.q[l], 0, sizeof(float) * P * p.o_ld[l], st));
   float* zl = scratch + s.zlast;
   const int F = p.d_out - 1;
-  const bool split_head = out_bar && tc_on(TC_BWD) && F >= 64 && (F % 4) == 0 && tc::pad64(F) <= 64 * tc::WR_MAX_SLICES;
+  // 257 = 1 udf-head row + 256 feature rows: the feature block is the K (at most 256) of a contraction on the weights-resident
+  // tensor kernel, the head row a rank-1 update in its epilogue (and a weighted column sum for its weight gradient).
+  const bool split_head = out_bar && tc_on(TC_BWD) && F >= 64 && (F % 4) == 0 && F <= 256;
   if (split_head) {
-    // 257 = 1 udf-head row + 256 feature rows: the feature block is a K = 256 contraction for the weights-resident tensor
-    // kernel, the head row a rank-1 update in its epilogue (and a weighted column sum for its weight gradient).
     float* zf = zl;
     float* z0 = zl + P * F;
     zlast_split_kernel<<<nblk(P * p.d_out, 256), 256, 0, st>>>(ub, ld_ub, fb, ld_fb, ctx + c.sgn, 1.0f / p.scale, F, P, zf, z0);

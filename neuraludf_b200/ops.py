@@ -111,8 +111,8 @@ class UdfHandle:
         ps = self.params()
         _require_cuda(*ps)
         lib_ = L.lib()
-        # the folded images depend on the engine and on which chains run fused (chain mask, plane mode)
-        key = tuple((p.data_ptr(), p._version) for p in ps) + (lib_.nudf_get_engine(), lib_.nudf_get_tc_mask(), lib_.nudf_get_chain_planes())
+        # the folded images depend on the engine and on which chains run fused (chain mask)
+        key = tuple((p.data_ptr(), p._version) for p in ps) + (lib_.nudf_get_engine(), lib_.nudf_get_tc_mask())
         if key == self._key:
             return
         d = L.UdfDesc()

@@ -24,7 +24,7 @@ def test_library_exports_every_declared_symbol():
     for name in declared:
         assert hasattr(L, name), "libnudf.so does not export %s" % name
     assert sorted(_lib.exported_symbols()) == declared, "python binding and include/nudf.h disagree"
-    assert L.nudf_abi_version() == 3
+    assert L.nudf_abi_version() == 4
 
 
 def test_descriptor_validation_runs_without_gpu():

@@ -32,17 +32,15 @@ def _loss(ret):
     return loss + 0.5 * ((ret["patch_colors"] - 0.4).abs().mean(dim=(1, 2)) * pm).sum() / (pm.sum() + 1e-5)
 
 
-@pytest.mark.parametrize("engine", [0, 1, 2])
+@pytest.mark.parametrize("engine", [0, 1])
 def test_render_core_blending_vs_reference(golden, fx, engine):
-    """engine 0: exact fp32; 1: tensor engine (default chains); 2: tensor engine with the plane-fed reverse-sweep / tangent
-    chains and plane-fed weight gradients (nudf_set_chain_planes)"""
+    """engine 0: exact fp32; 1: tensor engine (default chains)"""
     from neuraludf_b200 import _lib
     from neuraludf_b200.models.udf_renderer_blending import UDFRendererBlending
     from oracle.make_golden import GRAD_STRIDE
     L = _lib.lib()
-    old, old_pl = L.nudf_get_engine(), L.nudf_get_chain_planes()
-    L.nudf_set_engine(min(engine, 1))
-    L.nudf_set_chain_planes(1 if engine == 2 else 0)
+    old = L.nudf_get_engine()
+    L.nudf_set_engine(engine)
     try:
         udf, col, nerf, var, beta = build_modules(golden, DEV)
         ren = UDFRendererBlending(nerf, udf, var, col, beta, n_samples=S, n_importance=0, n_outside=N_OUT,
@@ -92,7 +90,6 @@ def test_render_core_blending_vs_reference(golden, fx, engine):
         assert float(col.lin4.weight_v.grad[3:].abs().max()) > 0
     finally:
         L.nudf_set_engine(old)
-        L.nudf_set_chain_planes(old_pl)
 
 
 def test_whole_render_with_blending_runs_and_trains_all_networks(golden):

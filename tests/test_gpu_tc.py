@@ -87,72 +87,6 @@ def test_wgrad_tc_vs_fp64(P, n_out, n_in):
         assert e < 5e-5, (engine, e)
 
 
-def _planes(L, lib, x):
-    rows, cols = x.shape
-    buf = torch.empty(lib.nudf_planes_elems(rows, cols) + 512, dtype=torch.int16, device=DEV)
-    off = (-buf.data_ptr() % 1024) // 2
-    pl = buf[off:off + lib.nudf_planes_elems(rows, cols)]
-    pl.fill_(0x7FC0)                                  # bf16 NaN everywhere: pad rows must be rewritten by the packer
-    L.check(lib.nudf_pack_planes(L.ptr(x), x.stride(0), rows, cols, L.ptr(pl), L.stream_ptr()), "pack")
-    return pl
-
-
-@pytest.mark.parametrize("rows,cols", [(1, 5), (130, 64), (257, 217), (4096, 256)])
-def test_planes_round_trip(rows, cols):
-    """fp32 -> split-bf16 planes -> fp32: 16 mantissa bits survive (relative error <= 2^-16)"""
-    L, lib = _lib()
-    g = torch.Generator().manual_seed(rows + cols)
-    x = (torch.randn(rows, cols, generator=g) * torch.logspace(-3, 3, cols)[None, :]).to(DEV).contiguous()
-    pl = _planes(L, lib, x)
-    y = torch.full_like(x, float("nan"))
-    L.check(lib.nudf_unpack_planes(L.ptr(pl), rows, cols, L.ptr(y), y.stride(0), L.stream_ptr()), "unpack")
-    assert float(((y - x).abs() / x.abs().clamp(min=1e-30)).max()) <= 2.0 ** -16
-
-
-@pytest.mark.parametrize("M,N,K,act", [(4096, 256, 256, 2), (300, 217, 256, 0), (129, 256, 39, 0), (1000, 39, 217, 0), (65536, 256, 256, 2)])
-def test_dense_planes_vs_fp64(M, N, K, act):
-    """one layer on the plane-fed weights-resident kernel (A operand fetched as plane blocks by cp.async.bulk)"""
-    L, lib = _lib()
-    g = torch.Generator().manual_seed(M + N + K)
-    X = torch.randn(M, K, generator=g, dtype=torch.float64) * 0.5
-    W = torch.randn(N, K, generator=g, dtype=torch.float64) / K ** 0.5
-    b = torch.randn(N, generator=g, dtype=torch.float64) * 0.1
-    ref = X @ W.t() + b
-    if act == 2:
-        ref = torch.nn.functional.softplus(ref, beta=100)
-    Xd = X.float().to(DEV).contiguous()
-    rows_pad = (M + 127) // 128 * 128
-    buf = torch.empty(lib.nudf_planes_elems(rows_pad, K) + 512, dtype=torch.int16, device=DEV)
-    off = (-buf.data_ptr() % 1024) // 2
-    pl = buf[off:off + lib.nudf_planes_elems(rows_pad, K)]
-    pl.fill_(0x7FC0)                                  # NaN in the rows beyond M: they must not leak into valid rows
-    L.check(lib.nudf_pack_planes(L.ptr(Xd), K, M, K, L.ptr(pl), L.stream_ptr()), "pack")
-    img = _image(W.float().to(DEV).contiguous(), N, K, 0)
-    Y = torch.full((M, N), float("nan"), device=DEV)
-    bd = b.float().to(DEV)
-    L.check(lib.nudf_dense_forward_planes(L.ptr(pl), L.ptr(img), L.ptr(bd), L.ptr(Y), N, M, N, K, act, L.stream_ptr()), "dense_planes")
-    e = err_inf(Y, ref) / scale_inf(ref)
-    report("tc.dense_planes[%d,%d,%d]" % (M, N, K), rel=e)
-    assert e < 3e-5, e
-
-
-@pytest.mark.parametrize("P,n_out,n_in", [(4096, 256, 256), (1000, 128, 64), (70, 257, 39), (65536, 256, 256), (333, 217, 256)])
-def test_wgrad_planes_vs_fp64(P, n_out, n_in):
-    """weight-gradient contraction with both operands fetched as plane blocks (MN-major UMMA operands)"""
-    L, lib = _lib()
-    g = torch.Generator().manual_seed(P + n_out)
-    dZ = torch.randn(P, n_out, generator=g, dtype=torch.float64)
-    X = torch.randn(P, n_in, generator=g, dtype=torch.float64)
-    ref = dZ.t() @ X
-    dZp = _planes(L, lib, dZ.float().to(DEV).contiguous())
-    Xp = _planes(L, lib, X.float().to(DEV).contiguous())
-    dW = torch.zeros(n_out, n_in, device=DEV)
-    L.check(lib.nudf_wgrad_planes(L.ptr(dZp), L.ptr(Xp), n_out, n_in, P, L.ptr(dW), n_in, L.stream_ptr()), "wgrad_planes")
-    e = err_inf(dW, ref) / scale_inf(ref)
-    report("tc.wgrad_planes[%d,%d,%d]" % (P, n_out, n_in), rel=e)
-    assert e < 5e-5, e
-
-
 @pytest.mark.parametrize("mask", [0, 62, -1, 63])
 def test_render_core_accuracy_by_tc_mask(golden, mask):
     """How far each choice of tensor-engine chains moves render_core from the fp64 reference (reported; the default

@@ -21,26 +21,14 @@ for npl in (2, 3):
     im = torch.zeros(lib.nudf_tc_image_elems(256, 256, npl), dtype=torch.int16, device=dev)
     lib.nudf_tc_prepare_weights(L.ptr(W), 256, 256, 256, 0, npl, L.ptr(im), st)
     imgs[npl] = im
-def planes(x):
-    n = lib.nudf_planes_elems(x.shape[0], x.shape[1])
-    buf = torch.empty(n + 512, dtype=torch.int16, device=dev)
-    off = (-buf.data_ptr() % 1024) // 2
-    pl = buf[off:off + n]
-    lib.nudf_pack_planes(L.ptr(x), x.stride(0), x.shape[0], x.shape[1], L.ptr(pl), st)
-    return pl
 
-
-Xp, Yp = planes(X), planes(Y)
 if len(sys.argv) > 1 and sys.argv[1] == "time":
     flush = torch.empty(64 * 1024 * 1024, device=dev)
     calls = {
         "wgrad_tc_fp32_operands": lambda: lib.nudf_wgrad(L.ptr(Y), 256, L.ptr(X), 256, 256, 256, P, L.ptr(dW), 256, 1, st),
-        "wgrad_tc_plane_operands": lambda: lib.nudf_wgrad_planes(L.ptr(Yp), L.ptr(Xp), 256, 256, P, L.ptr(dW), 256, st),
         "dense_fp32_ffma2": lambda: lib.nudf_dense_forward(L.ptr(X), 256, L.ptr(W), 256, L.ptr(b), L.ptr(Y), 256, P, 256, 256, 2, st),
         "wgrad_fp32_ffma2": lambda: lib.nudf_wgrad(L.ptr(Y), 256, L.ptr(X), 256, 256, 256, P, L.ptr(dW), 256, 0, st),
         "dense_tc_fp32_operand": lambda: lib.nudf_dense_forward_tc(L.ptr(X), 256, L.ptr(imgs[2]), 2, L.ptr(b), L.ptr(Y), 256, P, 256, 256, 2, st),
-        "dense_tc_plane_operand": lambda: lib.nudf_dense_forward_planes(L.ptr(Xp), L.ptr(imgs[2]), L.ptr(b), L.ptr(Y), 256, P, 256, 256, 2, st),
-        "pack_planes": lambda: lib.nudf_pack_planes(L.ptr(X), 256, P, 256, L.ptr(Xp), st),
     }
     for name, call in calls.items():
         if len(sys.argv) > 2 and name != sys.argv[2]:
@@ -56,8 +44,6 @@ if len(sys.argv) > 1 and sys.argv[1] == "time":
         print("%s: %.1f us" % (name, t / 10 * 1e3))
     sys.exit(0)
 for _ in range(2):
-    lib.nudf_wgrad_planes(L.ptr(Yp), L.ptr(Xp), 256, 256, P, L.ptr(dW), 256, st)
-    lib.nudf_dense_forward_planes(L.ptr(Xp), L.ptr(imgs[2]), L.ptr(b), L.ptr(Y), 256, P, 256, 256, 2, st)
     lib.nudf_dense_forward(L.ptr(X), 256, L.ptr(W), 256, L.ptr(b), L.ptr(Y), 256, P, 256, 256, 2, st)
     lib.nudf_dense_forward_tc(L.ptr(X), 256, L.ptr(imgs[2]), 2, L.ptr(b), L.ptr(Y), 256, P, 256, 256, 2, st)
     lib.nudf_dense_forward_tc(L.ptr(X), 256, L.ptr(imgs[3]), 3, L.ptr(b), L.ptr(Y), 256, P, 256, 256, 2, st)
