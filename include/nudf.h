@@ -32,8 +32,8 @@ const char* nudf_last_error(void);
  * when built with the tensor path).  Small / odd-shaped contractions always use the FFMA engine. */
 int nudf_set_engine(int engine);
 int nudf_get_engine(void);
-/* Which contraction chains may use the tensor engine (bit mask; default 254 = all but the UDF value chain, whose exact
- * fp16-slice kernel is 1.5x the reference's fp32 noise on the udf head; the colour / NeRF++ forward uses three bf16 planes): 1 UDF forward value, 2 reverse sweep (grad_x udf), 4 tangent,
+/* Which contraction chains may use the tensor engine (bit mask; default 255 = all; the UDF value chain and the colour /
+ * NeRF++ forward use three bf16 planes, the udf-head row stays exact fp32): 1 UDF forward value, 2 reverse sweep (grad_x udf), 4 tangent,
  * 8 backward, 16 weight gradients, 32 colour-network backward, 64 NeRF++ backward, 128 colour / NeRF++ forward. */
 int nudf_set_tc_mask(int mask);
 int nudf_get_tc_mask(void);

@@ -2,15 +2,17 @@
 //   engine 0: exact-fp32 FFMA kernel (gemm_simt.cuh) -- always used for small / odd shapes;
 //   engine 1: wgmma split-bf16 tensor-core kernels (gemm_tc.cuh) when the caller supplies the pre-split weight
 //             image built at fold time (gemm_nt / gemm_nn) or for the weight-gradient contraction (gemm_tn).
-// Which chains may use the tensor engine is a bit mask (NUDF_TC_MASK, see tc_mask()): the forward value chain needs
-// fp32-grade accuracy (udf feeds exp(-25000 u) and sigmoid(400 u)), the other chains tolerate the 3xBF16 split.
+// Which chains may use the tensor engine is a bit mask (NUDF_TC_MASK, see tc_mask()): the forward passes need fp32-grade
+// accuracy (udf feeds exp(-25000 u) and sigmoid(400 u); ReLU gates), so they take three bf16 planes / six products, the
+// gradient chains tolerate the 2-plane (3-product) split.
 #pragma once
 #include <stdlib.h>
 #include "gemm_tc.cuh"
 
 namespace nudf {
 
-// TC_FWD: UDF value chain (exact fp16 slices, tc::gemm_wx; off by default, capi.cu); TC_REV/TAN/BWD: UDF gradient, tangent and backward chains; TC_WGRAD:
+// TC_FWD: UDF value chain (hidden layers and feature rows on gemm_w<3>; the udf-head row stays an exact-fp32 dot product,
+// udf_net.cu); TC_REV/TAN/BWD: UDF gradient, tangent and backward chains; TC_WGRAD:
 // weight gradients; TC_COLOR / TC_NERF: BACKWARD data GEMMs of the ReLU networks (2 planes); TC_RELU_FWD: their forward passes,
 // with 3 planes / 6 products (gemm_w<3>, per-K-slice accumulators summed in fp32): a 4e-6 perturbation of a pre-activation (the
 // 2-plane split) flips ~60x more ReLU gates than the reference's own fp32 rounding does, which shows up as O(1/batch) jumps in

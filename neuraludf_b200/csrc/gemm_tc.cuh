@@ -7,7 +7,6 @@
 // through shared memory to the fused epilogue functor (4 consecutive columns of a row per call: coalesced).
 #pragma once
 #include <cuda_bf16.h>
-#include <cuda_fp16.h>
 
 #include "gemm_simt.cuh"
 
@@ -145,55 +144,51 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// r + half an ulp of r with the sign of r (the exponent bits times 2^-24): a result the tensor core truncated toward zero,
+// moved to the middle of its truncation interval
+__device__ __forceinline__ float unbias_rz(float r) { return fmaf(__uint_as_float(__float_as_uint(r) & 0xff800000u), 0x1p-24f, r); }
 
-// D[64 x 128] (+)= A[64 x 16] B[128 x 16]^T from shared memory (both K-major), bf16 or (F16) fp16 operands
-#define NUDF_WGMMA_M64N128K16(TYPE) \
-  asm volatile( \
-      "{\n" \
-      ".reg .pred p;\n" \
-      "setp.ne.b32 p, %66, 0;\n" \
-      "wgmma.mma_async.sync.aligned.m64n128k16.f32." TYPE "." TYPE " " \
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, " \
-      "%26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, " \
-      "%50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n" \
-      "}\n" \
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), \
-        "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), \
-        "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), \
-        "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), \
-        "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), \
-        "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), \
-        "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]) \
-      : "l"(da), "l"(db), "r"(accumulate))
-template <bool F16 = false>
+// D[64 x 128] (+)= A[64 x 16] B[128 x 16]^T from shared memory (both K-major), bf16 operands
 __device__ __forceinline__ void wgmma_128(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
-  if constexpr (F16) NUDF_WGMMA_M64N128K16("f16");
-  else NUDF_WGMMA_M64N128K16("bf16");
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, "
+      "%26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, "
+      "%50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+        "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
+        "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),
+        "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]),
+        "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]),
+        "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]),
+        "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(accumulate));
 }
 
 // The wgmma group of one 64-wide K slice, smallest products first; plane p at +p * stride, 32 B per 16-wide K step.
+// With 3 planes only the five correction products (lo * hi, hi * lo, mid * mid, mid * hi, hi * mid: ~2^-8 of the result's
+// scale, so the tensor core's truncation of each wgmma result to fp32 costs ~2^-32 of it); gemm_w_kernel issues the hi * hi
+// steps one at a time into fresh accumulators and adds them up in fp32 with round-to-nearest.
 template <int NP>
 __device__ __forceinline__ void mma_slice(float (&d)[64], uint32_t a, uint32_t a_stride, uint32_t b, uint32_t b_stride, bool zero_first) {
+  auto desc = [](uint32_t base, uint32_t stride, int p, int j) { return make_desc(base + p * stride + 32u * j); };
 #pragma unroll
   for (int j = 0; j < BK / 16; ++j) {
-    uint64_t da[NP], db[NP];
-#pragma unroll
-    for (int p = 0; p < NP; ++p) {
-      da[p] = make_desc(a + p * a_stride + 32u * j);
-      db[p] = make_desc(b + p * b_stride + 32u * j);
-    }
     const uint32_t acc0 = (zero_first && j == 0) ? 0u : 1u;
-    if (NP == 2) {
-      wgmma_128(d, da[1], db[0], acc0);
-      wgmma_128(d, da[0], db[1], 1u);
-      wgmma_128(d, da[0], db[0], 1u);
+    if constexpr (NP == 2) {
+      wgmma_128(d, desc(a, a_stride, 1, j), desc(b, b_stride, 0, j), acc0);
+      wgmma_128(d, desc(a, a_stride, 0, j), desc(b, b_stride, 1, j), 1u);
+      wgmma_128(d, desc(a, a_stride, 0, j), desc(b, b_stride, 0, j), 1u);
     } else {
-      wgmma_128(d, da[NP - 1], db[0], acc0);        // lo * hi
-      wgmma_128(d, da[0], db[NP - 1], 1u);          // hi * lo
-      wgmma_128(d, da[1], db[1], 1u);               // mid * mid
-      wgmma_128(d, da[1], db[0], 1u);               // mid * hi
-      wgmma_128(d, da[0], db[1], 1u);               // hi * mid
-      wgmma_128(d, da[0], db[0], 1u);               // hi * hi
+      wgmma_128(d, desc(a, a_stride, 2, j), desc(b, b_stride, 0, j), acc0);   // lo * hi
+      wgmma_128(d, desc(a, a_stride, 0, j), desc(b, b_stride, 2, j), 1u);     // hi * lo
+      wgmma_128(d, desc(a, a_stride, 1, j), desc(b, b_stride, 1, j), 1u);     // mid * mid
+      wgmma_128(d, desc(a, a_stride, 1, j), desc(b, b_stride, 0, j), 1u);     // mid * hi
+      wgmma_128(d, desc(a, a_stride, 0, j), desc(b, b_stride, 1, j), 1u);     // hi * mid
     }
   }
 }
@@ -375,7 +370,10 @@ gemm_w_kernel(const float* __restrict__ A, int64_t lda, int64_t M, int N, int K,
     fence_proxy_async();
   }
   __syncthreads();
-  // 3 planes: each K slice in fresh registers, added to the running sum in fp32 (short truncating accumulation chains)
+  // 3 planes: the corrections of each K slice and each 16-wide hi * hi step in fresh registers, summed in fp32 with
+  // round-to-nearest.  The tensor core truncates a wgmma result toward zero; every hi * hi result is a single truncation of
+  // 16 full-size products, so adding half an ulp of it (with its sign) leaves an unbiased error.  Without that the bias of
+  // the 16 truncations per output (K = 256) adds up coherently over the points of a parameter-gradient sum.
   float acc[64], tot[NP == 3 ? 64 : 1];
 #pragma unroll
   for (int q = 0; q < 64; ++q) acc[q] = 0.f;
@@ -394,6 +392,15 @@ gemm_w_kernel(const float* __restrict__ A, int64_t lda, int64_t M, int N, int K,
     if constexpr (NP == 3) {
 #pragma unroll
       for (int q = 0; q < 64; ++q) tot[q] += acc[q];
+#pragma unroll
+      for (int j = 0; j < BK / 16; ++j) {
+        wg_fence();
+        wgmma_128(acc, make_desc(st + wg * (64 * 128) + 32u * j), make_desc(st + a_bytes + 32u * j), 0u);   // hi * hi
+        wg_commit();
+        wg_wait_all();
+#pragma unroll
+        for (int q = 0; q < 64; ++q) tot[q] += unbias_rz(acc[q]);
+      }
     }
     fence_proxy_async();
     __syncthreads();
@@ -479,134 +486,6 @@ gemm_tn_kernel(const float* __restrict__ A, int64_t lda, const float* __restrict
   tile_epilogue(acc_s, m0, M, n0, N, epi, tid);
 }
 
-// ---------------------------------------------------------------------------------------------------------------
-// Exact fp16-slice layer for the UDF value chain (its udf head feeds exp(-25000 u)), Y = epi(A W^T):
-//   operand row r:  a = 2^(e_r - 11) (a0 + a1), a0 = rint(a 2^(11 - e_r)) (|a0| <= 2048, exact in fp16), a1 = fp16(remainder),
-//                   2^e_r > max_k |a_rk| (one power of two per row, from a pre-pass over the CTA's rows);
-//   weights:        w = 2^(E - 13) (w0 + w1 + w2), w0 = 1024 rint(w 2^(3 - E)), w1 = fp16(1024 remainder), w2 = fp16(second
-//                   remainder), 2^E > max |W| of the layer (images and meta[1] = 2^(E - 13): udf_chain.cuh).
-// Main accumulator M = sum a0 w0: integer multiples of 2^10 below 2^32, so the tensor core's fp32 accumulation is exact.
-// Correction C = sum a0 w1 + a0 w2 + a1 w0 + a1 w1 is ~2^-3 of M.  y = 2^(e_r + E - 24) (M + C); dropped: a1 w2 (2^-24).
-// ---------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ int pow2_above(float mx) {     // e with 2^e > mx (0 for mx = 0)
-  int e = 0;
-  frexpf(mx, &e);
-  return e;
-}
-template <class Epi>
-__global__ void __launch_bounds__(THREADS, 1)
-gemm_wx_kernel(const float* __restrict__ A, int64_t lda, int64_t M, int N, int K, const uint16_t* __restrict__ img,
-               const float* __restrict__ meta, Epi epi) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = align1024(smem_raw);
-  const int tid = threadIdx.x, wg = tid >> 7, c = tid & 15, rsub = tid >> 4;
-  const int n0 = blockIdx.y * BN;
-  const int rows_b = tile_rows(N, blockIdx.y, 3);            // 3-plane images have 128-row tiles: one per CTA
-  const int n_slices = pad64(K) / 64;
-  constexpr uint32_t a_bytes = 2 * A_HALF_BYTES, stage_bytes = a_bytes + 3 * B_HALF_BYTES;
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + 2 * stage_bytes);
-  float* rin = reinterpret_cast<float*>(full + 2);            // 2^(11 - e_r)
-  float* rout = rin + BM;                                      // 2^(e_r - 11) 2^(E - 13)
-  const int64_t m0 = (int64_t)blockIdx.x * BM;
-  const uint16_t* img_t = img + tile_offset(N, K, blockIdx.y, 3);
-  const bool vec_ok = ((lda & 3) == 0) && aligned16(A);
-  auto issue_copies = [&](int ks) {
-    const uint32_t wb = (uint32_t)rows_b * 128u;
-    mbar_arrive_expect_tx(&full[ks & 1], 3 * wb);
-    for (int p = 0; p < 3; ++p)
-      bulk_g2s(smem + (ks & 1) * stage_bytes + a_bytes + p * B_HALF_BYTES, img_t + ((int64_t)ks * 3 + p) * rows_b * 64, wb, &full[ks & 1]);
-  };
-  auto stage_a = [&](int ks, uint8_t* sa) {                   // a0 / a1 planes of K slice ks
-    float4 v[BM * 16 / THREADS];
-    fetch_a<THREADS>(A, lda, m0, M, ks * BK, K, tid, vec_ok, v);
-#pragma unroll
-    for (int pass = 0; pass < BM * 16 / THREADS; ++pass) {
-      const int r = pass * (THREADS / 16) + rsub;
-      const float x[4] = {v[pass].x * rin[r], v[pass].y * rin[r], v[pass].z * rin[r], v[pass].w * rin[r]};
-      const float i[4] = {rintf(x[0]), rintf(x[1]), rintf(x[2]), rintf(x[3])};
-      const __half2 h0 = __floats2half2_rn(i[0], i[1]), h1 = __floats2half2_rn(i[2], i[3]);
-      const __half2 l0 = __floats2half2_rn(x[0] - i[0], x[1] - i[1]), l1 = __floats2half2_rn(x[2] - i[2], x[3] - i[3]);
-      const uint32_t off = sw128((uint32_t)r, (uint32_t)(c * 4));
-      *reinterpret_cast<uint2*>(sa + off) = make_uint2(*reinterpret_cast<const uint32_t*>(&h0), *reinterpret_cast<const uint32_t*>(&h1));
-      *reinterpret_cast<uint2*>(sa + A_HALF_BYTES + off) =
-          make_uint2(*reinterpret_cast<const uint32_t*>(&l0), *reinterpret_cast<const uint32_t*>(&l1));
-    }
-  };
-  if (tid == 0) {
-    mbar_init(&full[0], 1);
-    mbar_init(&full[1], 1);
-    fence_barrier_init();
-    if (n_slices > 0) issue_copies(0);
-  }
-  // per-row power of two: 16 lanes per row, 16 rows per pass
-  const float wsc = meta[1];
-  for (int pass = 0; pass < BM * 16 / THREADS; ++pass) {
-    const int r = pass * (THREADS / 16) + rsub;
-    float mx = 0.f;
-    if (m0 + r < M)
-      for (int k = 4 * c; k < K; k += 64) {
-        const float* p = A + (m0 + r) * lda + k;
-        if (vec_ok && k + 3 < K) {
-          const float4 t = *reinterpret_cast<const float4*>(p);
-          mx = fmaxf(mx, fmaxf(fmaxf(fabsf(t.x), fabsf(t.y)), fmaxf(fabsf(t.z), fabsf(t.w))));
-        } else {
-          for (int j = 0; j < 4 && k + j < K; ++j) mx = fmaxf(mx, fabsf(p[j]));
-        }
-      }
-#pragma unroll
-    for (int o = 8; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-    if (c == 0) {
-      const int e = pow2_above(mx);
-      rin[r] = ldexpf(1.f, 11 - e);
-      rout[r] = ldexpf(wsc, e - 11);
-    }
-  }
-  __syncthreads();
-  if (n_slices > 0) {
-    stage_a(0, smem);
-    fence_proxy_async();
-  }
-  __syncthreads();
-  // M accumulates exactly across all slices; C starts fresh in every K slice and is added to ctot in fp32 with round-to-
-  // nearest (short truncating accumulation chains)
-  float accm[64], accc[64], ctot[64];
-#pragma unroll
-  for (int q = 0; q < 64; ++q) { accm[q] = 0.f; accc[q] = 0.f; ctot[q] = 0.f; }
-  for (int ks = 0; ks < n_slices; ++ks) {
-    const int s = ks & 1;
-    if (tid == 0 && ks + 1 < n_slices) issue_copies(ks + 1);
-    mbar_wait(&full[s], (uint32_t)((ks >> 1) & 1));
-    const uint32_t a = smem_u32(smem + s * stage_bytes) + wg * (64 * 128), b = smem_u32(smem + s * stage_bytes) + a_bytes;
-    wg_fence();
-#pragma unroll
-    for (int j = 0; j < BK / 16; ++j) {
-      const uint64_t a0 = make_desc(a + 32 * j), a1 = make_desc(a + A_HALF_BYTES + 32 * j);
-      const uint64_t w0 = make_desc(b + 32 * j), w1 = make_desc(b + B_HALF_BYTES + 32 * j), w2 = make_desc(b + 2 * B_HALF_BYTES + 32 * j);
-      wgmma_128<true>(accm, a0, w0, (ks == 0 && j == 0) ? 0u : 1u);
-      wgmma_128<true>(accc, a1, w1, j == 0 ? 0u : 1u);
-      wgmma_128<true>(accc, a1, w0, 1u);
-      wgmma_128<true>(accc, a0, w2, 1u);
-      wgmma_128<true>(accc, a0, w1, 1u);
-    }
-    wg_commit();
-    if (ks + 1 < n_slices) stage_a(ks + 1, smem + (s ^ 1) * stage_bytes);
-    wg_wait_all();
-#pragma unroll
-    for (int q = 0; q < 64; ++q) ctot[q] += accc[q];
-    fence_proxy_async();
-    __syncthreads();
-  }
-#pragma unroll
-  for (int q = 0; q < 64; ++q) {                               // fragment rows: 16 warp + lane / 4 (+ 8 for q % 4 >= 2)
-    const int r = 64 * wg + 16 * ((tid & 127) >> 5) + ((tid & 31) >> 2) + ((q & 2) ? 8 : 0);
-    accm[q] = (accm[q] + ctot[q]) * rout[r];
-  }
-  float* acc_s = reinterpret_cast<float*>(smem);
-  acc_to_smem(accm, acc_s, wg, tid & 127);
-  __syncthreads();
-  tile_epilogue(acc_s, m0, M, n0, N, epi, tid);
-}
-
 static inline int sm_count() {
   static int n = 0;
   if (n == 0) {
@@ -636,23 +515,6 @@ static inline int gemm_w(const float* A, int64_t lda, int64_t M, int N, int K, c
   return 0;
 }
 
-// exact fp16-slice layer (gemm_wx_kernel); img / meta from chain::run_prep_jobs (udf_chain.cuh)
-template <class Epi>
-static inline int gemm_wx(const float* A, int64_t lda, int64_t M, int N, int K, const uint16_t* img, const float* meta, const Epi& epi,
-                          cudaStream_t st) {
-  if (M <= 0 || N <= 0) return 0;
-  const size_t smem = 2 * (size_t)(2 * A_HALF_BYTES + 3 * B_HALF_BYTES) + 2 * sizeof(uint64_t) + 2 * BM * sizeof(float) + 1024;
-  static bool attr_set = false;
-  if (!attr_set) {
-    NUDF_CUDA_OK(cudaFuncSetAttribute(gemm_wx_kernel<Epi>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_set = true;
-  }
-  dim3 grid((unsigned)cdiv(M, BM), (unsigned)n_tiles(N, 3));
-  LaunchTimer lt_(epi_family<Epi>::value, st);
-  gemm_wx_kernel<Epi><<<grid, THREADS, smem, st>>>(A, lda, M, N, K, img, meta, epi);
-  NUDF_LAUNCH_OK();
-  return 0;
-}
 // split the points so that (M tiles x N tiles x splits) fills the SMs once, with at least `min_points` points per CTA
 static inline int tn_splits(int M, int N, int64_t K, int64_t min_points) {
   const int tiles = (int)(cdiv(M, BM) * cdiv(N, BN));
@@ -700,7 +562,7 @@ static inline int gemm_tn(const float* A, int64_t lda, const float* B, int64_t l
 
 // several weight images in one launch: grid.y = job
 struct PrepWJob { const float* W; uint16_t* img; int ldw, N, K, transposed, np; };
-struct PrepWJobs { int n; PrepWJob j[48]; };
+struct PrepWJobs { int n; PrepWJob j[64]; };
 static __global__ void tc_prep_weights_jobs_kernel(const __grid_constant__ PrepWJobs jobs) {
   const PrepWJob& J = jobs.j[blockIdx.y];
   tc_prep_weights_body(J.W, J.ldw, J.N, J.K, J.transposed, J.np, J.img, (int64_t)blockIdx.x * blockDim.x + threadIdx.x,

@@ -6,7 +6,6 @@
 #include "common.cuh"
 #include "ew_kernels.cuh"
 #include "gemm_engine.cuh"
-#include "udf_chain.cuh"
 #include <string.h>
 
 namespace nudf {
@@ -18,8 +17,7 @@ struct UdfPlan {
   int64_t w_off[NUDF_MAX_LAYERS], w_ld[NUDF_MAX_LAYERS], w_total;
   int64_t b_off[NUDF_MAX_LAYERS], b_total;
   int64_t img_nt[NUDF_MAX_LAYERS], img_nn[NUDF_MAX_LAYERS], img_nn1, img_total;   // uint16 offsets of the bf16 hi/lo weight images
-  int64_t img_chain[NUDF_MAX_LAYERS];   // uint16 offsets of the value chain's exact fp16 slice images (udf_chain.cuh): X W_l^T operands
-  int64_t sb_off[NUDF_MAX_LAYERS], sb_total;   // float offsets (after the images) of the chain's per-layer [scale meta (4) | bias table]
+  int64_t img_fwd[NUDF_MAX_LAYERS], img_feat;   // value chain: 3-plane X W^T images of the hidden layers and of the feature rows
   int pe_ld, y_ld;
   int a_ld[NUDF_MAX_LAYERS];    // ld of A[l] (input of layer l), l >= 1
   int o_ld[NUDF_MAX_LAYERS];    // ld of D[l] / Q[l] (out_dim rounded)
@@ -58,12 +56,12 @@ static int make_plan(const nudf_udf_desc* d, UdfPlan* p) {
   // feature rows 1.. of the last layer as a (N = in, K = d_out - 1) operand: the udf-head row is applied as a rank-1 update
   p->img_nn1 = ioff;
   if (p->d_out > 1) ioff += tc::image_elems(p->in_dim[p->n_lin - 1], p->d_out - 1, 2);
-  ioff = round_up(ioff, 512);           // the chain image is fetched with cp.async.bulk: keep its slices 1024-byte aligned
-  for (int l = 0; l < p->n_lin; ++l) { p->img_chain[l] = ioff; ioff += chain::ch_layer_elems(p->out_dim[l], p->in_dim[l]); }
+  // value chain (6 products per MAC): hidden layers, then the feature rows 1.. of the last layer (its udf-head row 0 stays
+  // exact fp32: udf_head_kernel)
+  for (int l = 0; l < p->n_lin - 1; ++l) { p->img_fwd[l] = ioff; ioff += tc::image_elems(p->out_dim[l], p->in_dim[l], 3); }
+  p->img_feat = ioff;
+  if (p->d_out > 1) ioff += tc::image_elems(p->d_out - 1, p->in_dim[p->n_lin - 1], 3);
   p->img_total = round_up(ioff, 8);
-  int64_t soff = 0;
-  for (int l = 0; l < p->n_lin; ++l) { p->sb_off[l] = soff; soff += 4 + (int64_t)chain::CH_NT * chain::ch_n_tiles(p->out_dim[l]); }
-  p->sb_total = soff;
   NUDF_REQUIRE(p->in_dim[0] == p->d_pe, "in_dim[0] must equal the positional-encoding width");
   NUDF_REQUIRE(p->out_dim[p->n_lin - 1] == p->d_out, "last layer width must equal d_out");
   for (int l = 1; l < p->n_lin; ++l) {
@@ -151,6 +149,22 @@ __global__ void udf_finalize_kernel(const float* __restrict__ y, int y_ld, int d
     feat[row * ld_f + c - 1] = v;
   }
 }
+// udf head: y[row * y_ld] = A[row, :K] . w0 + b0, exact fp32 (it feeds exp(-25000 u)); one warp per point, lane j sums
+// k = j, j + 32, ... and a fixed butterfly adds the lanes, so a point gets the same bits in any batch and position
+__global__ void udf_head_kernel(const float* __restrict__ A, int64_t lda, const float* __restrict__ w0, const float* __restrict__ b0,
+                                int K, int64_t P, float* __restrict__ y, int y_ld) {
+  const int64_t row = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (row >= P) return;
+  const float* a = A + row * lda;
+  float s = 0.f;
+#pragma unroll 8
+  for (int k = lane; k < K; k += 32) s = fmaf(a[k], w0[k], s);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if (lane == 0) y[row * y_ld] = s + (b0 != nullptr ? b0[0] : 0.f);
+}
+
 __global__ void udf_value_only_kernel(const float* __restrict__ y, int y_ld, int64_t P, float inv_scale, float* __restrict__ udf) {
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < P) udf[i] = fabsf(y[i * y_ld]) * inv_scale;
@@ -297,31 +311,23 @@ static int fold_all(const UdfPlan& p, const nudf_udf_desc* d, float* wfold, cuda
     if (int rc = run_fold_jobs(jobs, false, st)) return rc;
   }
   if (get_engine() == 1) {
+    // split-bf16 images of the tensor-core layer kernels (gemm_tc.cuh), all in one launch
     uint16_t* img = reinterpret_cast<uint16_t*>(wfold + p.w_total);
     const int last = p.n_lin - 1;
-    // split-bf16 images of the tensor-core layer kernels (gemm_tc.cuh)
+    const float* wfeat = wfold + p.w_off[last] + p.w_ld[last];    // rows 1.. of the last layer
+    tc::PrepWJobs pj;
+    pj.n = 0;
     for (int l = 0; l < p.n_lin; ++l) {
-      if (int rc = tc::prep_weights(wfold + p.w_off[l], p.w_ld[l], p.out_dim[l], p.in_dim[l], 0, 2, img + p.img_nt[l], st)) return rc;
-      if (int rc = tc::prep_weights(wfold + p.w_off[l], p.w_ld[l], p.in_dim[l], p.out_dim[l], 1, 2, img + p.img_nn[l], st)) return rc;
+      pj.j[pj.n++] = tc::PrepWJob{wfold + p.w_off[l], img + p.img_nt[l], (int)p.w_ld[l], p.out_dim[l], p.in_dim[l], 0, 2};
+      pj.j[pj.n++] = tc::PrepWJob{wfold + p.w_off[l], img + p.img_nn[l], (int)p.w_ld[l], p.in_dim[l], p.out_dim[l], 1, 2};
     }
-    if (p.d_out > 1)
-      if (int rc = tc::prep_weights(wfold + p.w_off[last] + p.w_ld[last], p.w_ld[last], p.in_dim[last], p.d_out - 1, 1, 2, img + p.img_nn1, st))
-        return rc;
+    if (p.d_out > 1) pj.j[pj.n++] = tc::PrepWJob{wfeat, img + p.img_nn1, (int)p.w_ld[last], p.in_dim[last], p.d_out - 1, 1, 2};
     if (tc_on(TC_FWD)) {
-      // exact fp16 slice images of the hidden layers for the value chain (udf_chain.cuh): one power-of-two scale per layer
-      float* tab = wfold + p.w_total + p.img_total / 2;     // per layer: [4 floats of scale meta | bias table]
-      chain::PrepJobs jobs;
-      jobs.n = 0;
-      chain::ScaleJobs sj;
-      sj.n = last;
-      for (int l = 0; l < last; ++l) {
-        float* meta = tab + p.sb_off[l];
-        const float* W = wfold + p.w_off[l];
-        sj.j[l] = chain::ScaleJob{W, meta, (int)p.w_ld[l], p.out_dim[l], p.in_dim[l]};
-        jobs.j[jobs.n++] = chain::PrepJob{W, nullptr, meta, img + p.img_chain[l], nullptr, (int)p.w_ld[l], p.out_dim[l], p.in_dim[l], 0, 0};
-      }
-      if (int rc = chain::run_prep_jobs(sj, jobs, st)) return rc;
+      for (int l = 0; l < last; ++l)
+        pj.j[pj.n++] = tc::PrepWJob{wfold + p.w_off[l], img + p.img_fwd[l], (int)p.w_ld[l], p.out_dim[l], p.in_dim[l], 0, 3};
+      if (p.d_out > 1) pj.j[pj.n++] = tc::PrepWJob{wfeat, img + p.img_feat, (int)p.w_ld[last], p.d_out - 1, p.in_dim[last], 0, 3};
     }
+    if (int rc = tc::prep_weights_jobs(pj, st)) return rc;
   }
   return 0;
 }
@@ -330,29 +336,33 @@ static inline const uint16_t* img_base(const UdfPlan& p, const float* wfold) {
   return reinterpret_cast<const uint16_t*>(wfold + p.w_total);
 }
 
+// Y[:, 0] (udf head) and, with `features`, Y[:, 1:] of the last layer, with every layer's input saved in the context
 static int value_chain(const UdfPlan& p, const nudf_udf_desc* d, const float* wfold, const float* pts, int64_t P,
-                       float* ctx, const UdfCtx& c, cudaStream_t st) {
+                       float* ctx, const UdfCtx& c, bool features, cudaStream_t st) {
   float* e0 = ctx + c.e0;
   float* askip = nullptr; int askip_ld = 0, askip_col = 0;
   if (p.skip >= 1) { askip = ctx + c.a[p.skip]; askip_ld = p.a_ld[p.skip]; askip_col = p.out_dim[p.skip - 1]; }
   pe_forward_kernel<<<nblk(P, 128), 128, 0, st>>>(pts, P, p.L, p.scale, e0, p.pe_ld, askip, askip_ld, askip_col);
   NUDF_LAUNCH_OK();
-  for (int l = 0; l < p.n_lin; ++l) {
+  const uint16_t* img = img_base(p, wfold);
+  const int last = p.n_lin - 1;
+  for (int l = 0; l < last; ++l) {
     const float* A = l == 0 ? e0 : ctx + c.a[l];
     int64_t lda = l == 0 ? p.pe_ld : p.a_ld[l];
-    const float* W = wfold + p.w_off[l];
-    int rc;
-    if (l < p.n_lin - 1) {
-      EpiAct epi{ctx + c.a[l + 1], p.a_ld[l + 1], d->bias[l], ACT_SOFTPLUS100, (l + 1 == p.skip) ? NUDF_SQRT1_2 : 1.0f};
-      const float* meta = wfold + p.w_total + p.img_total / 2 + p.sb_off[l];     // [2^(3 - E), 2^(E - 13), ...]
-      rc = tc_on(TC_FWD) ? tc::gemm_wx(A, lda, P, p.out_dim[l], p.in_dim[l], img_base(p, wfold) + p.img_chain[l], meta, epi, st)
-                         : gemm_nt(A, lda, W, p.w_ld[l], P, p.out_dim[l], p.in_dim[l], epi, st);
-    } else {
-      // the last layer always runs on the exact-fp32 engine: its row 0 is the udf head
-      EpiAct epi{ctx + c.y, p.y_ld, d->bias[l], ACT_NONE, 1.0f};
-      rc = gemm_nt(A, lda, W, p.w_ld[l], P, p.out_dim[l], p.in_dim[l], epi, st);
-    }
-    if (rc) return rc;
+    EpiAct epi{ctx + c.a[l + 1], p.a_ld[l + 1], d->bias[l], ACT_SOFTPLUS100, (l + 1 == p.skip) ? NUDF_SQRT1_2 : 1.0f};
+    if (int rc = gemm_nt(A, lda, wfold + p.w_off[l], p.w_ld[l], P, p.out_dim[l], p.in_dim[l], epi, st, img + p.img_fwd[l], TC_FWD, 3))
+      return rc;
+  }
+  const float* A = ctx + c.a[last];
+  const float* W = wfold + p.w_off[last];
+  udf_head_kernel<<<nblk(P * 32, 256), 256, 0, st>>>(A, p.a_ld[last], W, d->bias[last], p.in_dim[last], P, ctx + c.y, p.y_ld);
+  NUDF_LAUNCH_OK();
+  if (features && p.d_out > 1) {
+    const float* bias = d->bias[last] != nullptr ? d->bias[last] + 1 : nullptr;
+    EpiAct epi{ctx + c.y + 1, p.y_ld, bias, ACT_NONE, 1.0f};      // unaligned columns: st4 stores them one by one
+    if (int rc = gemm_nt(A, p.a_ld[last], W + p.w_ld[last], p.w_ld[last], P, p.d_out - 1, p.in_dim[last], epi, st, img + p.img_feat,
+                         TC_FWD, 3))
+      return rc;
   }
   return 0;
 }
@@ -402,7 +412,7 @@ extern "C" {
 int64_t nudf_udf_folded_floats(const nudf_udf_desc* d) {
   UdfPlan p;
   if (make_plan(d, &p)) return -1;
-  return p.w_total + p.img_total / 2 + p.sb_total;   // fp32 folded weights, the 16-bit weight images (2 per float), the chain's (scale, bias) tables
+  return p.w_total + p.img_total / 2;   // fp32 folded weights, then the 16-bit weight images (2 per float)
 }
 
 int nudf_udf_fold_weights(const nudf_udf_desc* d, float* wfold, void* stream) {
@@ -438,7 +448,7 @@ static int udf_forward_impl(const nudf_udf_desc* d, const float* wfold, const fl
   cudaStream_t st = (cudaStream_t)stream;
   UdfCtx c;
   ctx_layout(p, P, grad != nullptr, &c);
-  if (int rc = value_chain(p, d, wfold, pts, P, ctx, c, st)) return rc;
+  if (int rc = value_chain(p, d, wfold, pts, P, ctx, c, feat != nullptr, st)) return rc;
   udf_finalize_kernel<<<nblk(P * p.d_out, 256), 256, 0, st>>>(ctx + c.y, p.y_ld, p.d_out, P, 1.0f / p.scale, udf, ld_u, feat, ld_f,
                                                               ctx + c.sgn);
   NUDF_LAUNCH_OK();
@@ -470,11 +480,8 @@ int nudf_udf_value(const nudf_udf_desc* d, const float* wfold, const float* pts,
   NUDF_REQUIRE(work != nullptr, "null pointer (work)");
   UdfCtx c;
   ctx_layout(p, P, 0, &c);
-  // value-only: the last layer needs only its row 0 (the udf head); the 256 feature rows are skipped.
-  UdfPlan pv = p;
-  pv.out_dim[p.n_lin - 1] = 1;
-  nudf_udf_desc dv = *d;
-  if (int rc = value_chain(pv, &dv, wfold, pts, P, work, c, st)) return rc;
+  // value-only: of the last layer only row 0 (the udf head), through the same kernel as the full forward
+  if (int rc = value_chain(p, d, wfold, pts, P, work, c, false, st)) return rc;
   udf_value_only_kernel<<<nblk(P, 256), 256, 0, st>>>(work + c.y, p.y_ld, P, 1.0f / p.scale, udf);
   NUDF_LAUNCH_OK();
   return 0;
