@@ -447,6 +447,42 @@ int nudf_mp_hole_emit(const double* verts, const int64_t* edges, const uint8_t* 
 int nudf_mp_smooth_step(const double* verts_in, double* verts_out, const int64_t* border, int64_t n_border,
                         const int64_t* rowptr, const int64_t* cols, double lambda, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * Colour loss of the training step (replaces loss/loss.py ColorLoss with loss/patch_metric.py; neuraludf_b200/loss.py)
+ * ------------------------------------------------------------------------------------------------------------
+ * fp32, row-major, contiguous.  N rays, P = (2 h_patch + 1)^2 patch pixels (row-major, the patch's x fastest). */
+#define NUDF_PATCH_L1 0
+#define NUDF_PATCH_SSD 1
+#define NUDF_PATCH_SSIM 2
+#define NUDF_PATCH_NCC 3
+/* floats of the workspace both calls take (the forward writes it, the backward reads it); ws must be 8-byte aligned */
+#define NUDF_COLOR_LOSS_WS_FLOATS(n_rays) (4 * (int64_t)(n_rays) + 8)
+typedef struct nudf_color_loss_args {
+  int32_t n_rays;            /* N, 1 .. 16384 */
+  int32_t h_patch;           /* 1 .. 15 */
+  int32_t patch_type;        /* NUDF_PATCH_* */
+  float weights[4];          /* color_base, color, color_pixel, color_patch weights (loss.py:119-123) */
+  const float* color_base;   /* [N,3] each; NULL: the term is absent */
+  const float* color;
+  const float* color_pixel;
+  const float* gt_color;     /* [N,3] */
+  const float* pixel_mask;   /* [N] or NULL: denominator sum(mask) + 1e-4 of color_base / color, else the mean over N * 3 */
+  const float* patch_colors; /* [N,P,3]; NULL: no patch term */
+  const float* gt_patch_colors; /* [N,P,3] */
+  const uint8_t* patch_mask; /* [N] 0/1 or NULL: denominator count + 1e-4 of color_pixel, and the patch term's mask (required
+                              * with it) */
+  const float* window;       /* [P] Gaussian window of patch_metric.create_window (ssim / ncc) */
+} nudf_color_loss_args;
+/* losses[5] <- loss, color_base_loss, color_loss, color_pixel_loss, color_patch_loss (absent terms 0); kept[N] (with a patch
+ * term) <- 1 for the masked rays left after excluding the first int(0.3f * count(mask)) rays of the descending order of
+ * error * mask (NaN largest, equal keys in ray order; loss.py:78-84).  Two launches, no host synchronisation. */
+int nudf_color_loss_forward(const nudf_color_loss_args* args, float* losses, uint8_t* kept, float* ws, void* stream);
+/* d_* (same shapes as the predictions; NULL: not written) <- gradients of  sum_i losses_bar[i] * losses[i].  losses_bar:
+ * HOST array of 5 DEVICE pointers to one float each, NULL = zero.  kept and ws: as the forward left them. */
+int nudf_color_loss_backward(const nudf_color_loss_args* args, const float* const* losses_bar, const uint8_t* kept,
+                             const float* ws, float* d_color_base, float* d_color, float* d_color_pixel, float* d_patch_colors,
+                             void* stream);
+
 #ifdef __cplusplus
 }
 #endif

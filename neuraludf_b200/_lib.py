@@ -65,6 +65,21 @@ class RenderBar(ctypes.Structure):
                                         "ray_sums")]
 
 
+PATCH_TYPES = {"l1": 0, "ssd": 1, "ssim": 2, "ncc": 3}
+
+
+def color_loss_ws_floats(n_rays):
+    """NUDF_COLOR_LOSS_WS_FLOATS of include/nudf.h"""
+    return 4 * n_rays + 8
+
+
+class ColorLossArgs(ctypes.Structure):
+    _fields_ = [("n_rays", ctypes.c_int32), ("h_patch", ctypes.c_int32), ("patch_type", ctypes.c_int32),
+                ("weights", ctypes.c_float * 4)] + [(n, c_void_p) for n in (
+                    "color_base", "color", "color_pixel", "gt_color", "pixel_mask", "patch_colors", "gt_patch_colors",
+                    "patch_mask", "window")]
+
+
 LAUNCH_FAMILIES = ["udf_fwd_chain_fused", "tc_layer_reverse_sweep", "tc_layer_tangent", "tc_layer_backward", "tc_layer_other",
                    "tc_weight_gradient", "ffma_gemm", "ray_kernels", "elementwise", "udf_bwd_chain_fused"]
 
@@ -187,6 +202,8 @@ _SIGNATURES = {
     "nudf_mp_hole_emit": (ctypes.c_int, [c_void_p] * 3 + [ctypes.c_int64, c_void_p, c_void_p, ctypes.c_int64]
                           + [c_void_p] * 3),
     "nudf_mp_smooth_step": (ctypes.c_int, [c_void_p] * 3 + [ctypes.c_int64, c_void_p, c_void_p, ctypes.c_double, c_void_p]),
+    "nudf_color_loss_forward": (ctypes.c_int, [c_void_p] * 5),
+    "nudf_color_loss_backward": (ctypes.c_int, [c_void_p] * 9),
 }
 
 

@@ -6,7 +6,8 @@
 mirrors before the runner is executed from the reference root; everything else the runner imports (`dataset`, `loss`, ...)
 still resolves from the reference checkout (its `models/` directory is a namespace package).  `custom_mc` (the Cython
 MeshUDF marching cubes that extract_mesh.py imports) is bound to neuraludf_b200.mesh when the reference's own build cannot
-be imported by the running interpreter.
+be imported by the running interpreter.  With NUDF_DEVICE_LOSS=1 in the environment, `loss.loss` and `loss.patch_metric`
+are bound to neuraludf_b200.loss (the colour loss on the device); without it the runner's own loss files run.
 """
 import importlib
 import importlib.machinery
@@ -33,7 +34,26 @@ def install_shadow_modules(reference_root=None):
         sys.modules["models." + name] = mod
         setattr(pkg, name, mod)
     _install_custom_mc(reference_root)
+    if os.environ.get("NUDF_DEVICE_LOSS") == "1":
+        _install_device_loss(reference_root)
     return pkg
+
+
+def _install_device_loss(reference_root):
+    """Serves `loss.loss` (ColorLoss, ...) and `loss.patch_metric` (SSIM, NCC, ...) from neuraludf_b200.loss."""
+    from neuraludf_b200 import loss
+    pkg = sys.modules.get("loss")
+    if pkg is None:
+        pkg = types.ModuleType("loss")
+        pkg.__path__ = []
+        sys.modules["loss"] = pkg
+    if reference_root is not None:
+        p = os.path.join(reference_root, "loss")
+        if os.path.isdir(p) and p not in list(pkg.__path__):
+            pkg.__path__ = list(pkg.__path__) + [p]
+    for name in ("loss", "patch_metric"):
+        sys.modules["loss." + name] = loss
+        setattr(pkg, name, loss)
 
 
 def _native_custom_mc(reference_root):
