@@ -1,10 +1,11 @@
 // Tensor-core GEMM engine for sm_90a (wgmma) with an fp32-grade split-bf16 operand scheme:
 //   D = sum over K slices of A_hi*B_hi + A_hi*B_lo + A_lo*B_hi  (2 planes, ~4e-6 vs fp64), or with 3 planes hi/mid/lo the 6
 //   products of weight >= 2^-16 (fp32-grade); x = hi + lo, hi = bf16(x), lo = bf16(x - hi) (SURVEY.md section 0, fact 3).
-// One CTA = 2 warpgroups, a 128 x 128 output tile, a 2-stage shared-memory ring over 64-wide K slices: warpgroup w issues
-// wgmma.m64n128k16 for rows 64w.. (K-major SWIZZLE_128B operands, fp32 accumulators in registers) while all threads stage
+// One CTA = 2 warpgroups, a 128 x WN output tile, a 2-stage shared-memory ring over 64-wide K slices: warpgroup w issues
+// wgmma.m64n{WN}k16 for rows 64w.. (K-major SWIZZLE_128B operands, fp32 accumulators in registers) while all threads stage
 // the next activation slice as bf16 planes; weight slices arrive by cp.async.bulk on an mbarrier.  The accumulators go
-// through shared memory to the fused epilogue functor (4 consecutive columns of a row per call: coalesced).
+// through shared memory to the fused epilogue functor (4 consecutive columns of a row per call: coalesced).  WN = 256 for
+// 2-plane layers wider than 128 columns, so that each activation row block is read from HBM and split into planes once.
 #pragma once
 #include <cuda_bf16.h>
 
@@ -14,12 +15,13 @@ namespace nudf {
 namespace tc {
 
 constexpr int BM = 128;
-constexpr int BN = 128;        // output columns per CTA
+constexpr int BN = 128;        // output columns per CTA of gemm_tn_kernel and of the narrow gemm_w_kernel tile
 constexpr int BK = 64;
 constexpr int THREADS = 256;   // 2 warpgroups: MMA issue, operand staging and epilogue
 constexpr int A_HALF_BYTES = BM * BK * 2;   // 16 KB: one plane of a [128 x 64] operand slice
 constexpr int B_HALF_BYTES = BN * BK * 2;
-constexpr int ACC_LD = BN + 4;              // floats per row of the accumulator tile in shared memory
+__host__ __device__ constexpr int b_plane_bytes(int wn) { return wn * BK * 2; }   // one plane of a [wn x 64] weight slice
+__host__ __device__ constexpr int acc_ld(int wn) { return wn + 4; }   // floats per row of the accumulator tile in smem
 
 __host__ __device__ inline int pad16(int n) { return (n + 15) & ~15; }
 __host__ __device__ inline int pad64(int k) { return (k + 63) & ~63; }
@@ -144,6 +146,13 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait_but_one() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
+// keeps the compiler from moving reads of an accumulator array across the (volatile) wait that completes it
+template <int N>
+__device__ __forceinline__ void fence_operand(float (&d)[N]) {
+#pragma unroll
+  for (int q = 0; q < N; ++q) asm volatile("" : "+f"(d[q])::"memory");
+}
 // r + half an ulp of r with the sign of r (the exponent bits times 2^-24): a result the tensor core truncated toward zero,
 // moved to the middle of its truncation interval
 __device__ __forceinline__ float unbias_rz(float r) { return fmaf(__uint_as_float(__float_as_uint(r) & 0xff800000u), 0x1p-24f, r); }
@@ -168,64 +177,131 @@ __device__ __forceinline__ void wgmma_128(float (&d)[64], uint64_t da, uint64_t 
         "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
       : "l"(da), "l"(db), "r"(accumulate));
 }
+// D[64 x 128] = A[64 x 16] B[128 x 16]^T into fresh registers: write-only outputs, so that the compiler keeps no
+// earlier value of d alive
+__device__ __forceinline__ void wgmma_128_fresh(float (&d)[64], uint64_t da, uint64_t db) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, "
+      "%26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, "
+      "%50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n"
+      "}\n"
+      : "=f"(d[0]), "=f"(d[1]), "=f"(d[2]), "=f"(d[3]), "=f"(d[4]), "=f"(d[5]), "=f"(d[6]), "=f"(d[7]), "=f"(d[8]), "=f"(d[9]),
+        "=f"(d[10]), "=f"(d[11]), "=f"(d[12]), "=f"(d[13]), "=f"(d[14]), "=f"(d[15]), "=f"(d[16]), "=f"(d[17]), "=f"(d[18]),
+        "=f"(d[19]), "=f"(d[20]), "=f"(d[21]), "=f"(d[22]), "=f"(d[23]), "=f"(d[24]), "=f"(d[25]), "=f"(d[26]), "=f"(d[27]),
+        "=f"(d[28]), "=f"(d[29]), "=f"(d[30]), "=f"(d[31]), "=f"(d[32]), "=f"(d[33]), "=f"(d[34]), "=f"(d[35]), "=f"(d[36]),
+        "=f"(d[37]), "=f"(d[38]), "=f"(d[39]), "=f"(d[40]), "=f"(d[41]), "=f"(d[42]), "=f"(d[43]), "=f"(d[44]), "=f"(d[45]),
+        "=f"(d[46]), "=f"(d[47]), "=f"(d[48]), "=f"(d[49]), "=f"(d[50]), "=f"(d[51]), "=f"(d[52]), "=f"(d[53]), "=f"(d[54]),
+        "=f"(d[55]), "=f"(d[56]), "=f"(d[57]), "=f"(d[58]), "=f"(d[59]), "=f"(d[60]), "=f"(d[61]), "=f"(d[62]), "=f"(d[63])
+      : "l"(da), "l"(db), "r"(0u));
+}
+
+// D[64 x 256] (+)= A[64 x 16] B[256 x 16]^T, the same operands as wgmma_128 with twice the rows of B
+__device__ __forceinline__ void wgmma_256(float (&d)[128], uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %130, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, "
+      "%25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, "
+      "%71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, "
+      "%94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, "
+      "%114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, 0, 0;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]),
+        "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]),
+        "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]),
+        "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]),
+        "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]),
+        "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]),
+        "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]),
+        "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]),
+        "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]),
+        "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]),
+        "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]),
+        "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]),
+        "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(da), "l"(db), "r"(accumulate));
+}
 
 // The wgmma group of one 64-wide K slice, smallest products first; plane p at +p * stride, 32 B per 16-wide K step.
 // With 3 planes only the five correction products (lo * hi, hi * lo, mid * mid, mid * hi, hi * mid: ~2^-8 of the result's
-// scale, so the tensor core's truncation of each wgmma result to fp32 costs ~2^-32 of it); gemm_w_kernel issues the hi * hi
-// steps one at a time into fresh accumulators and adds them up in fp32 with round-to-nearest.
-template <int NP>
-__device__ __forceinline__ void mma_slice(float (&d)[64], uint32_t a, uint32_t a_stride, uint32_t b, uint32_t b_stride, bool zero_first) {
+// scale, so the tensor core's truncation of each wgmma result to fp32 costs ~2^-32 of it); gemm_w_kernel issues each hi * hi
+// step into fresh accumulators and adds them up in fp32 with round-to-nearest.
+// WN (128 or 256) is the width of the weight slice and of the accumulator fragment.
+template <int WN>
+__device__ __forceinline__ void wgmma_n(float (&d)[WN / 2], uint64_t da, uint64_t db, uint32_t accumulate) {
+  if constexpr (WN == 256) wgmma_256(d, da, db, accumulate);
+  else wgmma_128(d, da, db, accumulate);
+}
+template <int NP, int WN>
+__device__ __forceinline__ void mma_slice(float (&d)[WN / 2], uint32_t a, uint32_t a_stride, uint32_t b, uint32_t b_stride, bool zero_first) {
   auto desc = [](uint32_t base, uint32_t stride, int p, int j) { return make_desc(base + p * stride + 32u * j); };
 #pragma unroll
   for (int j = 0; j < BK / 16; ++j) {
     const uint32_t acc0 = (zero_first && j == 0) ? 0u : 1u;
     if constexpr (NP == 2) {
-      wgmma_128(d, desc(a, a_stride, 1, j), desc(b, b_stride, 0, j), acc0);
-      wgmma_128(d, desc(a, a_stride, 0, j), desc(b, b_stride, 1, j), 1u);
-      wgmma_128(d, desc(a, a_stride, 0, j), desc(b, b_stride, 0, j), 1u);
+      wgmma_n<WN>(d, desc(a, a_stride, 1, j), desc(b, b_stride, 0, j), acc0);
+      wgmma_n<WN>(d, desc(a, a_stride, 0, j), desc(b, b_stride, 1, j), 1u);
+      wgmma_n<WN>(d, desc(a, a_stride, 0, j), desc(b, b_stride, 0, j), 1u);
     } else {
-      wgmma_128(d, desc(a, a_stride, 2, j), desc(b, b_stride, 0, j), acc0);   // lo * hi
-      wgmma_128(d, desc(a, a_stride, 0, j), desc(b, b_stride, 2, j), 1u);     // hi * lo
-      wgmma_128(d, desc(a, a_stride, 1, j), desc(b, b_stride, 1, j), 1u);     // mid * mid
-      wgmma_128(d, desc(a, a_stride, 1, j), desc(b, b_stride, 0, j), 1u);     // mid * hi
-      wgmma_128(d, desc(a, a_stride, 0, j), desc(b, b_stride, 1, j), 1u);     // hi * mid
+      wgmma_n<WN>(d, desc(a, a_stride, 2, j), desc(b, b_stride, 0, j), acc0);   // lo * hi
+      wgmma_n<WN>(d, desc(a, a_stride, 0, j), desc(b, b_stride, 2, j), 1u);     // hi * lo
+      wgmma_n<WN>(d, desc(a, a_stride, 1, j), desc(b, b_stride, 1, j), 1u);     // mid * mid
+      wgmma_n<WN>(d, desc(a, a_stride, 1, j), desc(b, b_stride, 0, j), 1u);     // mid * hi
+      wgmma_n<WN>(d, desc(a, a_stride, 0, j), desc(b, b_stride, 1, j), 1u);     // hi * mid
     }
   }
 }
 
-// m64n128 accumulator fragment of warpgroup wg -> row-major [128 x ACC_LD] fp32 tile in shared memory
-__device__ __forceinline__ void acc_to_smem(const float (&d)[64], float* acc_s, int wg, int wtid) {
+// m64n{WN} accumulator fragment of warpgroup wg -> row-major [128 x acc_ld(WN)] fp32 tile in shared memory
+template <int WN>
+__device__ __forceinline__ void acc_to_smem(const float (&d)[WN / 2], float* acc_s, int wg, int wtid) {
+  constexpr int LD = acc_ld(WN);
   const int r = 64 * wg + 16 * (wtid >> 5) + ((wtid & 31) >> 2);
   const int c = 2 * (wtid & 3);
 #pragma unroll
-  for (int g = 0; g < 16; ++g) {
-    *reinterpret_cast<float2*>(acc_s + r * ACC_LD + 8 * g + c) = make_float2(d[4 * g], d[4 * g + 1]);
-    *reinterpret_cast<float2*>(acc_s + (r + 8) * ACC_LD + 8 * g + c) = make_float2(d[4 * g + 2], d[4 * g + 3]);
+  for (int g = 0; g < WN / 8; ++g) {
+    *reinterpret_cast<float2*>(acc_s + r * LD + 8 * g + c) = make_float2(d[4 * g], d[4 * g + 1]);
+    *reinterpret_cast<float2*>(acc_s + (r + 8) * LD + 8 * g + c) = make_float2(d[4 * g + 2], d[4 * g + 3]);
   }
 }
-// Fused epilogue of the tile at (m0, n0): a warp covers 128 consecutive columns of a row, two row groups' loads in flight
-template <class Epi>
+// Fused epilogue of the [128 x WN] tile at (m0, n0): a warp covers 128 consecutive columns of a row per pass (WN / 128
+// column halves per row), two row groups' loads in flight.  Columns at or beyond n_valid_end are never passed on.
+template <int WN, class Epi>
 __device__ __forceinline__ void tile_epilogue(const float* acc_s, int64_t m0, int64_t M, int n0, int n_valid_end, const Epi& epi, int tid) {
+  constexpr int LD = acc_ld(WN);
   const int cq = tid & 31;
-  const int col = n0 + 4 * cq;
-  int nv = n_valid_end - col;
-  nv = nv < 4 ? nv : 4;
-  if (nv <= 0) return;
-  for (int r0 = tid >> 5; r0 < BM; r0 += 2 * (THREADS / 32)) {
-    typename Epi::Aux aux[2];
+#pragma unroll 1
+  for (int h = 0; h < WN / 128; ++h) {
+    const int cl = 128 * h + 4 * cq;
+    const int col = n0 + cl;
+    int nv = n_valid_end - col;
+    nv = nv < 4 ? nv : 4;
+    if (nv <= 0) break;
+    for (int r0 = tid >> 5; r0 < BM; r0 += 2 * (THREADS / 32)) {
+      typename Epi::Aux aux[2];
 #pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      const int64_t row = m0 + r0 + i * (THREADS / 32);
-      if (row < M) epi.load(row, col, nv, aux[i]);
-    }
+      for (int i = 0; i < 2; ++i) {
+        const int64_t row = m0 + r0 + i * (THREADS / 32);
+        if (row < M) epi.load(row, col, nv, aux[i]);
+      }
 #pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      const int r = r0 + i * (THREADS / 32);
-      const int64_t row = m0 + r;
-      if (row < M) {
-        const float4 t = *reinterpret_cast<const float4*>(acc_s + r * ACC_LD + 4 * cq);
-        const float x[4] = {t.x, t.y, t.z, t.w};
-        epi.apply(row, col, x, nv, aux[i]);
+      for (int i = 0; i < 2; ++i) {
+        const int r = r0 + i * (THREADS / 32);
+        const int64_t row = m0 + r;
+        if (row < M) {
+          const float4 t = *reinterpret_cast<const float4*>(acc_s + r * LD + cl);
+          const float x[4] = {t.x, t.y, t.z, t.w};
+          epi.apply(row, col, x, nv, aux[i]);
+        }
       }
     }
   }
@@ -332,23 +408,29 @@ __device__ __forceinline__ void stage_block_t(const float* __restrict__ X, int64
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// C[M x N] = epi( A[M x K] * B^T ),  B given as a pre-split NP-plane weight image.  grid = (ceil(M/128), ceil(N/128)).
+// C[M x N] = epi( A[M x K] * B^T ),  B given as a pre-split NP-plane weight image, WN output columns per CTA.
+// 1-D grid of ceil(M/128) * ceil(N/WN) CTAs with the column tile fastest: the column tiles of a row block run back to
+// back, so that a second read of its activations hits L2.  Weight rows beyond the image tile (N = 217 -> 224 rows) leave
+// stale shared memory in the last rows of the slice; they only feed columns >= N, which the epilogue never passes on.
 // ---------------------------------------------------------------------------------------------------------------
-template <int NP, class Epi>
+template <int NP, int WN, class Epi>
 __global__ void __launch_bounds__(THREADS, 1)
 gemm_w_kernel(const float* __restrict__ A, int64_t lda, int64_t M, int N, int K, const uint16_t* __restrict__ img, Epi epi) {
+  static_assert(WN == 128 || (WN == 256 && NP == 2), "WN = 256 only with 2 planes (3 planes need 2 x WN/2 accumulators)");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = align1024(smem_raw);
   const int tid = threadIdx.x, wg = tid >> 7;
-  const int n0 = blockIdx.y * BN;
+  const int n_ct = (N + WN - 1) / WN;
+  const int n0 = (int)(blockIdx.x % (unsigned)n_ct) * WN;
+  const int64_t m0 = (int64_t)(blockIdx.x / (unsigned)n_ct) * BM;
   const int t = n0 / nt_of(NP);                             // image tile of this CTA's columns
   const int rows_t = tile_rows(N, t, NP);
   const int row_in_tile = n0 - t * nt_of(NP);
-  int rows_h = rows_t - row_in_tile; rows_h = rows_h < BN ? rows_h : BN;   // weight rows of this CTA (multiple of 16)
+  int rows_h = rows_t - row_in_tile; rows_h = rows_h < WN ? rows_h : WN;   // weight rows of this CTA (multiple of 16)
   const int n_slices = pad64(K) / 64;
-  const uint32_t a_bytes = NP * A_HALF_BYTES, stage_bytes = a_bytes + NP * B_HALF_BYTES;
+  constexpr uint32_t B_PLANE = b_plane_bytes(WN);
+  const uint32_t a_bytes = NP * A_HALF_BYTES, stage_bytes = a_bytes + NP * B_PLANE;
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + 2 * stage_bytes);
-  const int64_t m0 = (int64_t)blockIdx.x * BM;
   const uint16_t* img_t = img + tile_offset(N, K, t, NP) + (int64_t)row_in_tile * 64;
   const bool vec_ok = ((lda & 3) == 0) && aligned16(A);
 
@@ -356,7 +438,7 @@ gemm_w_kernel(const float* __restrict__ A, int64_t lda, int64_t M, int N, int K,
     uint8_t* st = smem + (ks & 1) * stage_bytes;
     const uint32_t wb = (uint32_t)rows_h * 128u;
     mbar_arrive_expect_tx(&full[ks & 1], NP * wb);
-    for (int p = 0; p < NP; ++p) bulk_g2s(st + a_bytes + p * B_HALF_BYTES, img_t + ((int64_t)ks * NP + p) * rows_t * 64, wb, &full[ks & 1]);
+    for (int p = 0; p < NP; ++p) bulk_g2s(st + a_bytes + p * B_PLANE, img_t + ((int64_t)ks * NP + p) * rows_t * 64, wb, &full[ks & 1]);
   };
   if (tid == 0) {
     mbar_init(&full[0], 1);
@@ -374,42 +456,60 @@ gemm_w_kernel(const float* __restrict__ A, int64_t lda, int64_t M, int N, int K,
   // round-to-nearest.  The tensor core truncates a wgmma result toward zero; every hi * hi result is a single truncation of
   // 16 full-size products, so adding half an ulp of it (with its sign) leaves an unbiased error.  Without that the bias of
   // the 16 truncations per output (K = 256) adds up coherently over the points of a parameter-gradient sum.
-  float acc[64], tot[NP == 3 ? 64 : 1];
+  // The hi * hi steps alternate between acc2 and acc, so that step j + 1 is in flight while step j is added; tot still
+  // takes the corrections, hh0, hh1, hh2, hh3 in that order.
+  constexpr int NACC = WN / 2, NTOT = NP == 3 ? 64 : 1;
+  float acc[NACC], tot[NTOT], acc2[NTOT];
 #pragma unroll
-  for (int q = 0; q < 64; ++q) acc[q] = 0.f;
+  for (int q = 0; q < NACC; ++q) acc[q] = 0.f;
 #pragma unroll
-  for (int q = 0; q < (NP == 3 ? 64 : 1); ++q) tot[q] = 0.f;
+  for (int q = 0; q < NTOT; ++q) tot[q] = 0.f;
   for (int ks = 0; ks < n_slices; ++ks) {
     const int s = ks & 1;
     if (tid == 0 && ks + 1 < n_slices) issue_copies(ks + 1);   // stage s ^ 1 was released by the wait + barrier of ks - 1
     mbar_wait(&full[s], (uint32_t)((ks >> 1) & 1));
     const uint32_t st = smem_u32(smem + s * stage_bytes);
     wg_fence();
-    mma_slice<NP>(acc, st + wg * (64 * 128), A_HALF_BYTES, st + a_bytes, B_HALF_BYTES, NP == 3 || ks == 0);
+    mma_slice<NP, WN>(acc, st + wg * (64 * 128), A_HALF_BYTES, st + a_bytes, B_PLANE, NP == 3 || ks == 0);
     wg_commit();
     if (ks + 1 < n_slices) stage_a_direct<NP, THREADS>(A, lda, m0, M, (ks + 1) * BK, K, smem + (s ^ 1) * stage_bytes, tid, vec_ok);
     wg_wait_all();
     if constexpr (NP == 3) {
-#pragma unroll
-      for (int q = 0; q < 64; ++q) tot[q] += acc[q];
-#pragma unroll
-      for (int j = 0; j < BK / 16; ++j) {
+      static_assert(BK / 16 == 4, "four hi * hi steps per K slice");
+      auto hi_hi = [&](float (&d)[64], int j) {
         wg_fence();
-        wgmma_128(acc, make_desc(st + wg * (64 * 128) + 32u * j), make_desc(st + a_bytes + 32u * j), 0u);   // hi * hi
+        wgmma_128_fresh(d, make_desc(st + wg * (64 * 128) + 32u * j), make_desc(st + a_bytes + 32u * j));
         wg_commit();
-        wg_wait_all();
+      };
+      auto add_unbiased = [&](float (&d)[64]) {              // after the wait that completes d
+        fence_operand(d);
 #pragma unroll
-        for (int q = 0; q < 64; ++q) tot[q] += unbias_rz(acc[q]);
-      }
+        for (int q = 0; q < 64; ++q) tot[q] += unbias_rz(d[q]);
+      };
+      hi_hi(acc2, 0);
+      fence_operand(acc);
+#pragma unroll
+      for (int q = 0; q < 64; ++q) tot[q] += acc[q];          // corrections
+      hi_hi(acc, 1);
+      wg_wait_but_one();
+      add_unbiased(acc2);                                     // hh0
+      hi_hi(acc2, 2);
+      wg_wait_but_one();
+      add_unbiased(acc);                                      // hh1
+      hi_hi(acc, 3);
+      wg_wait_but_one();
+      add_unbiased(acc2);                                     // hh2
+      wg_wait_all();
+      add_unbiased(acc);                                      // hh3
     }
     fence_proxy_async();
     __syncthreads();
   }
   float* acc_s = reinterpret_cast<float*>(smem);              // the operand stages are free by now
-  if constexpr (NP == 3) acc_to_smem(tot, acc_s, wg, tid & 127);
-  else acc_to_smem(acc, acc_s, wg, tid & 127);
+  if constexpr (NP == 3) acc_to_smem<WN>(tot, acc_s, wg, tid & 127);
+  else acc_to_smem<WN>(acc, acc_s, wg, tid & 127);
   __syncthreads();
-  tile_epilogue(acc_s, m0, M, n0, N, epi, tid);
+  tile_epilogue<WN>(acc_s, m0, M, n0, N, epi, tid);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -458,7 +558,7 @@ gemm_tn_kernel(const float* __restrict__ A, int64_t lda, const float* __restrict
     const int s = i & 1;
     const uint32_t st = smem_u32(smem + s * stage_bytes);
     wg_fence();
-    mma_slice<2>(acc, st + wg * (64 * 128), A_HALF_BYTES, st + 2 * A_HALF_BYTES, B_HALF_BYTES, i == 0);
+    mma_slice<2, BN>(acc, st + wg * (64 * 128), A_HALF_BYTES, st + 2 * A_HALF_BYTES, B_HALF_BYTES, i == 0);
     wg_commit();
     if (i + 1 < n_sl) stage(i + 1, smem + (s ^ 1) * stage_bytes);
     wg_wait_all();
@@ -481,9 +581,9 @@ gemm_tn_kernel(const float* __restrict__ A, int64_t lda, const float* __restrict
         }
   }
   float* acc_s = reinterpret_cast<float*>(smem);
-  acc_to_smem(acc, acc_s, wg, tid & 127);
+  acc_to_smem<BN>(acc, acc_s, wg, tid & 127);
   __syncthreads();
-  tile_epilogue(acc_s, m0, M, n0, N, epi, tid);
+  tile_epilogue<BN>(acc_s, m0, M, n0, N, epi, tid);
 }
 
 static inline int sm_count() {
@@ -496,23 +596,33 @@ static inline int sm_count() {
 }
 
 
-inline size_t w_smem_bytes(int np) { return 2 * (size_t)np * (A_HALF_BYTES + B_HALF_BYTES) + 2 * sizeof(uint64_t) + 1024; }
+// 2 stages x NP planes of the A and weight slices; the [128 x acc_ld(WN)] fp32 accumulator tile reuses them
+constexpr size_t w_smem_bytes(int np, int wn) { return 2 * (size_t)np * (A_HALF_BYTES + b_plane_bytes(wn)) + 2 * sizeof(uint64_t) + 1024; }
+static_assert(BM * acc_ld(2 * BN) * sizeof(float) <= 2 * 2 * (size_t)(A_HALF_BYTES + b_plane_bytes(2 * BN)), "accumulator tile");
 constexpr size_t TN_SMEM = 2 * (size_t)(2 * A_HALF_BYTES + 2 * B_HALF_BYTES) + 2 * sizeof(uint64_t) + 1024;
 
+template <int NP, int WN, class Epi>
+static inline int gemm_w_launch(const float* A, int64_t lda, int64_t M, int N, int K, const uint16_t* img, const Epi& epi, cudaStream_t st) {
+  constexpr size_t smem = w_smem_bytes(NP, WN);
+  static bool attr_set = false;   // per template instantiation
+  if (!attr_set) {
+    NUDF_CUDA_OK(cudaFuncSetAttribute(gemm_w_kernel<NP, WN, Epi>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    attr_set = true;
+  }
+  const unsigned grid = (unsigned)(cdiv(M, BM) * cdiv(N, WN));
+  LaunchTimer lt_(epi_family<Epi>::value, st);
+  gemm_w_kernel<NP, WN, Epi><<<grid, THREADS, smem, st>>>(A, lda, M, N, K, img, epi);
+  NUDF_LAUNCH_OK();
+  return 0;
+}
+// The output width per CTA follows from the shape: 256 columns for 2-plane layers wider than 128 (one read and split of
+// each activation row block instead of two), 128 otherwise (3 planes, and 2-plane layers of at most 128 columns).
 template <int NP, class Epi>
 static inline int gemm_w(const float* A, int64_t lda, int64_t M, int N, int K, const uint16_t* img, const Epi& epi, cudaStream_t st) {
   if (M <= 0 || N <= 0) return 0;
-  const size_t smem = w_smem_bytes(NP);
-  static bool attr_set = false;   // per template instantiation
-  if (!attr_set) {
-    NUDF_CUDA_OK(cudaFuncSetAttribute(gemm_w_kernel<NP, Epi>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_set = true;
-  }
-  dim3 grid((unsigned)cdiv(M, BM), (unsigned)cdiv(N, BN));
-  LaunchTimer lt_(epi_family<Epi>::value, st);
-  gemm_w_kernel<NP, Epi><<<grid, THREADS, smem, st>>>(A, lda, M, N, K, img, epi);
-  NUDF_LAUNCH_OK();
-  return 0;
+  if constexpr (NP == 2)
+    if (N > BN) return gemm_w_launch<2, 2 * BN, Epi>(A, lda, M, N, K, img, epi, st);
+  return gemm_w_launch<NP, BN, Epi>(A, lda, M, N, K, img, epi, st);
 }
 
 // split the points so that (M tiles x N tiles x splits) fills the SMs once, with at least `min_points` points per CTA
