@@ -41,13 +41,14 @@ static inline int gemm_nn(const float* A, int64_t lda, const float* W, int64_t l
 int colsum(const float* X, int64_t ldx, const float* w, float wscale, int64_t P, int N, float* out, cudaStream_t st);
 
 // colsum_a (optional): colsum_a[m] += sum_k A[k, m] -- the bias gradient that goes with a weight gradient; fused into the
-// tensor-engine kernel's operand staging, a separate reduction kernel on the FFMA path.
+// tensor-engine kernel's operand staging, a separate reduction kernel on the FFMA path.  Each engine picks its own split
+// over the points: tc::gemm_tn from the shape (tn_k_chunk), the FFMA kernel one split per SIMT_TN_POINTS points.
+constexpr int64_t SIMT_TN_POINTS = 2048;
 template <class Epi>
 static inline int gemm_tn(const float* A, int64_t lda, const float* B, int64_t ldb, int M, int N, int64_t K,
-                          const Epi& epi, cudaStream_t st, int split_k, int chain = TC_WGRAD, float* colsum_a = nullptr) {
-  if (tc_on(chain) && M >= 32 && N >= 32 && K >= 128)
-    return tc::gemm_tn(A, lda, B, ldb, M, N, K, epi, st, tc::tn_splits(M, N, K, 512), colsum_a);
-  if (int rc = gemm_simt<false, false, Epi>(A, lda, B, ldb, M, N, K, epi, st, split_k)) return rc;
+                          const Epi& epi, cudaStream_t st, int chain = TC_WGRAD, float* colsum_a = nullptr) {
+  if (tc_on(chain) && M >= 32 && N >= 32 && K >= 128) return tc::gemm_tn(A, lda, B, ldb, M, N, K, epi, st, colsum_a);
+  if (int rc = gemm_simt<false, false, Epi>(A, lda, B, ldb, M, N, K, epi, st, (int)cdiv(K, SIMT_TN_POINTS))) return rc;
   if (colsum_a != nullptr) return colsum(A, lda, nullptr, 1.f, K, M, colsum_a, st);
   return 0;
 }

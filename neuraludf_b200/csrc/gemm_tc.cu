@@ -33,15 +33,9 @@ int nudf_wgrad(const float* dZ, int64_t ldz, const float* X, int64_t ldx, int32_
                int64_t ldw, int32_t engine, void* stream) {
   NUDF_REQUIRE(dZ && X && dW, "null pointer");
   EpiAtomicAdd e{dW, ldw};
-  if (engine == 1) {
-    const int tiles = (int)(cdiv(n_out, 128) * cdiv(n_in, 256));
-    int splits = tc::sm_count() / tiles;
-    const int max_splits = (int)cdiv(P, 512);
-    if (splits > max_splits) splits = max_splits;
-    if (splits < 1) splits = 1;
-    return tc::gemm_tn(dZ, ldz, X, ldx, n_out, n_in, P, e, (cudaStream_t)stream, splits);
-  }
-  return gemm_simt<false, false, EpiAtomicAdd>(dZ, ldz, X, ldx, n_out, n_in, P, e, (cudaStream_t)stream, (int)cdiv(P, 2048));
+  // the same partition over the points as inside the networks' backward passes (gemm_engine.cuh)
+  if (engine == 1) return tc::gemm_tn(dZ, ldz, X, ldx, n_out, n_in, P, e, (cudaStream_t)stream);
+  return gemm_simt<false, false, EpiAtomicAdd>(dZ, ldz, X, ldx, n_out, n_in, P, e, (cudaStream_t)stream, (int)cdiv(P, SIMT_TN_POINTS));
 }
 
 }  // extern "C"

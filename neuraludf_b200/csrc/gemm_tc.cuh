@@ -358,15 +358,14 @@ __device__ __forceinline__ void stage_a_direct(const float* __restrict__ A, int6
 // One warp stages a [32 rows x 64 k] block of the K-major tile  T(r, k) = X[(k0 + k) * ld + m0 + r]  as 2 bf16 planes
 // (on-the-fly transpose; the contraction index k runs over points).  Lane l owns the m-quad (l & 7) and, in iteration q,
 // the k pair 4q + (l >> 3): every warp-level load covers 4 rows of X x 128 contiguous bytes (4 L1 wavefronts instead of
-// the 32 of a lane-per-row mapping); all 16 loads of a lane are issued before the first conversion.
-template <bool CSUM = false>
-__device__ __forceinline__ void stage_block_t(const float* __restrict__ X, int64_t ld, int m0, int m_total, int r0, int rows,
-                                              int64_t k0, int64_t k_end, uint8_t* s_hi, uint8_t* s_lo, int lane, bool vec_ok,
-                                              float* csum = nullptr) {
+// the 32 of a lane-per-row mapping).  Two steps, so that the 16 loads of a lane stay in flight while the tensor cores work
+// on the previous slice: fetch_block_t loads the block into registers, store_block_t splits them into the stage.
+// Tile rows are padded to 16 and blocks cover 32: both skip the quads beyond the tile.
+__device__ __forceinline__ void fetch_block_t(const float* __restrict__ X, int64_t ld, int m0, int m_total, int r0, int rows,
+                                              int64_t k0, int64_t k_end, int lane, bool vec_ok, float4 (&v)[8][2]) {
   const int mq = lane & 7, kq = lane >> 3;
-  if (r0 + 4 * mq >= rows) return;      // tile rows are padded to 16, blocks cover 32: skip quads beyond the tile
+  if (r0 + 4 * mq >= rows) return;
   const int m = m0 + r0 + 4 * mq;
-  float4 v[8][2];
 #pragma unroll
   for (int q = 0; q < 8; ++q) {
 #pragma unroll
@@ -386,6 +385,12 @@ __device__ __forceinline__ void stage_block_t(const float* __restrict__ X, int64
       }
     }
   }
+}
+template <bool CSUM = false>
+__device__ __forceinline__ void store_block_t(const float4 (&v)[8][2], int r0, int rows, uint8_t* s_hi, uint8_t* s_lo, int lane,
+                                              float* csum = nullptr) {
+  const int mq = lane & 7, kq = lane >> 3;
+  if (r0 + 4 * mq >= rows) return;
   if (CSUM) {                             // per-lane partial column sums of X (bias gradients), fp32
 #pragma unroll
     for (int q = 0; q < 8; ++q) {
@@ -515,7 +520,9 @@ gemm_w_kernel(const float* __restrict__ A, int64_t lda, int64_t M, int N, int K,
 // ---------------------------------------------------------------------------------------------------------------
 // C[M x N] += A[K x M]^T B[K x N]  (weight gradients; contraction over points, split over gridDim.z), row-major operands.
 // grid = (ceil(M/128), ceil(N/128), splits).  Epi is the caller's epilogue with one split, EpiSplitStore into the split-K
-// workspace with several.  Warps 0-3 stage the [128 x 64] A^T slice, warps 4-7 the B^T slice (stage_block_t).
+// workspace with several.  Warps 0-3 stage the [128 x 64] A^T slice, warps 4-7 the B^T slice (fetch_block_t /
+// store_block_t).  Slice i + 1 waits in registers while the tensor cores work on slice i: iteration i issues the wgmma
+// group of slice i, splits slice i + 1 into the free stage, issues the loads of slice i + 2, then waits for the group.
 // colsum (optional): colsum[m] += sum_k A[k, m], the bias gradient, from the values the A stagers hold anyway; one writer
 // per column and split (cs_ws: [split][M], or the output itself with one split).
 // ---------------------------------------------------------------------------------------------------------------
@@ -534,21 +541,29 @@ gemm_tn_kernel(const float* __restrict__ A, int64_t lda, const float* __restrict
   const int n_sl = ke > kb ? (int)((ke - kb + BK - 1) / BK) : 0;
   constexpr uint32_t stage_bytes = 2u * A_HALF_BYTES + 2u * B_HALF_BYTES;
   const bool do_csum = colsum != nullptr && blockIdx.y == 0;
+  const bool a_vec = ((lda & 3) == 0) && aligned16(A) && ((m0 & 3) == 0);
+  const bool b_vec = ((ldb & 3) == 0) && aligned16(B);
+  const bool b_warp = warp >= 4 && 32 * (warp - 4) < rows_b;
   float csum[4] = {0.f, 0.f, 0.f, 0.f};
+  float4 v[8][2];                                           // this thread's part of the next K slice
 
-  auto stage = [&](int i, uint8_t* st) {                    // K slice i into stage st
+  auto fetch = [&](int i) {                                 // K slice i into v
     const int64_t k0 = kb + (int64_t)i * BK;
+    if (warp < 4) fetch_block_t(A, lda, m0, M, 32 * warp, BM, k0, ke, lane, a_vec, v);
+    else if (b_warp) fetch_block_t(B, ldb, n0, N, 32 * (warp - 4), rows_b, k0, ke, lane, b_vec, v);
+  };
+  auto store = [&](uint8_t* st) {                           // v into stage st
     if (warp < 4) {
-      const bool a_vec = ((lda & 3) == 0) && aligned16(A) && ((m0 & 3) == 0);
-      if (do_csum) stage_block_t<true>(A, lda, m0, M, 32 * warp, BM, k0, ke, st, st + A_HALF_BYTES, lane, a_vec, csum);
-      else stage_block_t(A, lda, m0, M, 32 * warp, BM, k0, ke, st, st + A_HALF_BYTES, lane, a_vec);
-    } else if (32 * (warp - 4) < rows_b) {
-      const bool b_vec = ((ldb & 3) == 0) && aligned16(B);
-      stage_block_t(B, ldb, n0, N, 32 * (warp - 4), rows_b, k0, ke, st + 2 * A_HALF_BYTES, st + 2 * A_HALF_BYTES + B_HALF_BYTES, lane, b_vec);
+      if (do_csum) store_block_t<true>(v, 32 * warp, BM, st, st + A_HALF_BYTES, lane, csum);
+      else store_block_t(v, 32 * warp, BM, st, st + A_HALF_BYTES, lane);
+    } else if (b_warp) {
+      store_block_t(v, 32 * (warp - 4), rows_b, st + 2 * A_HALF_BYTES, st + 2 * A_HALF_BYTES + B_HALF_BYTES, lane);
     }
   };
   if (n_sl == 0) return;
-  stage(0, smem);
+  fetch(0);
+  store(smem);
+  if (n_sl > 1) fetch(1);
   fence_proxy_async();
   __syncthreads();
   float acc[64];
@@ -560,7 +575,10 @@ gemm_tn_kernel(const float* __restrict__ A, int64_t lda, const float* __restrict
     wg_fence();
     mma_slice<2, BN>(acc, st + wg * (64 * 128), A_HALF_BYTES, st + 2 * A_HALF_BYTES, B_HALF_BYTES, i == 0);
     wg_commit();
-    if (i + 1 < n_sl) stage(i + 1, smem + (s ^ 1) * stage_bytes);
+    if (i + 1 < n_sl) {
+      store(smem + (s ^ 1) * stage_bytes);                  // stage s ^ 1 was released by the wait + barrier of i - 1
+      if (i + 2 < n_sl) fetch(i + 2);
+    }
     wg_wait_all();
     fence_proxy_async();
     __syncthreads();
@@ -625,23 +643,27 @@ static inline int gemm_w(const float* A, int64_t lda, int64_t M, int N, int K, c
   return gemm_w_launch<NP, BN, Epi>(A, lda, M, N, K, img, epi, st);
 }
 
-// split the points so that (M tiles x N tiles x splits) fills the SMs once, with at least `min_points` points per CTA
-static inline int tn_splits(int M, int N, int64_t K, int64_t min_points) {
-  const int tiles = (int)(cdiv(M, BM) * cdiv(N, BN));
-  int splits = sm_count() / tiles;
-  const int max_splits = (int)cdiv(K, min_points);
-  if (splits > max_splits) splits = max_splits;
-  return splits < 1 ? 1 : splits;
+// The split of a weight-gradient contraction over its points (split-K), from the shape alone: the same inputs give the
+// same partition, hence the same bits, on every device.  (M tiles x N tiles x splits) fills the 132 SMs of an H100 SXM
+// once, each split has at least TN_MIN_POINTS points and a whole number of BK slices, and the per-split partial tiles
+// and column sums fit the split-K workspace.  Returns the points per split.
+constexpr int TN_WAVE_CTAS = 132;
+constexpr int64_t TN_MIN_POINTS = 512;
+static inline int64_t tn_k_chunk(int M, int N, int64_t K) {
+  const int64_t tiles = cdiv(M, BM) * cdiv(N, BN);
+  int64_t splits = TN_WAVE_CTAS / tiles;
+  if (splits > cdiv(K, TN_MIN_POINTS)) splits = cdiv(K, TN_MIN_POINTS);
+  splits = ws_splits(splits < 1 ? 1 : (int)splits, (int64_t)M * N + M);
+  return round_up(cdiv(K, splits), BK);
 }
 
 // C[M x N] += A[K x M]^T B[K x N] over row-major operands; colsum_a (optional) += the column sums of A
 template <class Epi>
 static inline int gemm_tn(const float* A, int64_t lda, const float* B, int64_t ldb, int M, int N, int64_t K, const Epi& epi,
-                          cudaStream_t st, int splits, float* colsum_a = nullptr) {
+                          cudaStream_t st, float* colsum_a = nullptr) {
   if (M <= 0 || N <= 0 || K <= 0) return 0;
-  splits = ws_splits(splits < 1 ? 1 : splits, (int64_t)M * N + M);
-  const int64_t k_chunk = round_up(cdiv(K, splits), BK);
-  splits = (int)cdiv(K, k_chunk);
+  const int64_t k_chunk = tn_k_chunk(M, N, K);
+  const int splits = (int)cdiv(K, k_chunk);
   dim3 grid((unsigned)cdiv(M, BM), (unsigned)cdiv(N, BN), (unsigned)splits);
   LaunchTimer lt_(FAM_TC_WGRAD, st);
   if (splits == 1) {

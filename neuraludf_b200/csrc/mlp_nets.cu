@@ -224,9 +224,8 @@ static int wgrad(const float* dZ, int64_t ldz, const float* X, int64_t ldx, int 
     if (int rc = splitk_reduce(ws, chunks, n_out, n_in, EpiAtomicAdd{dW, ldw}, st)) return rc;
     return db != nullptr ? vec_reduce(part_b, chunks, n_out, db, st) : 0;
   }
-  int split = (int)cdiv(P, 2048);
   EpiAtomicAdd ew{dW, ldw};
-  return gemm_tn(dZ, ldz, X, ldx, n_out, n_in, P, ew, st, split, TC_WGRAD, db);
+  return gemm_tn(dZ, ldz, X, ldx, n_out, n_in, P, ew, st, TC_WGRAD, db);
 }
 
 // =================================================================================================================

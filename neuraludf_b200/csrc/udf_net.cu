@@ -522,7 +522,6 @@ static int udf_backward_impl(const nudf_udf_desc* d, const float* wfold, const f
   UdfScratch s;
   scratch_layout(p, P, &s);
   const int last = p.n_lin - 1;
-  const int split = (int)cdiv(P, 2048);
 
   // ---- tangent chain (second-order terms) ----
   if (grad_bar) {
@@ -534,7 +533,7 @@ static int udf_backward_impl(const nudf_udf_desc* d, const float* wfold, const f
     for (int l = 0; l < last; ++l) {
       // dW_l += D_l^T Adot_l
       EpiAtomicAdd ew{dwfold + p.w_off[l], p.w_ld[l]};
-      if (int rc = gemm_tn(ctx + c.d[l], p.o_ld[l], adot, ld_adot, p.out_dim[l], p.in_dim[l], P, ew, st, split)) return rc;
+      if (int rc = gemm_tn(ctx + c.d[l], p.o_ld[l], adot, ld_adot, p.out_dim[l], p.in_dim[l], P, ew, st)) return rc;
       float* nxt = scratch + s.adot[l & 1];
       int64_t ld_nxt = p.a_ld[l + 1];
       EpiTan et;
@@ -575,7 +574,7 @@ static int udf_backward_impl(const nudf_udf_desc* d, const float* wfold, const f
     const float* Wl = wfold + p.w_off[last];
     float* dWl = dwfold + p.w_off[last];
     EpiAtomicAdd ew{dWl + p.w_ld[last], p.w_ld[last]};
-    if (int rc = gemm_tn(zf, F, ctx + c.a[last], p.a_ld[last], F, p.in_dim[last], P, ew, st, split, TC_WGRAD, dbias + p.b_off[last] + 1))
+    if (int rc = gemm_tn(zf, F, ctx + c.a[last], p.a_ld[last], F, p.in_dim[last], P, ew, st, TC_WGRAD, dbias + p.b_off[last] + 1))
       return rc;
     if (int rc = colsum(ctx + c.a[last], p.a_ld[last], z0, 1.0f, P, p.in_dim[last], dWl, st)) return rc;
     if (int rc = colsum(z0, 1, nullptr, 1.0f, P, 1, dbias + p.b_off[last], st)) return rc;
@@ -590,7 +589,7 @@ static int udf_backward_impl(const nudf_udf_desc* d, const float* wfold, const f
     zlast_kernel<<<nblk(P * p.y_ld, 256), 256, 0, st>>>(ub, ld_ub, fb, ld_fb, ctx + c.sgn, 1.0f / p.scale, p.d_out, p.y_ld, P, zl);
     NUDF_LAUNCH_OK();
     EpiAtomicAdd ew{dwfold + p.w_off[last], p.w_ld[last]};
-    if (int rc = gemm_tn(zl, p.y_ld, ctx + c.a[last], p.a_ld[last], p.out_dim[last], p.in_dim[last], P, ew, st, split, TC_WGRAD,
+    if (int rc = gemm_tn(zl, p.y_ld, ctx + c.a[last], p.a_ld[last], p.out_dim[last], p.in_dim[last], P, ew, st, TC_WGRAD,
                          dbias + p.b_off[last]))
       return rc;
     EpiBwd eb;
@@ -606,7 +605,7 @@ static int udf_backward_impl(const nudf_udf_desc* d, const float* wfold, const f
     const float* A = l == 0 ? ctx + c.e0 : ctx + c.a[l];
     int64_t lda = l == 0 ? p.pe_ld : p.a_ld[l];
     EpiAtomicAdd ew{dwfold + p.w_off[l], p.w_ld[l]};
-    if (int rc = gemm_tn(zb, p.o_ld[l], A, lda, p.out_dim[l], p.in_dim[l], P, ew, st, split, TC_WGRAD, dbias + p.b_off[l])) return rc;
+    if (int rc = gemm_tn(zb, p.o_ld[l], A, lda, p.out_dim[l], p.in_dim[l], P, ew, st, TC_WGRAD, dbias + p.b_off[l])) return rc;
     if (l > 0) {
       EpiBwd eb;
       eb.n_main = p.out_dim[l - 1]; eb.post_scale = (l == p.skip) ? NUDF_SQRT1_2 : 1.0f;
