@@ -225,6 +225,28 @@ int nudf_render_composite_forward(const nudf_render_cfg* cfg, const float* heads
                                   const float* bg_alpha, const float* bg_color, const nudf_render_out* out,
                                   void* stream);
 
+/* per-ray outputs of the forward-only view renderer; each may be NULL.  They may point into a larger image at the chunk's
+ * first ray, so that a whole view is written in place. */
+typedef struct nudf_view_out {
+  float* color;        /* [N,3]  as nudf_render_composite_forward's `color` (same bits) */
+  float* color_pixel;  /* [N,3]  pixel-blend composite (needs c_pix) */
+  float* depth;        /* [N,1]  as nudf_render_composite_forward's `depth` (same bits) */
+  float* normal;       /* [N,3]  rot @ sum_i gradients_flip_i * weights_i * inside_sphere_i over the S foreground samples */
+  float* weight_sum;   /* [N,1]  foreground weight sum */
+} nudf_view_out;
+
+/* Forward-only compositing of whole views (the image outputs of exp_runner_blending.py's validate(), :621-682): the alpha,
+ * visibility scan and weights of nudf_render_composite_forward (the same device code), no per-sample outputs, no state for
+ * a backward pass.  Inputs as nudf_render_composite_forward, without sampled_color_base, plus
+ *   c_pix  [N*S,3] per-sample pixel-blend colour (nudf_blend_forward's c_pix) or NULL.  When n_outside > 0 the blend
+ *          colour of a sample outside the unit sphere is replaced by bg_color of its own column (:503-507), so bg_color
+ *          must then hold all S+O columns;
+ *   rot    HOST row-major 3x3 applied to the normal (the inverse of the view's pose rotation, :681). */
+int nudf_render_view_forward(const nudf_render_cfg* cfg, const float* heads, const float* rays_d, const float* pts,
+                             const float* mid_z, const float* dists, const float* udf, int64_t ld_udf, const float* grads,
+                             const float* sampled_color, const float* c_pix, const float* bg_alpha, const float* bg_color,
+                             const float* rot, const nudf_view_out* out, void* stream);
+
 typedef struct nudf_render_bar {   /* upstream gradients, any may be NULL */
   const float* color_base; const float* color; const float* depth;       /* [N,3] [N,3] [N,1] */
   const float* weight_sum; const float* weight_sum_fg_bg;                 /* [N,1] */

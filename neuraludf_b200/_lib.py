@@ -56,6 +56,13 @@ class RenderOut(ctypes.Structure):
     _fields_ = [(n, c_void_p) for n in RENDER_OUT_FIELDS]
 
 
+VIEW_OUT_FIELDS = ["color", "color_pixel", "depth", "normal", "weight_sum"]
+
+
+class ViewOut(ctypes.Structure):
+    _fields_ = [(n, c_void_p) for n in VIEW_OUT_FIELDS]
+
+
 class BlendCfg(ctypes.Structure):
     _fields_ = [(n, ctypes.c_int32) for n in ("n_rays", "n_samples", "n_views", "height", "width", "h_patch")]
 
@@ -145,6 +152,7 @@ _SIGNATURES = {
     "nudf_ray_points": (ctypes.c_int, [c_void_p, c_void_p, c_void_p, ctypes.c_int32, ctypes.c_int32, ctypes.c_float,
                                        c_void_p, c_void_p, c_void_p, c_void_p]),
     "nudf_render_composite_forward": (ctypes.c_int, [c_void_p] * 2 + [c_void_p] * 5 + [ctypes.c_int64] + [c_void_p] * 7),
+    "nudf_render_view_forward": (ctypes.c_int, [c_void_p] * 2 + [c_void_p] * 5 + [ctypes.c_int64] + [c_void_p] * 8),
     "nudf_render_composite_backward": (ctypes.c_int, [c_void_p] * 2 + [c_void_p] * 5 + [ctypes.c_int64] + [c_void_p] * 14),
     "nudf_up_sample": (ctypes.c_int, [ctypes.c_int32, c_void_p, c_void_p, c_void_p, c_void_p, ctypes.c_int32,
                                       ctypes.c_int32, ctypes.c_int32, ctypes.c_float, ctypes.c_float, ctypes.c_float,

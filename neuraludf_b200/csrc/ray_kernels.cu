@@ -181,6 +181,109 @@ __device__ __forceinline__ RaySmem carve(float* base, int SO, int n_arrays_check
 }
 constexpr int RK_ARRAYS = 10;
 
+// Compositing sums every forward entry point shares: colour, depth and the weight sums, accumulated in one fixed order
+// per accumulator and with explicitly rounded products / fused multiply-adds (the compiler's contraction choices depend
+// on the surrounding kernel), so that every entry point returns the same bits for them.  `ex` adds the caller's own per-sample terms:
+// ex.fg(i, p, w, u, g, gq) for a foreground sample (p = flat sample index), ex.bg(i, q, w, col) for a background column
+// (q = flat [N, S+O] index, col its colour).
+struct RaySums { float cc[3]; float depth, ws_fg, ws_all; };
+
+template <class Extra>
+__device__ __forceinline__ RaySums ray_composite(const nudf_render_cfg& cfg, const RayIn& in, int r, int lane, RaySmem sm,
+                                                 Extra& ex) {
+  const int S = cfg.n_samples, O = cfg.n_outside, SO = S + O;
+  const int64_t base = (int64_t)r * S;
+  const float d[3] = {in.rays_d[r * 3 + 0], in.rays_d[r * 3 + 1], in.rays_d[r * 3 + 2]};
+  RaySums s = {{0.f, 0.f, 0.f}, 0.f, 0.f, 0.f};
+  for (int i = lane; i < SO; i += 32) {
+    const float w = __fmul_rn(sm.alpha[i], sm.T[i]);
+    s.ws_all = __fadd_rn(s.ws_all, w);
+    if (i < S) {
+      const int64_t p = base + i;
+      s.ws_fg = __fadd_rn(s.ws_fg, w);
+      float u = in.udf[p * in.ld_udf];
+      const float g[3] = {in.grads[p * 3 + 0], in.grads[p * 3 + 1], in.grads[p * 3 + 2]};
+      GradQ gq = grad_quantities(g, d, cfg.use_norm_grad_for_cosine);
+#pragma unroll
+      for (int c = 0; c < 3; ++c) s.cc[c] = __fmaf_rn(w, in.sc[p * 3 + c], s.cc[c]);
+      s.depth = __fmaf_rn(w, in.mid_z[p], s.depth);
+      ex.fg(i, p, w, u, g, gq);
+    } else {
+      const int64_t q = (int64_t)r * SO + i;
+      float col[3];
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        col[c] = in.bg_color[q * 3 + c];
+        s.cc[c] = __fmaf_rn(w, col[c], s.cc[c]);
+      }
+      ex.bg(i, q, w, col);
+    }
+  }
+#pragma unroll
+  for (int c = 0; c < 3; ++c) s.cc[c] = warp_sum(s.cc[c]);
+  s.depth = warp_sum(s.depth); s.ws_fg = warp_sum(s.ws_fg); s.ws_all = warp_sum(s.ws_all);
+  return s;
+}
+
+// colour of the ray: composite plus the constant background colour behind it (:527-528)
+__device__ __forceinline__ float ray_color(const nudf_render_cfg& cfg, const RaySums& s, int c) {
+  float col = s.cc[c];
+  if (cfg.has_background_rgb) col = __fmaf_rn(cfg.background_rgb[c], __fsub_rn(1.0f, s.ws_all), col);
+  return col;
+}
+
+// sphere test of the regularisers and of the normal map (:512, :527): |pts| < 1
+__device__ __forceinline__ float sample_norm(const RayIn& in, int64_t p) {
+  float px = in.pts[p * 3 + 0], py = in.pts[p * 3 + 1], pz = in.pts[p * 3 + 2];
+  return sqrtf(px * px + py * py + pz * pz);
+}
+
+// render_core's own per-sample terms: colour_base, normals, regulariser sums, per-sample diagnostics
+struct CoreExtra {
+  const nudf_render_cfg& cfg; const RayIn& in; const nudf_render_out& out; const RaySmem& sm; int r;
+  float cb[3] = {0, 0, 0}, nrm[3] = {0, 0, 0};
+  float s_relax_ge = 0.f, s_relax = 0.f, s_near_ge = 0.f, s_near = 0.f, s_sparse = 0.f;
+  __device__ CoreExtra(const nudf_render_cfg& cfg_, const RayIn& in_, const nudf_render_out& out_, const RaySmem& sm_, int r_)
+      : cfg(cfg_), in(in_), out(out_), sm(sm_), r(r_) {}
+  __device__ __forceinline__ void weight(int i, float w) {
+    if (out.weights) out.weights[(int64_t)r * (cfg.n_samples + cfg.n_outside) + i] = w;
+  }
+  __device__ __forceinline__ void fg(int i, int64_t p, float w, float u, const float g[3], const GradQ& gq) {
+    weight(i, w);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      cb[c] += w * in.scb[p * 3 + c];
+      nrm[c] += w * gq.flip * g[c];
+    }
+    float pn = sample_norm(in, p);
+    float inside = pn < 1.0f ? 1.f : 0.f, relax = pn < 1.2f ? 1.f : 0.f, near = u < 0.05f ? 1.f : 0.f;
+    float ge = (gq.gmag - 1.0f) * (gq.gmag - 1.0f);
+    s_relax_ge += relax * ge; s_relax += relax; s_near_ge += near * ge; s_near += near;
+    s_sparse += expf(-cfg.sparse_scale_factor * u);
+    // per-sample diagnostics
+    float raw, aocc;
+    occ_forward(u, in.dists[p], in.heads[1], in.heads[2], &raw, &aocc);
+    if (out.gradient_mag) out.gradient_mag[p] = gq.gmag;
+    if (out.true_cos) out.true_cos[p] = gq.tc;
+    if (out.vis_prob) out.vis_prob[p] = clampf_(sm.P[i], 0.f, 1.f);
+    if (out.alpha) out.alpha[p] = sm.alpha[i];
+    if (out.alpha_plus) out.alpha_plus[p] = sm.ap[i];
+    if (out.alpha_minus) out.alpha_minus[p] = sm.am[i];
+    if (out.alpha_occ) out.alpha_occ[p] = aocc;
+    if (out.raw_occ) out.raw_occ[p] = raw;
+    if (out.inside_sphere) out.inside_sphere[p] = inside;
+    if (out.gradients_flip) {
+#pragma unroll
+      for (int c = 0; c < 3; ++c) out.gradients_flip[p * 3 + c] = gq.flip * g[c];
+    }
+  }
+  __device__ __forceinline__ void bg(int i, int64_t q, float w, const float col[3]) {
+    weight(i, w);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) cb[c] = __fmaf_rn(w, col[c], cb[c]);
+  }
+};
+
 __global__ void __launch_bounds__(RK_WARPS * 32)
 composite_forward_kernel(nudf_render_cfg cfg, RayIn in, nudf_render_out out) {
   extern __shared__ float smem[];
@@ -191,71 +294,20 @@ composite_forward_kernel(nudf_render_cfg cfg, RayIn in, nudf_render_out out) {
   RaySmem sm = carve(smem + (size_t)warp * RK_ARRAYS * SO, SO, RK_ARRAYS);
   ray_forward_state(cfg, in, r, lane, sm);
 
-  const int64_t base = (int64_t)r * S;
-  const float d[3] = {in.rays_d[r * 3 + 0], in.rays_d[r * 3 + 1], in.rays_d[r * 3 + 2]};
-  float cb[3] = {0, 0, 0}, cc[3] = {0, 0, 0}, nrm[3] = {0, 0, 0};
-  float depth = 0.f, ws_fg = 0.f, ws_all = 0.f;
-  float s_relax_ge = 0.f, s_relax = 0.f, s_near_ge = 0.f, s_near = 0.f, s_sparse = 0.f;
-  for (int i = lane; i < SO; i += 32) {
-    float w = sm.alpha[i] * sm.T[i];
-    if (out.weights) out.weights[(int64_t)r * SO + i] = w;
-    ws_all += w;
-    if (i < S) {
-      const int64_t p = base + i;
-      ws_fg += w;
-      float u = in.udf[p * in.ld_udf];
-      const float g[3] = {in.grads[p * 3 + 0], in.grads[p * 3 + 1], in.grads[p * 3 + 2]};
-      GradQ gq = grad_quantities(g, d, cfg.use_norm_grad_for_cosine);
+  CoreExtra ex(cfg, in, out, sm, r);
+  const RaySums s = ray_composite(cfg, in, r, lane, sm, ex);
+  float* cb = ex.cb; float* nrm = ex.nrm;
+  const float* cc = s.cc;
+  const float depth = s.depth, ws_fg = s.ws_fg, ws_all = s.ws_all;
 #pragma unroll
-      for (int c = 0; c < 3; ++c) {
-        cb[c] += w * in.scb[p * 3 + c];
-        cc[c] += w * in.sc[p * 3 + c];
-        nrm[c] += w * gq.flip * g[c];
-      }
-      depth += w * in.mid_z[p];
-      float px = in.pts[p * 3 + 0], py = in.pts[p * 3 + 1], pz = in.pts[p * 3 + 2];
-      float pn = sqrtf(px * px + py * py + pz * pz);
-      float inside = pn < 1.0f ? 1.f : 0.f, relax = pn < 1.2f ? 1.f : 0.f, near = u < 0.05f ? 1.f : 0.f;
-      float ge = (gq.gmag - 1.0f) * (gq.gmag - 1.0f);
-      s_relax_ge += relax * ge; s_relax += relax; s_near_ge += near * ge; s_near += near;
-      s_sparse += expf(-cfg.sparse_scale_factor * u);
-      // per-sample diagnostics
-      float raw, aocc;
-      occ_forward(u, in.dists[p], in.heads[1], in.heads[2], &raw, &aocc);
-      if (out.gradient_mag) out.gradient_mag[p] = gq.gmag;
-      if (out.true_cos) out.true_cos[p] = gq.tc;
-      if (out.vis_prob) out.vis_prob[p] = clampf_(sm.P[i], 0.f, 1.f);
-      if (out.alpha) out.alpha[p] = sm.alpha[i];
-      if (out.alpha_plus) out.alpha_plus[p] = sm.ap[i];
-      if (out.alpha_minus) out.alpha_minus[p] = sm.am[i];
-      if (out.alpha_occ) out.alpha_occ[p] = aocc;
-      if (out.raw_occ) out.raw_occ[p] = raw;
-      if (out.inside_sphere) out.inside_sphere[p] = inside;
-      if (out.gradients_flip) {
-#pragma unroll
-        for (int c = 0; c < 3; ++c) out.gradients_flip[p * 3 + c] = gq.flip * g[c];
-      }
-    } else {
-      const int64_t q = (int64_t)r * SO + i;
-#pragma unroll
-      for (int c = 0; c < 3; ++c) {
-        float col = in.bg_color[q * 3 + c];
-        cb[c] += w * col; cc[c] += w * col;
-      }
-    }
-  }
-#pragma unroll
-  for (int c = 0; c < 3; ++c) { cb[c] = warp_sum(cb[c]); cc[c] = warp_sum(cc[c]); nrm[c] = warp_sum(nrm[c]); }
-  depth = warp_sum(depth); ws_fg = warp_sum(ws_fg); ws_all = warp_sum(ws_all);
-  s_relax_ge = warp_sum(s_relax_ge); s_relax = warp_sum(s_relax); s_near_ge = warp_sum(s_near_ge);
-  s_near = warp_sum(s_near); s_sparse = warp_sum(s_sparse);
+  for (int c = 0; c < 3; ++c) { cb[c] = warp_sum(cb[c]); nrm[c] = warp_sum(nrm[c]); }
+  const float s_relax_ge = warp_sum(ex.s_relax_ge), s_relax = warp_sum(ex.s_relax), s_near_ge = warp_sum(ex.s_near_ge);
+  const float s_near = warp_sum(ex.s_near), s_sparse = warp_sum(ex.s_sparse);
   if (lane == 0) {
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
-      float col = cc[c];
-      if (cfg.has_background_rgb) col += cfg.background_rgb[c] * (1.0f - ws_all);
       if (out.color_base) out.color_base[r * 3 + c] = cb[c];
-      if (out.color) out.color[r * 3 + c] = col;
+      if (out.color) out.color[r * 3 + c] = ray_color(cfg, s, c);
       if (out.normals) out.normals[r * 3 + c] = nrm[c];
     }
     if (out.depth) out.depth[r] = depth;
@@ -271,6 +323,70 @@ composite_forward_kernel(nudf_render_cfg cfg, RayIn in, nudf_render_out out) {
       const float chk = cc[0] + cc[1] + cc[2] + cb[0] + cb[1] + cb[2] + depth + ws_all + s_relax_ge + s_near_ge + s_sparse;
       if (!isfinite(chk)) atomicOr(out.status, NUDF_STATUS_NONFINITE_RENDER);
     }
+  }
+}
+
+// The view renderer's per-sample terms: the pixel-blend composite and validate()'s normal map
+// (exp_runner_blending.py:641-668: sum of gradients_flip * weights * inside_sphere over the foreground samples).
+struct ViewExtra {
+  const RayIn& in; const float* c_pix; int64_t row;   // row = r * (S + O): first background column of the ray
+  int has_bg;
+  float cp[3] = {0, 0, 0}, nrm[3] = {0, 0, 0};
+  __device__ ViewExtra(const RayIn& in_, const float* c_pix_, int64_t row_, int has_bg_)
+      : in(in_), c_pix(c_pix_), row(row_), has_bg(has_bg_) {}
+  __device__ __forceinline__ void fg(int i, int64_t p, float w, float u, const float g[3], const GradQ& gq) {
+    const bool inside = sample_norm(in, p) < 1.0f;
+    if (inside) {
+#pragma unroll
+      for (int c = 0; c < 3; ++c) nrm[c] += gq.flip * g[c] * w;
+    }
+    if (c_pix) {
+      // outside the unit sphere the blended colour is replaced by the NeRF++ colour of the same column (:503-507)
+      const int64_t q = row + i;
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        float col = (has_bg && !inside) ? in.bg_color[q * 3 + c] : c_pix[p * 3 + c];
+        cp[c] += col * w;
+      }
+    }
+  }
+  __device__ __forceinline__ void bg(int i, int64_t q, float w, const float col[3]) {
+#pragma unroll
+    for (int c = 0; c < 3; ++c) cp[c] += col[c] * w;
+  }
+};
+
+struct ViewArgs {
+  const float* c_pix;   // [N*S,3] or null
+  float rot[9];         // row-major camera-from-world rotation of the normal map
+  nudf_view_out out;
+};
+
+__global__ void __launch_bounds__(RK_WARPS * 32)
+view_forward_kernel(nudf_render_cfg cfg, RayIn in, ViewArgs va) {
+  extern __shared__ float smem[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int r = blockIdx.x * RK_WARPS + warp;
+  if (r >= cfg.n_rays) return;
+  const int S = cfg.n_samples, O = cfg.n_outside, SO = S + O;
+  RaySmem sm = carve(smem + (size_t)warp * RK_ARRAYS * SO, SO, RK_ARRAYS);
+  ray_forward_state(cfg, in, r, lane, sm);
+
+  ViewExtra ex(in, va.c_pix, (int64_t)r * SO, O > 0);
+  const RaySums s = ray_composite(cfg, in, r, lane, sm, ex);
+  float cp[3], nw[3];
+#pragma unroll
+  for (int c = 0; c < 3; ++c) { cp[c] = warp_sum(ex.cp[c]); nw[c] = warp_sum(ex.nrm[c]); }
+  if (lane == 0) {
+    const nudf_view_out& o = va.out;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      if (o.color) o.color[r * 3 + c] = ray_color(cfg, s, c);
+      if (o.color_pixel) o.color_pixel[r * 3 + c] = cp[c];
+      if (o.normal) o.normal[r * 3 + c] = va.rot[c * 3 + 0] * nw[0] + va.rot[c * 3 + 1] * nw[1] + va.rot[c * 3 + 2] * nw[2];
+    }
+    if (o.depth) o.depth[r] = s.depth;
+    if (o.weight_sum) o.weight_sum[r] = s.ws_fg;
   }
 }
 
@@ -492,6 +608,27 @@ int nudf_render_composite_forward(const nudf_render_cfg* cfg, const float* heads
     NUDF_CUDA_OK(cudaFuncSetAttribute(composite_forward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   LaunchTimer lt_(FAM_RAY, (cudaStream_t)stream);
   composite_forward_kernel<<<(unsigned)cdiv(cfg->n_rays, RK_WARPS), RK_WARPS * 32, smem, (cudaStream_t)stream>>>(*cfg, in, *out);
+  NUDF_LAUNCH_OK();
+  return 0;
+}
+
+int nudf_render_view_forward(const nudf_render_cfg* cfg, const float* heads, const float* rays_d, const float* pts,
+                             const float* mid_z, const float* dists, const float* udf, int64_t ld_udf, const float* grads,
+                             const float* sampled_color, const float* c_pix, const float* bg_alpha, const float* bg_color,
+                             const float* rot, const nudf_view_out* out, void* stream) {
+  if (int rc = check_cfg(cfg, bg_alpha, bg_color)) return rc;
+  NUDF_REQUIRE(heads && rays_d && pts && mid_z && dists && udf && grads && sampled_color && rot && out, "null pointer");
+  if (cfg->n_rays <= 0) return 0;
+  RayIn in{heads, rays_d, pts, mid_z, dists, udf, ld_udf, grads, nullptr, sampled_color, bg_alpha, bg_color};
+  ViewArgs va;
+  va.c_pix = c_pix;
+  for (int k = 0; k < 9; ++k) va.rot[k] = rot[k];
+  va.out = *out;
+  size_t smem = (size_t)RK_WARPS * RK_ARRAYS * (cfg->n_samples + cfg->n_outside) * sizeof(float);
+  if (smem > 48 * 1024)
+    NUDF_CUDA_OK(cudaFuncSetAttribute(view_forward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  LaunchTimer lt_(FAM_RAY, (cudaStream_t)stream);
+  view_forward_kernel<<<(unsigned)cdiv(cfg->n_rays, RK_WARPS), RK_WARPS * 32, smem, (cudaStream_t)stream>>>(*cfg, in, va);
   NUDF_LAUNCH_OK();
   return 0;
 }

@@ -152,10 +152,13 @@ class UDFRendererBlending:
         return z_vals
 
     @torch.no_grad()
-    def importance_sample_mix(self, rays_o, rays_d, z_vals, sample_dist):
+    def importance_sample_mix(self, rays_o, rays_d, z_vals, sample_dist, gamma=None):
+        """`gamma`: the clipped gamma as a float, when the caller has already read it (render.render_view reads it once
+        per view); otherwise it is read here."""
         pts = ops.points_on_rays(rays_o, rays_d, z_vals)
         udf = self.udf_network.udf_values(pts).reshape(z_vals.shape)
-        gamma = float(self.beta_network.get_gamma().clip(1e-6, 1e6))   # one host read, as in the reference (:792)
+        if gamma is None:
+            gamma = float(self.beta_network.get_gamma().clip(1e-6, 1e6))   # one host read, as in the reference (:792)
         K = self.up_sample_steps
         m = self.n_importance // (K + 1)
         for i in range(K):

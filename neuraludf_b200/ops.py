@@ -726,3 +726,137 @@ def outside_points(rays_o, rays_d, z, col0, sample_dist):
     L.check(lib.nudf_outside_points(L.ptr(rays_o), L.ptr(rays_d), L.ptr(z), N, n, col0, float(sample_dist), L.ptr(pts4),
                                     L.ptr(dists), L.stream_ptr()), "nudf_outside_points")
     return pts4, dists
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# forward-only view rendering: the network forwards and the compositing pass outside autograd, every per-chunk array
+# carved from one caller-owned workspace
+# ---------------------------------------------------------------------------------------------------------------
+def udf_forward_split_into(handle, pts, udf, feat, grad, ctx):
+    """nudf_udf_forward_split into given buffers: udf [P], feat [P, d_out - 1], grad [P,3]; ctx is scratch (no backward)."""
+    lib = L.lib()
+    handle.refresh()
+    L.check(lib.nudf_udf_forward_split(ctypes.byref(handle.desc), L.ptr(handle.wfold), L.ptr(pts), pts.shape[0], L.ptr(udf),
+                                       L.ptr(feat), feat.shape[1], L.ptr(grad), L.ptr(ctx), L.stream_ptr()),
+            "nudf_udf_forward_split")
+
+
+def color_forward_into(handle, pts, dirs, samples_per_ray, feat, cb, c, bl, ctx):
+    lib = L.lib()
+    handle.refresh()
+    L.check(lib.nudf_color_forward(ctypes.byref(handle.desc), L.ptr(handle.wfold), L.ptr(pts), L.ptr(dirs),
+                                   int(samples_per_ray), L.ptr(feat), feat.stride(0), pts.shape[0], L.ptr(cb), L.ptr(c),
+                                   L.ptr(bl), L.ptr(ctx), L.stream_ptr()), "nudf_color_forward")
+
+
+def nerf_forward_into(handle, pts, dirs, samples_per_ray, sigma, rgb, ctx):
+    lib = L.lib()
+    L.check(lib.nudf_nerf_forward(ctypes.byref(handle.desc()), L.ptr(handle.images()), L.ptr(pts), L.ptr(dirs),
+                                  int(samples_per_ray), pts.shape[0], L.ptr(sigma), L.ptr(rgb), L.ptr(ctx), L.stream_ptr()),
+            "nudf_nerf_forward")
+
+
+def view_composite(cfg, heads, rays_d, pts, mid, dists, udf, grads, sc, c_pix, bg_alpha, bg_color, rot, outs):
+    """nudf_render_view_forward: outs maps color / color_pixel / depth / normal / weight_sum to [N, .] tensors (views
+    into the image buffers are fine) or None; rot is a host 3x3 (nested sequence or array)."""
+    lib = L.lib()
+    ro = L.ViewOut()
+    for k in L.VIEW_OUT_FIELDS:
+        t = outs.get(k)
+        setattr(ro, k, None if t is None else t.data_ptr())
+    r9 = (ctypes.c_float * 9)(*[float(v) for row in rot for v in row])
+    L.check(lib.nudf_render_view_forward(ctypes.byref(cfg), L.ptr(heads), L.ptr(rays_d), L.ptr(pts), L.ptr(mid), L.ptr(dists),
+                                         L.ptr(udf), 1, L.ptr(grads), L.ptr(sc), L.ptr(c_pix), L.ptr(bg_alpha),
+                                         L.ptr(bg_color), r9, ctypes.byref(ro), L.stream_ptr()), "nudf_render_view_forward")
+
+
+class ViewWorkspace:
+    """One fp32 buffer holding every array of one chunk of the forward-only view pipeline (render.render_view).
+
+    The network forwards keep no state for a backward pass, so their context buffers are scratch: the UDF, colour and
+    NeRF++ forwards (and the sampling stage's UDF value queries) share one region sized for the largest of them.  The
+    chunk size is the largest ray count whose arrays fit `budget_bytes`, from the library's nudf_*_ctx_floats queries."""
+
+    def __init__(self, renderer, n_rays, budget_bytes, device, n_views=0):
+        lib = L.lib()
+        udf_h = renderer.udf_network._handle
+        udf_h.refresh()
+        col_h = renderer.color_network._handle
+        col_h.refresh()
+        self.S0, self.S = renderer.n_samples, renderer.n_samples + renderer.n_importance
+        self.O = renderer.n_outside
+        self.F = udf_h.meta[2] - 1
+        self.nb = col_h.meta[3]
+        self.blend = n_views > 0
+        # NeRF++ columns evaluated per ray: all S+O when the pixel blend needs the inside columns too (render() does the same)
+        self.m = (self.S + self.O if self.blend else self.O) if self.O > 0 else 0
+        nerf_d = renderer.nerf._handle.desc() if self.O > 0 else None
+        S, SO, m = self.S, self.S + self.O, self.m
+
+        def ctx(n):
+            c = [lib.nudf_udf_ctx_floats(ctypes.byref(udf_h.desc), n * S, 1),
+                 lib.nudf_udf_ctx_floats(ctypes.byref(udf_h.desc), n * self.S0, 0),
+                 lib.nudf_color_ctx_floats(ctypes.byref(col_h.desc), n * S)]
+            if m:
+                c.append(lib.nudf_nerf_ctx_floats(ctypes.byref(nerf_d), n * m))
+            return max(c)
+
+        # per ray: pts, mid, dists, udf, feat, grad, cb, c, logits (+ c_pix) of S samples; NeRF++ inputs / outputs of m
+        # columns and the [S+O] background arrays; sampling and z-sorting temporaries (z, udf, points of each round)
+        self._per_ray = (S * (3 + 1 + 1 + 1 + self.F + 3 + 3 + 3 + self.nb + (3 if self.blend else 0))
+                         + m * (4 + 1 + 1 + 3) + SO * (1 + 3) + 8 * SO)
+        self._ctx = ctx
+        # the sampling stage's UDF value queries allocate their own scratch while the workspace is live: counted twice
+        total = lambda n: n * self._per_ray + 2 * ctx(n)
+        probe = min(4096, n_rays)
+        n = max(1, min(n_rays, int(budget_bytes // 4 * probe // total(probe))))
+        while n > 1 and total(n) * 4 > budget_bytes:
+            n = max(1, n * 15 // 16)
+        self.chunk = n
+        self.buf = torch.empty(n * (self._per_ray - 8 * SO) + ctx(n) + 64 * 16, dtype=torch.float32, device=device)
+
+    def carve(self, n):
+        """views of the workspace for a chunk of n <= self.chunk rays"""
+        S, SO, m = self.S, self.S + self.O, self.m
+        off = [0]
+        buf = self.buf
+
+        def take(*shape):             # every array starts on a 256-byte boundary (vector loads in the kernels)
+            k = 1
+            for s in shape:
+                k *= s
+            t = buf[off[0]:off[0] + k].view(*shape)
+            off[0] += -(-k // 64) * 64
+            return t
+        w = {"pts": take(n * S, 3), "mid": take(n, S), "dists": take(n, S), "udf": take(n * S), "feat": take(n * S, self.F),
+             "grad": take(n * S, 3), "cb": take(n * S, 3), "c": take(n * S, 3), "bl": take(n * S, self.nb)}
+        if self.blend:
+            w["c_pix"] = take(n * S, 3)
+        if m:
+            w.update(pts4=take(n * m, 4), odists=take(n, m), sigma=take(n * m, 1), rgb=take(n * m, 3), bg_alpha=take(n, SO),
+                     bg_color=take(n, SO, 3))
+        w["ctx"] = buf[off[0]:]
+        assert w["ctx"].numel() >= self._ctx(n)
+        return w
+
+
+def blend_pixels_into(pts, proj, imgs, logits, n_rays, n_samples, c_pix):
+    """nudf_blend_forward without patches (hom = NULL): pixel-blend colour c_pix [P,3] of every sample.  Pixel blending
+    does not depend on the patch size, so this serves any h_patch_size."""
+    lib = L.lib()
+    V, _, H, W = imgs.shape
+    cfg = L.BlendCfg(n_rays, n_samples, V, H, W, 0)
+    L.check(lib.nudf_blend_forward(ctypes.byref(cfg), L.ptr(pts), L.ptr(proj), None, None, L.ptr(imgs), L.ptr(logits),
+                                   logits.stride(0), L.ptr(c_pix), None, None, L.stream_ptr()), "nudf_blend_forward")
+
+
+def ray_points_into(rays_o, rays_d, z_vals, sample_dist, pts, mid, dists):
+    N, S = z_vals.shape
+    L.check(L.lib().nudf_ray_points(L.ptr(rays_o), L.ptr(rays_d), L.ptr(z_vals), N, S, float(sample_dist), L.ptr(pts),
+                                    L.ptr(mid), L.ptr(dists), L.stream_ptr()), "nudf_ray_points")
+
+
+def outside_points_into(rays_o, rays_d, z, col0, sample_dist, pts4, dists):
+    N, n = z.shape
+    L.check(L.lib().nudf_outside_points(L.ptr(rays_o), L.ptr(rays_d), L.ptr(z), N, n, col0, float(sample_dist), L.ptr(pts4),
+                                        L.ptr(dists), L.stream_ptr()), "nudf_outside_points")
