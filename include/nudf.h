@@ -364,6 +364,26 @@ int nudf_mc_vertices(const float* df, int32_t n0, int32_t n1, int32_t n2, const 
                      const uint8_t* mask, const int64_t* keys, int64_t n_keys, float* verts, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * Threshold marching cubes (replaces PyMCubes' marching_cubes in the runner's validate_mesh; neuraludf_b200/mesh.py's
+ * iso_marching_cubes_index drives the stages).  The MeshUDF construction above on the corner values v = fl32(f - level)
+ * (corner positive when v > 0), with no pseudo-signs and no polarity; the lattice is read in place, never shifted.
+ * df: DEVICE fp32 lattice [n0, n1, n2]; level must be finite.  Faces are wound so that their normals (right-hand rule)
+ * point from the > level side into the <= level side.  All buffers are caller-provided; nothing is allocated.
+ * ------------------------------------------------------------------------------------------------------------ */
+/* flags[g] (g < n0 * n1 * n2) = 1 when the cell with lower corner g has a corner with v > 0, one with v <= 0 and none NaN */
+int nudf_iso_active(const float* df, int32_t n0, int32_t n1, int32_t n2, float level, uint8_t* flags, void* stream);
+/* triangles per cell (<= 12), as nudf_mc_count */
+int nudf_iso_count(const float* df, int32_t n0, int32_t n1, int32_t n2, float level, const int64_t* cells, int64_t n_cells,
+                   int32_t* counts, void* stream);
+/* vertex keys of the triangles, as nudf_mc_emit: 3 * corner + axis, then 3 * n0 * n1 * n2 + 4 * t + l for loop centres */
+int nudf_iso_emit(const float* df, int32_t n0, int32_t n1, int32_t n2, float level, const int64_t* cells, int64_t n_cells,
+                  const int64_t* offsets, int64_t* keys, void* stream);
+/* verts[n_keys, 3] fp64 lattice-index coordinates: edge points at t = v_a / (v_a - v_b) from the lower corner (fp64 from the
+ * fp32 v, no contraction), loop centres at the mean of their loop's edge points summed in loop order */
+int nudf_iso_vertices(const float* df, int32_t n0, int32_t n1, int32_t n2, float level, const int64_t* cells, int64_t n_cells,
+                      const int64_t* keys, int64_t n_keys, double* verts, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------
  * Point-cloud evaluation (the DTU / DeepFashion3D Chamfer protocols; neuraludf_b200/evaluate.py drives the stages)
  * ------------------------------------------------------------------------------------------------------------
  * Points are DEVICE fp64 [n, 3]; all buffers are caller-provided, nothing is allocated.  Host arrays are marked HOST. */

@@ -179,6 +179,13 @@ _SIGNATURES = {
     "nudf_mc_emit": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [c_void_p, ctypes.c_int64] + [c_void_p] * 4),
     "nudf_mc_vertices": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [c_void_p, ctypes.c_int64, c_void_p, c_void_p,
                                                                             ctypes.c_int64, c_void_p, c_void_p]),
+    "nudf_iso_active": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [ctypes.c_float, c_void_p, c_void_p]),
+    "nudf_iso_count": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [ctypes.c_float, c_void_p, ctypes.c_int64, c_void_p,
+                                                                          c_void_p]),
+    "nudf_iso_emit": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [ctypes.c_float, c_void_p, ctypes.c_int64]
+                      + [c_void_p] * 3),
+    "nudf_iso_vertices": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [ctypes.c_float, c_void_p, ctypes.c_int64,
+                                                                             c_void_p, ctypes.c_int64, c_void_p, c_void_p]),
     "nudf_pc_sample_count": (ctypes.c_int, [c_void_p, ctypes.c_int64, c_void_p, ctypes.c_int64, ctypes.c_double, c_void_p,
                                             c_void_p]),
     "nudf_pc_sample_emit": (ctypes.c_int, [c_void_p, ctypes.c_int64, c_void_p, ctypes.c_int64, ctypes.c_double, c_void_p,

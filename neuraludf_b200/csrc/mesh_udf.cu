@@ -20,6 +20,8 @@
 // candidates and normals, a lattice whose values equal the dense ones wherever those are <= max_t and are > max_t elsewhere
 // (+inf included: max <= max_t fails) meshes exactly like the dense one -- what grid.udf_band's narrow band relies on.
 // tests/proto/udf_mc.py restates every stage in NumPy with the same float32 operation order.
+// Threshold meshing (nudf_iso_*) runs stages 4-5 on v = fl32(f - level) instead of the pseudo-signed udf (the corner rules
+// UdfCorners / IsoCorners), with its own active-cell test and fp64 vertices; tests/proto/iso_mc.py restates it.
 #include <algorithm>
 
 #include "../../include/nudf.h"
@@ -193,16 +195,39 @@ __global__ void k_uf_final(const int64_t* __restrict__ par, const uint8_t* __res
   }
 }
 
-// the crossing loops of one cell: local edge ids concatenated in loop[], lengths in len[]; returns the loop count (<= 4)
-__device__ int cell_loops(const float* __restrict__ df, const Dims& D, int64_t g, int m, int8_t loop[12], int8_t len[4]) {
-  float v[8];
+// Corner-value rules of the shared triangulation (cell_loops, loop_triangles): rule(D, t, g, v) writes the values v[8] of
+// cell g = cells[t]; corner c is positive when v[c] > 0.  Faces are wound towards v > 0, or with kDescent towards v <= 0.
+struct UdfCorners {             // MeshUDF: the udf with the cell's pseudo-sign
+  const float* __restrict__ df;
+  const uint8_t* __restrict__ mask;
+  static constexpr bool kDescent = false;
+  __device__ __forceinline__ void operator()(const Dims& D, int64_t t, int64_t g, float v[8]) const {
+    const int m = mask[t];
+#pragma unroll
+    for (int c = 0; c < 8; ++c) {
+      const float u = df[g + D.coff(c)];
+      v[c] = ((m >> c) & 1) ? -u : u;
+    }
+  }
+};
+
+struct IsoCorners {             // threshold meshing: v = fl32(f - level), faces wound from the > level side into the <= level side
+  const float* __restrict__ df;
+  float level;
+  static constexpr bool kDescent = true;
+  __device__ __forceinline__ void operator()(const Dims& D, int64_t, int64_t g, float v[8]) const {
+#pragma unroll
+    for (int c = 0; c < 8; ++c) v[c] = __fsub_rn(df[g + D.coff(c)], level);
+  }
+};
+
+// the crossing loops of one cell with corner values v: local edge ids concatenated in loop[], lengths in len[]; returns the
+// loop count (<= 4)
+__device__ int cell_loops(const float v[8], int8_t loop[12], int8_t len[4]) {
   int p = 0;
 #pragma unroll
-  for (int c = 0; c < 8; ++c) {
-    const float u = df[g + D.coff(c)];
-    v[c] = ((m >> c) & 1) ? -u : u;
+  for (int c = 0; c < 8; ++c)
     if (v[c] > 0.f) p |= 1 << c;
-  }
   if (p == 0 || p == 0xFF) return 0;
   int8_t nxt[12];
 #pragma unroll
@@ -266,12 +291,12 @@ __device__ __forceinline__ bool canonical_loop(const int8_t* __restrict__ l, int
 // chords is chosen by a dynamic programme over the polygon (cost[i][j] of loop[i..j], ties -> smallest apex k), emitted
 // in pre-order.  When every triangulation needs one (reachable: some loops of 7+ edges through ambiguous faces), the
 // loop is fanned around its own centre vertex instead, whose spokes no other cell shares.  Triangles are written in
-// reversed loop order; returns the count (n - 2, or n with the centre).  The programme runs on the loop in canonical
-// order (canonical_loop) and the winding is flipped back, so a global sign flip (which reverses every loop) gives the
-// same triangles with the opposite winding.
-__device__ int loop_triangles(const int8_t* __restrict__ lin, int n, int li, int8_t (*tri)[3]) {
+// reversed loop order (loop order with `descent`); returns the count (n - 2, or n with the centre).  The programme runs
+// on the loop in canonical order (canonical_loop) and the winding is flipped back, so a global sign flip (which reverses
+// every loop) gives the same triangles with the opposite winding.
+__device__ int loop_triangles(const int8_t* __restrict__ lin, int n, int li, int8_t (*tri)[3], bool descent) {
   int8_t l[12];
-  const bool rev = canonical_loop(lin, n, l);
+  const bool rev = canonical_loop(lin, n, l) != descent;
   const int a = rev ? 2 : 1, b = rev ? 1 : 2;     // winding slots
   int fm[12];
   int8_t cost[12][12], apex[12][12];
@@ -313,34 +338,38 @@ __device__ int loop_triangles(const int8_t* __restrict__ lin, int n, int li, int
   return nt;
 }
 
-// triangles of one cell (<= 12); entries are local edge ids or kCentre + loop
-__device__ int cell_triangles(const float* __restrict__ df, const Dims& D, int64_t g, int m, int8_t tri[12][3]) {
+// triangles of one cell (<= 12) under the corner rule cv; entries are local edge ids or kCentre + loop
+template <class C>
+__device__ int cell_triangles(const C& cv, const Dims& D, int64_t t, int64_t g, int8_t tri[12][3]) {
+  float v[8];
+  cv(D, t, g, v);
   int8_t loop[12], len[4];
-  const int nl = cell_loops(df, D, g, m, loop, len);
+  const int nl = cell_loops(v, loop, len);
   int nt = 0, off = 0;
   for (int li = 0; li < nl; ++li) {
-    nt += loop_triangles(loop + off, len[li], li, tri + nt);
+    nt += loop_triangles(loop + off, len[li], li, tri + nt, C::kDescent);
     off += len[li];
   }
   return nt;
 }
 
-__global__ void k_count(const float* __restrict__ df, Dims D, const int64_t* __restrict__ cells, int64_t n,
-                        const uint8_t* __restrict__ mask, int32_t* __restrict__ counts) {
+template <class C>
+__global__ void k_count(C cv, Dims D, const int64_t* __restrict__ cells, int64_t n, int32_t* __restrict__ counts) {
   for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < n; t += (int64_t)gridDim.x * blockDim.x) {
     int8_t tri[12][3];
-    counts[t] = cell_triangles(df, D, cells[t], mask[t], tri);
+    counts[t] = cell_triangles(cv, D, t, cells[t], tri);
   }
 }
 
 // vertex keys: 3 * corner + axis for a lattice-edge point; 3 * n_points + 4 * t + l for the centre of loop l of cells[t]
-__global__ void k_emit(const float* __restrict__ df, Dims D, const int64_t* __restrict__ cells, int64_t n,
-                       const uint8_t* __restrict__ mask, const int64_t* __restrict__ offsets, int64_t* __restrict__ keys) {
+template <class C>
+__global__ void k_emit(C cv, Dims D, const int64_t* __restrict__ cells, int64_t n, const int64_t* __restrict__ offsets,
+                       int64_t* __restrict__ keys) {
   const int64_t centre0 = 3 * D.n0 * D.n1 * D.n2;
   for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < n; t += (int64_t)gridDim.x * blockDim.x) {
     int8_t tri[12][3];
     const int64_t g = cells[t];
-    const int nt = cell_triangles(df, D, g, mask[t], tri);
+    const int nt = cell_triangles(cv, D, t, g, tri);
     int64_t* out = keys + 3 * offsets[t];
     for (int i = 0; i < nt; ++i)
       for (int k = 0; k < 3; ++k) {
@@ -348,6 +377,19 @@ __global__ void k_emit(const float* __restrict__ df, Dims D, const int64_t* __re
         out[3 * i + k] = e >= kCentre ? centre0 + 4 * t + (e - kCentre) : 3 * (g + D.coff(edge_lo(e))) + (e >> 2);
       }
   }
+}
+
+// the loop li of cells[c] in canonical order (the order its centre vertex sums its edge points in); returns its length
+template <class C>
+__device__ int centre_loop(const C& cv, const Dims& D, int64_t c, int64_t g, int li, int8_t cl[12]) {
+  float v[8];
+  cv(D, c, g, v);
+  int8_t loop[12], len[4];
+  cell_loops(v, loop, len);
+  int off = 0;
+  for (int i = 0; i < li; ++i) off += len[i];
+  canonical_loop(loop + off, len[li], cl);
+  return len[li];
 }
 
 // lattice-index coordinates of the point on the edge (lower corner gk, axis ax): t = u_a / (u_a + u_b)
@@ -371,20 +413,70 @@ __global__ void k_vertices(const float* __restrict__ df, Dims D, const int64_t* 
       edge_point(df, D, key / 3, (int)(key % 3), x);
     } else {                   // centre of a loop: the mean of its edge points, summed in canonical loop order
       const int64_t c = (key - centre0) >> 2, g = cells[c];
-      const int li = (int)((key - centre0) & 3);
-      int8_t loop[12], len[4];
-      cell_loops(df, D, g, mask[c], loop, len);
-      int off = 0;
-      for (int i = 0; i < li; ++i) off += len[i];
       int8_t cl[12];
-      canonical_loop(loop + off, len[li], cl);
+      const int len = centre_loop(UdfCorners{df, mask}, D, c, g, (int)((key - centre0) & 3), cl);
       float s[3] = {0.f, 0.f, 0.f}, y[3];
-      for (int i = 0; i < len[li]; ++i) {
+      for (int i = 0; i < len; ++i) {
         const int e = cl[i];
         edge_point(df, D, g + D.coff(edge_lo(e)), e >> 2, y);
         for (int k = 0; k < 3; ++k) s[k] = __fadd_rn(s[k], y[k]);
       }
-      for (int k = 0; k < 3; ++k) x[k] = __fdiv_rn(s[k], (float)len[li]);
+      for (int k = 0; k < 3; ++k) x[k] = __fdiv_rn(s[k], (float)len);
+    }
+    for (int k = 0; k < 3; ++k) verts[t * 3 + k] = x[k];
+  }
+}
+
+// Threshold meshing of f at `level` (nudf_iso_*): the construction above on v = fl32(f - level), with no pseudo-signs and
+// no polarity.  A cell is active when its corners take both sides (some v > 0, some v <= 0) and none is NaN.
+__global__ void k_iso_active(const float* __restrict__ df, Dims D, float level, int64_t n, uint8_t* __restrict__ flag) {
+  for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < n; t += (int64_t)gridDim.x * blockDim.x) {
+    uint8_t on = 0;
+    if (D.is_cell(t)) {
+      bool pos = false, neg = false, nan = false;
+#pragma unroll
+      for (int c = 0; c < 8; ++c) {
+        const float v = __fsub_rn(df[t + D.coff(c)], level);
+        pos |= v > 0.f;
+        neg |= v <= 0.f;
+        nan |= v != v;
+      }
+      on = pos && neg && !nan;
+    }
+    flag[t] = on;
+  }
+}
+
+// fp64 lattice-index coordinates of the point on the edge (lower corner gk, axis ax): t = v_a / (v_a - v_b) of the fp32 v
+__device__ __forceinline__ void iso_edge_point(const float* __restrict__ df, const Dims& D, float level, int64_t gk, int ax,
+                                               double x[3]) {
+  const double va = __fsub_rn(df[gk], level), vb = __fsub_rn(df[gk + D.stride(ax)], level);
+  const double tt = __ddiv_rn(va, __dsub_rn(va, vb));
+  for (int k = 0; k < 3; ++k) {
+    const double c = (double)D.coord(gk, k);
+    x[k] = k == ax ? __dadd_rn(c, tt) : c;
+  }
+}
+
+__global__ void k_iso_vertices(const float* __restrict__ df, Dims D, float level, const int64_t* __restrict__ cells,
+                               const int64_t* __restrict__ keys, int64_t n, double* __restrict__ verts) {
+  const int64_t centre0 = 3 * D.n0 * D.n1 * D.n2;
+  for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < n; t += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t key = keys[t];
+    double x[3];
+    if (key < centre0) {
+      iso_edge_point(df, D, level, key / 3, (int)(key % 3), x);
+    } else {                   // centre of a loop: the mean of its edge points, summed in canonical loop order
+      const int64_t c = (key - centre0) >> 2, g = cells[c];
+      int8_t cl[12];
+      const int len = centre_loop(IsoCorners{df, level}, D, c, g, (int)((key - centre0) & 3), cl);
+      double s[3] = {0.0, 0.0, 0.0}, y[3];
+      for (int i = 0; i < len; ++i) {
+        const int e = cl[i];
+        iso_edge_point(df, D, level, g + D.coff(edge_lo(e)), e >> 2, y);
+        for (int k = 0; k < 3; ++k) s[k] = __dadd_rn(s[k], y[k]);
+      }
+      for (int k = 0; k < 3; ++k) x[k] = __ddiv_rn(s[k], (double)len);
     }
     for (int k = 0; k < 3; ++k) verts[t * 3 + k] = x[k];
   }
@@ -478,7 +570,7 @@ int nudf_mc_count(const float* df, int32_t n0, int32_t n1, int32_t n2, const int
   MC_DIMS_OK();
   NUDF_REQUIRE(df && cells && mask && counts && n_cells >= 0, "null pointer or negative count");
   if (n_cells == 0) return 0;
-  k_count<<<grid_for(n_cells), 128, 0, (cudaStream_t)stream>>>(df, dims(n0, n1, n2), cells, n_cells, mask, counts);
+  k_count<<<grid_for(n_cells), 128, 0, (cudaStream_t)stream>>>(UdfCorners{df, mask}, dims(n0, n1, n2), cells, n_cells, counts);
   NUDF_LAUNCH_OK();
   return 0;
 }
@@ -488,7 +580,8 @@ int nudf_mc_emit(const float* df, int32_t n0, int32_t n1, int32_t n2, const int6
   MC_DIMS_OK();
   NUDF_REQUIRE(df && cells && mask && offsets && keys && n_cells >= 0, "null pointer or negative count");
   if (n_cells == 0) return 0;
-  k_emit<<<grid_for(n_cells), 128, 0, (cudaStream_t)stream>>>(df, dims(n0, n1, n2), cells, n_cells, mask, offsets, keys);
+  k_emit<<<grid_for(n_cells), 128, 0, (cudaStream_t)stream>>>(UdfCorners{df, mask}, dims(n0, n1, n2), cells, n_cells, offsets,
+                                                               keys);
   NUDF_LAUNCH_OK();
   return 0;
 }
@@ -499,6 +592,52 @@ int nudf_mc_vertices(const float* df, int32_t n0, int32_t n1, int32_t n2, const 
   NUDF_REQUIRE(df && cells && mask && keys && verts && n_cells >= 0 && n_keys >= 0, "null pointer or negative count");
   if (n_keys == 0) return 0;
   k_vertices<<<grid_for(n_keys), 128, 0, (cudaStream_t)stream>>>(df, dims(n0, n1, n2), cells, mask, keys, n_keys, verts);
+  NUDF_LAUNCH_OK();
+  return 0;
+}
+
+#define ISO_LEVEL_OK() NUDF_REQUIRE(level == level && level - level == 0.f, "level must be finite")
+
+int nudf_iso_active(const float* df, int32_t n0, int32_t n1, int32_t n2, float level, uint8_t* flags, void* stream) {
+  MC_DIMS_OK();
+  ISO_LEVEL_OK();
+  NUDF_REQUIRE(df && flags, "null pointer");
+  const int64_t n = (int64_t)n0 * n1 * n2;
+  k_iso_active<<<grid_for(n), 256, 0, (cudaStream_t)stream>>>(df, dims(n0, n1, n2), level, n, flags);
+  NUDF_LAUNCH_OK();
+  return 0;
+}
+
+int nudf_iso_count(const float* df, int32_t n0, int32_t n1, int32_t n2, float level, const int64_t* cells, int64_t n_cells,
+                   int32_t* counts, void* stream) {
+  MC_DIMS_OK();
+  ISO_LEVEL_OK();
+  NUDF_REQUIRE(df && cells && counts && n_cells >= 0, "null pointer or negative count");
+  if (n_cells == 0) return 0;
+  k_count<<<grid_for(n_cells), 128, 0, (cudaStream_t)stream>>>(IsoCorners{df, level}, dims(n0, n1, n2), cells, n_cells, counts);
+  NUDF_LAUNCH_OK();
+  return 0;
+}
+
+int nudf_iso_emit(const float* df, int32_t n0, int32_t n1, int32_t n2, float level, const int64_t* cells, int64_t n_cells,
+                  const int64_t* offsets, int64_t* keys, void* stream) {
+  MC_DIMS_OK();
+  ISO_LEVEL_OK();
+  NUDF_REQUIRE(df && cells && offsets && keys && n_cells >= 0, "null pointer or negative count");
+  if (n_cells == 0) return 0;
+  k_emit<<<grid_for(n_cells), 128, 0, (cudaStream_t)stream>>>(IsoCorners{df, level}, dims(n0, n1, n2), cells, n_cells, offsets,
+                                                               keys);
+  NUDF_LAUNCH_OK();
+  return 0;
+}
+
+int nudf_iso_vertices(const float* df, int32_t n0, int32_t n1, int32_t n2, float level, const int64_t* cells, int64_t n_cells,
+                      const int64_t* keys, int64_t n_keys, double* verts, void* stream) {
+  MC_DIMS_OK();
+  ISO_LEVEL_OK();
+  NUDF_REQUIRE(df && cells && keys && verts && n_cells >= 0 && n_keys >= 0, "null pointer or negative count");
+  if (n_keys == 0) return 0;
+  k_iso_vertices<<<grid_for(n_keys), 128, 0, (cudaStream_t)stream>>>(df, dims(n0, n1, n2), level, cells, keys, n_keys, verts);
   NUDF_LAUNCH_OK();
   return 0;
 }

@@ -7,6 +7,8 @@ filter, extract_mesh.py:205-214); `udf_mesh_band` is the same with the lattice e
 for the reference's `custom_mc._marching_cubes_lewiner.udf_mc_lewiner`, served to the unmodified runner by
 `launch.install_shadow_modules` when the reference's Cython build cannot be imported.  The kernels are in
 csrc/mesh_udf.cu (stages and deviations documented there); tests/proto/udf_mc.py is their NumPy restatement.
+`iso_marching_cubes_index` / `iso_marching_cubes` are threshold marching cubes on the same kernels (the runner's
+validate_mesh without PyMCubes; `python -m neuraludf_b200.mesh --threshold T`), restated in tests/proto/iso_mc.py.
 """
 import ctypes
 
@@ -89,6 +91,87 @@ def marching_cubes_index(df, dims, normals, idx=None):
           "nudf_mc_vertices")
     info["vertex_keys"] = ukeys
     return verts, inv.reshape(-1, 3).to(torch.int64), info
+
+
+def _iso_level(level):
+    """the level as the kernels compare it: rounded to fp32 once (the lattice is fp32); non-finite -> ValueError"""
+    lv = float(level)
+    if not np.isfinite(lv) or not np.isfinite(np.float32(lv)):
+        raise ValueError("level must be finite (got %r)" % (level,))
+    return float(np.float32(lv))
+
+
+@torch.no_grad()
+def iso_marching_cubes_index(df, dims, level):
+    """Threshold marching cubes of the fp32 lattice df (shape `dims`, on a CUDA device) at `level`, all on the device:
+    (verts [V,3] fp64 in lattice-index units, column k along array axis k; faces [F,3] int64; info).
+
+    The MeshUDF construction (csrc/mesh_udf.cu) on v = fl32(f - fl32(level)): a cell is active when some corner has v > 0,
+    some v <= 0 and none is NaN; ambiguous faces by the asymptotic decider; each loop triangulated with no chord in a cube
+    face, so every interior edge has exactly two faces.  Edge points sit at t = v_a / (v_a - v_b) (fp64); loop centres at
+    the mean of their loop's edge points.  Vertices are numbered by ascending key (lattice edges 3 * corner + axis, then loop
+    centres).  Faces are wound so that their normals point towards decreasing values (from the > level side into the
+    <= level side: skimage's 'descent').  info: `active` (sorted active cells), `face_keys` [F,3], `vertex_keys`."""
+    L = _lib.lib()
+    st = _lib.stream_ptr()
+    n0, n1, n2 = (int(d) for d in dims)
+    if min(n0, n1, n2) < 2:
+        raise ValueError("lattice dimensions must be at least 2 (got %s)" % ((n0, n1, n2),))
+    level = _iso_level(level)
+    dev = df.device
+    if dev.type != "cuda":
+        raise ValueError("marching cubes runs on a CUDA device (df is on %s)" % dev)
+    df = df.reshape(-1)
+    if df.dtype != torch.float32:
+        raise ValueError("df must be float32 (got %s)" % df.dtype)
+    df = df.contiguous()
+    if df.numel() != n0 * n1 * n2:
+        raise ValueError("df has %d values, dims %s need %d" % (df.numel(), (n0, n1, n2), n0 * n1 * n2))
+    flags = torch.empty(df.numel(), dtype=torch.uint8, device=dev)
+    check(L.nudf_iso_active(ptr(df), n0, n1, n2, level, ptr(flags), st), "nudf_iso_active")
+    cells = torch.nonzero(flags).reshape(-1).contiguous()
+    n = cells.numel()
+    empty = (torch.zeros(0, 3, dtype=torch.float64, device=dev), torch.zeros(0, 3, dtype=torch.int64, device=dev))
+    info = {"active": cells, "face_keys": empty[1], "vertex_keys": torch.zeros(0, dtype=torch.int64, device=dev)}
+    if n == 0:
+        return empty[0], empty[1], info
+    counts = torch.empty(n, dtype=torch.int32, device=dev)
+    check(L.nudf_iso_count(ptr(df), n0, n1, n2, level, ptr(cells), n, ptr(counts), st), "nudf_iso_count")
+    csum = torch.cumsum(counts, 0, dtype=torch.int64)
+    n_faces = int(csum[-1])
+    offsets = (csum - counts).contiguous()
+    keys = torch.empty(3 * n_faces, dtype=torch.int64, device=dev)
+    check(L.nudf_iso_emit(ptr(df), n0, n1, n2, level, ptr(cells), n, ptr(offsets), ptr(keys), st), "nudf_iso_emit")
+    info["face_keys"] = keys.reshape(-1, 3)
+    if n_faces == 0:
+        return empty[0], empty[1], info
+    ukeys, inv = torch.unique(keys, sorted=True, return_inverse=True)
+    ukeys = ukeys.contiguous()
+    verts = torch.empty(ukeys.numel(), 3, dtype=torch.float64, device=dev)
+    check(L.nudf_iso_vertices(ptr(df), n0, n1, n2, level, ptr(cells), n, ptr(ukeys), ukeys.numel(), ptr(verts), st),
+          "nudf_iso_vertices")
+    info["vertex_keys"] = ukeys
+    return verts, inv.reshape(-1, 3).to(torch.int64), info
+
+
+def iso_marching_cubes(volume, isovalue):
+    """Threshold marching cubes with `mcubes.marching_cubes(volume, isovalue)`'s call signature, on the CUDA kernels:
+    NumPy (vertices fp64 [V,3] in array-index units, triangles int64 [F,3]).
+
+    `volume` is meshed as fp32 and `isovalue` is rounded to fp32 once.  A level that nothing crosses gives empty (0, 3)
+    arrays.  A volume that is not 3-D or has a dimension below 2, or a non-finite level, raises ValueError.  Faces are wound
+    towards decreasing values (the convention NeuS-family code relies on when it meshes -sdf at 0).  The vertex numbering
+    and the triangulation of ambiguous cells are this project's (iso_marching_cubes_index), not PyMCubes'."""
+    volume = np.asarray(volume)
+    if volume.ndim != 3:
+        raise ValueError("volume must be a 3-D array (got %d dimensions)" % volume.ndim)
+    if min(volume.shape) < 2:
+        raise ValueError("volume must be at least 2 x 2 x 2 (got %s)" % (volume.shape,))
+    _iso_level(isovalue)
+    dev = torch.device("cuda", torch.cuda.current_device())
+    df = torch.from_numpy(np.ascontiguousarray(volume, np.float32)).to(dev)
+    verts, faces, _ = iso_marching_cubes_index(df, volume.shape, isovalue)
+    return verts.cpu().numpy(), faces.cpu().numpy()
 
 
 def udf_marching_cubes(df, N, idx, normals):
@@ -271,18 +354,40 @@ def udf_network_from_state(sd, scale=1.0):
     return net
 
 
+def threshold_box(cameras=None):
+    """The box and world transform of the runner's validate_mesh: (bbox_min, bbox_max) fp32 [3] as dataset/dataset.py:112-123
+    forms object_bbox_min / max from the cameras file's fp32 scale_mat_0 (both camera roles read the same file in the shipped
+    confs) and its fp64 object scale_mat_0, or +-1.01 without a cameras file; and the fp32 scale_mat_0 (None without)."""
+    bmin = np.array([-1.01, -1.01, -1.01, 1.0])
+    bmax = np.array([1.01, 1.01, 1.01, 1.0])
+    if cameras is None:
+        return bmin[:3].astype(np.float32), bmax[:3].astype(np.float32), None
+    cam = np.load(cameras)
+    sm = cam["scale_mat_0"].astype(np.float32)
+    obj = cam["scale_mat_0"]
+    lo = np.linalg.inv(sm) @ obj @ bmin[:, None]
+    hi = np.linalg.inv(sm) @ obj @ bmax[:, None]
+    return lo[:3, 0].astype(np.float32), hi[:3, 0].astype(np.float32), sm
+
+
 def main(argv=None):
     """python -m neuraludf_b200.mesh: a runner checkpoint's UDF network -> PLY mesh (see INTEGRATION.md)"""
     import argparse
     from neuraludf_b200.evaluate import write_ply_mesh
     ap = argparse.ArgumentParser(prog="python -m neuraludf_b200.mesh",
-                                 description="Mesh the UDF network of a runner checkpoint: the mesh as udf_mesh makes it, or with "
-                                             "--postprocess the mesh the runner's extract_udf_mesh exports.")
+                                 description="Mesh the UDF network of a runner checkpoint: the mesh as udf_mesh makes it, with "
+                                             "--postprocess the mesh the runner's extract_udf_mesh exports, or with --threshold "
+                                             "the mesh the runner's validate_mesh exports.")
     ap.add_argument("--ckpt", required=True, help="checkpoint written by the runner (its udf_network_fine state dict is used)")
     ap.add_argument("--resolution", type=int, default=512, help="lattice points per axis")
-    ap.add_argument("--cameras", default=None, help="cameras_sphere.npz: map the mesh to world space with its scale_mat_0")
-    ap.add_argument("--dist_threshold_ratio", type=float, default=1.0)
-    ap.add_argument("--lipschitz", type=float, default=2.0, help="Lipschitz bound of the band's culling test")
+    ap.add_argument("--cameras", default=None, help="cameras_sphere.npz: map the mesh to world space with its scale_mat_0 "
+                                                    "(with --threshold it also sets the box, as the runner's dataset does)")
+    ap.add_argument("--threshold", type=float, default=None,
+                    help="threshold meshing of the udf at this level on validate_mesh's lattice (the box +-1.01, or the "
+                         "object box of --cameras) instead of the MeshUDF pipeline: the mesh the runner's "
+                         "validate_mesh(world_space=True) exports with --cameras; the runner passes --threshold 0.005")
+    ap.add_argument("--dist_threshold_ratio", type=float, default=None, help="vertex filter in voxels (default 1)")
+    ap.add_argument("--lipschitz", type=float, default=None, help="Lipschitz bound of the band's culling test (default 2)")
     ap.add_argument("--scale", type=float, default=1.0, help="the conf's udf_network.scale")
     ap.add_argument("--dense", action="store_true", help="evaluate the whole lattice (udf_mesh) instead of the narrow band")
     ap.add_argument("--postprocess", action="store_true",
@@ -291,10 +396,27 @@ def main(argv=None):
                          "passes --dist_threshold_ratio 5")
     ap.add_argument("--out", required=True, help="output PLY")
     a = ap.parse_args(argv)
+    if a.threshold is not None:
+        for flag, given in (("--postprocess", a.postprocess), ("--dense", a.dense), ("--lipschitz", a.lipschitz is not None),
+                            ("--dist_threshold_ratio", a.dist_threshold_ratio is not None)):
+            if given:
+                ap.error("--threshold cannot be combined with %s" % flag)
+    a.dist_threshold_ratio = 1.0 if a.dist_threshold_ratio is None else a.dist_threshold_ratio
+    a.lipschitz = 2.0 if a.lipschitz is None else a.lipschitz
     if not torch.cuda.is_available():
         raise SystemExit("meshing runs on a CUDA device")
     ck = torch.load(a.ckpt, map_location="cpu", weights_only=True)
     net = udf_network_from_state(ck["udf_network_fine"] if "udf_network_fine" in ck else ck, a.scale).cuda()
+    if a.threshold is not None:                   # exp_runner_blending.py:746-761, renderer.extract_geometry
+        from neuraludf_b200.models.udf_renderer_blending import extract_geometry
+        bmin, bmax, sm = threshold_box(a.cameras)
+        v, faces = extract_geometry(torch.tensor(bmin, dtype=torch.float32), torch.tensor(bmax, dtype=torch.float32),
+                                    a.resolution, a.threshold, lambda pts: net.udf_values(pts), torch.device("cuda"))
+        if sm is not None:
+            v = v * sm[0, 0] + sm[:3, 3][None]
+        write_ply_mesh(a.out, v, faces)
+        print("%s: %d vertices, %d faces" % (a.out, v.shape[0], faces.shape[0]))
+        return v, np.asarray(faces)
     if a.postprocess:
         verts, faces, _ = udf_mesh_post(net, a.resolution, a.dist_threshold_ratio, dense=a.dense, lipschitz=a.lipschitz)
     elif a.dense:

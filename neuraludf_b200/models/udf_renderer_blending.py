@@ -29,10 +29,9 @@ from .patch_projector import PatchProjector
 GRID_BLOCK = 64     # the reference queries dense grids in 64^3 blocks (:16-49); 262 144 points per kernel chain here
 
 
-def _grid_query(bound_min, bound_max, resolution, query_func, device, channels):
-    """Evaluate query_func on the resolution^3 lattice spanned by the bounds, block by block; returns a float32 numpy
-    array [R, R, R] (channels == 0) or [R, R, R, channels].  The grid is assembled on the device and copied to the host
-    once (the reference copies and synchronises after every block)."""
+def _grid_query_device(bound_min, bound_max, resolution, query_func, device, channels):
+    """Evaluate query_func on the resolution^3 lattice spanned by the bounds, block by block; returns a float32 tensor
+    [R, R, R] (channels == 0) or [R, R, R, channels] on the device."""
     axes = [torch.linspace(float(bound_min[a]), float(bound_max[a]), resolution, device=device) for a in range(3)]
     out = torch.zeros([resolution] * 3 + ([channels] if channels else []), dtype=torch.float32, device=device)
     starts = range(0, resolution, GRID_BLOCK)
@@ -41,7 +40,13 @@ def _grid_query(bound_min, bound_max, resolution, query_func, device, channels):
         pts = torch.cartesian_prod(*blk)                               # x slowest, z fastest (meshgrid 'ij' order)
         shape = [len(b) for b in blk] + ([channels] if channels else [])
         out[i0:i0 + shape[0], j0:j0 + shape[1], k0:k0 + shape[2]] = query_func(pts).detach().reshape(shape).float()
-    return out.cpu().numpy()
+    return out
+
+
+def _grid_query(bound_min, bound_max, resolution, query_func, device, channels):
+    """_grid_query_device as a float32 numpy array: the grid is assembled on the device and copied to the host once (the
+    reference copies and synchronises after every block)."""
+    return _grid_query_device(bound_min, bound_max, resolution, query_func, device, channels).cpu().numpy()
 
 
 def extract_fields(bound_min, bound_max, resolution, query_func, device):
@@ -56,10 +61,22 @@ def extract_gradient_fields(bound_min, bound_max, resolution, query_func, device
 
 
 def extract_geometry(bound_min, bound_max, resolution, threshold, query_func, device):
-    """reference :52-63 (needs PyMCubes, like the reference)."""
-    import mcubes
-    u = extract_fields(bound_min, bound_max, resolution, query_func, device)
-    vertices, triangles = mcubes.marching_cubes(u, threshold)
+    """reference :52-63.  With PyMCubes importable, exactly the reference's path.  Without it, the lattice stays on the
+    device and is meshed there (mesh.iso_marching_cubes_index: fp32 threshold, faces wound towards decreasing values, this
+    project's vertex numbering and ambiguous-cell triangulation); the vertices then take the reference's mapping below."""
+    try:
+        import mcubes
+    except ImportError:
+        mcubes = None
+    if mcubes is not None:
+        u = extract_fields(bound_min, bound_max, resolution, query_func, device)
+        vertices, triangles = mcubes.marching_cubes(u, threshold)
+    else:
+        from ..mesh import iso_marching_cubes_index
+        with torch.no_grad():
+            u = _grid_query_device(bound_min, bound_max, resolution, query_func, device, 0)
+            v, f, _ = iso_marching_cubes_index(u, u.shape, threshold)
+        vertices, triangles = v.cpu().numpy(), f.cpu().numpy()
     b_max_np = bound_max.detach().cpu().numpy()
     b_min_np = bound_min.detach().cpu().numpy()
     vertices = vertices / (resolution - 1.0) * (b_max_np - b_min_np)[None, :] + b_min_np[None, :]
