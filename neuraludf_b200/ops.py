@@ -395,9 +395,10 @@ class NerfHandle:
         return [self.params()]
 
     def images(self):
-        """bf16 hi/lo weight images for the tensor engine, rebuilt when a parameter changed (None on the fp32 engine)."""
+        """bf16 hi/lo weight images for the tensor engine, rebuilt when a parameter changed (None on the fp32 engine, or
+        when neither the NeRF++ backward (chain bit 64) nor the ReLU-network forward (bit 128) runs on the tensor cores)."""
         lib = L.lib()
-        if lib.nudf_get_engine() != 1 or not (lib.nudf_get_tc_mask() & 64):
+        if lib.nudf_get_engine() != 1 or not (lib.nudf_get_tc_mask() & (64 | 128)):
             return None
         ps = self.params()
         key = tuple((p.data_ptr(), p._version) for p in ps)
