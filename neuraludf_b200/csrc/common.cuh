@@ -113,6 +113,11 @@ float* split_workspace(cudaStream_t st);
 
 static inline int64_t cdiv(int64_t a, int64_t b) { return (a + b - 1) / b; }
 static inline int64_t round_up(int64_t a, int64_t b) { return cdiv(a, b) * b; }
+// the ctx / scratch layouts of the networks: offsets in floats, every block starts 16-byte aligned
+struct Bump {
+  int64_t off = 0;
+  int64_t take(int64_t n) { int64_t o = off; off += round_up(n, 4); return o; }
+};
 
 __device__ __forceinline__ bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 

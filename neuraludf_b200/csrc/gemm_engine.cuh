@@ -22,18 +22,20 @@ enum TcChain { TC_FWD = 1, TC_REV = 2, TC_TAN = 4, TC_BWD = 8, TC_WGRAD = 16, TC
 int get_engine();
 int tc_mask();
 static inline bool tc_on(int chain) { return get_engine() == 1 && (tc_mask() & chain) != 0; }
+// the operand shapes B(N, K) the weights-resident tensor-core kernel takes; the planners (dense_layer.cuh) build images of these only
+static inline bool tc_shape_ok(int N, int64_t K) { return K >= 32 && N >= 16; }
 
 template <class Epi>
 static inline int gemm_nt(const float* A, int64_t lda, const float* W, int64_t ldw, int64_t M, int N, int64_t K,
                           const Epi& epi, cudaStream_t st, const uint16_t* img = nullptr, int chain = 0, int planes = 2) {
-  if (img != nullptr && tc_on(chain) && K >= 32 && N >= 16)
+  if (img != nullptr && tc_on(chain) && tc_shape_ok(N, K))
     return planes == 3 ? tc::gemm_w<3>(A, lda, M, N, (int)K, img, epi, st) : tc::gemm_w<2>(A, lda, M, N, (int)K, img, epi, st);
   return gemm_simt<true, true, Epi>(A, lda, W, ldw, M, N, K, epi, st, 1);
 }
 template <class Epi>
 static inline int gemm_nn(const float* A, int64_t lda, const float* W, int64_t ldw, int64_t M, int N, int64_t K,
                           const Epi& epi, cudaStream_t st, const uint16_t* img = nullptr, int chain = 0) {
-  if (img != nullptr && tc_on(chain) && K >= 32 && N >= 16)
+  if (img != nullptr && tc_on(chain) && tc_shape_ok(N, K))
     return tc::gemm_w<2>(A, lda, M, N, (int)K, img, epi, st);
   return gemm_simt<true, false, Epi>(A, lda, W, ldw, M, N, K, epi, st, 1);
 }

@@ -4,7 +4,7 @@
 #include "../../include/nudf.h"
 #include "common.cuh"
 #include "ew_kernels.cuh"
-#include "gemm_engine.cuh"
+#include "dense_layer.cuh"
 
 namespace nudf {
 
@@ -209,8 +209,10 @@ wgrad_small_kernel(const float* __restrict__ dZ, int64_t ldz, const float* __res
   if (blockIdx.x == 0 && threadIdx.x < n_out) part_b[(int64_t)blockIdx.y * n_out + threadIdx.x] = bs;
 }
 
-static int wgrad(const float* dZ, int64_t ldz, const float* X, int64_t ldx, int n_out, int n_in, int64_t P, float* dW,
-                 int64_t ldw, float* db, cudaStream_t st) {
+// dW += dZ^T X, db += column sums of dZ, for the layer's shape (dW has the layer's leading dimension)
+static int wgrad(const DenseLayer& L, const float* dZ, int64_t ldz, const float* X, int64_t ldx, int64_t P, float* dW, float* db,
+                 cudaStream_t st) {
+  const int n_out = L.n_out, n_in = L.n_in;
   if (n_out <= 16 && P > 0) {
     int64_t chunk = 256;
     while (cdiv(P, chunk) * (int64_t)n_out * (n_in + 1) > SPLIT_WS_FLOATS) chunk *= 2;
@@ -221,59 +223,51 @@ static int wgrad(const float* dZ, int64_t ldz, const float* X, int64_t ldx, int 
     dim3 grid((unsigned)cdiv(n_in, 128), (unsigned)chunks);
     wgrad_small_kernel<16><<<grid, 512, 0, st>>>(dZ, ldz, X, ldx, n_out, n_in, P, chunk, ws, part_b);
     NUDF_LAUNCH_OK();
-    if (int rc = splitk_reduce(ws, chunks, n_out, n_in, EpiAtomicAdd{dW, ldw}, st)) return rc;
+    if (int rc = splitk_reduce(ws, chunks, n_out, n_in, EpiAtomicAdd{dW, L.ldw}, st)) return rc;
     return db != nullptr ? vec_reduce(part_b, chunks, n_out, db, st) : 0;
   }
-  EpiAtomicAdd ew{dW, ldw};
+  EpiAtomicAdd ew{dW, L.ldw};
   return gemm_tn(dZ, ldz, X, ldx, n_out, n_in, P, ew, st, TC_WGRAD, db);
 }
 
 // =================================================================================================================
 // colour network
 // =================================================================================================================
+enum { BASE = 0, MAIN = 1 };
 struct ColorPlan {
   int n_lin, F, H, d_out, n_blend, Lv, d_view;
-  int dims_b[NUDF_MAX_LAYERS + 1], dims_m[NUDF_MAX_LAYERS + 1];
-  int64_t wb_off[NUDF_MAX_LAYERS], wm_off[NUDF_MAX_LAYERS], wb_ld[NUDF_MAX_LAYERS], wm_ld[NUDF_MAX_LAYERS], w_total;
-  int64_t bb_off[NUDF_MAX_LAYERS], bm_off[NUDF_MAX_LAYERS], b_total;
-  int64_t ib_nt[NUDF_MAX_LAYERS], ib_nn[NUDF_MAX_LAYERS], im_nt[NUDF_MAX_LAYERS], im_nn[NUDF_MAX_LAYERS], img_total;
+  DenseLayer stack[2][NUDF_MAX_LAYERS];        // [BASE] and [MAIN], n_lin layers each
+  int64_t w_total, b_total, img_total;
   int ld_xb, ld_xm, ld_ym, c_cb, c_hid;
 };
 
-static int color_plan(const nudf_color_desc* d, ColorPlan* p) {
+// wfold (optional): the folded buffer the layers' weights and images are read from
+static int color_plan(const nudf_color_desc* d, ColorPlan* p, const float* wfold = nullptr) {
   NUDF_REQUIRE(d != nullptr, "null desc");
   NUDF_REQUIRE(d->n_lin >= 3 && d->n_lin <= NUDF_MAX_LAYERS, "n_lin out of range");
   p->n_lin = d->n_lin; p->F = d->d_feature; p->H = d->d_hidden; p->d_out = d->d_out; p->n_blend = d->n_blend;
   p->Lv = d->multires_view;
   p->d_view = 3 * (1 + 2 * p->Lv);
   NUDF_REQUIRE(p->d_out >= 1 && p->d_out <= 4, "d_out must be <= 4");
-  p->dims_b[0] = 3 + p->F;
-  p->dims_m[0] = p->d_view + p->d_out + p->H;
-  for (int l = 1; l < p->n_lin; ++l) { p->dims_b[l] = p->H; p->dims_m[l] = p->H; }
-  p->dims_b[p->n_lin] = p->d_out;
-  p->dims_m[p->n_lin] = p->d_out + p->n_blend;
-  int64_t off = 0, boff = 0;
-  for (int l = 0; l < p->n_lin; ++l) {
-    p->wb_ld[l] = round_up(p->dims_b[l], 4);
-    p->wb_off[l] = off; off = round_up(off + (int64_t)p->dims_b[l + 1] * p->wb_ld[l], 4);
-    p->bb_off[l] = boff; boff += p->dims_b[l + 1];
-  }
-  for (int l = 0; l < p->n_lin; ++l) {
-    p->wm_ld[l] = round_up(p->dims_m[l], 4);
-    p->wm_off[l] = off; off = round_up(off + (int64_t)p->dims_m[l + 1] * p->wm_ld[l], 4);
-    p->bm_off[l] = boff; boff += p->dims_m[l + 1];
-  }
+  const float* const* bias[2] = {d->base_b, d->main_b};
+  int64_t off = 0, boff = 0, ioff = 0;
+  for (int s = 0; s < 2; ++s)                  // folded weights and biases: the base stack's layers, then the main stack's
+    for (int l = 0; l < p->n_lin; ++l) {
+      DenseLayer& L = p->stack[s][l];
+      L.n_in = l > 0 ? p->H : (s == BASE ? 3 + p->F : p->d_view + p->d_out + p->H);
+      L.n_out = l < p->n_lin - 1 ? p->H : (s == BASE ? p->d_out : p->d_out + p->n_blend);
+      L.bias = bias[s][l];
+      L.ldw = round_up(L.n_in, 4);
+      L.w_off = off; off = round_up(off + (int64_t)L.n_out * L.ldw, 4);
+      L.b_off = boff; boff += L.n_out;
+      ioff = plan_images(L, 1 << IMG_NT3 | 1 << IMG_NN2, ioff);    // forward images: 3 planes (6 products)
+    }
   p->w_total = off; p->b_total = boff;
-  int64_t ioff = 0;
-  for (int l = 0; l < p->n_lin; ++l) {
-    p->ib_nt[l] = ioff; ioff += tc::image_elems(p->dims_b[l + 1], p->dims_b[l], 3);    // forward images: 3 planes (6 products)
-    p->ib_nn[l] = ioff; ioff += tc::image_elems(p->dims_b[l], p->dims_b[l + 1], 2);
-    p->im_nt[l] = ioff; ioff += tc::image_elems(p->dims_m[l + 1], p->dims_m[l], 3);
-    p->im_nn[l] = ioff; ioff += tc::image_elems(p->dims_m[l], p->dims_m[l + 1], 2);
-  }
   p->img_total = round_up(ioff, 8);
+  bind_layers(p->stack[BASE], p->n_lin, wfold, p->w_total);
+  bind_layers(p->stack[MAIN], p->n_lin, wfold, p->w_total);
   p->ld_xb = (int)round_up(3 + p->F, 4);
-  p->ld_xm = (int)round_up(p->dims_m[0], 4);
+  p->ld_xm = (int)round_up(p->stack[MAIN][0].n_in, 4);
   p->ld_ym = (int)round_up(p->d_out + p->n_blend, 4);
   p->c_cb = p->d_view; p->c_hid = p->d_view + p->d_out;
   return 0;
@@ -281,23 +275,27 @@ static int color_plan(const nudf_color_desc* d, ColorPlan* p) {
 
 struct ColorCtx { int64_t xb, hb[NUDF_MAX_LAYERS], xm, hm[NUDF_MAX_LAYERS], ym, cs, total; };
 static void color_ctx_layout(const ColorPlan& p, int64_t P, ColorCtx* c) {
-  int64_t off = 0;
-  auto take = [&](int64_t n) { int64_t o = off; off += round_up(n, 4); return o; };
-  c->xb = take(P * p.ld_xb);
-  for (int l = 1; l <= p.n_lin - 2; ++l) c->hb[l] = take(P * p.H);   // outputs of base layers 0..n_lin-3
-  c->xm = take(P * p.ld_xm);
-  for (int l = 1; l <= p.n_lin - 1; ++l) c->hm[l] = take(P * p.H);   // outputs of main layers 0..n_lin-2
-  c->ym = take(P * p.ld_ym);
-  c->cs = take(P * 4);
-  c->total = off;
+  Bump b;
+  c->xb = b.take(P * p.ld_xb);
+  for (int l = 1; l <= p.n_lin - 2; ++l) c->hb[l] = b.take(P * p.H);   // outputs of base layers 0..n_lin-3
+  c->xm = b.take(P * p.ld_xm);
+  for (int l = 1; l <= p.n_lin - 1; ++l) c->hm[l] = b.take(P * p.H);   // outputs of main layers 0..n_lin-2
+  c->ym = b.take(P * p.ld_ym);
+  c->cs = b.take(P * 4);
+  c->total = b.off;
 }
 struct ColorScratch { int64_t buf[2], dym, dyb, dcbx, total; };
 static void color_scratch_layout(const ColorPlan& p, int64_t P, ColorScratch* s) {
-  int64_t off = 0;
-  auto take = [&](int64_t n) { int64_t o = off; off += round_up(n, 4); return o; };
-  s->buf[0] = take(P * p.H); s->buf[1] = take(P * p.H);
-  s->dym = take(P * p.ld_ym); s->dyb = take(P * 4); s->dcbx = take(P * 4);
-  s->total = off;
+  Bump b;
+  s->buf[0] = b.take(P * p.H); s->buf[1] = b.take(P * p.H);
+  s->dym = b.take(P * p.ld_ym); s->dyb = b.take(P * 4); s->dcbx = b.take(P * 4);
+  s->total = b.off;
+}
+
+// forward of one colour-network layer: the narrow heads (dense_small_forward_kernel) stream X once, the others are a layer GEMM
+static int color_layer_forward(const DenseLayer& L, const float* X, int64_t ldx, int64_t P, const EpiAct& e, cudaStream_t st) {
+  if (L.n_out <= 16 && L.n_in <= 128) return dense_small_forward(X, ldx, L.W, L.ldw, P, L.n_out, L.n_in, e, st);
+  return layer_nt(L, X, ldx, P, e, TC_RELU_FWD, st);
 }
 
 }  // namespace nudf
@@ -306,8 +304,8 @@ using namespace nudf;
 
 extern "C" {
 
-// One dense layer Y = act(X W^T + b): the primitive every network above is built from, exported for micro-benchmarks
-// (bench.py times the dominant 256x256 layer through it) and for callers that want a single fused layer.
+// One dense layer Y = act(X W^T + b): the primitive every network above is built from, exported for the tests and the
+// micro-benchmarks under tools/ and for callers that want a single fused layer.
 int nudf_dense_forward(const float* X, int64_t ldx, const float* W, int64_t ldw, const float* bias, float* Y, int64_t ldy,
                        int64_t M, int32_t N, int32_t K, int32_t act, void* stream) {
   NUDF_REQUIRE(X && W && Y, "null pointer");
@@ -325,30 +323,21 @@ int64_t nudf_color_folded_floats(const nudf_color_desc* d) {
 
 int nudf_color_fold_weights(const nudf_color_desc* d, float* wfold, void* stream) {
   ColorPlan p;
-  if (int rc = color_plan(d, &p)) return rc;
+  if (int rc = color_plan(d, &p, wfold)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
-  {                                                     // all layers of both stacks: one launch
-    FoldJobs jobs;
-    jobs.n = 0;
-    for (int l = 0; l < p.n_lin; ++l) {
-      jobs.j[jobs.n++] = FoldJob{d->base_g[l], d->base_v[l], nullptr, nullptr, nullptr, wfold + p.wb_off[l], p.dims_b[l + 1], p.dims_b[l], (int)p.wb_ld[l]};
-      jobs.j[jobs.n++] = FoldJob{d->main_g[l], d->main_v[l], nullptr, nullptr, nullptr, wfold + p.wm_off[l], p.dims_m[l + 1], p.dims_m[l], (int)p.wm_ld[l]};
-    }
-    if (int rc = run_fold_jobs(jobs, false, st)) return rc;
-  }
-  if (get_engine() == 1) {
-    uint16_t* img = reinterpret_cast<uint16_t*>(wfold + p.w_total);
-    tc::PrepWJobs pj;
-    pj.n = 0;
-    for (int l = 0; l < p.n_lin; ++l) {
-      pj.j[pj.n++] = tc::PrepWJob{wfold + p.wb_off[l], img + p.ib_nt[l], (int)p.wb_ld[l], p.dims_b[l + 1], p.dims_b[l], 0, 3};
-      pj.j[pj.n++] = tc::PrepWJob{wfold + p.wb_off[l], img + p.ib_nn[l], (int)p.wb_ld[l], p.dims_b[l], p.dims_b[l + 1], 1, 2};
-      pj.j[pj.n++] = tc::PrepWJob{wfold + p.wm_off[l], img + p.im_nt[l], (int)p.wm_ld[l], p.dims_m[l + 1], p.dims_m[l], 0, 3};
-      pj.j[pj.n++] = tc::PrepWJob{wfold + p.wm_off[l], img + p.im_nn[l], (int)p.wm_ld[l], p.dims_m[l], p.dims_m[l + 1], 1, 2};
-    }
-    if (int rc = tc::prep_weights_jobs(pj, st)) return rc;
-  }
-  return 0;
+  const float* const* g[2] = {d->base_g, d->main_g};
+  const float* const* v[2] = {d->base_v, d->main_v};
+  FoldJobs jobs;                                        // all layers of both stacks: one launch
+  jobs.n = 0;
+  for (int s = 0; s < 2; ++s)
+    for (int l = 0; l < p.n_lin; ++l) add_fold_job(jobs, p.stack[s][l], g[s][l], v[s][l], wfold);
+  if (int rc = run_fold_jobs(jobs, false, st)) return rc;
+  if (get_engine() != 1) return 0;
+  tc::PrepWJobs pj;
+  pj.n = 0;
+  for (int s = 0; s < 2; ++s)
+    for (int l = 0; l < p.n_lin; ++l) add_prep_jobs(pj, p.stack[s][l], reinterpret_cast<uint16_t*>(wfold + p.w_total), IMG_ALL);
+  return tc::prep_weights_jobs(pj, st);
 }
 
 int64_t nudf_color_ctx_floats(const nudf_color_desc* d, int64_t P) {
@@ -370,7 +359,7 @@ int nudf_color_forward(const nudf_color_desc* d, const float* wfold, const float
                        int32_t samples_per_ray, const float* feat, int64_t ld_feat, int64_t P, float* color_base,
                        float* color, float* blend, float* ctx, void* stream) {
   ColorPlan p;
-  if (int rc = color_plan(d, &p)) return rc;
+  if (int rc = color_plan(d, &p, wfold)) return rc;
   if (P <= 0) return 0;
   NUDF_REQUIRE(wfold && pts && dirs && feat && ctx, "null pointer");
   NUDF_REQUIRE(ld_feat >= p.F, "ld_feat too small");
@@ -385,20 +374,16 @@ int nudf_color_forward(const nudf_color_desc* d, const float* wfold, const float
   ew_pe_kernel<<<ew_blocks(P, 128), 128, 0, st>>>(dirs, 3, p.Lv, spr, P, xm, p.ld_xm, 0, nullptr, 0, 0);
   NUDF_LAUNCH_OK();
   const int nl = p.n_lin;
-  const uint16_t* cimg = reinterpret_cast<const uint16_t*>(wfold + p.w_total);
   // base stack
   for (int l = 0; l < nl; ++l) {
     const float* X = l == 0 ? xb : (l == nl - 1 ? xm + p.c_hid : ctx + c.hb[l]);
     int64_t ldx = l == 0 ? p.ld_xb : (l == nl - 1 ? p.ld_xm : p.H);
     EpiAct e;
-    e.bias = d->base_b[l]; e.post_scale = 1.0f;
+    e.bias = p.stack[BASE][l].bias; e.post_scale = 1.0f;
     if (l < nl - 2) { e.C = ctx + c.hb[l + 1]; e.ldc = p.H; e.act = ACT_RELU; }
     else if (l == nl - 2) { e.C = xm + p.c_hid; e.ldc = p.ld_xm; e.act = ACT_RELU; }      // x_hidden (fields.py:472-473)
     else { e.C = xm + p.c_cb; e.ldc = p.ld_xm; e.act = ACT_SIGMOID; }                      // color_base (:475-476)
-    if (p.dims_b[l + 1] <= 16 && p.dims_b[l] <= 128) {
-      if (int rc = dense_small_forward(X, ldx, wfold + p.wb_off[l], p.wb_ld[l], P, p.dims_b[l + 1], p.dims_b[l], e, st)) return rc;
-    } else if (int rc = gemm_nt(X, ldx, wfold + p.wb_off[l], p.wb_ld[l], P, p.dims_b[l + 1], p.dims_b[l], e, st,
-                                cimg + p.ib_nt[l], TC_RELU_FWD, 3)) return rc;
+    if (int rc = color_layer_forward(p.stack[BASE][l], X, ldx, P, e, st)) return rc;
   }
   if (color_base) {
     ew_copy_cols_kernel<<<ew_blocks(P * p.d_out, 256), 256, 0, st>>>(xm + p.c_cb, p.ld_xm, color_base, p.d_out, 0, p.d_out, P, 1.f);
@@ -409,13 +394,10 @@ int nudf_color_forward(const nudf_color_desc* d, const float* wfold, const float
     const float* X = l == 0 ? xm : ctx + c.hm[l];
     int64_t ldx = l == 0 ? p.ld_xm : p.H;
     EpiAct e;
-    e.bias = d->main_b[l]; e.post_scale = 1.0f;
+    e.bias = p.stack[MAIN][l].bias; e.post_scale = 1.0f;
     if (l < nl - 1) { e.C = ctx + c.hm[l + 1]; e.ldc = p.H; e.act = ACT_RELU; }
     else { e.C = ctx + c.ym; e.ldc = p.ld_ym; e.act = ACT_NONE; }
-    if (p.dims_m[l + 1] <= 16 && p.dims_m[l] <= 128) {
-      if (int rc = dense_small_forward(X, ldx, wfold + p.wm_off[l], p.wm_ld[l], P, p.dims_m[l + 1], p.dims_m[l], e, st)) return rc;
-    } else if (int rc = gemm_nt(X, ldx, wfold + p.wm_off[l], p.wm_ld[l], P, p.dims_m[l + 1], p.dims_m[l], e, st,
-                                cimg + p.im_nt[l], TC_RELU_FWD, 3)) return rc;
+    if (int rc = color_layer_forward(p.stack[MAIN][l], X, ldx, P, e, st)) return rc;
   }
   color_head_kernel<<<ew_blocks(P * (p.d_out + p.n_blend), 256), 256, 0, st>>>(ctx + c.ym, p.ld_ym, p.d_out, p.n_blend, P,
                                                                               color, ctx + c.cs, 4, blend);
@@ -427,7 +409,7 @@ int nudf_color_backward(const nudf_color_desc* d, const float* wfold, int64_t P,
                         const float* blend_bar, const float* ctx_c, float* scratch, float* dfeat, int64_t ld_df,
                         float* dwfold, float* dbias, void* stream) {
   ColorPlan p;
-  if (int rc = color_plan(d, &p)) return rc;
+  if (int rc = color_plan(d, &p, wfold)) return rc;
   NUDF_REQUIRE(wfold && ctx_c && scratch && dwfold && dbias, "null pointer");
   cudaStream_t st = (cudaStream_t)stream;
   NUDF_CUDA_OK(cudaMemsetAsync(dwfold, 0, sizeof(float) * p.w_total, st));
@@ -439,7 +421,6 @@ int nudf_color_backward(const nudf_color_desc* d, const float* wfold, int64_t P,
   ColorScratch s;
   color_scratch_layout(p, P, &s);
   const int nl = p.n_lin;
-  const uint16_t* cimg = reinterpret_cast<const uint16_t*>(wfold + p.w_total);
   float* xm = ctx + c.xm;
   float* dym = scratch + s.dym;
   sigmoid_head_bwd_kernel<<<ew_blocks(P * p.ld_ym, 256), 256, 0, st>>>(c_bar, p.d_out, nullptr, 0, ctx + c.cs, 4, p.d_out,
@@ -449,19 +430,17 @@ int nudf_color_backward(const nudf_color_desc* d, const float* wfold, int64_t P,
   const float* dz = dym; int64_t ldz = p.ld_ym;
   int flip = 0;
   for (int l = nl - 1; l >= 0; --l) {
+    const DenseLayer& L = p.stack[MAIN][l];
     const float* X = l == 0 ? xm : ctx + c.hm[l];
     int64_t ldx = l == 0 ? p.ld_xm : p.H;
-    if (int rc = wgrad(dz, ldz, X, ldx, p.dims_m[l + 1], p.dims_m[l], P, dwfold + p.wm_off[l], p.wm_ld[l],
-                       dbias + p.bm_off[l], st)) return rc;
+    if (int rc = wgrad(L, dz, ldz, X, ldx, P, dwfold + L.w_off, dbias + L.b_off, st)) return rc;
     float* out = scratch + s.buf[flip];
     if (l >= 1) {
       EpiReluBwd e{0, p.H, ctx + c.hm[l], p.H, out, p.H, 0};
-      if (int rc = gemm_nn(dz, ldz, wfold + p.wm_off[l], p.wm_ld[l], P, p.dims_m[l], p.dims_m[l + 1], e, st,
-                           cimg + p.im_nn[l], TC_COLOR)) return rc;
+      if (int rc = layer_nn(L, dz, ldz, P, e, TC_COLOR, st)) return rc;
     } else {
-      EpiColorMainIn e{p.c_cb, p.c_hid, p.dims_m[0], scratch + s.dcbx, 4, xm + p.c_hid, p.ld_xm, out, p.H};
-      if (int rc = gemm_nn(dz, ldz, wfold + p.wm_off[0], p.wm_ld[0], P, p.dims_m[0], p.dims_m[1], e, st,
-                           cimg + p.im_nn[0], TC_COLOR)) return rc;
+      EpiColorMainIn e{p.c_cb, p.c_hid, L.n_in, scratch + s.dcbx, 4, xm + p.c_hid, p.ld_xm, out, p.H};
+      if (int rc = layer_nn(L, dz, ldz, P, e, TC_COLOR, st)) return rc;
     }
     dz = out; ldz = p.H; flip ^= 1;
   }
@@ -473,28 +452,25 @@ int nudf_color_backward(const nudf_color_desc* d, const float* wfold, int64_t P,
   NUDF_LAUNCH_OK();
   // ---- base stack ----
   {
-    const int l = nl - 1;
-    if (int rc = wgrad(dyb, 4, xm + p.c_hid, p.ld_xm, p.dims_b[l + 1], p.dims_b[l], P, dwfold + p.wb_off[l], p.wb_ld[l],
-                       dbias + p.bb_off[l], st)) return rc;
+    const DenseLayer& L = p.stack[BASE][nl - 1];       // colour_base head: K = d_out <= 4, no image, the FFMA kernel
+    if (int rc = wgrad(L, dyb, 4, xm + p.c_hid, p.ld_xm, P, dwfold + L.w_off, dbias + L.b_off, st)) return rc;
     EpiReluBwd e{0, p.H, xm + p.c_hid, p.ld_xm, dzb, p.H, 1};
-    if (int rc = gemm_nn(dyb, 4, wfold + p.wb_off[l], p.wb_ld[l], P, p.dims_b[l], p.dims_b[l + 1], e, st)) return rc;
+    if (int rc = layer_nn(L, dyb, 4, P, e, TC_COLOR, st)) return rc;
   }
   dz = dzb; ldz = p.H;
   for (int l = nl - 2; l >= 0; --l) {
+    const DenseLayer& L = p.stack[BASE][l];
     const float* X = l == 0 ? ctx + c.xb : ctx + c.hb[l];
     int64_t ldx = l == 0 ? p.ld_xb : p.H;
-    if (int rc = wgrad(dz, ldz, X, ldx, p.dims_b[l + 1], p.dims_b[l], P, dwfold + p.wb_off[l], p.wb_ld[l],
-                       dbias + p.bb_off[l], st)) return rc;
+    if (int rc = wgrad(L, dz, ldz, X, ldx, P, dwfold + L.w_off, dbias + L.b_off, st)) return rc;
     if (l >= 1) {
       float* out = scratch + s.buf[flip];
       EpiReluBwd e{0, p.H, ctx + c.hb[l], p.H, out, p.H, 0};
-      if (int rc = gemm_nn(dz, ldz, wfold + p.wb_off[l], p.wb_ld[l], P, p.dims_b[l], p.dims_b[l + 1], e, st,
-                           cimg + p.ib_nn[l], TC_COLOR)) return rc;
+      if (int rc = layer_nn(L, dz, ldz, P, e, TC_COLOR, st)) return rc;
       dz = out; flip ^= 1;
     } else if (dfeat) {
       EpiReluBwd e{3, 3 + p.F, nullptr, 0, dfeat, ld_df, 0};
-      if (int rc = gemm_nn(dz, ldz, wfold + p.wb_off[0], p.wb_ld[0], P, p.dims_b[0], p.dims_b[1], e, st,
-                           cimg + p.ib_nn[0], TC_COLOR)) return rc;
+      if (int rc = layer_nn(L, dz, ldz, P, e, TC_COLOR, st)) return rc;
     }
   }
   return 0;
@@ -505,12 +481,14 @@ int nudf_color_unfold_grads(const nudf_color_desc* d, const float* dwfold, float
   ColorPlan p;
   if (int rc = color_plan(d, &p)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
+  const float* const* g[2] = {d->base_g, d->main_g};
+  const float* const* v[2] = {d->base_v, d->main_v};
+  float* const* dg[2] = {dg_base, dg_main};
+  float* const* dv[2] = {dv_base, dv_main};
   FoldJobs jobs;
   jobs.n = 0;
-  for (int l = 0; l < p.n_lin; ++l) {
-    jobs.j[jobs.n++] = FoldJob{d->base_g[l], d->base_v[l], dwfold + p.wb_off[l], dg_base[l], dv_base[l], nullptr, p.dims_b[l + 1], p.dims_b[l], (int)p.wb_ld[l]};
-    jobs.j[jobs.n++] = FoldJob{d->main_g[l], d->main_v[l], dwfold + p.wm_off[l], dg_main[l], dv_main[l], nullptr, p.dims_m[l + 1], p.dims_m[l], (int)p.wm_ld[l]};
-  }
+  for (int s = 0; s < 2; ++s)
+    for (int l = 0; l < p.n_lin; ++l) add_unfold_job(jobs, p.stack[s][l], g[s][l], v[s][l], dwfold, dg[s][l], dv[s][l]);
   return run_fold_jobs(jobs, true, st);
 }
 
@@ -520,13 +498,15 @@ int nudf_color_unfold_grads(const nudf_color_desc* d, const float* dwfold, float
 }  // extern "C"
 
 namespace nudf {
+enum { VIEWS = 0, FEATURE = 1, ALPHA = 2, RGB = 3 };
 struct NerfPlan {
   int D, W, d_in, L, Lv, skip, ch, chv, ld_f, ld_x5;
-  int in_dim[NUDF_MAX_LAYERS];
-  // tensor-engine weight images (uint16 offsets): per pts layer X W^T and dY W operands, feature layer, views layer
-  int64_t ipts_nt[NUDF_MAX_LAYERS], ipts_nn[NUDF_MAX_LAYERS], ifeat_nt, ifeat_nn, iviews_nt, iviews_nn, img_total;
+  // the D pts layers, then [D + VIEWS .. D + RGB]: the order of nudf_nerf_backward's dparams (weight, bias) pairs
+  DenseLayer layer[NUDF_MAX_LAYERS + 4];
+  int64_t img_total;
 };
-static int nerf_plan(const nudf_nerf_desc* d, NerfPlan* p) {
+// wimg (optional): the image block of nudf_nerf_prepare; null = exact-fp32 engine
+static int nerf_plan(const nudf_nerf_desc* d, NerfPlan* p, const float* wimg = nullptr) {
   NUDF_REQUIRE(d != nullptr, "null desc");
   NUDF_REQUIRE(d->D >= 2 && d->D <= NUDF_MAX_LAYERS, "D out of range");
   p->D = d->D; p->W = d->W; p->d_in = d->d_in; p->L = d->multires; p->Lv = d->multires_view; p->skip = d->skip;
@@ -534,39 +514,44 @@ static int nerf_plan(const nudf_nerf_desc* d, NerfPlan* p) {
   NUDF_REQUIRE(p->d_in >= 1 && p->d_in <= 4, "d_in out of range");
   p->ch = p->d_in * (1 + 2 * p->L);
   p->chv = 3 * (1 + 2 * p->Lv);
-  for (int i = 0; i < p->D; ++i) p->in_dim[i] = i == 0 ? p->ch : (i - 1 == p->skip ? p->W + p->ch : p->W);
   p->ld_f = (int)round_up(p->W + p->chv, 4);
   p->ld_x5 = (int)round_up(p->W + p->ch, 4);
   int64_t io = 0;
-  for (int i = 0; i < p->D; ++i) {
-    p->ipts_nt[i] = io; io += tc::image_elems(p->W, p->in_dim[i], 3);    // forward images: 3 planes (6 products)
-    p->ipts_nn[i] = io; io += tc::image_elems(p->in_dim[i], p->W, 2);
-  }
-  p->ifeat_nt = io; io += tc::image_elems(p->W, p->W, 3);
-  p->ifeat_nn = io; io += tc::image_elems(p->W, p->W, 2);
-  p->iviews_nt = io; io += tc::image_elems(p->W / 2, p->W + p->chv, 3);
-  p->iviews_nn = io; io += tc::image_elems(p->W + p->chv, p->W / 2, 2);
+  auto set = [&](int i, const float* W, const float* b, int n_out, int n_in, int want) {
+    DenseLayer& L = p->layer[i];
+    L.W = W; L.bias = b; L.n_out = n_out; L.n_in = n_in;
+    L.ldw = n_in; L.w_off = L.b_off = 0;                    // plain nn.Linear parameters, read in place
+    L.img = reinterpret_cast<const uint16_t*>(wimg);
+    io = plan_images(L, want, io);
+  };
+  // forward images with 3 planes (6 products); the backward pass ends at the first layer's weight gradient: no dY W image there.
+  // The alpha and rgb heads (1 and 3 outputs) are no tensor-core shape: they own no image and run on the FFMA kernel.
+  const int both = 1 << IMG_NT3 | 1 << IMG_NN2;
+  for (int i = 0; i < p->D; ++i)
+    set(i, d->pts_w[i], d->pts_b[i], p->W, i == 0 ? p->ch : (i - 1 == p->skip ? p->W + p->ch : p->W), i == 0 ? 1 << IMG_NT3 : both);
+  set(p->D + VIEWS, d->views_w, d->views_b, p->W / 2, p->W + p->chv, both);
+  set(p->D + FEATURE, d->feature_w, d->feature_b, p->W, p->W, both);
+  set(p->D + ALPHA, d->alpha_w, d->alpha_b, 1, p->W, both);
+  set(p->D + RGB, d->rgb_w, d->rgb_b, 3, p->W / 2, both);
   p->img_total = round_up(io, 8);
   return 0;
 }
 struct NerfCtx { int64_t e, h[NUDF_MAX_LAYERS], f, hv, total; };
 // h[i] = post-ReLU output of pts layer i; for i == skip it lives inside the concatenated buffer at column ch.
 static void nerf_ctx_layout(const NerfPlan& p, int64_t P, NerfCtx* c) {
-  int64_t off = 0;
-  auto take = [&](int64_t n) { int64_t o = off; off += round_up(n, 4); return o; };
-  c->e = take(P * round_up(p.ch, 4));
-  for (int i = 0; i < p.D; ++i) c->h[i] = take(P * (i == p.skip ? p.ld_x5 : p.W));
-  c->f = take(P * p.ld_f);
-  c->hv = take(P * (p.W / 2));
-  c->total = off;
+  Bump b;
+  c->e = b.take(P * round_up(p.ch, 4));
+  for (int i = 0; i < p.D; ++i) c->h[i] = b.take(P * (i == p.skip ? p.ld_x5 : p.W));
+  c->f = b.take(P * p.ld_f);
+  c->hv = b.take(P * (p.W / 2));
+  c->total = b.off;
 }
-struct NerfScratch { int64_t buf[2], dzv, dsig, total; };
+struct NerfScratch { int64_t buf[2], dzv, total; };
 static void nerf_scratch_layout(const NerfPlan& p, int64_t P, NerfScratch* s) {
-  int64_t off = 0;
-  auto take = [&](int64_t n) { int64_t o = off; off += round_up(n, 4); return o; };
-  s->buf[0] = take(P * p.W); s->buf[1] = take(P * p.W);
-  s->dzv = take(P * (p.W / 2));
-  s->total = off;
+  Bump b;
+  s->buf[0] = b.take(P * p.W); s->buf[1] = b.take(P * p.W);
+  s->dzv = b.take(P * (p.W / 2));
+  s->total = b.off;
 }
 // layer-i output location
 static inline float* nerf_h(const NerfPlan& p, float* ctx, const NerfCtx& c, int i, int64_t* ld) {
@@ -591,20 +576,12 @@ int64_t nudf_nerf_image_floats(const nudf_nerf_desc* d) {
 
 int nudf_nerf_prepare(const nudf_nerf_desc* d, float* wimg, void* stream) {
   NerfPlan p;
-  if (int rc = nerf_plan(d, &p)) return rc;
+  if (int rc = nerf_plan(d, &p, wimg)) return rc;
   NUDF_REQUIRE(wimg != nullptr, "null wimg");
   cudaStream_t st = (cudaStream_t)stream;
-  uint16_t* img = reinterpret_cast<uint16_t*>(wimg);
-  tc::PrepWJobs pj;                                        // all images in one launch; forward (X W^T) images with 3 planes
+  tc::PrepWJobs pj;                                        // all images in one launch
   pj.n = 0;
-  for (int i = 0; i < p.D; ++i) {
-    pj.j[pj.n++] = tc::PrepWJob{d->pts_w[i], img + p.ipts_nt[i], p.in_dim[i], p.W, p.in_dim[i], 0, 3};
-    pj.j[pj.n++] = tc::PrepWJob{d->pts_w[i], img + p.ipts_nn[i], p.in_dim[i], p.in_dim[i], p.W, 1, 2};
-  }
-  pj.j[pj.n++] = tc::PrepWJob{d->feature_w, img + p.ifeat_nt, p.W, p.W, p.W, 0, 3};
-  pj.j[pj.n++] = tc::PrepWJob{d->feature_w, img + p.ifeat_nn, p.W, p.W, p.W, 1, 2};
-  pj.j[pj.n++] = tc::PrepWJob{d->views_w, img + p.iviews_nt, p.W + p.chv, p.W / 2, p.W + p.chv, 0, 3};
-  pj.j[pj.n++] = tc::PrepWJob{d->views_w, img + p.iviews_nn, p.W + p.chv, p.W + p.chv, p.W / 2, 1, 2};
+  for (int i = 0; i < p.D + 4; ++i) add_prep_jobs(pj, p.layer[i], reinterpret_cast<uint16_t*>(wimg), IMG_ALL);
   return tc::prep_weights_jobs(pj, st);
 }
 
@@ -626,7 +603,7 @@ int64_t nudf_nerf_scratch_floats(const nudf_nerf_desc* d, int64_t P) {
 int nudf_nerf_forward(const nudf_nerf_desc* d, const float* wimg, const float* pts, const float* dirs, int32_t samples_per_ray,
                       int64_t P, float* sigma, float* rgb, float* ctx, void* stream) {
   NerfPlan p;
-  if (int rc = nerf_plan(d, &p)) return rc;
+  if (int rc = nerf_plan(d, &p, wimg)) return rc;
   if (P <= 0) return 0;
   NUDF_REQUIRE(pts && dirs && sigma && rgb && ctx, "null pointer");
   cudaStream_t st = (cudaStream_t)stream;
@@ -634,7 +611,6 @@ int nudf_nerf_forward(const nudf_nerf_desc* d, const float* wimg, const float* p
   NerfCtx c;
   nerf_ctx_layout(p, P, &c);
   const int ld_e = (int)round_up(p.ch, 4);
-  const uint16_t* img = reinterpret_cast<const uint16_t*>(wimg);   // null: exact-fp32 engine
   float* x5 = (p.skip >= 0) ? ctx + c.h[p.skip] : nullptr;
   ew_pe_kernel<<<ew_blocks(P, 128), 128, 0, st>>>(pts, p.d_in, p.L, 1, P, ctx + c.e, ld_e, 0, x5, p.ld_x5, 0);
   NUDF_LAUNCH_OK();
@@ -644,26 +620,27 @@ int nudf_nerf_forward(const nudf_nerf_desc* d, const float* wimg, const float* p
     int64_t ldx, ldh;
     const float* X = nerf_x(p, ctx, c, i, &ldx);
     float* Hh = nerf_h(p, ctx, c, i, &ldh);
-    EpiAct e{Hh, ldh, d->pts_b[i], ACT_RELU, 1.0f};
-    if (int rc = gemm_nt(X, ldx, d->pts_w[i], p.in_dim[i], P, p.W, p.in_dim[i], e, st, img ? img + p.ipts_nt[i] : nullptr, TC_RELU_FWD, 3)) return rc;
+    EpiAct e{Hh, ldh, p.layer[i].bias, ACT_RELU, 1.0f};
+    if (int rc = layer_nt(p.layer[i], X, ldx, P, e, TC_RELU_FWD, st)) return rc;
   }
+  const DenseLayer* head = p.layer + p.D;
   int64_t ldl;
   const float* Hl = nerf_h(p, ctx, c, p.D - 1, &ldl);
   {
-    EpiAct e{sigma, 1, d->alpha_b, ACT_NONE, 1.0f};
-    if (int rc = gemm_nt(Hl, ldl, d->alpha_w, p.W, P, 1, p.W, e, st)) return rc;
+    EpiAct e{sigma, 1, head[ALPHA].bias, ACT_NONE, 1.0f};
+    if (int rc = layer_nt(head[ALPHA], Hl, ldl, P, e, TC_RELU_FWD, st)) return rc;
   }
   {
-    EpiAct e{ctx + c.f, p.ld_f, d->feature_b, ACT_NONE, 1.0f};
-    if (int rc = gemm_nt(Hl, ldl, d->feature_w, p.W, P, p.W, p.W, e, st, img ? img + p.ifeat_nt : nullptr, TC_RELU_FWD, 3)) return rc;
+    EpiAct e{ctx + c.f, p.ld_f, head[FEATURE].bias, ACT_NONE, 1.0f};
+    if (int rc = layer_nt(head[FEATURE], Hl, ldl, P, e, TC_RELU_FWD, st)) return rc;
   }
   {
-    EpiAct e{ctx + c.hv, p.W / 2, d->views_b, ACT_RELU, 1.0f};
-    if (int rc = gemm_nt(ctx + c.f, p.ld_f, d->views_w, p.W + p.chv, P, p.W / 2, p.W + p.chv, e, st, img ? img + p.iviews_nt : nullptr, TC_RELU_FWD, 3)) return rc;
+    EpiAct e{ctx + c.hv, p.W / 2, head[VIEWS].bias, ACT_RELU, 1.0f};
+    if (int rc = layer_nt(head[VIEWS], ctx + c.f, p.ld_f, P, e, TC_RELU_FWD, st)) return rc;
   }
   {
-    EpiAct e{rgb, 3, d->rgb_b, ACT_NONE, 1.0f};
-    if (int rc = gemm_nt(ctx + c.hv, p.W / 2, d->rgb_w, p.W / 2, P, 3, p.W / 2, e, st)) return rc;
+    EpiAct e{rgb, 3, head[RGB].bias, ACT_NONE, 1.0f};
+    if (int rc = layer_nt(head[RGB], ctx + c.hv, p.W / 2, P, e, TC_RELU_FWD, st)) return rc;
   }
   return 0;
 }
@@ -671,72 +648,60 @@ int nudf_nerf_forward(const nudf_nerf_desc* d, const float* wimg, const float* p
 int nudf_nerf_backward(const nudf_nerf_desc* d, const float* wimg, int64_t P, const float* sigma_bar, const float* rgb_bar,
                        const float* ctx_c, float* scratch, float* const* dparams, void* stream) {
   NerfPlan p;
-  if (int rc = nerf_plan(d, &p)) return rc;
+  if (int rc = nerf_plan(d, &p, wimg)) return rc;
   NUDF_REQUIRE(sigma_bar && rgb_bar && ctx_c && scratch && dparams, "null pointer");
   cudaStream_t st = (cudaStream_t)stream;
-  const uint16_t* img = reinterpret_cast<const uint16_t*>(wimg);
   const int D = p.D, W = p.W, W2 = p.W / 2;
-  float* const* dpts = dparams;                 // [2*i], [2*i+1]
-  float* dviews_w = dparams[2 * D + 0]; float* dviews_b = dparams[2 * D + 1];
-  float* dfeat_w = dparams[2 * D + 2];  float* dfeat_b = dparams[2 * D + 3];
-  float* dalpha_w = dparams[2 * D + 4]; float* dalpha_b = dparams[2 * D + 5];
-  float* drgb_w = dparams[2 * D + 6];   float* drgb_b = dparams[2 * D + 7];
-  for (int i = 0; i < D; ++i) {
-    NUDF_CUDA_OK(cudaMemsetAsync(dpts[2 * i], 0, sizeof(float) * W * p.in_dim[i], st));
-    NUDF_CUDA_OK(cudaMemsetAsync(dpts[2 * i + 1], 0, sizeof(float) * W, st));
+  for (int i = 0; i < D + 4; ++i) {                        // dparams[2 i], [2 i + 1] = weight and bias gradient of layer i
+    NUDF_CUDA_OK(cudaMemsetAsync(dparams[2 * i], 0, sizeof(float) * p.layer[i].n_out * p.layer[i].n_in, st));
+    NUDF_CUDA_OK(cudaMemsetAsync(dparams[2 * i + 1], 0, sizeof(float) * p.layer[i].n_out, st));
   }
-  NUDF_CUDA_OK(cudaMemsetAsync(dviews_w, 0, sizeof(float) * W2 * (W + p.chv), st));
-  NUDF_CUDA_OK(cudaMemsetAsync(dviews_b, 0, sizeof(float) * W2, st));
-  NUDF_CUDA_OK(cudaMemsetAsync(dfeat_w, 0, sizeof(float) * W * W, st));
-  NUDF_CUDA_OK(cudaMemsetAsync(dfeat_b, 0, sizeof(float) * W, st));
-  NUDF_CUDA_OK(cudaMemsetAsync(dalpha_w, 0, sizeof(float) * W, st));
-  NUDF_CUDA_OK(cudaMemsetAsync(dalpha_b, 0, sizeof(float) * 1, st));
-  NUDF_CUDA_OK(cudaMemsetAsync(drgb_w, 0, sizeof(float) * 3 * W2, st));
-  NUDF_CUDA_OK(cudaMemsetAsync(drgb_b, 0, sizeof(float) * 3, st));
   if (P <= 0) return 0;
   float* ctx = const_cast<float*>(ctx_c);
   NerfCtx c;
   nerf_ctx_layout(p, P, &c);
   NerfScratch s;
   nerf_scratch_layout(p, P, &s);
+  const DenseLayer* head = p.layer + D;
+  float* const* dhead = dparams + 2 * D;
   // rgb head
-  if (int rc = wgrad(rgb_bar, 3, ctx + c.hv, W2, 3, W2, P, drgb_w, W2, drgb_b, st)) return rc;
+  if (int rc = wgrad(head[RGB], rgb_bar, 3, ctx + c.hv, W2, P, dhead[2 * RGB], dhead[2 * RGB + 1], st)) return rc;
   float* dzv = scratch + s.dzv;
   {
     EpiReluBwd e{0, W2, ctx + c.hv, W2, dzv, W2, 0};
-    if (int rc = gemm_nn(rgb_bar, 3, d->rgb_w, W2, P, W2, 3, e, st)) return rc;
+    if (int rc = layer_nn(head[RGB], rgb_bar, 3, P, e, TC_NERF, st)) return rc;
   }
   // views layer
-  if (int rc = wgrad(dzv, W2, ctx + c.f, p.ld_f, W2, W + p.chv, P, dviews_w, W + p.chv, dviews_b, st)) return rc;
+  if (int rc = wgrad(head[VIEWS], dzv, W2, ctx + c.f, p.ld_f, P, dhead[2 * VIEWS], dhead[2 * VIEWS + 1], st)) return rc;
   float* dfeat = scratch + s.buf[0];
   {
     EpiReluBwd e{0, W, nullptr, 0, dfeat, W, 0};
-    if (int rc = gemm_nn(dzv, W2, d->views_w, W + p.chv, P, W + p.chv, W2, e, st, img ? img + p.iviews_nn : nullptr, TC_NERF)) return rc;
+    if (int rc = layer_nn(head[VIEWS], dzv, W2, P, e, TC_NERF, st)) return rc;
   }
   // feature + alpha heads -> dZ of the last pts layer
   int64_t ldl;
   const float* Hl = nerf_h(p, ctx, c, D - 1, &ldl);
-  if (int rc = wgrad(dfeat, W, Hl, ldl, W, W, P, dfeat_w, W, dfeat_b, st)) return rc;
-  if (int rc = wgrad(sigma_bar, 1, Hl, ldl, 1, W, P, dalpha_w, W, dalpha_b, st)) return rc;
+  if (int rc = wgrad(head[FEATURE], dfeat, W, Hl, ldl, P, dhead[2 * FEATURE], dhead[2 * FEATURE + 1], st)) return rc;
+  if (int rc = wgrad(head[ALPHA], sigma_bar, 1, Hl, ldl, P, dhead[2 * ALPHA], dhead[2 * ALPHA + 1], st)) return rc;
   float* dz = scratch + s.buf[1];
   {
     EpiReluBwd e0{0, W, nullptr, 0, dz, W, 0};
-    if (int rc = gemm_nn(sigma_bar, 1, d->alpha_w, W, P, W, 1, e0, st)) return rc;
+    if (int rc = layer_nn(head[ALPHA], sigma_bar, 1, P, e0, TC_NERF, st)) return rc;
     EpiReluBwd e1{0, W, Hl, ldl, dz, W, 1};
-    if (int rc = gemm_nn(dfeat, W, d->feature_w, W, P, W, W, e1, st, img ? img + p.ifeat_nn : nullptr, TC_NERF)) return rc;
+    if (int rc = layer_nn(head[FEATURE], dfeat, W, P, e1, TC_NERF, st)) return rc;
   }
   int flip = 0;  // dz lives in buf[1]; next output goes to buf[0]
   for (int i = D - 1; i >= 0; --i) {
     int64_t ldx;
     const float* X = nerf_x(p, ctx, c, i, &ldx);
-    if (int rc = wgrad(dz, W, X, ldx, W, p.in_dim[i], P, dpts[2 * i], p.in_dim[i], dpts[2 * i + 1], st)) return rc;
+    if (int rc = wgrad(p.layer[i], dz, W, X, ldx, P, dparams[2 * i], dparams[2 * i + 1], st)) return rc;
     if (i == 0) break;
     float* out = scratch + s.buf[flip];
     int64_t ldh;
     const float* Hprev = nerf_h(p, ctx, c, i - 1, &ldh);
     int col_lo = (i - 1 == p.skip) ? p.ch : 0;
     EpiReluBwd e{col_lo, col_lo + W, Hprev, ldh, out, W, 0};
-    if (int rc = gemm_nn(dz, W, d->pts_w[i], p.in_dim[i], P, p.in_dim[i], W, e, st, img ? img + p.ipts_nn[i] : nullptr, TC_NERF)) return rc;
+    if (int rc = layer_nn(p.layer[i], dz, W, P, e, TC_NERF, st)) return rc;
     dz = out; flip ^= 1;
   }
   return 0;

@@ -5,7 +5,7 @@
 #include "../../include/nudf.h"
 #include "common.cuh"
 #include "ew_kernels.cuh"
-#include "gemm_engine.cuh"
+#include "dense_layer.cuh"
 #include <string.h>
 
 namespace nudf {
@@ -13,18 +13,18 @@ namespace nudf {
 struct UdfPlan {
   int n_lin, d_in, L, d_pe, d_out, skip;
   float scale;
-  int in_dim[NUDF_MAX_LAYERS], out_dim[NUDF_MAX_LAYERS];
-  int64_t w_off[NUDF_MAX_LAYERS], w_ld[NUDF_MAX_LAYERS], w_total;
-  int64_t b_off[NUDF_MAX_LAYERS], b_total;
-  int64_t img_nt[NUDF_MAX_LAYERS], img_nn[NUDF_MAX_LAYERS], img_nn1, img_total;   // uint16 offsets of the bf16 hi/lo weight images
-  int64_t img_fwd[NUDF_MAX_LAYERS], img_feat;   // value chain: 3-plane X W^T images of the hidden layers and of the feature rows
+  // the n_lin layers, then the feature rows 1.. of the last one as an operand of their own: its udf-head row 0 stays an exact-fp32
+  // dot product in the value chain (udf_head_kernel) and a rank-1 update in the backward chain (EpiBwdR1)
+  DenseLayer layer[NUDF_MAX_LAYERS + 1];
+  int64_t w_total, b_total, img_total;   // fp32 folded weights, biases, uint16 elements of the bf16 weight images
   int pe_ld, y_ld;
   int a_ld[NUDF_MAX_LAYERS];    // ld of A[l] (input of layer l), l >= 1
   int o_ld[NUDF_MAX_LAYERS];    // ld of D[l] / Q[l] (out_dim rounded)
   int max_ld;
 };
 
-static int make_plan(const nudf_udf_desc* d, UdfPlan* p) {
+// wfold (optional): the folded buffer the layers' weights and images are read from
+static int make_plan(const nudf_udf_desc* d, UdfPlan* p, const float* wfold = nullptr) {
   NUDF_REQUIRE(d != nullptr, "null desc");
   NUDF_REQUIRE(d->n_lin >= 2 && d->n_lin <= NUDF_MAX_LAYERS, "n_lin out of range");
   NUDF_REQUIRE(d->d_in == 3, "d_in must be 3");
@@ -36,37 +36,38 @@ static int make_plan(const nudf_udf_desc* d, UdfPlan* p) {
   int64_t off = 0, boff = 0;
   p->max_ld = 0;
   for (int l = 0; l < p->n_lin; ++l) {
-    p->in_dim[l] = d->in_dim[l]; p->out_dim[l] = d->out_dim[l];
-    NUDF_REQUIRE(p->in_dim[l] > 0 && p->out_dim[l] > 0, "bad layer dims");
-    p->w_ld[l] = round_up(p->in_dim[l], 4);
-    p->w_off[l] = off; off += (int64_t)p->out_dim[l] * p->w_ld[l];
+    DenseLayer& L = p->layer[l];
+    L.n_in = d->in_dim[l]; L.n_out = d->out_dim[l]; L.bias = d->bias[l];
+    NUDF_REQUIRE(L.n_in > 0 && L.n_out > 0, "bad layer dims");
+    L.ldw = round_up(L.n_in, 4);
+    L.w_off = off; off += (int64_t)L.n_out * L.ldw;
     off = round_up(off, 4);
-    p->b_off[l] = boff; boff += p->out_dim[l];
-    p->a_ld[l] = (int)round_up(p->in_dim[l], 8);        // the fused chains move 8-column octets: whole octets stay inside a tensor
-    p->o_ld[l] = (int)round_up(p->out_dim[l], 8);
+    L.b_off = boff; boff += L.n_out;
+    p->a_ld[l] = (int)round_up(L.n_in, 8);        // the fused chains move 8-column octets: whole octets stay inside a tensor
+    p->o_ld[l] = (int)round_up(L.n_out, 8);
     if (p->a_ld[l] > p->max_ld) p->max_ld = p->a_ld[l];
     if (p->o_ld[l] > p->max_ld) p->max_ld = p->o_ld[l];
   }
   p->w_total = off; p->b_total = boff;
+  const int last = p->n_lin - 1;
+  DenseLayer& F = p->layer[p->n_lin];
+  F = p->layer[last];
+  F.n_out = p->d_out - 1; F.w_off += F.ldw; F.b_off += 1;
+  if (F.bias != nullptr) F.bias += 1;
+  // hidden layers: value chain (3 planes), tangent chain, reverse / backward chains.  The tangent chain stops below the last layer,
+  // whose whole-matrix dY W image serves the backward chain when the head is not split off; the feature rows serve the value
+  // chain and the split backward (none when d_out == 1: plan_images drops the empty shape)
   int64_t ioff = 0;
-  for (int l = 0; l < p->n_lin; ++l) {
-    p->img_nt[l] = ioff; ioff += tc::image_elems(p->out_dim[l], p->in_dim[l], 2);   // operand of X W^T  (N = out, K = in)
-    p->img_nn[l] = ioff; ioff += tc::image_elems(p->in_dim[l], p->out_dim[l], 2);   // operand of dY W   (N = in,  K = out)
-  }
-  // feature rows 1.. of the last layer as a (N = in, K = d_out - 1) operand: the udf-head row is applied as a rank-1 update
-  p->img_nn1 = ioff;
-  if (p->d_out > 1) ioff += tc::image_elems(p->in_dim[p->n_lin - 1], p->d_out - 1, 2);
-  // value chain (6 products per MAC): hidden layers, then the feature rows 1.. of the last layer (its udf-head row 0 stays
-  // exact fp32: udf_head_kernel)
-  for (int l = 0; l < p->n_lin - 1; ++l) { p->img_fwd[l] = ioff; ioff += tc::image_elems(p->out_dim[l], p->in_dim[l], 3); }
-  p->img_feat = ioff;
-  if (p->d_out > 1) ioff += tc::image_elems(p->d_out - 1, p->in_dim[p->n_lin - 1], 3);
+  for (int l = 0; l < last; ++l) ioff = plan_images(p->layer[l], 1 << IMG_NT2 | 1 << IMG_NT3 | 1 << IMG_NN2, ioff);
+  ioff = plan_images(p->layer[last], 1 << IMG_NN2, ioff);
+  ioff = plan_images(F, 1 << IMG_NT3 | 1 << IMG_NN2, ioff);
   p->img_total = round_up(ioff, 8);
-  NUDF_REQUIRE(p->in_dim[0] == p->d_pe, "in_dim[0] must equal the positional-encoding width");
-  NUDF_REQUIRE(p->out_dim[p->n_lin - 1] == p->d_out, "last layer width must equal d_out");
+  bind_layers(p->layer, p->n_lin + 1, wfold, p->w_total);
+  NUDF_REQUIRE(p->layer[0].n_in == p->d_pe, "in_dim[0] must equal the positional-encoding width");
+  NUDF_REQUIRE(p->layer[last].n_out == p->d_out, "last layer width must equal d_out");
   for (int l = 1; l < p->n_lin; ++l) {
-    int expect = p->out_dim[l - 1] + (l == p->skip ? p->d_pe : 0);
-    NUDF_REQUIRE(p->in_dim[l] == expect, "layer dims are not chained consistently");
+    int expect = p->layer[l - 1].n_out + (l == p->skip ? p->d_pe : 0);
+    NUDF_REQUIRE(p->layer[l].n_in == expect, "layer dims are not chained consistently");
   }
   p->pe_ld = (int)round_up(p->d_pe, 8);
   p->y_ld = (int)round_up(p->d_out, 8);
@@ -78,31 +79,29 @@ struct UdfCtx {
   int64_t e0, a[NUDF_MAX_LAYERS], y, sgn, d[NUDF_MAX_LAYERS], gpe, ge, total;
 };
 static void ctx_layout(const UdfPlan& p, int64_t P, int with_grad, UdfCtx* c) {
-  int64_t off = 0;
-  auto take = [&](int64_t n) { int64_t o = off; off += round_up(n, 4); return o; };
-  c->e0 = take(P * p.pe_ld);
-  for (int l = 1; l < p.n_lin; ++l) c->a[l] = take(P * p.a_ld[l]);
-  c->y = take(P * p.y_ld);
-  c->sgn = take(P);
+  Bump b;
+  c->e0 = b.take(P * p.pe_ld);
+  for (int l = 1; l < p.n_lin; ++l) c->a[l] = b.take(P * p.a_ld[l]);
+  c->y = b.take(P * p.y_ld);
+  c->sgn = b.take(P);
   if (with_grad) {
-    for (int l = 0; l < p.n_lin - 1; ++l) c->d[l] = take(P * p.o_ld[l]);
-    c->gpe = take(P * p.pe_ld);
-    c->ge = take(P * p.pe_ld);
+    for (int l = 0; l < p.n_lin - 1; ++l) c->d[l] = b.take(P * p.o_ld[l]);
+    c->gpe = b.take(P * p.pe_ld);
+    c->ge = b.take(P * p.pe_ld);
   }
-  c->total = off;
+  c->total = b.off;
 }
 struct UdfScratch {
   int64_t edot, adot[2], q[NUDF_MAX_LAYERS], zlast, total;
 };
 static void scratch_layout(const UdfPlan& p, int64_t P, UdfScratch* s) {
-  int64_t off = 0;
-  auto take = [&](int64_t n) { int64_t o = off; off += round_up(n, 4); return o; };
-  s->edot = take(P * p.pe_ld);
-  s->adot[0] = take(P * p.max_ld);
-  s->adot[1] = take(P * p.max_ld);
-  for (int l = 0; l < p.n_lin - 1; ++l) s->q[l] = take(P * p.o_ld[l]);
-  s->zlast = take(P * p.y_ld);
-  s->total = off;
+  Bump b;
+  s->edot = b.take(P * p.pe_ld);
+  s->adot[0] = b.take(P * p.max_ld);
+  s->adot[1] = b.take(P * p.max_ld);
+  for (int l = 0; l < p.n_lin - 1; ++l) s->q[l] = b.take(P * p.o_ld[l]);
+  s->zlast = b.take(P * p.y_ld);
+  s->total = b.off;
 }
 
 // ---- element-wise kernels ---------------------------------------------------------------------------------------
@@ -303,76 +302,51 @@ static inline unsigned nblk(int64_t n, int t) { return (unsigned)cdiv(n, t); }
 // ---- host orchestration -----------------------------------------------------------------------------------------
 
 static int fold_all(const UdfPlan& p, const nudf_udf_desc* d, float* wfold, cudaStream_t st) {
-  {
-    FoldJobs jobs;
-    jobs.n = p.n_lin;
-    for (int l = 0; l < p.n_lin; ++l)
-      jobs.j[l] = FoldJob{d->weight_g[l], d->weight_v[l], nullptr, nullptr, nullptr, wfold + p.w_off[l], p.out_dim[l], p.in_dim[l], (int)p.w_ld[l]};
-    if (int rc = run_fold_jobs(jobs, false, st)) return rc;
-  }
-  if (get_engine() == 1) {
-    // split-bf16 images of the tensor-core layer kernels (gemm_tc.cuh), all in one launch
-    uint16_t* img = reinterpret_cast<uint16_t*>(wfold + p.w_total);
-    const int last = p.n_lin - 1;
-    const float* wfeat = wfold + p.w_off[last] + p.w_ld[last];    // rows 1.. of the last layer
-    tc::PrepWJobs pj;
-    pj.n = 0;
-    for (int l = 0; l < p.n_lin; ++l) {
-      pj.j[pj.n++] = tc::PrepWJob{wfold + p.w_off[l], img + p.img_nt[l], (int)p.w_ld[l], p.out_dim[l], p.in_dim[l], 0, 2};
-      pj.j[pj.n++] = tc::PrepWJob{wfold + p.w_off[l], img + p.img_nn[l], (int)p.w_ld[l], p.in_dim[l], p.out_dim[l], 1, 2};
-    }
-    if (p.d_out > 1) pj.j[pj.n++] = tc::PrepWJob{wfeat, img + p.img_nn1, (int)p.w_ld[last], p.in_dim[last], p.d_out - 1, 1, 2};
-    if (tc_on(TC_FWD)) {
-      for (int l = 0; l < last; ++l)
-        pj.j[pj.n++] = tc::PrepWJob{wfold + p.w_off[l], img + p.img_fwd[l], (int)p.w_ld[l], p.out_dim[l], p.in_dim[l], 0, 3};
-      if (p.d_out > 1) pj.j[pj.n++] = tc::PrepWJob{wfeat, img + p.img_feat, (int)p.w_ld[last], p.d_out - 1, p.in_dim[last], 0, 3};
-    }
-    if (int rc = tc::prep_weights_jobs(pj, st)) return rc;
-  }
-  return 0;
-}
-
-static inline const uint16_t* img_base(const UdfPlan& p, const float* wfold) {
-  return reinterpret_cast<const uint16_t*>(wfold + p.w_total);
+  FoldJobs jobs;
+  jobs.n = 0;
+  for (int l = 0; l < p.n_lin; ++l) add_fold_job(jobs, p.layer[l], d->weight_g[l], d->weight_v[l], wfold);
+  if (int rc = run_fold_jobs(jobs, false, st)) return rc;
+  if (get_engine() != 1) return 0;
+  // split-bf16 images of the tensor-core layer kernels (gemm_tc.cuh), all in one launch; the 3-plane ones only when the value
+  // chain runs there
+  tc::PrepWJobs pj;
+  pj.n = 0;
+  const int kinds = 1 << IMG_NT2 | 1 << IMG_NN2 | (tc_on(TC_FWD) ? 1 << IMG_NT3 : 0);
+  for (int l = 0; l <= p.n_lin; ++l) add_prep_jobs(pj, p.layer[l], reinterpret_cast<uint16_t*>(wfold + p.w_total), kinds);
+  return tc::prep_weights_jobs(pj, st);
 }
 
 // Y[:, 0] (udf head) and, with `features`, Y[:, 1:] of the last layer, with every layer's input saved in the context
-static int value_chain(const UdfPlan& p, const nudf_udf_desc* d, const float* wfold, const float* pts, int64_t P,
-                       float* ctx, const UdfCtx& c, bool features, cudaStream_t st) {
+static int value_chain(const UdfPlan& p, const float* pts, int64_t P, float* ctx, const UdfCtx& c, bool features, cudaStream_t st) {
   float* e0 = ctx + c.e0;
   float* askip = nullptr; int askip_ld = 0, askip_col = 0;
-  if (p.skip >= 1) { askip = ctx + c.a[p.skip]; askip_ld = p.a_ld[p.skip]; askip_col = p.out_dim[p.skip - 1]; }
+  if (p.skip >= 1) { askip = ctx + c.a[p.skip]; askip_ld = p.a_ld[p.skip]; askip_col = p.layer[p.skip - 1].n_out; }
   pe_forward_kernel<<<nblk(P, 128), 128, 0, st>>>(pts, P, p.L, p.scale, e0, p.pe_ld, askip, askip_ld, askip_col);
   NUDF_LAUNCH_OK();
-  const uint16_t* img = img_base(p, wfold);
   const int last = p.n_lin - 1;
   for (int l = 0; l < last; ++l) {
     const float* A = l == 0 ? e0 : ctx + c.a[l];
     int64_t lda = l == 0 ? p.pe_ld : p.a_ld[l];
-    EpiAct epi{ctx + c.a[l + 1], p.a_ld[l + 1], d->bias[l], ACT_SOFTPLUS100, (l + 1 == p.skip) ? NUDF_SQRT1_2 : 1.0f};
-    if (int rc = gemm_nt(A, lda, wfold + p.w_off[l], p.w_ld[l], P, p.out_dim[l], p.in_dim[l], epi, st, img + p.img_fwd[l], TC_FWD, 3))
-      return rc;
+    EpiAct epi{ctx + c.a[l + 1], p.a_ld[l + 1], p.layer[l].bias, ACT_SOFTPLUS100, (l + 1 == p.skip) ? NUDF_SQRT1_2 : 1.0f};
+    if (int rc = layer_nt(p.layer[l], A, lda, P, epi, TC_FWD, st)) return rc;
   }
   const float* A = ctx + c.a[last];
-  const float* W = wfold + p.w_off[last];
-  udf_head_kernel<<<nblk(P * 32, 256), 256, 0, st>>>(A, p.a_ld[last], W, d->bias[last], p.in_dim[last], P, ctx + c.y, p.y_ld);
+  const DenseLayer& Ll = p.layer[last];
+  udf_head_kernel<<<nblk(P * 32, 256), 256, 0, st>>>(A, p.a_ld[last], Ll.W, Ll.bias, Ll.n_in, P, ctx + c.y, p.y_ld);
   NUDF_LAUNCH_OK();
   if (features && p.d_out > 1) {
-    const float* bias = d->bias[last] != nullptr ? d->bias[last] + 1 : nullptr;
-    EpiAct epi{ctx + c.y + 1, p.y_ld, bias, ACT_NONE, 1.0f};      // unaligned columns: st4 stores them one by one
-    if (int rc = gemm_nt(A, p.a_ld[last], W + p.w_ld[last], p.w_ld[last], P, p.d_out - 1, p.in_dim[last], epi, st, img + p.img_feat,
-                         TC_FWD, 3))
-      return rc;
+    const DenseLayer& Lf = p.layer[p.n_lin];
+    EpiAct epi{ctx + c.y + 1, p.y_ld, Lf.bias, ACT_NONE, 1.0f};      // unaligned columns: st4 stores them one by one
+    if (int rc = layer_nt(Lf, A, p.a_ld[last], P, epi, TC_FWD, st)) return rc;
   }
   return 0;
 }
 
-static int reverse_chain(const UdfPlan& p, const float* wfold, const float* pts, int64_t P, float* ctx, const UdfCtx& c,
-                         float* grad, cudaStream_t st) {
+static int reverse_chain(const UdfPlan& p, const float* pts, int64_t P, float* ctx, const UdfCtx& c, float* grad, cudaStream_t st) {
   const int last = p.n_lin - 1;
   auto make_rev = [&](int l) {  // epilogue that turns G (wrt A[l]) into D[l-1]
     EpiRev e;
-    e.n_main = p.out_dim[l - 1];
+    e.n_main = p.layer[l - 1].n_out;
     e.post_scale = (l == p.skip) ? NUDF_SQRT1_2 : 1.0f;
     e.Anext = ctx + c.a[l]; e.lda = p.a_ld[l]; e.a_unscale = (l == p.skip) ? 1.41421356237309504880f : 1.0f;
     e.Dprev = ctx + c.d[l - 1]; e.ldd = p.o_ld[l - 1];
@@ -381,22 +355,18 @@ static int reverse_chain(const UdfPlan& p, const float* wfold, const float* pts,
   };
   {
     EpiRev e = make_rev(last);
-    int cols4 = (p.in_dim[last] + 3) / 4;
-    rev_init_kernel<EpiRev><<<nblk(P * cols4, 256), 256, 0, st>>>(ctx + c.sgn, wfold + p.w_off[last], p.in_dim[last],
-                                                                  1.0f / p.scale, P, e);
+    const int in_last = p.layer[last].n_in;
+    int cols4 = (in_last + 3) / 4;
+    rev_init_kernel<EpiRev><<<nblk(P * cols4, 256), 256, 0, st>>>(ctx + c.sgn, p.layer[last].W, in_last, 1.0f / p.scale, P, e);
     NUDF_LAUNCH_OK();
   }
   for (int l = last - 1; l >= 1; --l) {
     EpiRev e = make_rev(l);
-    int rc = gemm_nn(ctx + c.d[l], p.o_ld[l], wfold + p.w_off[l], p.w_ld[l], P, p.in_dim[l], p.out_dim[l], e, st,
-                     img_base(p, wfold) + p.img_nn[l], TC_REV);
-    if (rc) return rc;
+    if (int rc = layer_nn(p.layer[l], ctx + c.d[l], p.o_ld[l], P, e, TC_REV, st)) return rc;
   }
   {
     EpiRevFinal e{ctx + c.ge, p.pe_ld, p.skip >= 1 ? ctx + c.gpe : nullptr, p.pe_ld};
-    int rc = gemm_nn(ctx + c.d[0], p.o_ld[0], wfold + p.w_off[0], p.w_ld[0], P, p.in_dim[0], p.out_dim[0], e, st,
-                     img_base(p, wfold) + p.img_nn[0], TC_REV);
-    if (rc) return rc;
+    if (int rc = layer_nn(p.layer[0], ctx + c.d[0], p.o_ld[0], P, e, TC_REV, st)) return rc;
   }
   pe_vjp_kernel<<<nblk(P, 128), 128, 0, st>>>(pts, ctx + c.ge, p.pe_ld, P, p.L, p.scale, grad);
   NUDF_LAUNCH_OK();
@@ -417,7 +387,7 @@ int64_t nudf_udf_folded_floats(const nudf_udf_desc* d) {
 
 int nudf_udf_fold_weights(const nudf_udf_desc* d, float* wfold, void* stream) {
   UdfPlan p;
-  if (int rc = make_plan(d, &p)) return rc;
+  if (int rc = make_plan(d, &p, wfold)) return rc;
   NUDF_REQUIRE(wfold != nullptr, "null wfold");
   cudaStream_t st = (cudaStream_t)stream;
   return fold_all(p, d, wfold, st);
@@ -442,17 +412,17 @@ int64_t nudf_udf_scratch_floats(const nudf_udf_desc* d, int64_t P) {
 static int udf_forward_impl(const nudf_udf_desc* d, const float* wfold, const float* pts, int64_t P, float* udf, int64_t ld_u, float* feat,
                             int64_t ld_f, float* grad, float* ctx, void* stream) {
   UdfPlan p;
-  if (int rc = make_plan(d, &p)) return rc;
+  if (int rc = make_plan(d, &p, wfold)) return rc;
   if (P <= 0) return 0;
   NUDF_REQUIRE(wfold && pts && ctx, "null pointer");
   cudaStream_t st = (cudaStream_t)stream;
   UdfCtx c;
   ctx_layout(p, P, grad != nullptr, &c);
-  if (int rc = value_chain(p, d, wfold, pts, P, ctx, c, feat != nullptr, st)) return rc;
+  if (int rc = value_chain(p, pts, P, ctx, c, feat != nullptr, st)) return rc;
   udf_finalize_kernel<<<nblk(P * p.d_out, 256), 256, 0, st>>>(ctx + c.y, p.y_ld, p.d_out, P, 1.0f / p.scale, udf, ld_u, feat, ld_f,
                                                               ctx + c.sgn);
   NUDF_LAUNCH_OK();
-  if (grad) return reverse_chain(p, wfold, pts, P, ctx, c, grad, st);
+  if (grad) return reverse_chain(p, pts, P, ctx, c, grad, st);
   return 0;
 }
 
@@ -473,7 +443,7 @@ int nudf_udf_forward_split(const nudf_udf_desc* d, const float* wfold, const flo
 int nudf_udf_value(const nudf_udf_desc* d, const float* wfold, const float* pts, int64_t P, float* udf, float* work,
                    void* stream) {
   UdfPlan p;
-  if (int rc = make_plan(d, &p)) return rc;
+  if (int rc = make_plan(d, &p, wfold)) return rc;
   if (P <= 0) return 0;
   NUDF_REQUIRE(wfold && pts && udf, "null pointer");
   cudaStream_t st = (cudaStream_t)stream;
@@ -481,7 +451,7 @@ int nudf_udf_value(const nudf_udf_desc* d, const float* wfold, const float* pts,
   UdfCtx c;
   ctx_layout(p, P, 0, &c);
   // value-only: of the last layer only row 0 (the udf head), through the same kernel as the full forward
-  if (int rc = value_chain(p, d, wfold, pts, P, work, c, false, st)) return rc;
+  if (int rc = value_chain(p, pts, P, work, c, false, st)) return rc;
   udf_value_only_kernel<<<nblk(P, 256), 256, 0, st>>>(work + c.y, p.y_ld, P, 1.0f / p.scale, udf);
   NUDF_LAUNCH_OK();
   return 0;
@@ -509,7 +479,7 @@ static int udf_backward_impl(const nudf_udf_desc* d, const float* wfold, const f
                              float* dbias, void* stream) {
   const bool out_bar = ub != nullptr || fb != nullptr;      // some upstream gradient of the value / feature outputs
   UdfPlan p;
-  if (int rc = make_plan(d, &p)) return rc;
+  if (int rc = make_plan(d, &p, wfold)) return rc;
   NUDF_REQUIRE(wfold && dwfold && dbias, "null pointer");
   cudaStream_t st = (cudaStream_t)stream;
   NUDF_CUDA_OK(cudaMemsetAsync(dwfold, 0, sizeof(float) * p.w_total, st));
@@ -522,6 +492,7 @@ static int udf_backward_impl(const nudf_udf_desc* d, const float* wfold, const f
   UdfScratch s;
   scratch_layout(p, P, &s);
   const int last = p.n_lin - 1;
+  const DenseLayer& Ll = p.layer[last];
 
   // ---- tangent chain (second-order terms) ----
   if (grad_bar) {
@@ -531,9 +502,10 @@ static int udf_backward_impl(const nudf_udf_desc* d, const float* wfold, const f
     const float* adot = edot;
     int64_t ld_adot = p.pe_ld;
     for (int l = 0; l < last; ++l) {
+      const DenseLayer& L = p.layer[l];
       // dW_l += D_l^T Adot_l
-      EpiAtomicAdd ew{dwfold + p.w_off[l], p.w_ld[l]};
-      if (int rc = gemm_tn(ctx + c.d[l], p.o_ld[l], adot, ld_adot, p.out_dim[l], p.in_dim[l], P, ew, st)) return rc;
+      EpiAtomicAdd ew{dwfold + L.w_off, L.ldw};
+      if (int rc = gemm_tn(ctx + c.d[l], p.o_ld[l], adot, ld_adot, L.n_out, L.n_in, P, ew, st)) return rc;
       float* nxt = scratch + s.adot[l & 1];
       int64_t ld_nxt = p.a_ld[l + 1];
       EpiTan et;
@@ -542,18 +514,15 @@ static int udf_backward_impl(const nudf_udf_desc* d, const float* wfold, const f
       et.D = ctx + c.d[l]; et.ldd = p.o_ld[l];
       et.Q = scratch + s.q[l]; et.ldq = p.o_ld[l];
       et.AdotNext = nxt; et.ldn = ld_nxt; et.post_scale = (l + 1 == p.skip) ? NUDF_SQRT1_2 : 1.0f;
-      if (int rc = gemm_nt(adot, ld_adot, wfold + p.w_off[l], p.w_ld[l], P, p.out_dim[l], p.in_dim[l], et, st,
-                           img_base(p, wfold) + p.img_nt[l], TC_TAN))
-        return rc;
+      if (int rc = layer_nt(L, adot, ld_adot, P, et, TC_TAN, st)) return rc;
       if (l + 1 == p.skip) {
-        ew_copy_cols_kernel<<<nblk(P * p.d_pe, 256), 256, 0, st>>>(edot, p.pe_ld, nxt, ld_nxt, p.out_dim[l], p.d_pe, P,
-                                                                    NUDF_SQRT1_2);
+        ew_copy_cols_kernel<<<nblk(P * p.d_pe, 256), 256, 0, st>>>(edot, p.pe_ld, nxt, ld_nxt, L.n_out, p.d_pe, P, NUDF_SQRT1_2);
         NUDF_LAUNCH_OK();
       }
       adot = nxt; ld_adot = ld_nxt;
     }
     // g_last = W_last^T d_last with d_last = (sgn/scale) e_0  =>  dW_last[0,:] += sum_p (sgn/scale) Adot_last
-    if (int rc = colsum(adot, ld_adot, ctx + c.sgn, 1.0f / p.scale, P, p.in_dim[last], dwfold + p.w_off[last], st)) return rc;
+    if (int rc = colsum(adot, ld_adot, ctx + c.sgn, 1.0f / p.scale, P, Ll.n_in, dwfold + Ll.w_off, st)) return rc;
   }
 
   // ---- backward chain ----
@@ -567,53 +536,45 @@ static int udf_backward_impl(const nudf_udf_desc* d, const float* wfold, const f
   // tensor kernel, the head row a rank-1 update in its epilogue (and a weighted column sum for its weight gradient).
   const bool split_head = out_bar && tc_on(TC_BWD) && F >= 64 && (F % 4) == 0 && F <= 256;
   if (split_head) {
+    const DenseLayer& Lf = p.layer[p.n_lin];
     float* zf = zl;
     float* z0 = zl + P * F;
     zlast_split_kernel<<<nblk(P * p.d_out, 256), 256, 0, st>>>(ub, ld_ub, fb, ld_fb, ctx + c.sgn, 1.0f / p.scale, F, P, zf, z0);
     NUDF_LAUNCH_OK();
-    const float* Wl = wfold + p.w_off[last];
-    float* dWl = dwfold + p.w_off[last];
-    EpiAtomicAdd ew{dWl + p.w_ld[last], p.w_ld[last]};
-    if (int rc = gemm_tn(zf, F, ctx + c.a[last], p.a_ld[last], F, p.in_dim[last], P, ew, st, TC_WGRAD, dbias + p.b_off[last] + 1))
-      return rc;
-    if (int rc = colsum(ctx + c.a[last], p.a_ld[last], z0, 1.0f, P, p.in_dim[last], dWl, st)) return rc;
-    if (int rc = colsum(z0, 1, nullptr, 1.0f, P, 1, dbias + p.b_off[last], st)) return rc;
+    EpiAtomicAdd ew{dwfold + Lf.w_off, Lf.ldw};
+    if (int rc = gemm_tn(zf, F, ctx + c.a[last], p.a_ld[last], F, Lf.n_in, P, ew, st, TC_WGRAD, dbias + Lf.b_off)) return rc;
+    if (int rc = colsum(ctx + c.a[last], p.a_ld[last], z0, 1.0f, P, Ll.n_in, dwfold + Ll.w_off, st)) return rc;
+    if (int rc = colsum(z0, 1, nullptr, 1.0f, P, 1, dbias + Ll.b_off, st)) return rc;
     EpiBwdR1 eb;
-    eb.n_main = p.out_dim[last - 1]; eb.post_scale = (last == p.skip) ? NUDF_SQRT1_2 : 1.0f;
+    eb.n_main = p.layer[last - 1].n_out; eb.post_scale = (last == p.skip) ? NUDF_SQRT1_2 : 1.0f;
     eb.Anext = ctx + c.a[last]; eb.lda = p.a_ld[last]; eb.a_unscale = (last == p.skip) ? 1.41421356237309504880f : 1.0f;
     eb.QZ = scratch + s.q[last - 1]; eb.ldq = p.o_ld[last - 1];
-    eb.z0 = z0; eb.w0 = Wl;
-    if (int rc = gemm_nn(zf, F, Wl + p.w_ld[last], p.w_ld[last], P, p.in_dim[last], F, eb, st, img_base(p, wfold) + p.img_nn1, TC_BWD))
-      return rc;
+    eb.z0 = z0; eb.w0 = Ll.W;
+    if (int rc = layer_nn(Lf, zf, F, P, eb, TC_BWD, st)) return rc;
   } else if (out_bar) {
     zlast_kernel<<<nblk(P * p.y_ld, 256), 256, 0, st>>>(ub, ld_ub, fb, ld_fb, ctx + c.sgn, 1.0f / p.scale, p.d_out, p.y_ld, P, zl);
     NUDF_LAUNCH_OK();
-    EpiAtomicAdd ew{dwfold + p.w_off[last], p.w_ld[last]};
-    if (int rc = gemm_tn(zl, p.y_ld, ctx + c.a[last], p.a_ld[last], p.out_dim[last], p.in_dim[last], P, ew, st, TC_WGRAD,
-                         dbias + p.b_off[last]))
-      return rc;
+    EpiAtomicAdd ew{dwfold + Ll.w_off, Ll.ldw};
+    if (int rc = gemm_tn(zl, p.y_ld, ctx + c.a[last], p.a_ld[last], Ll.n_out, Ll.n_in, P, ew, st, TC_WGRAD, dbias + Ll.b_off)) return rc;
     EpiBwd eb;
-    eb.n_main = p.out_dim[last - 1]; eb.post_scale = (last == p.skip) ? NUDF_SQRT1_2 : 1.0f;
+    eb.n_main = p.layer[last - 1].n_out; eb.post_scale = (last == p.skip) ? NUDF_SQRT1_2 : 1.0f;
     eb.Anext = ctx + c.a[last]; eb.lda = p.a_ld[last]; eb.a_unscale = (last == p.skip) ? 1.41421356237309504880f : 1.0f;
     eb.QZ = scratch + s.q[last - 1]; eb.ldq = p.o_ld[last - 1];
-    if (int rc = gemm_nn(zl, p.y_ld, wfold + p.w_off[last], p.w_ld[last], P, p.in_dim[last], p.out_dim[last], eb, st,
-                         img_base(p, wfold) + p.img_nn[last], TC_BWD))
-      return rc;
+    if (int rc = layer_nn(Ll, zl, p.y_ld, P, eb, TC_BWD, st)) return rc;
   }
   for (int l = last - 1; l >= 0; --l) {
+    const DenseLayer& L = p.layer[l];
     const float* zb = scratch + s.q[l];  // now holds Zbar_l
     const float* A = l == 0 ? ctx + c.e0 : ctx + c.a[l];
     int64_t lda = l == 0 ? p.pe_ld : p.a_ld[l];
-    EpiAtomicAdd ew{dwfold + p.w_off[l], p.w_ld[l]};
-    if (int rc = gemm_tn(zb, p.o_ld[l], A, lda, p.out_dim[l], p.in_dim[l], P, ew, st, TC_WGRAD, dbias + p.b_off[l])) return rc;
+    EpiAtomicAdd ew{dwfold + L.w_off, L.ldw};
+    if (int rc = gemm_tn(zb, p.o_ld[l], A, lda, L.n_out, L.n_in, P, ew, st, TC_WGRAD, dbias + L.b_off)) return rc;
     if (l > 0) {
       EpiBwd eb;
-      eb.n_main = p.out_dim[l - 1]; eb.post_scale = (l == p.skip) ? NUDF_SQRT1_2 : 1.0f;
+      eb.n_main = p.layer[l - 1].n_out; eb.post_scale = (l == p.skip) ? NUDF_SQRT1_2 : 1.0f;
       eb.Anext = ctx + c.a[l]; eb.lda = p.a_ld[l]; eb.a_unscale = (l == p.skip) ? 1.41421356237309504880f : 1.0f;
       eb.QZ = scratch + s.q[l - 1]; eb.ldq = p.o_ld[l - 1];
-      if (int rc = gemm_nn(zb, p.o_ld[l], wfold + p.w_off[l], p.w_ld[l], P, p.in_dim[l], p.out_dim[l], eb, st,
-                           img_base(p, wfold) + p.img_nn[l], TC_BWD))
-        return rc;
+      if (int rc = layer_nn(L, zb, p.o_ld[l], P, eb, TC_BWD, st)) return rc;
     }
   }
   return 0;
@@ -624,9 +585,8 @@ int nudf_udf_unfold_grads(const nudf_udf_desc* d, const float* dwfold, float* co
   if (int rc = make_plan(d, &p)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   FoldJobs jobs;
-  jobs.n = p.n_lin;
-  for (int l = 0; l < p.n_lin; ++l)
-    jobs.j[l] = FoldJob{d->weight_g[l], d->weight_v[l], dwfold + p.w_off[l], dg[l], dv[l], nullptr, p.out_dim[l], p.in_dim[l], (int)p.w_ld[l]};
+  jobs.n = 0;
+  for (int l = 0; l < p.n_lin; ++l) add_unfold_job(jobs, p.layer[l], d->weight_g[l], d->weight_v[l], dwfold, dg[l], dv[l]);
   return run_fold_jobs(jobs, true, st);
 }
 

@@ -76,6 +76,44 @@ def _ptr_array(tensors):
     return arr
 
 
+def _refold(h, ps, extra, make_desc, size_fn, fold_fn):
+    """The handles' shared bookkeeping.  h.wfold (folded weights and / or tensor-core weight images) is cached on
+    (data_ptr, Tensor._version) of every parameter in ps plus `extra`; on a change it is resized to size_fn's float count
+    and rebuilt by fold_fn from a fresh descriptor.  Returns that descriptor, or None when nothing changed."""
+    key = tuple((p.data_ptr(), p._version) for p in ps) + extra
+    if key == h._key:
+        return None
+    d = make_desc()
+    n = size_fn(ctypes.byref(d))
+    if n < 0:
+        L.check(-1, size_fn.__name__)
+    dev = ps[0].device
+    if h.wfold is None or h.wfold.numel() != n or h.wfold.device != dev:
+        h.wfold = torch.empty(n, dtype=torch.float32, device=dev)
+    L.check(fold_fn(ctypes.byref(d), L.ptr(h.wfold), L.stream_ptr()), fold_fn.__name__)
+    h._key = key
+    return d
+
+
+def _grad_targets(h, mods):
+    """Where a backward pass writes the gradients of the weight-normed layers `mods` (in the order of the library's
+    dbias): (sink, db, dg, dv, dbs).  With an armed gradient sink (dp.GradBucket) they are views of the data-parallel
+    bucket, else fresh tensors; db is the ONE contiguous bias block the library writes, dbs its per-layer slices."""
+    sink = h.grad_sink if (h.grad_sink is not None and h.grad_sink.begin()) else None
+    if sink is not None:
+        db = sink.block([m.bias for m in mods])
+        return (sink, db, [sink.view(m.weight_g) for m in mods], [sink.view(m.weight_v) for m in mods],
+                [sink.view(m.bias) for m in mods])
+    nb = sum(int(m.bias.numel()) for m in mods)
+    db = torch.empty(nb, dtype=torch.float32, device=mods[0].bias.device)
+    dbs, off = [], 0
+    for m in mods:
+        n = m.bias.numel()
+        dbs.append(db[off:off + n])
+        off += n
+    return None, db, [torch.empty_like(m.weight_g) for m in mods], [torch.empty_like(m.weight_v) for m in mods], dbs
+
+
 # ---------------------------------------------------------------------------------------------------------------
 # UDF network
 # ---------------------------------------------------------------------------------------------------------------
@@ -110,11 +148,14 @@ class UdfHandle:
     def refresh(self):
         ps = self.params()
         _require_cuda(*ps)
-        lib_ = L.lib()
+        lib = L.lib()
         # the folded images depend on the engine and on which chains run fused (chain mask)
-        key = tuple((p.data_ptr(), p._version) for p in ps) + (lib_.nudf_get_engine(), lib_.nudf_get_tc_mask())
-        if key == self._key:
-            return
+        d = _refold(self, ps, (lib.nudf_get_engine(), lib.nudf_get_tc_mask()), self._make_desc, lib.nudf_udf_folded_floats,
+                    lib.nudf_udf_fold_weights)
+        if d is not None:
+            self.desc = d
+
+    def _make_desc(self):
         d = L.UdfDesc()
         d.n_lin = len(self.layers)
         d.d_in, d.multires, d.d_out, d.skip_layer, d.scale = self.meta
@@ -126,16 +167,13 @@ class UdfHandle:
             d.weight_g[l] = m.weight_g.data_ptr()
             d.weight_v[l] = m.weight_v.data_ptr()
             d.bias[l] = m.bias.data_ptr()
-        lib = L.lib()
-        n = lib.nudf_udf_folded_floats(ctypes.byref(d))
-        if n < 0:
-            L.check(-1, "nudf_udf_folded_floats")
-        dev = ps[0].device
-        if self.wfold is None or self.wfold.numel() != n or self.wfold.device != dev:
-            self.wfold = torch.empty(n, dtype=torch.float32, device=dev)
-        L.check(lib.nudf_udf_fold_weights(ctypes.byref(d), L.ptr(self.wfold), L.stream_ptr()), "nudf_udf_fold_weights")
-        self.desc = d
-        self._key = key
+        return d
+
+
+def _udf_ctx(handle, P, with_grad, dev):
+    """the context buffer of a forward over P points (with_grad: also what the gradient and backward chains keep)"""
+    n = L.lib().nudf_udf_ctx_floats(ctypes.byref(handle.desc), P, 1 if with_grad else 0)
+    return torch.empty(max(n, 1), dtype=torch.float32, device=dev)
 
 
 class _UdfFunction(torch.autograd.Function):
@@ -151,13 +189,11 @@ class _UdfFunction(torch.autograd.Function):
         d_out = handle.meta[2]
         dev = pts.device
         grad = torch.empty(P, 3, dtype=torch.float32, device=dev) if with_grad else None
-        nctx = lib.nudf_udf_ctx_floats(ctypes.byref(handle.desc), P, 1 if with_grad else 0)
-        buf = torch.empty(max(nctx, 1), dtype=torch.float32, device=dev)
+        buf = _udf_ctx(handle, P, with_grad, dev)
         if split:
             a = torch.empty(P, 1, dtype=torch.float32, device=dev)
             b = torch.empty(P, d_out - 1, dtype=torch.float32, device=dev)
-            L.check(lib.nudf_udf_forward_split(ctypes.byref(handle.desc), L.ptr(handle.wfold), L.ptr(pts), P, L.ptr(a), L.ptr(b), d_out - 1,
-                                               L.ptr(grad), L.ptr(buf), L.stream_ptr()), "nudf_udf_forward_split")
+            udf_forward_split_into(handle, pts, a, b, grad, buf)
         else:
             a = torch.empty(P, d_out, dtype=torch.float32, device=dev)
             b = torch.empty(0, device=dev)
@@ -186,22 +222,7 @@ class _UdfFunction(torch.autograd.Function):
         nscr = lib.nudf_udf_scratch_floats(ctypes.byref(h.desc), P)
         scratch = torch.empty(max(nscr, 1), dtype=torch.float32, device=dev)
         dw = torch.empty_like(h.wfold)
-        sink = h.grad_sink if (h.grad_sink is not None and h.grad_sink.begin()) else None
-        if sink is not None:                  # gradients land directly in the data-parallel bucket (dp.GradBucket)
-            db = sink.block([m.bias for m in h.layers])
-            dgs = [sink.view(m.weight_g) for m in h.layers]
-            dvs = [sink.view(m.weight_v) for m in h.layers]
-            dbs = [sink.view(m.bias) for m in h.layers]
-        else:
-            nb = sum(int(m.bias.numel()) for m in h.layers)
-            db = torch.empty(nb, dtype=torch.float32, device=dev)
-            dgs = [torch.empty_like(m.weight_g) for m in h.layers]
-            dvs = [torch.empty_like(m.weight_v) for m in h.layers]
-            dbs, off = [], 0
-            for m in h.layers:
-                n = m.bias.numel()
-                dbs.append(db[off:off + n])
-                off += n
+        sink, db, dgs, dvs, dbs = _grad_targets(h, h.layers)
         if ctx.split:
             L.check(lib.nudf_udf_backward_split(ctypes.byref(h.desc), L.ptr(h.wfold), L.ptr(pts), P, L.ptr(a_bar), L.ptr(b_bar),
                                                 b_bar.shape[1] if b_bar is not None else 0, L.ptr(grad_bar), L.ptr(buf),
@@ -240,8 +261,7 @@ def udf_value(handle, pts):
     _require_cuda(pts)
     P = pts.shape[0]
     udf = torch.empty(P, dtype=torch.float32, device=pts.device)
-    n = lib.nudf_udf_ctx_floats(ctypes.byref(handle.desc), P, 0)
-    work = torch.empty(max(n, 1), dtype=torch.float32, device=pts.device)
+    work = _udf_ctx(handle, P, False, pts.device)
     L.check(lib.nudf_udf_value(ctypes.byref(handle.desc), L.ptr(handle.wfold), L.ptr(pts), P, L.ptr(udf), L.ptr(work),
                                L.stream_ptr()), "nudf_udf_value")
     return udf
@@ -277,9 +297,12 @@ class ColorHandle:
     def refresh(self):
         ps = self.params()
         _require_cuda(*ps)
-        key = tuple((p.data_ptr(), p._version) for p in ps) + (L.lib().nudf_get_engine(),)
-        if key == self._key:
-            return
+        lib = L.lib()
+        d = _refold(self, ps, (lib.nudf_get_engine(),), self._make_desc, lib.nudf_color_folded_floats, lib.nudf_color_fold_weights)
+        if d is not None:
+            self.desc = d
+
+    def _make_desc(self):
         d = L.ColorDesc()
         d.n_lin = len(self.base)
         d.d_feature, d.d_hidden, d.d_out, d.n_blend, d.multires_view = self.meta
@@ -287,16 +310,7 @@ class ColorHandle:
             d.base_g[l], d.base_v[l], d.base_b[l] = m.weight_g.data_ptr(), m.weight_v.data_ptr(), m.bias.data_ptr()
         for l, m in enumerate(self.main):
             d.main_g[l], d.main_v[l], d.main_b[l] = m.weight_g.data_ptr(), m.weight_v.data_ptr(), m.bias.data_ptr()
-        lib = L.lib()
-        n = lib.nudf_color_folded_floats(ctypes.byref(d))
-        if n < 0:
-            L.check(-1, "nudf_color_folded_floats")
-        dev = ps[0].device
-        if self.wfold is None or self.wfold.numel() != n or self.wfold.device != dev:
-            self.wfold = torch.empty(n, dtype=torch.float32, device=dev)
-        L.check(lib.nudf_color_fold_weights(ctypes.byref(d), L.ptr(self.wfold), L.stream_ptr()), "nudf_color_fold_weights")
-        self.desc = d
-        self._key = key
+        return d
 
 
 class _ColorFunction(torch.autograd.Function):
@@ -316,9 +330,7 @@ class _ColorFunction(torch.autograd.Function):
         bl = torch.empty(P, n_blend, dtype=torch.float32, device=dev)
         n = lib.nudf_color_ctx_floats(ctypes.byref(handle.desc), P)
         buf = torch.empty(max(n, 1), dtype=torch.float32, device=dev)
-        L.check(lib.nudf_color_forward(ctypes.byref(handle.desc), L.ptr(handle.wfold), L.ptr(pts), L.ptr(dirs),
-                                       int(samples_per_ray), L.ptr(feat), feat.stride(0), P, L.ptr(cb), L.ptr(c),
-                                       L.ptr(bl), L.ptr(buf), L.stream_ptr()), "nudf_color_forward")
+        color_forward_into(handle, pts, dirs, samples_per_ray, feat, cb, c, bl, buf)
         ctx.handle, ctx.P, ctx.key = handle, P, handle._key
         ctx.save_for_backward(buf)
         return cb, c, bl
@@ -338,41 +350,19 @@ class _ColorFunction(torch.autograd.Function):
         scratch = torch.empty(max(nscr, 1), dtype=torch.float32, device=dev)
         dfeat = torch.empty(P, d_feature, dtype=torch.float32, device=dev)
         dw = torch.empty_like(h.wfold)
-        mods = list(h.base) + list(h.main)
-        sink = h.grad_sink if (h.grad_sink is not None and h.grad_sink.begin()) else None
-        if sink is not None:
-            db = sink.block([m.bias for m in mods])
-            new_g = lambda m: sink.view(m.weight_g)
-            new_v = lambda m: sink.view(m.weight_v)
-            bb = [sink.view(m.bias) for m in h.base]
-            bm = [sink.view(m.bias) for m in h.main]
-        else:
-            nb = sum(int(m.bias.numel()) for m in mods)
-            db = torch.empty(nb, dtype=torch.float32, device=dev)
-            new_g = lambda m: torch.empty_like(m.weight_g)
-            new_v = lambda m: torch.empty_like(m.weight_v)
-            off = 0            # bias layout in the library: base layers first, then main layers
-            bb, bm = [], []
-            for m in h.base:
-                n = m.bias.numel(); bb.append(db[off:off + n]); off += n
-            for m in h.main:
-                n = m.bias.numel(); bm.append(db[off:off + n]); off += n
+        nbase = len(h.base)             # bias layout in the library: base layers first, then main layers
+        sink, db, dg, dv, dbs = _grad_targets(h, list(h.base) + list(h.main))
         L.check(lib.nudf_color_backward(ctypes.byref(h.desc), L.ptr(h.wfold), P, L.ptr(cb_bar), L.ptr(c_bar),
                                         L.ptr(bl_bar), L.ptr(buf), L.ptr(scratch), L.ptr(dfeat), d_feature, L.ptr(dw),
                                         L.ptr(db), L.stream_ptr()), "nudf_color_backward")
-        dgb = [new_g(m) for m in h.base]
-        dvb = [new_v(m) for m in h.base]
-        dgm = [new_g(m) for m in h.main]
-        dvm = [new_v(m) for m in h.main]
-        L.check(lib.nudf_color_unfold_grads(ctypes.byref(h.desc), L.ptr(dw), _ptr_array(dgb), _ptr_array(dvb),
-                                            _ptr_array(dgm), _ptr_array(dvm), L.stream_ptr()), "nudf_color_unfold_grads")
+        L.check(lib.nudf_color_unfold_grads(ctypes.byref(h.desc), L.ptr(dw), _ptr_array(dg[:nbase]), _ptr_array(dv[:nbase]),
+                                            _ptr_array(dg[nbase:]), _ptr_array(dv[nbase:]), L.stream_ptr()),
+                "nudf_color_unfold_grads")
         if sink is not None:
             sink.ready()
         grads = []
-        for l in range(len(h.main)):
-            grads += [dgm[l], dvm[l], bm[l]]
-        for l in range(len(h.base)):
-            grads += [dgb[l], dvb[l], bb[l]]
+        for l in list(range(nbase, len(dg))) + list(range(nbase)):     # params() order: main layers, then base layers
+            grads += [dg[l], dv[l], dbs[l]]
         return (None, None, dfeat, None, None) + tuple(grads)
 
 
@@ -388,7 +378,7 @@ class NerfHandle:
         self.m = module
         self.meta = (D, W, d_in, multires, multires_view, skip)
         self._key = None
-        self.wimg = None
+        self.wfold = None            # NeRF++ has plain weights: the buffer holds the weight images only
         self.grad_sink = None
 
     def sink_layout(self):
@@ -400,16 +390,8 @@ class NerfHandle:
         lib = L.lib()
         if lib.nudf_get_engine() != 1 or not (lib.nudf_get_tc_mask() & (64 | 128)):
             return None
-        ps = self.params()
-        key = tuple((p.data_ptr(), p._version) for p in ps)
-        if key != self._key:
-            d = self.desc()
-            n = lib.nudf_nerf_image_floats(ctypes.byref(d))
-            if self.wimg is None or self.wimg.numel() != n or self.wimg.device != ps[0].device:
-                self.wimg = torch.empty(n, dtype=torch.float32, device=ps[0].device)
-            L.check(lib.nudf_nerf_prepare(ctypes.byref(d), L.ptr(self.wimg), L.stream_ptr()), "nudf_nerf_prepare")
-            self._key = key
-        return self.wimg
+        _refold(self, self.params(), (), self.desc, lib.nudf_nerf_image_floats, lib.nudf_nerf_prepare)
+        return self.wfold
 
     def params(self):
         m = self.m
@@ -450,8 +432,7 @@ class _NerfFunction(torch.autograd.Function):
         n = lib.nudf_nerf_ctx_floats(ctypes.byref(d), P)
         buf = torch.empty(max(n, 1), dtype=torch.float32, device=dev)
         wimg = handle.images()
-        L.check(lib.nudf_nerf_forward(ctypes.byref(d), L.ptr(wimg), L.ptr(pts), L.ptr(dirs), int(samples_per_ray), P,
-                                      L.ptr(sigma), L.ptr(rgb), L.ptr(buf), L.stream_ptr()), "nudf_nerf_forward")
+        nerf_forward_into(d, wimg, pts, dirs, samples_per_ray, sigma, rgb, buf)
         ctx.handle, ctx.P, ctx.wimg = handle, P, wimg
         ctx.save_for_backward(buf, *params)
         return sigma, rgb
@@ -485,7 +466,6 @@ def nerf_forward(handle, pts, dirs, samples_per_ray=0):
 # ray geometry + compositing
 # ---------------------------------------------------------------------------------------------------------------
 def ray_points(rays_o, rays_d, z_vals, sample_dist):
-    lib = L.lib()
     rays_o, rays_d, z_vals = _f32c(rays_o), _f32c(rays_d), _f32c(z_vals)
     _require_cuda(rays_o, rays_d, z_vals)
     N, S = z_vals.shape
@@ -493,8 +473,7 @@ def ray_points(rays_o, rays_d, z_vals, sample_dist):
     pts = torch.empty(N * S, 3, dtype=torch.float32, device=dev)
     mid = torch.empty(N, S, dtype=torch.float32, device=dev)
     dists = torch.empty(N, S, dtype=torch.float32, device=dev)
-    L.check(lib.nudf_ray_points(L.ptr(rays_o), L.ptr(rays_d), L.ptr(z_vals), N, S, float(sample_dist), L.ptr(pts),
-                                L.ptr(mid), L.ptr(dists), L.stream_ptr()), "nudf_ray_points")
+    ray_points_into(rays_o, rays_d, z_vals, sample_dist, pts, mid, dists)
     return pts, mid, dists
 
 
@@ -613,7 +592,6 @@ class _BlendFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, logits, pts, proj, hom, px, imgs, n_rays, n_samples, h_patch):
-        lib = L.lib()
         P = n_rays * n_samples
         V, _, H, W = imgs.shape
         cfg = L.BlendCfg(n_rays, n_samples, V, H, W, h_patch)
@@ -622,9 +600,7 @@ class _BlendFunction(torch.autograd.Function):
         npx = (2 * h_patch + 1) ** 2
         c_pat = torch.empty(P, npx, 3, device=pts.device) if hom is not None else None
         m_pat = torch.empty(P, device=pts.device) if hom is not None else None
-        L.check(lib.nudf_blend_forward(ctypes.byref(cfg), L.ptr(pts), L.ptr(proj), L.ptr(hom), L.ptr(px), L.ptr(imgs), L.ptr(logits),
-                                       logits.stride(0), L.ptr(c_pix), L.ptr(c_pat), L.ptr(m_pat), L.stream_ptr()),
-                "nudf_blend_forward")
+        blend_forward_into(cfg, pts, proj, hom, px, imgs, logits, c_pix, c_pat, m_pat)
         ctx.cfg, ctx.has_patch, ctx.n_logits = cfg, hom is not None, logits.shape[1]
         ctx.save_for_backward(logits, pts, proj, hom, px, imgs)
         if hom is None:
@@ -718,43 +694,39 @@ def points_on_rays(rays_o, rays_d, z):
 
 
 def outside_points(rays_o, rays_d, z, col0, sample_dist):
-    lib = L.lib()
     rays_o, rays_d, z = _f32c(rays_o), _f32c(rays_d), _f32c(z)
     N, n = z.shape
     m = n - col0
     pts4 = torch.empty(N * m, 4, dtype=torch.float32, device=z.device)
     dists = torch.empty(N, m, dtype=torch.float32, device=z.device)
-    L.check(lib.nudf_outside_points(L.ptr(rays_o), L.ptr(rays_d), L.ptr(z), N, n, col0, float(sample_dist), L.ptr(pts4),
-                                    L.ptr(dists), L.stream_ptr()), "nudf_outside_points")
+    outside_points_into(rays_o, rays_d, z, col0, sample_dist, pts4, dists)
     return pts4, dists
 
 
 # ---------------------------------------------------------------------------------------------------------------
-# forward-only view rendering: the network forwards and the compositing pass outside autograd, every per-chunk array
-# carved from one caller-owned workspace
+# The library calls that write into caller-owned tensors: the one call site of each entry point.  The allocating wrappers
+# and autograd forwards above allocate and call these; the forward-only view renderer (render.render_view) passes views of
+# its workspace.  A handle must have been refresh()ed by the caller (the autograd forwards need its descriptor earlier, to
+# size the context buffer, and a forward refreshes once).
 # ---------------------------------------------------------------------------------------------------------------
 def udf_forward_split_into(handle, pts, udf, feat, grad, ctx):
-    """nudf_udf_forward_split into given buffers: udf [P], feat [P, d_out - 1], grad [P,3]; ctx is scratch (no backward)."""
-    lib = L.lib()
-    handle.refresh()
-    L.check(lib.nudf_udf_forward_split(ctypes.byref(handle.desc), L.ptr(handle.wfold), L.ptr(pts), pts.shape[0], L.ptr(udf),
-                                       L.ptr(feat), feat.shape[1], L.ptr(grad), L.ptr(ctx), L.stream_ptr()),
+    """nudf_udf_forward_split into given buffers: udf [P] or [P,1], feat [P, d_out - 1], grad [P,3] or None; ctx is the
+    context buffer (scratch when there is no backward)."""
+    L.check(L.lib().nudf_udf_forward_split(ctypes.byref(handle.desc), L.ptr(handle.wfold), L.ptr(pts), pts.shape[0], L.ptr(udf),
+                                           L.ptr(feat), feat.shape[1], L.ptr(grad), L.ptr(ctx), L.stream_ptr()),
             "nudf_udf_forward_split")
 
 
 def color_forward_into(handle, pts, dirs, samples_per_ray, feat, cb, c, bl, ctx):
-    lib = L.lib()
-    handle.refresh()
-    L.check(lib.nudf_color_forward(ctypes.byref(handle.desc), L.ptr(handle.wfold), L.ptr(pts), L.ptr(dirs),
-                                   int(samples_per_ray), L.ptr(feat), feat.stride(0), pts.shape[0], L.ptr(cb), L.ptr(c),
-                                   L.ptr(bl), L.ptr(ctx), L.stream_ptr()), "nudf_color_forward")
+    L.check(L.lib().nudf_color_forward(ctypes.byref(handle.desc), L.ptr(handle.wfold), L.ptr(pts), L.ptr(dirs),
+                                       int(samples_per_ray), L.ptr(feat), feat.stride(0), pts.shape[0], L.ptr(cb), L.ptr(c),
+                                       L.ptr(bl), L.ptr(ctx), L.stream_ptr()), "nudf_color_forward")
 
 
-def nerf_forward_into(handle, pts, dirs, samples_per_ray, sigma, rgb, ctx):
-    lib = L.lib()
-    L.check(lib.nudf_nerf_forward(ctypes.byref(handle.desc()), L.ptr(handle.images()), L.ptr(pts), L.ptr(dirs),
-                                  int(samples_per_ray), pts.shape[0], L.ptr(sigma), L.ptr(rgb), L.ptr(ctx), L.stream_ptr()),
-            "nudf_nerf_forward")
+def nerf_forward_into(desc, wimg, pts, dirs, samples_per_ray, sigma, rgb, ctx):
+    """desc, wimg: NerfHandle.desc() and .images() (None: exact-fp32 engine)"""
+    L.check(L.lib().nudf_nerf_forward(ctypes.byref(desc), L.ptr(wimg), L.ptr(pts), L.ptr(dirs), int(samples_per_ray),
+                                      pts.shape[0], L.ptr(sigma), L.ptr(rgb), L.ptr(ctx), L.stream_ptr()), "nudf_nerf_forward")
 
 
 def view_composite(cfg, heads, rays_d, pts, mid, dists, udf, grads, sc, c_pix, bg_alpha, bg_color, rot, outs):
@@ -771,84 +743,18 @@ def view_composite(cfg, heads, rays_d, pts, mid, dists, udf, grads, sc, c_pix, b
                                          L.ptr(bg_color), r9, ctypes.byref(ro), L.stream_ptr()), "nudf_render_view_forward")
 
 
-class ViewWorkspace:
-    """One fp32 buffer holding every array of one chunk of the forward-only view pipeline (render.render_view).
-
-    The network forwards keep no state for a backward pass, so their context buffers are scratch: the UDF, colour and
-    NeRF++ forwards (and the sampling stage's UDF value queries) share one region sized for the largest of them.  The
-    chunk size is the largest ray count whose arrays fit `budget_bytes`, from the library's nudf_*_ctx_floats queries."""
-
-    def __init__(self, renderer, n_rays, budget_bytes, device, n_views=0):
-        lib = L.lib()
-        udf_h = renderer.udf_network._handle
-        udf_h.refresh()
-        col_h = renderer.color_network._handle
-        col_h.refresh()
-        self.S0, self.S = renderer.n_samples, renderer.n_samples + renderer.n_importance
-        self.O = renderer.n_outside
-        self.F = udf_h.meta[2] - 1
-        self.nb = col_h.meta[3]
-        self.blend = n_views > 0
-        # NeRF++ columns evaluated per ray: all S+O when the pixel blend needs the inside columns too (render() does the same)
-        self.m = (self.S + self.O if self.blend else self.O) if self.O > 0 else 0
-        nerf_d = renderer.nerf._handle.desc() if self.O > 0 else None
-        S, SO, m = self.S, self.S + self.O, self.m
-
-        def ctx(n):
-            c = [lib.nudf_udf_ctx_floats(ctypes.byref(udf_h.desc), n * S, 1),
-                 lib.nudf_udf_ctx_floats(ctypes.byref(udf_h.desc), n * self.S0, 0),
-                 lib.nudf_color_ctx_floats(ctypes.byref(col_h.desc), n * S)]
-            if m:
-                c.append(lib.nudf_nerf_ctx_floats(ctypes.byref(nerf_d), n * m))
-            return max(c)
-
-        # per ray: pts, mid, dists, udf, feat, grad, cb, c, logits (+ c_pix) of S samples; NeRF++ inputs / outputs of m
-        # columns and the [S+O] background arrays; sampling and z-sorting temporaries (z, udf, points of each round)
-        self._per_ray = (S * (3 + 1 + 1 + 1 + self.F + 3 + 3 + 3 + self.nb + (3 if self.blend else 0))
-                         + m * (4 + 1 + 1 + 3) + SO * (1 + 3) + 8 * SO)
-        self._ctx = ctx
-        # the sampling stage's UDF value queries allocate their own scratch while the workspace is live: counted twice
-        total = lambda n: n * self._per_ray + 2 * ctx(n)
-        probe = min(4096, n_rays)
-        n = max(1, min(n_rays, int(budget_bytes // 4 * probe // total(probe))))
-        while n > 1 and total(n) * 4 > budget_bytes:
-            n = max(1, n * 15 // 16)
-        self.chunk = n
-        self.buf = torch.empty(n * (self._per_ray - 8 * SO) + ctx(n) + 64 * 16, dtype=torch.float32, device=device)
-
-    def carve(self, n):
-        """views of the workspace for a chunk of n <= self.chunk rays"""
-        S, SO, m = self.S, self.S + self.O, self.m
-        off = [0]
-        buf = self.buf
-
-        def take(*shape):             # every array starts on a 256-byte boundary (vector loads in the kernels)
-            k = 1
-            for s in shape:
-                k *= s
-            t = buf[off[0]:off[0] + k].view(*shape)
-            off[0] += -(-k // 64) * 64
-            return t
-        w = {"pts": take(n * S, 3), "mid": take(n, S), "dists": take(n, S), "udf": take(n * S), "feat": take(n * S, self.F),
-             "grad": take(n * S, 3), "cb": take(n * S, 3), "c": take(n * S, 3), "bl": take(n * S, self.nb)}
-        if self.blend:
-            w["c_pix"] = take(n * S, 3)
-        if m:
-            w.update(pts4=take(n * m, 4), odists=take(n, m), sigma=take(n * m, 1), rgb=take(n * m, 3), bg_alpha=take(n, SO),
-                     bg_color=take(n, SO, 3))
-        w["ctx"] = buf[off[0]:]
-        assert w["ctx"].numel() >= self._ctx(n)
-        return w
+def blend_forward_into(cfg, pts, proj, hom, px, imgs, logits, c_pix, c_pat, m_pat):
+    """nudf_blend_forward; hom / px / c_pat / m_pat None = no patches"""
+    L.check(L.lib().nudf_blend_forward(ctypes.byref(cfg), L.ptr(pts), L.ptr(proj), L.ptr(hom), L.ptr(px), L.ptr(imgs), L.ptr(logits),
+                                       logits.stride(0), L.ptr(c_pix), L.ptr(c_pat), L.ptr(m_pat), L.stream_ptr()),
+            "nudf_blend_forward")
 
 
 def blend_pixels_into(pts, proj, imgs, logits, n_rays, n_samples, c_pix):
-    """nudf_blend_forward without patches (hom = NULL): pixel-blend colour c_pix [P,3] of every sample.  Pixel blending
-    does not depend on the patch size, so this serves any h_patch_size."""
-    lib = L.lib()
+    """The pixel-blend colour c_pix [P,3] of every sample, without patches.  Pixel blending does not depend on the patch
+    size, so this serves any h_patch_size."""
     V, _, H, W = imgs.shape
-    cfg = L.BlendCfg(n_rays, n_samples, V, H, W, 0)
-    L.check(lib.nudf_blend_forward(ctypes.byref(cfg), L.ptr(pts), L.ptr(proj), None, None, L.ptr(imgs), L.ptr(logits),
-                                   logits.stride(0), L.ptr(c_pix), None, None, L.stream_ptr()), "nudf_blend_forward")
+    blend_forward_into(L.BlendCfg(n_rays, n_samples, V, H, W, 0), pts, proj, None, None, imgs, logits, c_pix, None, None)
 
 
 def ray_points_into(rays_o, rays_d, z_vals, sample_dist, pts, mid, dists):

@@ -3,7 +3,7 @@
 
 `render_view` renders an [H, W] grid of rays chunk by chunk.  Each chunk runs the sampling of `render()` and then the
 UDF, colour and NeRF++ forwards, the pixel blend and `nudf_render_view_forward` (csrc/ray_kernels.cu) outside autograd,
-with every per-chunk array carved from one workspace (ops.ViewWorkspace) and no host read.  The compositing is the same
+with every per-chunk array carved from one workspace (ViewWorkspace) and no host read.  The compositing is the same
 device code as render_core's, so `color` and `depth` equal `render()`'s bit for bit on the same rays.
 
 Deviations from the runner (INTEGRATION.md "Rendering views"):
@@ -18,6 +18,7 @@ Deviations from the runner (INTEGRATION.md "Rendering views"):
 `load_scan` restates the reference's DTU-layout `Dataset` (downsample_factor 1), `rays_between` its `gen_rays_between`,
 and `python -m neuraludf_b200.render` renders a checkpoint's views into the runner's file layout.
 """
+import ctypes
 import glob
 import os
 
@@ -36,6 +37,76 @@ def _heads(renderer, device):
     beta = renderer.beta_network.get_beta().clip(1e-6, 1e6)
     gamma = renderer.beta_network.get_gamma().clip(1e-6, 1e6)
     return torch.cat([inv_s.reshape(1), beta.reshape(1), gamma.reshape(1)]).float().contiguous()
+
+
+class ViewWorkspace:
+    """One fp32 buffer holding every array of one chunk of the forward-only view pipeline (render.render_view).
+
+    The network forwards keep no state for a backward pass, so their context buffers are scratch: the UDF, colour and
+    NeRF++ forwards (and the sampling stage's UDF value queries) share one region sized for the largest of them.  The
+    chunk size is the largest ray count whose arrays fit `budget_bytes`, from the library's nudf_*_ctx_floats queries."""
+
+    def __init__(self, renderer, n_rays, budget_bytes, device, n_views=0):
+        lib = L.lib()
+        udf_h = renderer.udf_network._handle
+        udf_h.refresh()
+        col_h = renderer.color_network._handle
+        col_h.refresh()
+        self.S0, self.S = renderer.n_samples, renderer.n_samples + renderer.n_importance
+        self.O = renderer.n_outside
+        self.F = udf_h.meta[2] - 1
+        self.nb = col_h.meta[3]
+        self.blend = n_views > 0
+        # NeRF++ columns evaluated per ray: all S+O when the pixel blend needs the inside columns too (render() does the same)
+        self.m = (self.S + self.O if self.blend else self.O) if self.O > 0 else 0
+        nerf_d = renderer.nerf._handle.desc() if self.O > 0 else None
+        S, SO, m = self.S, self.S + self.O, self.m
+
+        def ctx(n):
+            c = [lib.nudf_udf_ctx_floats(ctypes.byref(udf_h.desc), n * S, 1),
+                 lib.nudf_udf_ctx_floats(ctypes.byref(udf_h.desc), n * self.S0, 0),
+                 lib.nudf_color_ctx_floats(ctypes.byref(col_h.desc), n * S)]
+            if m:
+                c.append(lib.nudf_nerf_ctx_floats(ctypes.byref(nerf_d), n * m))
+            return max(c)
+
+        # per ray: pts, mid, dists, udf, feat, grad, cb, c, logits (+ c_pix) of S samples; NeRF++ inputs / outputs of m
+        # columns and the [S+O] background arrays; sampling and z-sorting temporaries (z, udf, points of each round)
+        self._per_ray = (S * (3 + 1 + 1 + 1 + self.F + 3 + 3 + 3 + self.nb + (3 if self.blend else 0))
+                         + m * (4 + 1 + 1 + 3) + SO * (1 + 3) + 8 * SO)
+        self._ctx = ctx
+        # the sampling stage's UDF value queries allocate their own scratch while the workspace is live: counted twice
+        total = lambda n: n * self._per_ray + 2 * ctx(n)
+        probe = min(4096, n_rays)
+        n = max(1, min(n_rays, int(budget_bytes // 4 * probe // total(probe))))
+        while n > 1 and total(n) * 4 > budget_bytes:
+            n = max(1, n * 15 // 16)
+        self.chunk = n
+        self.buf = torch.empty(n * (self._per_ray - 8 * SO) + ctx(n) + 64 * 16, dtype=torch.float32, device=device)
+
+    def carve(self, n):
+        """views of the workspace for a chunk of n <= self.chunk rays"""
+        S, SO, m = self.S, self.S + self.O, self.m
+        off = [0]
+        buf = self.buf
+
+        def take(*shape):             # every array starts on a 256-byte boundary (vector loads in the kernels)
+            k = 1
+            for s in shape:
+                k *= s
+            t = buf[off[0]:off[0] + k].view(*shape)
+            off[0] += -(-k // 64) * 64
+            return t
+        w = {"pts": take(n * S, 3), "mid": take(n, S), "dists": take(n, S), "udf": take(n * S), "feat": take(n * S, self.F),
+             "grad": take(n * S, 3), "cb": take(n * S, 3), "c": take(n * S, 3), "bl": take(n * S, self.nb)}
+        if self.blend:
+            w["c_pix"] = take(n * S, 3)
+        if m:
+            w.update(pts4=take(n * m, 4), odists=take(n, m), sigma=take(n * m, 1), rgb=take(n * m, 3), bg_alpha=take(n, SO),
+                     bg_color=take(n, SO, 3))
+        w["ctx"] = buf[off[0]:]
+        assert w["ctx"].numel() >= self._ctx(n)
+        return w
 
 
 @torch.no_grad()
@@ -81,7 +152,7 @@ def render_view(renderer, rays_o, rays_d, near, far, *, color_maps=None, w2cs=No
         n_views = color_maps.shape[0]
         proj = (intrinsics[:, :3, :3] @ w2cs[:, :3, :]).reshape(n_views, 12).float().contiguous()
         imgs = color_maps.float().contiguous()
-    ws = ops.ViewWorkspace(renderer, N, workspace_bytes, dev, n_views)
+    ws = ViewWorkspace(renderer, N, workspace_bytes, dev, n_views)
     chunk = ws.chunk if max_chunk is None else max(1, min(ws.chunk, int(max_chunk)))
 
     f = lambda c: torch.empty(N, c, dtype=torch.float32, device=dev)
@@ -125,13 +196,15 @@ def render_view(renderer, rays_o, rays_d, near, far, *, color_maps=None, w2cs=No
             col0 = 0 if blend else S
             m = S + O - col0
             ops.outside_points_into(oc, dc, z_feed, col0, sample_dist, w["pts4"], w["odists"])
-            ops.nerf_forward_into(nerf_h, w["pts4"], dc, m, w["sigma"], w["rgb"], w["ctx"])
+            ops.nerf_forward_into(nerf_h.desc(), nerf_h.images(), w["pts4"], dc, m, w["sigma"], w["rgb"], w["ctx"])
             bg_alpha, bg_color = w["bg_alpha"], w["bg_color"]
             bg_alpha[:, col0:] = 1.0 - torch.exp(-torch.nn.functional.relu(w["sigma"].reshape(n, m)) * w["odists"])
             bg_color[:, col0:] = w["rgb"].reshape(n, m, 3)
         # ---- fine pass ----
         ops.ray_points_into(oc, dc, z, sample_dist, w["pts"], w["mid"], w["dists"])
+        udf_h.refresh()
         ops.udf_forward_split_into(udf_h, w["pts"], w["udf"], w["feat"], w["grad"], w["ctx"])
+        col_h.refresh()
         ops.color_forward_into(col_h, w["pts"], dc, S, w["feat"], w["cb"], w["c"], w["bl"], w["ctx"])
         c_pix = None
         if blend:

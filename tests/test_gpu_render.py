@@ -95,7 +95,7 @@ def test_render_view_workspace_budget(golden, scan):
     peak = torch.cuda.max_memory_allocated() - base
     report("render_view.memory", peak=peak, budget=budget, images=images)
     assert peak <= budget + images, (peak, budget, images)
-    ws = R.ops.ViewWorkspace(ren, rays_o.shape[0] * rays_o.shape[1], budget, rays_o.device, 8)
+    ws = R.ViewWorkspace(ren, rays_o.shape[0] * rays_o.shape[1], budget, rays_o.device, 8)
     assert ws.chunk < rays_o.shape[0] * rays_o.shape[1]           # the budget forces several chunks
 
 
