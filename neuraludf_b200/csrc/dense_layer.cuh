@@ -10,6 +10,13 @@ namespace nudf {
 // 2 planes (gradient chains).  A network names the ones its launches read as bits 1 << IMG_*.
 enum { IMG_NT2 = 0, IMG_NT3 = 1, IMG_NN2 = 2, IMG_KINDS = 3, IMG_ALL = (1 << IMG_KINDS) - 1 };
 
+// The fold and prepare job lists take every layer of a network in one launch and are filled without a bounds check.  The
+// colour network is the largest: two stacks of up to NUDF_MAX_LAYERS layers, each layer with at most two images (NT3, NN2).
+// The UDF network needs at most 3 NUDF_MAX_LAYERS images, NeRF++ at most 2 (NUDF_MAX_LAYERS + 4).
+static_assert(NUDF_MAX_JOBS >= 2 * NUDF_MAX_LAYERS, "FoldJobs must hold both stacks of the deepest colour network");
+static_assert(sizeof(tc::PrepWJobs::j) / sizeof(tc::PrepWJob) >= 4 * NUDF_MAX_LAYERS,
+              "PrepWJobs must hold every image of the deepest colour network");
+
 struct DenseLayer {
   int n_out, n_in;
   int64_t ldw;                  // W is [n_out, ldw]

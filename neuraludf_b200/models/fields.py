@@ -150,6 +150,11 @@ class ResidualRenderingNetwork(nn.Module):
             raise NotImplementedError("weight_norm=False is not supported by the CUDA path")
         if not squeeze_out:
             raise NotImplementedError("squeeze_out=False is not supported")
+        if d_in != 6:
+            # mode 'no_normal' feeds cat([points, feature]) (3 + d_feature wide) to lin_base0, which the reference sizes
+            # d_in - 3 + d_feature: any other d_in is a shape error there, and would fold garbage here
+            raise NotImplementedError("ResidualRenderingNetwork mode 'no_normal' needs d_in = 6 (points + view "
+                                      "direction), got d_in=%d" % (d_in,))
         self.mode = mode
         self.squeeze_out = squeeze_out
         self.d_out = d_out

@@ -275,6 +275,7 @@ class ColorHandle:
         self.base, self.main = base_layers, main_layers
         self.meta = (d_feature, d_hidden, d_out, n_blend, multires_view)
         self._key = None
+        self._checked = None         # the parameter pointers whose shapes _check_shapes() accepted
         self.desc = None
         self.wfold = None
         self.grad_sink = None
@@ -302,14 +303,39 @@ class ColorHandle:
         if d is not None:
             self.desc = d
 
+    def layer_shapes(self):
+        """[(n_out, n_in)] of the base layers, then of the main layers, as nudf_color_fold_weights reads them"""
+        F, H, d_out, n_blend, Lv = self.meta
+        n_lin = len(self.base)
+        d_view = 3 * (1 + 2 * Lv)
+        out = lambda l, head: H if l < n_lin - 1 else head
+        return ([(out(l, d_out), 3 + F if l == 0 else H) for l in range(n_lin)] +
+                [(out(l, d_out + n_blend), d_view + d_out + H if l == 0 else H) for l in range(n_lin)])
+
+    def _check_shapes(self):
+        """every parameter has the shape nudf_color_fold_weights reads it with: any other would be folded with the wrong row
+        length"""
+        if len(self.main) != len(self.base):
+            raise RuntimeError("colour network: %d main layers but %d base layers" % (len(self.main), len(self.base)))
+        nb = len(self.base)
+        for l, (m, (n_out, n_in)) in enumerate(zip(list(self.base) + list(self.main), self.layer_shapes())):
+            if m.weight_v.shape != (n_out, n_in) or m.weight_g.shape != (n_out, 1) or m.bias.shape != (n_out,):
+                raise RuntimeError("colour network %s: weight_v %s, weight_g %s, bias %s; the library plans [%d, %d]" % (
+                    "lin_base%d" % l if l < nb else "lin%d" % (l - nb), tuple(m.weight_v.shape), tuple(m.weight_g.shape),
+                    tuple(m.bias.shape), n_out, n_in))
+
     def _make_desc(self):
+        mods = list(self.base) + list(self.main)
+        ptrs = tuple(t.data_ptr() for m in mods for t in (m.weight_g, m.weight_v, m.bias))
+        if ptrs != self._checked:                 # the shapes can only have changed with the tensors
+            self._check_shapes()
+            self._checked = ptrs
         d = L.ColorDesc()
-        d.n_lin = len(self.base)
+        n = d.n_lin = len(self.base)
         d.d_feature, d.d_hidden, d.d_out, d.n_blend, d.multires_view = self.meta
-        for l, m in enumerate(self.base):
-            d.base_g[l], d.base_v[l], d.base_b[l] = m.weight_g.data_ptr(), m.weight_v.data_ptr(), m.bias.data_ptr()
-        for l, m in enumerate(self.main):
-            d.main_g[l], d.main_v[l], d.main_b[l] = m.weight_g.data_ptr(), m.weight_v.data_ptr(), m.bias.data_ptr()
+        for l in range(n):
+            d.base_g[l], d.base_v[l], d.base_b[l] = ptrs[3 * l:3 * l + 3]
+            d.main_g[l], d.main_v[l], d.main_b[l] = ptrs[3 * (n + l):3 * (n + l) + 3]
         return d
 
 
@@ -378,6 +404,7 @@ class NerfHandle:
         self.m = module
         self.meta = (D, W, d_in, multires, multires_view, skip)
         self._key = None
+        self._checked = None         # the parameter pointers whose shapes desc() accepted
         self.wfold = None            # NeRF++ has plain weights: the buffer holds the weight images only
         self.grad_sink = None
 
@@ -402,16 +429,33 @@ class NerfHandle:
             ps += [lin.weight, lin.bias]
         return ps
 
+    def layer_shapes(self):
+        """[(module, (n_out, n_in))] of every layer, in params() order, as nudf_nerf_forward / _backward read the plain
+        nn.Linear weights"""
+        D, W, d_in, multires, multires_view, skip = self.meta
+        ch, chv = d_in * (1 + 2 * multires), 3 * (1 + 2 * multires_view)
+        m = self.m
+        shapes = [(lin, (W, ch if i == 0 else (W + ch if i - 1 == skip else W))) for i, lin in enumerate(m.pts_linears)]
+        return shapes + [(m.views_linears[0], (W // 2, W + chv)), (m.feature_linear, (W, W)), (m.alpha_linear, (1, W)),
+                         (m.rgb_linear, (3, W // 2))]
+
     def desc(self):
         m = self.m
+        ptrs = tuple(t.data_ptr() for t in self.params())
+        if ptrs != self._checked:                 # the shapes can only have changed with the tensors
+            if len(m.pts_linears) != self.meta[0]:
+                raise RuntimeError("NeRF: %d pts_linears for D = %d" % (len(m.pts_linears), self.meta[0]))
+            for lin, (n_out, n_in) in self.layer_shapes():
+                if lin.weight.shape != (n_out, n_in) or lin.bias.shape != (n_out,):
+                    raise RuntimeError("NeRF layer of weight %s / bias %s; the library plans [%d, %d]" % (
+                        tuple(lin.weight.shape), tuple(lin.bias.shape), n_out, n_in))
+            self._checked = ptrs
         d = L.NerfDesc()
         d.D, d.W, d.d_in, d.multires, d.multires_view, d.skip = self.meta
-        for i, lin in enumerate(m.pts_linears):
-            d.pts_w[i], d.pts_b[i] = lin.weight.data_ptr(), lin.bias.data_ptr()
-        d.views_w, d.views_b = m.views_linears[0].weight.data_ptr(), m.views_linears[0].bias.data_ptr()
-        d.feature_w, d.feature_b = m.feature_linear.weight.data_ptr(), m.feature_linear.bias.data_ptr()
-        d.alpha_w, d.alpha_b = m.alpha_linear.weight.data_ptr(), m.alpha_linear.bias.data_ptr()
-        d.rgb_w, d.rgb_b = m.rgb_linear.weight.data_ptr(), m.rgb_linear.bias.data_ptr()
+        D = len(m.pts_linears)
+        for i in range(D):
+            d.pts_w[i], d.pts_b[i] = ptrs[2 * i:2 * i + 2]
+        d.views_w, d.views_b, d.feature_w, d.feature_b, d.alpha_w, d.alpha_b, d.rgb_w, d.rgb_b = ptrs[2 * D:]
         return d
 
 
