@@ -119,7 +119,7 @@ struct Bump {
   int64_t take(int64_t n) { int64_t o = off; off += round_up(n, 4); return o; }
 };
 
-__device__ __forceinline__ bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
+__host__ __device__ __forceinline__ bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
 // ---- weight-norm fold / unfold of ALL layers of a network in one launch ------------------------------------------------------
 // W = g v / ||v||  (row-wise; torch._weight_norm(v, g, dim=0), reference models/fields.py:110-113) and its adjoint

@@ -7,6 +7,8 @@
 // through shared memory to the fused epilogue functor (4 consecutive columns of a row per call: coalesced).  WN = 256 for
 // 2-plane layers wider than 128 columns, so that each activation row block is read from HBM and split into planes once.
 #pragma once
+#include <cuda.h>
+#include <cudaTypedefs.h>
 #include <cuda_bf16.h>
 
 #include "gemm_simt.cuh"
@@ -29,6 +31,22 @@ __host__ __device__ inline int pad64(int k) { return (k + 63) & ~63; }
 // byte offset of element (row, k) inside a [rows x 64] bf16 K-major SWIZZLE_128B tile (tile base 1024-aligned)
 __host__ __device__ inline uint32_t sw128(uint32_t row, uint32_t k) {
   return (row >> 3) * 1024u + (row & 7u) * 128u + ((((k >> 3) ^ (row & 7u)) & 7u) << 4) + ((k & 7u) << 1);
+}
+
+// gemm_tn_kernel's ring path: slices of TN_PS points, fp32 operand blocks as they lie in HBM ([point][128 columns]) in a
+// TN_RING-deep ring, and a double-buffered stage of bf16 planes (hi, lo of A, then of B)
+constexpr int TN_PS = 32;
+constexpr int TN_RING = 4;
+constexpr uint32_t TN_F32_OPND = TN_PS * BM * 4;            // 16 KB: one operand's [32 x 128] fp32 block
+constexpr uint32_t TN_F32_STAGE = 2 * TN_F32_OPND;          // A, then B
+constexpr uint32_t TN_PLANE = BM * TN_PS * 2;               // 8 KB: one bf16 plane of one operand
+constexpr uint32_t TN_PLANE_STAGE = 4 * TN_PLANE;
+struct TnMaps { CUtensorMap a, b; };                         // the ring path's 2-D tensor maps of A and B
+// byte offset of element (mn, k) inside a [128 x 32] bf16 MN-major SWIZZLE_128B plane (base 1024-aligned): two 64-wide
+// MN blocks of 4 KB, each four 1 KB atoms of 8 points x 128 B; the 16-byte chunk index is XOR-ed with the point's row
+// in its atom, as the hardware's 128B swizzle does with address bits 4-6 and 7-9
+__host__ __device__ inline uint32_t sw128_mn(uint32_t mn, uint32_t k) {
+  return (mn >> 6) * 4096u + (k >> 3) * 1024u + (k & 7u) * 128u + ((((mn >> 3) ^ k) & 7u) << 4) + ((mn & 7u) << 1);
 }
 
 __device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
@@ -138,10 +156,24 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, u
                : "memory");
 }
 
+// the [TN_PS x 128] fp32 box at (column c, point k) of a 2-D tensor map into shared memory, on an mbarrier
+__device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* map, int c, int k, uint64_t* bar) {
+  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
+               ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(c), "r"(k), "r"(smem_u32(bar))
+               : "memory");
+}
+
 // wgmma smem descriptor of a K-major operand: start, LBO, SBO (16-byte units), bits 62-63 = 1 (SWIZZLE_128B); SBO = 1024 B
 // (8-row atoms)
 __device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
   return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 62);
+}
+// wgmma smem descriptor of an MN-major SWIZZLE_128B operand in gemm_tn_kernel's plane layout (sw128_mn).  The PTX ISA's
+// canonical MN-major 128B-swizzle layout is ((8 x 16 B, m), (8, k)) : ((contiguous, LBO), (128 B, SBO)): an atom is 8
+// K rows of 128 contiguous bytes (64 bf16 along M or N), LBO is the step between 64-wide MN blocks (4096 B here, used
+// by B's 128 columns) and SBO the step between 8-point K groups (1024 B: the atoms of a block are consecutive).
+__device__ __forceinline__ uint64_t make_desc_mn(uint32_t smem_addr) {
+  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)(4096 >> 4) << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
 }
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
@@ -157,7 +189,9 @@ __device__ __forceinline__ void fence_operand(float (&d)[N]) {
 // moved to the middle of its truncation interval
 __device__ __forceinline__ float unbias_rz(float r) { return fmaf(__uint_as_float(__float_as_uint(r) & 0xff800000u), 0x1p-24f, r); }
 
-// D[64 x 128] (+)= A[64 x 16] B[128 x 16]^T from shared memory (both K-major), bf16 operands
+// D[64 x 128] (+)= A[64 x 16] B[128 x 16]^T from shared memory, bf16 operands; both K-major (MN_MAJOR = 0) or both
+// MN-major (1: the transpose immediates of A and B set, descriptors from make_desc_mn)
+template <int MN_MAJOR = 0>
 __device__ __forceinline__ void wgmma_128(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
   asm volatile(
       "{\n"
@@ -166,7 +200,7 @@ __device__ __forceinline__ void wgmma_128(float (&d)[64], uint64_t da, uint64_t 
       "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
       "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, "
       "%26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, "
-      "%50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n"
+      "%50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %67;\n"
       "}\n"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
         "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
@@ -175,7 +209,7 @@ __device__ __forceinline__ void wgmma_128(float (&d)[64], uint64_t da, uint64_t 
         "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]),
         "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]),
         "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-      : "l"(da), "l"(db), "r"(accumulate));
+      : "l"(da), "l"(db), "r"(accumulate), "n"(MN_MAJOR));
 }
 // D[64 x 128] = A[64 x 16] B[128 x 16]^T into fresh registers: write-only outputs, so that the compiler keeps no
 // earlier value of d alive
@@ -258,6 +292,18 @@ __device__ __forceinline__ void mma_slice(float (&d)[WN / 2], uint32_t a, uint32
       wgmma_n<WN>(d, desc(a, a_stride, 1, j), desc(b, b_stride, 0, j), 1u);     // mid * hi
       wgmma_n<WN>(d, desc(a, a_stride, 0, j), desc(b, b_stride, 1, j), 1u);     // hi * mid
     }
+  }
+}
+// The wgmma group of one TN_PS-point slice of gemm_tn_kernel's ring path: MN-major planes (lo at +TN_PLANE), 2 KB per
+// 16-point step, the products of each step in mma_slice<2>'s order
+__device__ __forceinline__ void mma_slice_mn(float (&d)[64], uint32_t a, uint32_t b, bool zero_first) {
+#pragma unroll
+  for (int j = 0; j < TN_PS / 16; ++j) {
+    const uint32_t acc0 = (zero_first && j == 0) ? 0u : 1u;
+    const uint32_t aj = a + 2048u * j, bj = b + 2048u * j;
+    wgmma_128<1>(d, make_desc_mn(aj + TN_PLANE), make_desc_mn(bj), acc0);
+    wgmma_128<1>(d, make_desc_mn(aj), make_desc_mn(bj + TN_PLANE), 1u);
+    wgmma_128<1>(d, make_desc_mn(aj), make_desc_mn(bj), 1u);
   }
 }
 
@@ -520,87 +566,181 @@ gemm_w_kernel(const float* __restrict__ A, int64_t lda, int64_t M, int N, int K,
 // ---------------------------------------------------------------------------------------------------------------
 // C[M x N] += A[K x M]^T B[K x N]  (weight gradients; contraction over points, split over gridDim.z), row-major operands.
 // grid = (ceil(M/128), ceil(N/128), splits).  Epi is the caller's epilogue with one split, EpiSplitStore into the split-K
-// workspace with several.  Warps 0-3 stage the [128 x 64] A^T slice, warps 4-7 the B^T slice (fetch_block_t /
-// store_block_t).  Slice i + 1 waits in registers while the tensor cores work on slice i: iteration i issues the wgmma
-// group of slice i, splits slice i + 1 into the free stage, issues the loads of slice i + 2, then waits for the group.
-// colsum (optional): colsum[m] += sum_k A[k, m], the bias gradient, from the values the A stagers hold anyway; one writer
-// per column and split (cs_ws: [split][M], or the output itself with one split).
+// workspace with several.  colsum (optional): colsum[m] += sum_k A[k, m], the bias gradient, from the fp32 values the A
+// stagers read anyway; one writer per column and split (cs_ws: [split][M], or the output itself with one split).
+// Both paths keep each column's sum in the same order: per k-quarter partials (points 8q + 2kq, 8q + 2kq + 1 of each
+// 64 points, pairs added first, in point order), then (q0 + q1) + (q2 + q3).
+//
+// RING (row strides a multiple of 4 floats and 16-byte-aligned bases, as 2-D tensor maps need): the operands reach
+// shared memory as they lie in HBM.  One thread issues a 2-D TMA copy per operand and slice (a [TN_PS points x 128
+// columns] fp32 box, 16 KB; columns past M / N and points past K arrive as zeros) into a TN_RING-deep ring on an
+// mbarrier, and refills a stage as soon as the barrier after its split has passed: up to TN_RING - 1 slices are in
+// flight per CTA beyond the one being split, in no registers.  While the wgmma group of slice i runs, all threads split
+// slice i + 1 into the free MN-major plane stage (warps 0-3 A, warps 4-7 B; warp w takes k-quarter kq = w & 3 of each 8
+// points, lane l columns 4l..4l+3), and the wgmma reads both operands with its transpose flags set.  Points of the
+// last slice past the chunk end (the next chunk's) are split as zeros.
+// Otherwise warps 0-3 stage the [128 x 64] A^T slice, warps 4-7 the B^T slice (fetch_block_t / store_block_t), K-major.
+// Slice i + 1 waits in registers while the tensor cores work on slice i: iteration i issues the wgmma group of slice i,
+// splits slice i + 1 into the free stage, issues the loads of slice i + 2, then waits for the group.
 // ---------------------------------------------------------------------------------------------------------------
-template <class Epi>
+template <class Epi, bool RING>
 __global__ void __launch_bounds__(THREADS, 1)
 gemm_tn_kernel(const float* __restrict__ A, int64_t lda, const float* __restrict__ B, int64_t ldb, int M, int N, int64_t K, int64_t k_chunk,
-               Epi epi, float* __restrict__ colsum, float* __restrict__ cs_ws) {
+               Epi epi, float* __restrict__ colsum, float* __restrict__ cs_ws, const __grid_constant__ TnMaps maps) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = align1024(smem_raw);
   const int tid = threadIdx.x, wg = tid >> 7, warp = tid >> 5, lane = tid & 31;
   const int m0 = blockIdx.x * BM;
   const int n0 = blockIdx.y * BN;
-  int rows_b = N - n0; rows_b = pad16(rows_b < BN ? rows_b : BN);
   const int64_t kb = (int64_t)blockIdx.z * k_chunk;
   const int64_t ke = (kb + k_chunk < K) ? kb + k_chunk : K;
-  const int n_sl = ke > kb ? (int)((ke - kb + BK - 1) / BK) : 0;
-  constexpr uint32_t stage_bytes = 2u * A_HALF_BYTES + 2u * B_HALF_BYTES;
   const bool do_csum = colsum != nullptr && blockIdx.y == 0;
-  const bool a_vec = ((lda & 3) == 0) && aligned16(A) && ((m0 & 3) == 0);
-  const bool b_vec = ((ldb & 3) == 0) && aligned16(B);
-  const bool b_warp = warp >= 4 && 32 * (warp - 4) < rows_b;
   float csum[4] = {0.f, 0.f, 0.f, 0.f};
-  float4 v[8][2];                                           // this thread's part of the next K slice
-
-  auto fetch = [&](int i) {                                 // K slice i into v
-    const int64_t k0 = kb + (int64_t)i * BK;
-    if (warp < 4) fetch_block_t(A, lda, m0, M, 32 * warp, BM, k0, ke, lane, a_vec, v);
-    else if (b_warp) fetch_block_t(B, ldb, n0, N, 32 * (warp - 4), rows_b, k0, ke, lane, b_vec, v);
-  };
-  auto store = [&](uint8_t* st) {                           // v into stage st
-    if (warp < 4) {
-      if (do_csum) store_block_t<true>(v, 32 * warp, BM, st, st + A_HALF_BYTES, lane, csum);
-      else store_block_t(v, 32 * warp, BM, st, st + A_HALF_BYTES, lane);
-    } else if (b_warp) {
-      store_block_t(v, 32 * (warp - 4), rows_b, st + 2 * A_HALF_BYTES, st + 2 * A_HALF_BYTES + B_HALF_BYTES, lane);
-    }
-  };
-  if (n_sl == 0) return;
-  fetch(0);
-  store(smem);
-  if (n_sl > 1) fetch(1);
-  fence_proxy_async();
-  __syncthreads();
+  if (ke <= kb) return;
   float acc[64];
 #pragma unroll
   for (int q = 0; q < 64; ++q) acc[q] = 0.f;
-  for (int i = 0; i < n_sl; ++i) {
-    const int s = i & 1;
-    const uint32_t st = smem_u32(smem + s * stage_bytes);
-    wg_fence();
-    mma_slice<2, BN>(acc, st + wg * (64 * 128), A_HALF_BYTES, st + 2 * A_HALF_BYTES, B_HALF_BYTES, i == 0);
-    wg_commit();
-    if (i + 1 < n_sl) {
-      store(smem + (s ^ 1) * stage_bytes);                  // stage s ^ 1 was released by the wait + barrier of i - 1
-      if (i + 2 < n_sl) fetch(i + 2);
+  if constexpr (RING) {
+    uint8_t* ring = smem;
+    uint8_t* planes = smem + TN_RING * TN_F32_STAGE;
+    float* cs_part = reinterpret_cast<float*>(planes + 2 * TN_PLANE_STAGE);   // [4 k-quarters][128 columns]
+    uint64_t* full = reinterpret_cast<uint64_t*>(cs_part + 4 * BM);
+    const int n_sl = (int)((ke - kb + TN_PS - 1) / TN_PS);
+    const int opnd = warp >> 2, kq = warp & 3;
+
+    auto issue = [&](int i) {                               // one thread: slice i into ring stage i % TN_RING
+      const int r = i % TN_RING;
+      const int k0 = (int)(kb + (int64_t)i * TN_PS);
+      uint8_t* st = ring + r * TN_F32_STAGE;
+      mbar_arrive_expect_tx(&full[r], TN_F32_STAGE);
+      tma_load_2d(st, &maps.a, m0, k0, &full[r]);
+      tma_load_2d(st + TN_F32_OPND, &maps.b, n0, k0, &full[r]);
+    };
+    // slice i from the ring into the plane stage dst.  Shared-memory traffic without bank conflicts: a warp's float4
+    // reads cover one point's 512 contiguous bytes, and each half-warp's 8-byte plane stores cover all 8 16-byte chunks
+    // of one 128-byte swizzled row (64 columns of one point), i.e. all 32 banks once.
+    auto split = [&](int i, uint8_t* dst) {
+      const int r = i % TN_RING;
+      mbar_wait(&full[r], (uint32_t)((i / TN_RING) & 1));
+      const float* f = reinterpret_cast<const float*>(ring + r * TN_F32_STAGE + opnd * TN_F32_OPND) + 4 * lane;
+      uint8_t* hi = dst + opnd * 2 * TN_PLANE;
+      const int64_t k0 = kb + (int64_t)i * TN_PS;
+#pragma unroll
+      for (int q = 0; q < TN_PS / 8; ++q) {
+        float4 v[2];
+#pragma unroll
+        for (int kk = 0; kk < 2; ++kk) {
+          const int p = 8 * q + 2 * kq + kk;
+          v[kk] = k0 + p < ke ? *reinterpret_cast<const float4*>(f + p * BM) : make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+        if (opnd == 0 && do_csum) {
+          csum[0] += v[0].x + v[1].x; csum[1] += v[0].y + v[1].y;
+          csum[2] += v[0].z + v[1].z; csum[3] += v[0].w + v[1].w;
+        }
+#pragma unroll
+        for (int kk = 0; kk < 2; ++kk) {
+          const float x[4] = {v[kk].x, v[kk].y, v[kk].z, v[kk].w};
+          uint2 pl[2];
+          split4<2>(x, pl);
+          const uint32_t off = sw128_mn(4u * lane, (uint32_t)(8 * q + 2 * kq + kk));
+          *reinterpret_cast<uint2*>(hi + off) = pl[0];
+          *reinterpret_cast<uint2*>(hi + TN_PLANE + off) = pl[1];
+        }
+      }
+    };
+    if (tid == 0) {
+      for (int r = 0; r < TN_RING; ++r) mbar_init(&full[r], 1);
+      fence_barrier_init();
+      for (int i = 0; i < TN_RING && i < n_sl; ++i) issue(i);
     }
-    wg_wait_all();
+    __syncthreads();
+    split(0, planes);
     fence_proxy_async();
     __syncthreads();
-  }
-  if (do_csum && warp < 4) {                                // lanes (mq, kq): reduce over the 4 kq lanes
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      csum[j] += __shfl_xor_sync(0xffffffffu, csum[j], 8);
-      csum[j] += __shfl_xor_sync(0xffffffffu, csum[j], 16);
+    if (tid == 0 && TN_RING < n_sl) issue(TN_RING);         // slice 0's ring stage is split
+    for (int i = 0; i < n_sl; ++i) {
+      const int s = i & 1;
+      const uint32_t st = smem_u32(planes + s * TN_PLANE_STAGE);
+      wg_fence();
+      mma_slice_mn(acc, st + wg * 4096u, st + 2 * TN_PLANE, i == 0);
+      wg_commit();
+      if (i + 1 < n_sl) split(i + 1, planes + (s ^ 1) * TN_PLANE_STAGE);   // released by the wait + barrier of i - 1
+      wg_wait_all();
+      fence_proxy_async();
+      __syncthreads();
+      if (tid == 0 && i + 1 + TN_RING < n_sl) issue(i + 1 + TN_RING);     // slice i + 1's ring stage is split
     }
-    const int m = m0 + 32 * warp + 4 * (lane & 7);
-    if ((lane >> 3) == 0)
+    if (do_csum && opnd == 0)
 #pragma unroll
-      for (int j = 0; j < 4; ++j)
-        if (m + j < M) {
-          if (cs_ws != nullptr) cs_ws[(int64_t)blockIdx.z * M + m + j] = csum[j];
-          else colsum[m + j] += csum[j];
-        }
+      for (int j = 0; j < 4; ++j) cs_part[kq * BM + 4 * lane + j] = csum[j];
+  } else {
+    int rows_b = N - n0; rows_b = pad16(rows_b < BN ? rows_b : BN);
+    const int n_sl = (int)((ke - kb + BK - 1) / BK);
+    constexpr uint32_t stage_bytes = 2u * A_HALF_BYTES + 2u * B_HALF_BYTES;
+    const bool a_vec = ((lda & 3) == 0) && aligned16(A) && ((m0 & 3) == 0);
+    const bool b_vec = ((ldb & 3) == 0) && aligned16(B);
+    const bool b_warp = warp >= 4 && 32 * (warp - 4) < rows_b;
+    float4 v[8][2];                                         // this thread's part of the next K slice
+
+    auto fetch = [&](int i) {                               // K slice i into v
+      const int64_t k0 = kb + (int64_t)i * BK;
+      if (warp < 4) fetch_block_t(A, lda, m0, M, 32 * warp, BM, k0, ke, lane, a_vec, v);
+      else if (b_warp) fetch_block_t(B, ldb, n0, N, 32 * (warp - 4), rows_b, k0, ke, lane, b_vec, v);
+    };
+    auto store = [&](uint8_t* st) {                         // v into stage st
+      if (warp < 4) {
+        if (do_csum) store_block_t<true>(v, 32 * warp, BM, st, st + A_HALF_BYTES, lane, csum);
+        else store_block_t(v, 32 * warp, BM, st, st + A_HALF_BYTES, lane);
+      } else if (b_warp) {
+        store_block_t(v, 32 * (warp - 4), rows_b, st + 2 * A_HALF_BYTES, st + 2 * A_HALF_BYTES + B_HALF_BYTES, lane);
+      }
+    };
+    fetch(0);
+    store(smem);
+    if (n_sl > 1) fetch(1);
+    fence_proxy_async();
+    __syncthreads();
+    for (int i = 0; i < n_sl; ++i) {
+      const int s = i & 1;
+      const uint32_t st = smem_u32(smem + s * stage_bytes);
+      wg_fence();
+      mma_slice<2, BN>(acc, st + wg * (64 * 128), A_HALF_BYTES, st + 2 * A_HALF_BYTES, B_HALF_BYTES, i == 0);
+      wg_commit();
+      if (i + 1 < n_sl) {
+        store(smem + (s ^ 1) * stage_bytes);                // stage s ^ 1 was released by the wait + barrier of i - 1
+        if (i + 2 < n_sl) fetch(i + 2);
+      }
+      wg_wait_all();
+      fence_proxy_async();
+      __syncthreads();
+    }
+    if (do_csum && warp < 4) {                              // lanes (mq, kq): reduce over the 4 kq lanes
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        csum[j] += __shfl_xor_sync(0xffffffffu, csum[j], 8);
+        csum[j] += __shfl_xor_sync(0xffffffffu, csum[j], 16);
+      }
+      const int m = m0 + 32 * warp + 4 * (lane & 7);
+      if ((lane >> 3) == 0)
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+          if (m + j < M) {
+            if (cs_ws != nullptr) cs_ws[(int64_t)blockIdx.z * M + m + j] = csum[j];
+            else colsum[m + j] += csum[j];
+          }
+    }
   }
-  float* acc_s = reinterpret_cast<float*>(smem);
+  float* acc_s = reinterpret_cast<float*>(smem);            // the operand stages (or the ring: every copy has landed)
   acc_to_smem<BN>(acc, acc_s, wg, tid & 127);
   __syncthreads();
+  if constexpr (RING) {
+    const float* cs_part = reinterpret_cast<const float*>(smem + TN_RING * TN_F32_STAGE + 2 * TN_PLANE_STAGE);
+    if (do_csum && tid < BM && m0 + tid < M) {
+      const float c = (cs_part[tid] + cs_part[BM + tid]) + (cs_part[2 * BM + tid] + cs_part[3 * BM + tid]);
+      if (cs_ws != nullptr) cs_ws[(int64_t)blockIdx.z * M + m0 + tid] = c;
+      else colsum[m0 + tid] += c;
+    }
+  }
   tile_epilogue<BN>(acc_s, m0, M, n0, N, epi, tid);
 }
 
@@ -618,6 +758,10 @@ static inline int sm_count() {
 constexpr size_t w_smem_bytes(int np, int wn) { return 2 * (size_t)np * (A_HALF_BYTES + b_plane_bytes(wn)) + 2 * sizeof(uint64_t) + 1024; }
 static_assert(BM * acc_ld(2 * BN) * sizeof(float) <= 2 * 2 * (size_t)(A_HALF_BYTES + b_plane_bytes(2 * BN)), "accumulator tile");
 constexpr size_t TN_SMEM = 2 * (size_t)(2 * A_HALF_BYTES + 2 * B_HALF_BYTES) + 2 * sizeof(uint64_t) + 1024;
+// the ring path: the fp32 ring, 2 plane stages, the k-quarter column-sum partials and one mbarrier per ring stage
+constexpr size_t TN_RING_SMEM = (size_t)TN_RING * TN_F32_STAGE + 2 * TN_PLANE_STAGE + 4 * BM * sizeof(float) + TN_RING * sizeof(uint64_t) + 1024;
+static_assert(BM * acc_ld(BN) * sizeof(float) <= (size_t)TN_RING * TN_F32_STAGE, "accumulator tile in the ring");
+static_assert(TN_RING_SMEM <= 227 * 1024, "one CTA per SM");
 
 template <int NP, int WN, class Epi>
 static inline int gemm_w_launch(const float* A, int64_t lda, int64_t M, int N, int K, const uint16_t* img, const Epi& epi, cudaStream_t st) {
@@ -657,6 +801,50 @@ static inline int64_t tn_k_chunk(int M, int N, int64_t K) {
   return round_up(cdiv(K, splits), BK);
 }
 
+// 2-D tensor map of a row-major fp32 operand [rows x cols] (row stride ld floats) in [TN_PS x 128] boxes, zero fill
+static inline int tn_tensor_map(CUtensorMap* map, const float* X, int64_t ld, int cols, int64_t rows) {
+  static PFN_cuTensorMapEncodeTiled encode = nullptr;
+  if (encode == nullptr) {
+    void* fn = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess ||
+        fn == nullptr) {
+      nudf::set_error("cuTensorMapEncodeTiled is not available from the driver");
+      return -2;
+    }
+    encode = reinterpret_cast<PFN_cuTensorMapEncodeTiled>(fn);
+  }
+  const cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+  const cuuint64_t strides[1] = {(cuuint64_t)ld * sizeof(float)};
+  const cuuint32_t box[2] = {(cuuint32_t)BM, (cuuint32_t)TN_PS};
+  const cuuint32_t elem[2] = {1, 1};
+  const CUresult r = encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(X), dims, strides, box, elem,
+                            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    nudf::set_error("cuTensorMapEncodeTiled failed (%d)", (int)r);
+    return -2;
+  }
+  return 0;
+}
+template <class Epi, bool RING>
+static inline int gemm_tn_launch(dim3 grid, const float* A, int64_t lda, const float* B, int64_t ldb, int M, int N, int64_t K,
+                                 int64_t k_chunk, const Epi& epi, float* colsum, float* cs_ws, cudaStream_t st) {
+  constexpr size_t smem = RING ? TN_RING_SMEM : TN_SMEM;
+  static bool attr_set = false;   // per template instantiation
+  if (!attr_set) {
+    NUDF_CUDA_OK(cudaFuncSetAttribute(gemm_tn_kernel<Epi, RING>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    attr_set = true;
+  }
+  TnMaps maps{};
+  if constexpr (RING) {
+    if (int rc = tn_tensor_map(&maps.a, A, lda, M, K)) return rc;
+    if (int rc = tn_tensor_map(&maps.b, B, ldb, N, K)) return rc;
+  }
+  gemm_tn_kernel<Epi, RING><<<grid, THREADS, smem, st>>>(A, lda, B, ldb, M, N, K, k_chunk, epi, colsum, cs_ws, maps);
+  NUDF_LAUNCH_OK();
+  return 0;
+}
 // C[M x N] += A[K x M]^T B[K x N] over row-major operands; colsum_a (optional) += the column sums of A
 template <class Epi>
 static inline int gemm_tn(const float* A, int64_t lda, const float* B, int64_t ldb, int M, int N, int64_t K, const Epi& epi,
@@ -666,28 +854,20 @@ static inline int gemm_tn(const float* A, int64_t lda, const float* B, int64_t l
   const int splits = (int)cdiv(K, k_chunk);
   dim3 grid((unsigned)cdiv(M, BM), (unsigned)cdiv(N, BN), (unsigned)splits);
   LaunchTimer lt_(FAM_TC_WGRAD, st);
+  // the ring path's tensor maps need row strides of whole 16-byte units and 16-byte-aligned bases
+  const bool ring = (lda & 3) == 0 && (ldb & 3) == 0 && aligned16(A) && aligned16(B);
   if (splits == 1) {
-    static bool attr_set = false;
-    if (!attr_set) {
-      NUDF_CUDA_OK(cudaFuncSetAttribute(gemm_tn_kernel<Epi>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TN_SMEM));
-      attr_set = true;
-    }
-    gemm_tn_kernel<Epi><<<grid, THREADS, TN_SMEM, st>>>(A, lda, B, ldb, M, N, K, k_chunk, epi, colsum_a, nullptr);
-    NUDF_LAUNCH_OK();
-    return 0;
+    if (ring) return gemm_tn_launch<Epi, true>(grid, A, lda, B, ldb, M, N, K, k_chunk, epi, colsum_a, nullptr, st);
+    return gemm_tn_launch<Epi, false>(grid, A, lda, B, ldb, M, N, K, k_chunk, epi, colsum_a, nullptr, st);
   }
   // deterministic split-K (gemm_simt.cuh): partial tiles and column sums go to the workspace, summed in split order
-  static bool attr_set_ws = false;
-  if (!attr_set_ws) {
-    NUDF_CUDA_OK(cudaFuncSetAttribute(gemm_tn_kernel<EpiSplitStore>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TN_SMEM));
-    attr_set_ws = true;
-  }
   float* ws = split_workspace(st);
   if (ws == nullptr) return -2;
   float* cs = ws + (int64_t)splits * M * N;
-  gemm_tn_kernel<EpiSplitStore><<<grid, THREADS, TN_SMEM, st>>>(A, lda, B, ldb, M, N, K, k_chunk, EpiSplitStore{ws, (int64_t)M * N, N},
-                                                                 colsum_a, cs);
-  NUDF_LAUNCH_OK();
+  const EpiSplitStore e{ws, (int64_t)M * N, N};
+  if (int rc = ring ? gemm_tn_launch<EpiSplitStore, true>(grid, A, lda, B, ldb, M, N, K, k_chunk, e, colsum_a, cs, st)
+                    : gemm_tn_launch<EpiSplitStore, false>(grid, A, lda, B, ldb, M, N, K, k_chunk, e, colsum_a, cs, st))
+    return rc;
   if (int rc = splitk_reduce(ws, splits, M, N, epi, st)) return rc;
   return colsum_a != nullptr ? vec_reduce(cs, splits, M, colsum_a, st) : 0;
 }
