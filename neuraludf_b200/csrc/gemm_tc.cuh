@@ -3,7 +3,8 @@
 //   products of weight >= 2^-16 (fp32-grade); x = hi + lo, hi = bf16(x), lo = bf16(x - hi) (SURVEY.md section 0, fact 3).
 // One CTA = 2 warpgroups, a 128 x WN output tile, a 2-stage shared-memory ring over 64-wide K slices: warpgroup w issues
 // wgmma.m64n{WN}k16 for rows 64w.. (K-major SWIZZLE_128B operands, fp32 accumulators in registers) while all threads stage
-// the next activation slice as bf16 planes; weight slices arrive by cp.async.bulk on an mbarrier.  The accumulators go
+// the next activation slice as bf16 planes (2-plane layers from a ring of TMA-copied fp32 slices, split in place, when
+// the operand allows it); weight slices arrive by cp.async.bulk on an mbarrier.  The accumulators go
 // through shared memory to the fused epilogue functor (4 consecutive columns of a row per call: coalesced).  WN = 256 for
 // 2-plane layers wider than 128 columns, so that each activation row block is read from HBM and split into planes once.
 #pragma once
@@ -48,6 +49,12 @@ struct TnMaps { CUtensorMap a, b; };                         // the ring path's 
 __host__ __device__ inline uint32_t sw128_mn(uint32_t mn, uint32_t k) {
   return (mn >> 6) * 4096u + (k >> 3) * 1024u + (k & 7u) * 128u + ((((mn >> 3) ^ k) & 7u) << 4) + ((mn & 7u) << 1);
 }
+
+// gemm_w_kernel's ring path (2 planes): slots of one fp32 [128 x 64] activation slice as it lies in HBM, each split in
+// place into its hi and lo planes; W_RING(WN) slots beside the two weight stages
+constexpr uint32_t W_SLOT = BM * BK * 4;                     // 32 KB
+static_assert(W_SLOT == 2 * A_HALF_BYTES, "a slot holds exactly the two bf16 planes of its slice");
+__host__ __device__ constexpr int w_ring(int wn) { return wn == 256 ? 3 : 4; }
 
 __device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
   __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
@@ -156,7 +163,7 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, u
                : "memory");
 }
 
-// the [TN_PS x 128] fp32 box at (column c, point k) of a 2-D tensor map into shared memory, on an mbarrier
+// the box of a 2-D tensor map whose first element is (column c, row k) into shared memory, on an mbarrier
 __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* map, int c, int k, uint64_t* bar) {
   asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
                ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(c), "r"(k), "r"(smem_u32(bar))
@@ -320,10 +327,16 @@ __device__ __forceinline__ void acc_to_smem(const float (&d)[WN / 2], float* acc
   }
 }
 // Fused epilogue of the [128 x WN] tile at (m0, n0): a warp covers 128 consecutive columns of a row per pass (WN / 128
-// column halves per row), two row groups' loads in flight.  Columns at or beyond n_valid_end are never passed on.
+// column halves per row), EPI_ROWS rows' loads in flight per warp.  Columns at or beyond n_valid_end are never passed on.
+// The accumulators are in shared memory by now, so the registers are free for the loads.  The reverse, tangent and
+// backward epilogues read one or two activation-sized tensors: with 8 rows per warp (half of its 16 rows per column
+// half) those reads keep HBM busy, where 2 rows left it waiting.  The others read at most a bias and mostly store; they
+// keep 2 rows, which measured faster for them.
+template <class Epi> constexpr int epi_rows_in_flight() { return epi_family<Epi>::value == FAM_TC_OTHER ? 2 : 8; }
 template <int WN, class Epi>
 __device__ __forceinline__ void tile_epilogue(const float* acc_s, int64_t m0, int64_t M, int n0, int n_valid_end, const Epi& epi, int tid) {
   constexpr int LD = acc_ld(WN);
+  constexpr int EPI_ROWS = epi_rows_in_flight<Epi>();
   const int cq = tid & 31;
 #pragma unroll 1
   for (int h = 0; h < WN / 128; ++h) {
@@ -332,15 +345,15 @@ __device__ __forceinline__ void tile_epilogue(const float* acc_s, int64_t m0, in
     int nv = n_valid_end - col;
     nv = nv < 4 ? nv : 4;
     if (nv <= 0) break;
-    for (int r0 = tid >> 5; r0 < BM; r0 += 2 * (THREADS / 32)) {
-      typename Epi::Aux aux[2];
+    for (int r0 = tid >> 5; r0 < BM; r0 += EPI_ROWS * (THREADS / 32)) {
+      typename Epi::Aux aux[EPI_ROWS];
 #pragma unroll
-      for (int i = 0; i < 2; ++i) {
+      for (int i = 0; i < EPI_ROWS; ++i) {
         const int64_t row = m0 + r0 + i * (THREADS / 32);
         if (row < M) epi.load(row, col, nv, aux[i]);
       }
 #pragma unroll
-      for (int i = 0; i < 2; ++i) {
+      for (int i = 0; i < EPI_ROWS; ++i) {
         const int r = r0 + i * (THREADS / 32);
         const int64_t row = m0 + r;
         if (row < M) {
@@ -463,11 +476,24 @@ __device__ __forceinline__ void store_block_t(const float4 (&v)[8][2], int r0, i
 // 1-D grid of ceil(M/128) * ceil(N/WN) CTAs with the column tile fastest: the column tiles of a row block run back to
 // back, so that a second read of its activations hits L2.  Weight rows beyond the image tile (N = 217 -> 224 rows) leave
 // stale shared memory in the last rows of the slice; they only feed columns >= N, which the epilogue never passes on.
+// Weight slices arrive by cp.async.bulk into two stages on mbarriers.  The activation slices take one of two paths:
+//
+// RING (2 planes; a row stride that is a multiple of 4 floats and a 16-byte-aligned base, as a 2-D tensor map needs):
+// one thread issues a 2-D TMA copy per 64-wide K slice (a [128 rows x 64 k] fp32 box, 32 KB; rows past M and columns
+// past K arrive as zeros, padding columns of the row stride are never read) into a w_ring(WN)-deep ring of slots on
+// mbarriers, all of them before the main loop.  While the wgmma group of slice ks runs, all threads split slice ks + 1
+// in place: each reads its 8 float4 (store_a's mapping: a warp reads 512 contiguous bytes), a CTA barrier, then the
+// hi / lo K-major SW128 planes go over the same 32 KB.  A slot is refilled as soon as the barrier after the wgmma group
+// that read it has passed.  The planes and the products are the register path's, so both give the same bits.
+// Otherwise all threads stage each slice through registers (stage_a_direct): the loads of slice ks + 1 are issued after
+// the wgmma group of slice ks, then split into the free stage.
 // ---------------------------------------------------------------------------------------------------------------
-template <int NP, int WN, class Epi>
+template <int NP, int WN, class Epi, bool RING>
 __global__ void __launch_bounds__(THREADS, 1)
-gemm_w_kernel(const float* __restrict__ A, int64_t lda, int64_t M, int N, int K, const uint16_t* __restrict__ img, Epi epi) {
+gemm_w_kernel(const float* __restrict__ A, int64_t lda, int64_t M, int N, int K, const uint16_t* __restrict__ img, Epi epi,
+              const __grid_constant__ CUtensorMap amap) {
   static_assert(WN == 128 || (WN == 256 && NP == 2), "WN = 256 only with 2 planes (3 planes need 2 x WN/2 accumulators)");
+  static_assert(!RING || NP == 2, "the ring path splits a slot into 2 planes in place");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = align1024(smem_raw);
   const int tid = threadIdx.x, wg = tid >> 7;
@@ -480,29 +506,7 @@ gemm_w_kernel(const float* __restrict__ A, int64_t lda, int64_t M, int N, int K,
   int rows_h = rows_t - row_in_tile; rows_h = rows_h < WN ? rows_h : WN;   // weight rows of this CTA (multiple of 16)
   const int n_slices = pad64(K) / 64;
   constexpr uint32_t B_PLANE = b_plane_bytes(WN);
-  const uint32_t a_bytes = NP * A_HALF_BYTES, stage_bytes = a_bytes + NP * B_PLANE;
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + 2 * stage_bytes);
   const uint16_t* img_t = img + tile_offset(N, K, t, NP) + (int64_t)row_in_tile * 64;
-  const bool vec_ok = ((lda & 3) == 0) && aligned16(A);
-
-  auto issue_copies = [&](int ks) {                         // one thread: weight slice ks
-    uint8_t* st = smem + (ks & 1) * stage_bytes;
-    const uint32_t wb = (uint32_t)rows_h * 128u;
-    mbar_arrive_expect_tx(&full[ks & 1], NP * wb);
-    for (int p = 0; p < NP; ++p) bulk_g2s(st + a_bytes + p * B_PLANE, img_t + ((int64_t)ks * NP + p) * rows_t * 64, wb, &full[ks & 1]);
-  };
-  if (tid == 0) {
-    mbar_init(&full[0], 1);
-    mbar_init(&full[1], 1);
-    fence_barrier_init();
-  }
-  __syncthreads();
-  if (n_slices > 0) {
-    if (tid == 0) issue_copies(0);
-    stage_a_direct<NP, THREADS>(A, lda, m0, M, 0, K, smem, tid, vec_ok);
-    fence_proxy_async();
-  }
-  __syncthreads();
   // 3 planes: the corrections of each K slice and each 16-wide hi * hi step in fresh registers, summed in fp32 with
   // round-to-nearest.  The tensor core truncates a wgmma result toward zero; every hi * hi result is a single truncation of
   // 16 full-size products, so adding half an ulp of it (with its sign) leaves an unbiased error.  Without that the bias of
@@ -515,48 +519,129 @@ gemm_w_kernel(const float* __restrict__ A, int64_t lda, int64_t M, int N, int K,
   for (int q = 0; q < NACC; ++q) acc[q] = 0.f;
 #pragma unroll
   for (int q = 0; q < NTOT; ++q) tot[q] = 0.f;
-  for (int ks = 0; ks < n_slices; ++ks) {
-    const int s = ks & 1;
-    if (tid == 0 && ks + 1 < n_slices) issue_copies(ks + 1);   // stage s ^ 1 was released by the wait + barrier of ks - 1
-    mbar_wait(&full[s], (uint32_t)((ks >> 1) & 1));
-    const uint32_t st = smem_u32(smem + s * stage_bytes);
-    wg_fence();
-    mma_slice<NP, WN>(acc, st + wg * (64 * 128), A_HALF_BYTES, st + a_bytes, B_PLANE, NP == 3 || ks == 0);
-    wg_commit();
-    if (ks + 1 < n_slices) stage_a_direct<NP, THREADS>(A, lda, m0, M, (ks + 1) * BK, K, smem + (s ^ 1) * stage_bytes, tid, vec_ok);
-    wg_wait_all();
-    if constexpr (NP == 3) {
-      static_assert(BK / 16 == 4, "four hi * hi steps per K slice");
-      auto hi_hi = [&](float (&d)[64], int j) {
-        wg_fence();
-        wgmma_128_fresh(d, make_desc(st + wg * (64 * 128) + 32u * j), make_desc(st + a_bytes + 32u * j));
-        wg_commit();
-      };
-      auto add_unbiased = [&](float (&d)[64]) {              // after the wait that completes d
-        fence_operand(d);
+
+  if constexpr (RING) {
+    // [w_ring(WN) activation slots][2 weight stages of 2 planes][a barrier per slot][a barrier per weight stage]
+    constexpr int NR = w_ring(WN);
+    constexpr uint32_t W_STAGE = 2 * B_PLANE;
+    uint8_t* wst = smem + NR * W_SLOT;
+    uint64_t* afull = reinterpret_cast<uint64_t*>(wst + 2 * W_STAGE);
+    uint64_t* wfull = afull + NR;
+    auto issue_a = [&](int i) {                             // one thread: activation slice i into slot i % NR
+      const int r = i % NR;
+      mbar_arrive_expect_tx(&afull[r], W_SLOT);
+      tma_load_2d(smem + r * W_SLOT, &amap, i * BK, (int)m0, &afull[r]);
+    };
+    auto issue_w = [&](int ks) {                            // one thread: weight slice ks into stage ks & 1
+      uint8_t* st = wst + (ks & 1) * W_STAGE;
+      const uint32_t wb = (uint32_t)rows_h * 128u;
+      mbar_arrive_expect_tx(&wfull[ks & 1], 2 * wb);
+      for (int p = 0; p < 2; ++p) bulk_g2s(st + p * B_PLANE, img_t + ((int64_t)ks * 2 + p) * rows_t * 64, wb, &wfull[ks & 1]);
+    };
+    auto split = [&](int i) {                               // slice i, once landed, into hi / lo planes over its slot
+      uint8_t* slot = smem + (i % NR) * W_SLOT;
+      mbar_wait(&afull[i % NR], (uint32_t)((i / NR) & 1));
+      float4 v[BM * 16 / THREADS];
+      const float4* f = reinterpret_cast<const float4*>(slot) + (tid >> 4) * (BK / 4) + (tid & 15);
 #pragma unroll
-        for (int q = 0; q < 64; ++q) tot[q] += unbias_rz(d[q]);
-      };
-      hi_hi(acc2, 0);
-      fence_operand(acc);
-#pragma unroll
-      for (int q = 0; q < 64; ++q) tot[q] += acc[q];          // corrections
-      hi_hi(acc, 1);
-      wg_wait_but_one();
-      add_unbiased(acc2);                                     // hh0
-      hi_hi(acc2, 2);
-      wg_wait_but_one();
-      add_unbiased(acc);                                      // hh1
-      hi_hi(acc, 3);
-      wg_wait_but_one();
-      add_unbiased(acc2);                                     // hh2
-      wg_wait_all();
-      add_unbiased(acc);                                      // hh3
+      for (int pass = 0; pass < BM * 16 / THREADS; ++pass) v[pass] = f[pass * (THREADS / 16) * (BK / 4)];
+      __syncthreads();                                      // every read of the slot before the first plane store
+      store_a<2, THREADS>(v, slot, tid);
+    };
+    if (tid == 0) {
+      for (int r = 0; r < NR; ++r) mbar_init(&afull[r], 1);
+      mbar_init(&wfull[0], 1);
+      mbar_init(&wfull[1], 1);
+      fence_barrier_init();
+      if (n_slices > 0) issue_w(0);
+      for (int i = 0; i < NR && i < n_slices; ++i) issue_a(i);
     }
-    fence_proxy_async();
     __syncthreads();
+    if (n_slices > 0) {
+      split(0);
+      fence_proxy_async();
+    }
+    __syncthreads();
+    for (int ks = 0; ks < n_slices; ++ks) {
+      const int s = ks & 1;
+      if (tid == 0 && ks + 1 < n_slices) issue_w(ks + 1);   // stage s ^ 1 was released by the wait + barrier of ks - 1
+      mbar_wait(&wfull[s], (uint32_t)((ks >> 1) & 1));
+      const uint32_t sa = smem_u32(smem + (ks % NR) * W_SLOT), sb = smem_u32(wst + s * W_STAGE);
+      wg_fence();
+      mma_slice<2, WN>(acc, sa + wg * (64 * 128), A_HALF_BYTES, sb, B_PLANE, ks == 0);
+      wg_commit();
+      if (ks + 1 < n_slices) split(ks + 1);
+      wg_wait_all();
+      fence_proxy_async();
+      __syncthreads();
+      if (tid == 0 && ks + NR < n_slices) issue_a(ks + NR);  // slot ks % NR: the group that read it has completed
+    }
+  } else {
+    const uint32_t a_bytes = NP * A_HALF_BYTES, stage_bytes = a_bytes + NP * B_PLANE;
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + 2 * stage_bytes);
+    const bool vec_ok = ((lda & 3) == 0) && aligned16(A);
+
+    auto issue_copies = [&](int ks) {                       // one thread: weight slice ks
+      uint8_t* st = smem + (ks & 1) * stage_bytes;
+      const uint32_t wb = (uint32_t)rows_h * 128u;
+      mbar_arrive_expect_tx(&full[ks & 1], NP * wb);
+      for (int p = 0; p < NP; ++p) bulk_g2s(st + a_bytes + p * B_PLANE, img_t + ((int64_t)ks * NP + p) * rows_t * 64, wb, &full[ks & 1]);
+    };
+    if (tid == 0) {
+      mbar_init(&full[0], 1);
+      mbar_init(&full[1], 1);
+      fence_barrier_init();
+    }
+    __syncthreads();
+    if (n_slices > 0) {
+      if (tid == 0) issue_copies(0);
+      stage_a_direct<NP, THREADS>(A, lda, m0, M, 0, K, smem, tid, vec_ok);
+      fence_proxy_async();
+    }
+    __syncthreads();
+    for (int ks = 0; ks < n_slices; ++ks) {
+      const int s = ks & 1;
+      if (tid == 0 && ks + 1 < n_slices) issue_copies(ks + 1);   // stage s ^ 1 was released by the wait + barrier of ks - 1
+      mbar_wait(&full[s], (uint32_t)((ks >> 1) & 1));
+      const uint32_t st = smem_u32(smem + s * stage_bytes);
+      wg_fence();
+      mma_slice<NP, WN>(acc, st + wg * (64 * 128), A_HALF_BYTES, st + a_bytes, B_PLANE, NP == 3 || ks == 0);
+      wg_commit();
+      if (ks + 1 < n_slices) stage_a_direct<NP, THREADS>(A, lda, m0, M, (ks + 1) * BK, K, smem + (s ^ 1) * stage_bytes, tid, vec_ok);
+      wg_wait_all();
+      if constexpr (NP == 3) {
+        static_assert(BK / 16 == 4, "four hi * hi steps per K slice");
+        auto hi_hi = [&](float (&d)[64], int j) {
+          wg_fence();
+          wgmma_128_fresh(d, make_desc(st + wg * (64 * 128) + 32u * j), make_desc(st + a_bytes + 32u * j));
+          wg_commit();
+        };
+        auto add_unbiased = [&](float (&d)[64]) {            // after the wait that completes d
+          fence_operand(d);
+#pragma unroll
+          for (int q = 0; q < 64; ++q) tot[q] += unbias_rz(d[q]);
+        };
+        hi_hi(acc2, 0);
+        fence_operand(acc);
+#pragma unroll
+        for (int q = 0; q < 64; ++q) tot[q] += acc[q];        // corrections
+        hi_hi(acc, 1);
+        wg_wait_but_one();
+        add_unbiased(acc2);                                   // hh0
+        hi_hi(acc2, 2);
+        wg_wait_but_one();
+        add_unbiased(acc);                                    // hh1
+        hi_hi(acc, 3);
+        wg_wait_but_one();
+        add_unbiased(acc2);                                   // hh2
+        wg_wait_all();
+        add_unbiased(acc);                                    // hh3
+      }
+      fence_proxy_async();
+      __syncthreads();
+    }
   }
-  float* acc_s = reinterpret_cast<float*>(smem);              // the operand stages are free by now
+  float* acc_s = reinterpret_cast<float*>(smem);              // the operand stages are free by now: every copy has landed
   if constexpr (NP == 3) acc_to_smem<WN>(tot, acc_s, wg, tid & 127);
   else acc_to_smem<WN>(acc, acc_s, wg, tid & 127);
   __syncthreads();
@@ -754,28 +839,69 @@ static inline int sm_count() {
 }
 
 
+// 2-D tensor map of a row-major fp32 operand [rows x cols] (row stride ld floats, a multiple of 4) in [box_rows x box_cols]
+// boxes; boxes reaching past the extent arrive zero-filled there
+static inline int tensor_map_2d(CUtensorMap* map, const float* X, int64_t ld, int64_t cols, int64_t rows, int box_cols, int box_rows) {
+  static PFN_cuTensorMapEncodeTiled encode = nullptr;
+  if (encode == nullptr) {
+    void* fn = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess ||
+        fn == nullptr) {
+      nudf::set_error("cuTensorMapEncodeTiled is not available from the driver");
+      return -2;
+    }
+    encode = reinterpret_cast<PFN_cuTensorMapEncodeTiled>(fn);
+  }
+  const cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+  const cuuint64_t strides[1] = {(cuuint64_t)ld * sizeof(float)};
+  const cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows};
+  const cuuint32_t elem[2] = {1, 1};
+  const CUresult r = encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(X), dims, strides, box, elem,
+                            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    nudf::set_error("cuTensorMapEncodeTiled failed (%d)", (int)r);
+    return -2;
+  }
+  return 0;
+}
 // 2 stages x NP planes of the A and weight slices; the [128 x acc_ld(WN)] fp32 accumulator tile reuses them
 constexpr size_t w_smem_bytes(int np, int wn) { return 2 * (size_t)np * (A_HALF_BYTES + b_plane_bytes(wn)) + 2 * sizeof(uint64_t) + 1024; }
 static_assert(BM * acc_ld(2 * BN) * sizeof(float) <= 2 * 2 * (size_t)(A_HALF_BYTES + b_plane_bytes(2 * BN)), "accumulator tile");
-constexpr size_t TN_SMEM = 2 * (size_t)(2 * A_HALF_BYTES + 2 * B_HALF_BYTES) + 2 * sizeof(uint64_t) + 1024;
-// the ring path: the fp32 ring, 2 plane stages, the k-quarter column-sum partials and one mbarrier per ring stage
-constexpr size_t TN_RING_SMEM = (size_t)TN_RING * TN_F32_STAGE + 2 * TN_PLANE_STAGE + 4 * BM * sizeof(float) + TN_RING * sizeof(uint64_t) + 1024;
-static_assert(BM * acc_ld(BN) * sizeof(float) <= (size_t)TN_RING * TN_F32_STAGE, "accumulator tile in the ring");
-static_assert(TN_RING_SMEM <= 227 * 1024, "one CTA per SM");
+// the ring path: w_ring(wn) fp32 slots, 2 weight stages of 2 planes, a barrier per slot and per stage; the accumulator
+// tile reuses the slots and stages
+constexpr size_t w_ring_operand_bytes(int wn) { return (size_t)w_ring(wn) * W_SLOT + 2 * 2 * (size_t)b_plane_bytes(wn); }
+constexpr size_t w_ring_smem_bytes(int wn) { return w_ring_operand_bytes(wn) + (w_ring(wn) + 2) * sizeof(uint64_t) + 1024; }
+static_assert(w_ring_smem_bytes(BN) <= 227 * 1024 && w_ring_smem_bytes(2 * BN) <= 227 * 1024, "one CTA per SM");
+static_assert(BM * acc_ld(BN) * sizeof(float) <= w_ring_operand_bytes(BN), "accumulator tile in the ring path's stages");
+static_assert(BM * acc_ld(2 * BN) * sizeof(float) <= w_ring_operand_bytes(2 * BN), "accumulator tile in the ring path's stages");
 
-template <int NP, int WN, class Epi>
+template <int NP, int WN, class Epi, bool RING>
 static inline int gemm_w_launch(const float* A, int64_t lda, int64_t M, int N, int K, const uint16_t* img, const Epi& epi, cudaStream_t st) {
-  constexpr size_t smem = w_smem_bytes(NP, WN);
+  constexpr size_t smem = RING ? w_ring_smem_bytes(WN) : w_smem_bytes(NP, WN);
   static bool attr_set = false;   // per template instantiation
   if (!attr_set) {
-    NUDF_CUDA_OK(cudaFuncSetAttribute(gemm_w_kernel<NP, WN, Epi>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    NUDF_CUDA_OK(cudaFuncSetAttribute(gemm_w_kernel<NP, WN, Epi, RING>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr_set = true;
   }
+  CUtensorMap amap{};
+  if constexpr (RING)
+    if (int rc = tensor_map_2d(&amap, A, lda, K, M, BK, BM)) return rc;
   const unsigned grid = (unsigned)(cdiv(M, BM) * cdiv(N, WN));
   LaunchTimer lt_(epi_family<Epi>::value, st);
-  gemm_w_kernel<NP, WN, Epi><<<grid, THREADS, smem, st>>>(A, lda, M, N, K, img, epi);
+  gemm_w_kernel<NP, WN, Epi, RING><<<grid, THREADS, smem, st>>>(A, lda, M, N, K, img, epi, amap);
   NUDF_LAUNCH_OK();
   return 0;
+}
+// The activation path follows from the operand: 2-plane layers take the ring when the row stride is a multiple of 4
+// floats and the base is 16-byte aligned (a 2-D tensor map needs both; every operand the networks pass has them), the
+// register path otherwise.  3-plane layers always take the register path.
+template <int NP, int WN, class Epi>
+static inline int gemm_w_path(const float* A, int64_t lda, int64_t M, int N, int K, const uint16_t* img, const Epi& epi, cudaStream_t st) {
+  if constexpr (NP == 2)
+    if (K > 0 && (lda & 3) == 0 && aligned16(A)) return gemm_w_launch<2, WN, Epi, true>(A, lda, M, N, K, img, epi, st);
+  return gemm_w_launch<NP, WN, Epi, false>(A, lda, M, N, K, img, epi, st);
 }
 // The output width per CTA follows from the shape: 256 columns for 2-plane layers wider than 128 (one read and split of
 // each activation row block instead of two), 128 otherwise (3 planes, and 2-plane layers of at most 128 columns).
@@ -783,8 +909,8 @@ template <int NP, class Epi>
 static inline int gemm_w(const float* A, int64_t lda, int64_t M, int N, int K, const uint16_t* img, const Epi& epi, cudaStream_t st) {
   if (M <= 0 || N <= 0) return 0;
   if constexpr (NP == 2)
-    if (N > BN) return gemm_w_launch<2, 2 * BN, Epi>(A, lda, M, N, K, img, epi, st);
-  return gemm_w_launch<NP, BN, Epi>(A, lda, M, N, K, img, epi, st);
+    if (N > BN) return gemm_w_path<2, 2 * BN, Epi>(A, lda, M, N, K, img, epi, st);
+  return gemm_w_path<NP, BN, Epi>(A, lda, M, N, K, img, epi, st);
 }
 
 // The split of a weight-gradient contraction over its points (split-K), from the shape alone: the same inputs give the
@@ -801,32 +927,12 @@ static inline int64_t tn_k_chunk(int M, int N, int64_t K) {
   return round_up(cdiv(K, splits), BK);
 }
 
-// 2-D tensor map of a row-major fp32 operand [rows x cols] (row stride ld floats) in [TN_PS x 128] boxes, zero fill
-static inline int tn_tensor_map(CUtensorMap* map, const float* X, int64_t ld, int cols, int64_t rows) {
-  static PFN_cuTensorMapEncodeTiled encode = nullptr;
-  if (encode == nullptr) {
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess ||
-        fn == nullptr) {
-      nudf::set_error("cuTensorMapEncodeTiled is not available from the driver");
-      return -2;
-    }
-    encode = reinterpret_cast<PFN_cuTensorMapEncodeTiled>(fn);
-  }
-  const cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  const cuuint64_t strides[1] = {(cuuint64_t)ld * sizeof(float)};
-  const cuuint32_t box[2] = {(cuuint32_t)BM, (cuuint32_t)TN_PS};
-  const cuuint32_t elem[2] = {1, 1};
-  const CUresult r = encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(X), dims, strides, box, elem,
-                            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    nudf::set_error("cuTensorMapEncodeTiled failed (%d)", (int)r);
-    return -2;
-  }
-  return 0;
-}
+constexpr size_t TN_SMEM = 2 * (size_t)(2 * A_HALF_BYTES + 2 * B_HALF_BYTES) + 2 * sizeof(uint64_t) + 1024;
+// the ring path: the fp32 ring, 2 plane stages, the k-quarter column-sum partials and one mbarrier per ring stage
+constexpr size_t TN_RING_SMEM = (size_t)TN_RING * TN_F32_STAGE + 2 * TN_PLANE_STAGE + 4 * BM * sizeof(float) + TN_RING * sizeof(uint64_t) + 1024;
+static_assert(BM * acc_ld(BN) * sizeof(float) <= (size_t)TN_RING * TN_F32_STAGE, "accumulator tile in the ring");
+static_assert(TN_RING_SMEM <= 227 * 1024, "one CTA per SM");
+
 template <class Epi, bool RING>
 static inline int gemm_tn_launch(dim3 grid, const float* A, int64_t lda, const float* B, int64_t ldb, int M, int N, int64_t K,
                                  int64_t k_chunk, const Epi& epi, float* colsum, float* cs_ws, cudaStream_t st) {
@@ -838,8 +944,8 @@ static inline int gemm_tn_launch(dim3 grid, const float* A, int64_t lda, const f
   }
   TnMaps maps{};
   if constexpr (RING) {
-    if (int rc = tn_tensor_map(&maps.a, A, lda, M, K)) return rc;
-    if (int rc = tn_tensor_map(&maps.b, B, ldb, N, K)) return rc;
+    if (int rc = tensor_map_2d(&maps.a, A, lda, M, K, BM, TN_PS)) return rc;
+    if (int rc = tensor_map_2d(&maps.b, B, ldb, N, K, BN, TN_PS)) return rc;
   }
   gemm_tn_kernel<Epi, RING><<<grid, THREADS, smem, st>>>(A, lda, B, ldb, M, N, K, k_chunk, epi, colsum, cs_ws, maps);
   NUDF_LAUNCH_OK();
