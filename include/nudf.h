@@ -462,6 +462,21 @@ int nudf_nb_count(const uint8_t* flags, int32_t n, int32_t s, int32_t t, const i
 /* idx / pts[offsets[i] ...] = those points of block kept[i] in (x, y, z) lexicographic order; offsets = exclusive scan */
 int nudf_nb_emit(const uint8_t* flags, int32_t n, int32_t s, int32_t t, const int64_t* kept, int64_t n_kept,
                  const int64_t* offsets, double voxel, int64_t* idx, float* pts, void* stream);
+/* The same stages on the lattice of three DEVICE fp32 axis tables ax, ay, az [N] (any box; grid.iso_band passes the
+ * torch.linspace tables of the dense threshold sweep): point (i, j, k) is (ax[i], ay[j], az[k]).  nudf_nb_count is shared. */
+/* nudf_nb_sublattice with the table coordinates */
+int nudf_nb_sublattice_box(int32_t n, int32_t s, const float* ax, const float* ay, const float* az, int64_t* idx, float* pts,
+                           void* stream);
+/* nudf_nb_block_test with r = half the diagonal of the block's table-coordinate box (fp64, |ax[hi] - ax[lo]| per axis),
+ * enlarged by 1e-6 relative plus pad (>= 0), and tau used as given (the caller's slack included); edge slopes
+ * |du| / (e_a h_a), h_a >= 0 the largest step of table a */
+int nudf_nb_block_test_box(const float* df, int32_t n, int32_t s, const uint8_t* parent_flags, int32_t parent_s,
+                           const float* ax, const float* ay, const float* az, double hx, double hy, double hz, double pad,
+                           double lipschitz, double tau, uint8_t* flags, uint32_t* max_slope, void* stream);
+/* nudf_nb_emit with the table coordinates */
+int nudf_nb_emit_box(const uint8_t* flags, int32_t n, int32_t s, int32_t t, const int64_t* kept, int64_t n_kept,
+                     const int64_t* offsets, const float* ax, const float* ay, const float* az, int64_t* idx, float* pts,
+                     void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Mesh post-processing (neuraludf_b200/mesh_post.py drives the steps; sorting, unique and compaction in torch)

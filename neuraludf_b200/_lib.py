@@ -212,6 +212,10 @@ _SIGNATURES = {
     "nudf_nb_count": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [c_void_p, ctypes.c_int64] + [c_void_p] * 2),
     "nudf_nb_emit": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [c_void_p, ctypes.c_int64, c_void_p, ctypes.c_double]
                      + [c_void_p] * 3),
+    "nudf_nb_sublattice_box": (ctypes.c_int, [ctypes.c_int32] * 2 + [c_void_p] * 6),
+    "nudf_nb_block_test_box": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 2 + [c_void_p, ctypes.c_int32] + [c_void_p] * 3
+                               + [ctypes.c_double] * 6 + [c_void_p] * 3),
+    "nudf_nb_emit_box": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [c_void_p, ctypes.c_int64] + [c_void_p] * 7),
     "nudf_mp_faces": (ctypes.c_int, [c_void_p, ctypes.c_int64, c_void_p, ctypes.c_int64] + [c_void_p] * 6),
     "nudf_mp_hole_count": (ctypes.c_int, [c_void_p, ctypes.c_int64, c_void_p, c_void_p, ctypes.c_int64, c_void_p, c_void_p]),
     "nudf_mp_hole_emit": (ctypes.c_int, [c_void_p] * 3 + [ctypes.c_int64, c_void_p, c_void_p, ctypes.c_int64]

@@ -8,7 +8,10 @@ is handed over as the dense distance grid plus a SPARSE list of near-surface cel
 ~7 MB at 256^3 instead of the reference's 67 MB + 201 MB dense normal grid and its ~130 blocking copies.
 `get_udf_normals_grid_slow` keeps the reference's return convention for `udf_mc_lewiner` (the Cython MeshUDF marching cubes,
 out of scope).  `udf_band` is the coarse-to-fine alternative to the dense sweep: it evaluates the lattice only where a
-Lipschitz bound cannot rule out udf < 2 voxels (kernels in csrc/mesh_band.cu)."""
+Lipschitz bound cannot rule out udf < 2 voxels (kernels in csrc/mesh_band.cu).  `iso_band` does the same for the threshold
+lattice of validate_mesh (any box, torch.linspace coordinates): it evaluates every point a threshold mesh at `level` can
+read."""
+import math
 import warnings
 
 import torch
@@ -115,9 +118,10 @@ def band_block_test(df, N, s, parent=None, parent_s=0, lipschitz=2.0, dist_voxel
     return out, float(slope.view(torch.float32))
 
 
-def band_points(flags, N, s, t):
+def band_points(flags, N, s, t, axes=None):
     """(flat indices [M] int64, points [M,3] fp32, kept block count): the stride-t points that the kept blocks of stride s
-    emit, each point once (the lowest-numbered kept block holding it), blocks ascending, each in lexicographic order"""
+    emit, each point once (the lowest-numbered kept block holding it), blocks ascending, each in lexicographic order;
+    coordinates on [-1,1]^3, or from the three fp32 tables `axes` (iso_band)"""
     L = _lib.lib()
     st = _lib.stream_ptr()
     kept = torch.nonzero(flags).reshape(-1)
@@ -129,9 +133,88 @@ def band_points(flags, N, s, t):
     offsets = (csum - counts).contiguous()
     idx = torch.empty(total, dtype=torch.int64, device=flags.device)
     pts = torch.empty(total, 3, device=flags.device)
-    check(L.nudf_nb_emit(ptr(flags), N, s, t, ptr(kept), n, ptr(offsets), 2.0 / (N - 1), ptr(idx), ptr(pts), st),
-          "nudf_nb_emit")
+    if axes is None:
+        check(L.nudf_nb_emit(ptr(flags), N, s, t, ptr(kept), n, ptr(offsets), 2.0 / (N - 1), ptr(idx), ptr(pts), st),
+              "nudf_nb_emit")
+    else:
+        check(L.nudf_nb_emit_box(ptr(flags), N, s, t, ptr(kept), n, ptr(offsets), *_table_ptrs(axes, N), ptr(idx), ptr(pts),
+                                 st), "nudf_nb_emit_box")
     return idx, pts, n
+
+
+def _table_ptrs(axes, N):
+    if len(axes) != 3 or any(x.dtype != torch.float32 or x.shape != (N,) or not x.is_contiguous() for x in axes):
+        raise ValueError("axes must be three contiguous float32 tables of %d coordinates" % N)
+    return [ptr(x) for x in axes]
+
+
+def band_sublattice_box(axes, s):
+    """band_sublattice with the coordinates of the fp32 tables `axes` (three [N] device tensors)"""
+    L = _lib.lib()
+    N = axes[0].numel()
+    m = -(-(N - 1) // s) + 1
+    idx = torch.empty(m ** 3, dtype=torch.int64, device=axes[0].device)
+    pts = torch.empty(m ** 3, 3, device=axes[0].device)
+    check(L.nudf_nb_sublattice_box(N, s, *_table_ptrs(axes, N), ptr(idx), ptr(pts), _lib.stream_ptr()),
+          "nudf_nb_sublattice_box")
+    return idx, pts
+
+
+def band_block_test_box(df, axes, s, parent, parent_s, spacing, pad, lipschitz, tau, flags=True):
+    """band_block_test on the lattice of the tables `axes` (csrc/mesh_band.cu's table rule): r from the block's table
+    coordinates plus `pad`, `tau` as given, edge slopes over `spacing` (the largest step per axis)"""
+    L = _lib.lib()
+    N = axes[0].numel()
+    nb = -(-(N - 1) // s)
+    out = torch.empty(nb ** 3, dtype=torch.uint8, device=df.device) if flags else None
+    slope = torch.zeros(1, dtype=torch.int32, device=df.device)
+    check(L.nudf_nb_block_test_box(ptr(df), N, s, ptr(parent), parent_s, *_table_ptrs(axes, N), *(float(x) for x in spacing),
+                                   float(pad), float(lipschitz), float(tau), ptr(out), ptr(slope), _lib.stream_ptr()),
+          "nudf_nb_block_test_box")
+    return out, float(slope.view(torch.float32))
+
+
+def _coarse_to_fine(values, N, strides, device, max_batch, sublattice, block_test, points):
+    """The level loop of udf_band and iso_band: (df [N^3] fp32 flat, +inf where never evaluated; info without
+    max_edge_slope).  values(pts [P,3]) -> [P] fp32; sublattice(s) -> (idx, pts); block_test(df, s, parent, parent_s,
+    flags) -> (flags or None, slope); points(flags, s, t) -> (idx, pts, kept blocks)."""
+    df = torch.full((N ** 3,), float("inf"), device=device)
+    info = {"strides": strides, "points": [], "kept_blocks": [], "edge_slope": []}
+    events = []
+
+    def mark():
+        events.append(torch.cuda.Event(enable_timing=True))
+        events[-1].record()
+
+    def evaluate(idx, pts):
+        for head in range(0, idx.numel(), max_batch):
+            df[idx[head:head + max_batch]] = values(pts[head:head + max_batch])
+        info["points"].append(int(idx.numel()))
+
+    mark()
+    evaluate(*sublattice(strides[0]))
+    mark()
+    parent = None
+    for k, s in enumerate(strides):
+        last = k + 1 == len(strides)
+        flags, slope = block_test(df, s, parent, strides[k - 1] if k else 0, not last)
+        info["edge_slope"].append(slope)
+        if last:
+            break
+        idx, pts, n_kept = points(flags, s, strides[k + 1])
+        info["kept_blocks"].append(n_kept)
+        evaluate(idx, pts)
+        del idx, pts
+        mark()
+        parent = flags
+    mark()
+    torch.cuda.synchronize(device)
+    ms = [a.elapsed_time(b) for a, b in zip(events, events[1:])]
+    # level 0: the stride-strides[0] lattice; level k: block test at strides[k-1], emission and evaluation of strides[k]
+    # points; slope_ms: the slope pass over the finest level
+    info["level_ms"], info["slope_ms"] = ms[:-1], ms[-1]
+    info["max_edge_slope"] = max(info["edge_slope"])
+    return df, info
 
 
 @torch.no_grad()
@@ -148,45 +231,91 @@ def udf_band(udf_network, N, lipschitz=2.0, strides=None, max_batch=1 << 21):
     `lipschitz` -- and level_ms (CUDA events)."""
     strides = _check_strides(default_strides(N) if strides is None else strides)
     device = _device(udf_network)
-    df = torch.full((N ** 3,), float("inf"), device=device)
-    info = {"strides": strides, "points": [], "kept_blocks": [], "edge_slope": []}
-    events = []
-
-    def mark():
-        events.append(torch.cuda.Event(enable_timing=True))
-        events[-1].record()
-
-    def evaluate(idx, pts):
-        for head in range(0, idx.numel(), max_batch):
-            df[idx[head:head + max_batch]] = udf_network.udf_values(pts[head:head + max_batch]).reshape(-1)
-        info["points"].append(int(idx.numel()))
-
-    mark()
-    evaluate(*band_sublattice(N, strides[0], device))
-    mark()
-    parent = None
-    for k, s in enumerate(strides):
-        last = k + 1 == len(strides)
-        flags, slope = band_block_test(df, N, s, parent, strides[k - 1] if k else 0, lipschitz, flags=not last)
-        info["edge_slope"].append(slope)
-        if last:
-            break
-        idx, pts, n_kept = band_points(flags, N, s, strides[k + 1])
-        info["kept_blocks"].append(n_kept)
-        evaluate(idx, pts)
-        del idx, pts
-        mark()
-        parent = flags
-    mark()
-    torch.cuda.synchronize(device)
-    ms = [a.elapsed_time(b) for a, b in zip(events, events[1:])]
-    # level 0: the stride-strides[0] lattice; level k: block test at strides[k-1], emission and evaluation of strides[k]
-    # points; slope_ms: the slope pass over the finest level
-    info["level_ms"], info["slope_ms"] = ms[:-1], ms[-1]
-    info["max_edge_slope"] = max(info["edge_slope"])
+    df, info = _coarse_to_fine(
+        lambda pts: udf_network.udf_values(pts).reshape(-1), N, strides, device, max_batch,
+        lambda s: band_sublattice(N, s, device),
+        lambda df, s, parent, parent_s, flags: band_block_test(df, N, s, parent, parent_s, lipschitz, flags=flags),
+        lambda flags, s, t: band_points(flags, N, s, t))
     if info["max_edge_slope"] > lipschitz:
         warnings.warn("udf_band: a lattice edge has slope %.3f > lipschitz=%.3f: the field is not %.3f-Lipschitz, so the band "
                       "may miss points with udf < 2 voxels" % (info["max_edge_slope"], lipschitz, lipschitz), RuntimeWarning,
+                      stacklevel=2)
+    return df, info
+
+
+def axis_tables(bound_min, bound_max, resolution, device):
+    """the coordinates of the threshold lattice on the box, per axis: torch.linspace(bound_min[a], bound_max[a], resolution)
+    (fp32 [resolution], on `device`), the tables the dense sweep of extract_geometry evaluates"""
+    return [torch.linspace(float(bound_min[a]), float(bound_max[a]), resolution, device=device) for a in range(3)]
+
+
+def table_spacing(axes):
+    """(h, e), three floats each, from the fp32 tables in fp64 (exact): h[a] the largest step |x[i+1] - x[i]| of table a and
+    e[a] its largest excursion against its direction, min over the two directions of max_{i<j} (x[i] - x[j]) or
+    max_{i<j} (x[j] - x[i]).  0 for a monotone table.  A point between two others on the lattice lies within e[a] of the
+    interval their coordinates span, which is what iso_band's culling needs of the rounding in torch.linspace."""
+    rows = []
+    for x in axes:
+        x = x.double()
+        up = (torch.cummax(x, 0).values - x).max()
+        down = (x - torch.cummin(x, 0).values).max()
+        rows.append(torch.stack([(x[1:] - x[:-1]).abs().max(), torch.minimum(up, down)]))
+    v = torch.stack(rows).cpu().tolist()
+    return [r[0] for r in v], [r[1] for r in v]
+
+
+def iso_cull(level, lipschitz, h, e):
+    """(tau, pad) of iso_band's block test, fp64: D = sqrt(h_x^2 + h_y^2 + h_z^2) bounds the distance between two corners of
+    one lattice cell; tau = level + L D, plus 1e-6 (|level| + L D) of slack against the rounding of D, tau and the block
+    radius, so that tau exceeds the exact level + L D; pad = 1.000001 |e| enlarges every block radius by the tables'
+    excursion (table_spacing)"""
+    d = math.sqrt(h[0] * h[0] + h[1] * h[1] + h[2] * h[2])
+    ld = lipschitz * d
+    tau = (level + ld) + 1e-6 * (abs(level) + ld)
+    pad = 1.000001 * math.sqrt(e[0] * e[0] + e[1] * e[1] + e[2] * e[2])
+    return tau, pad
+
+
+@torch.no_grad()
+def iso_band(query, bound_min, bound_max, resolution, level, lipschitz=2.0, strides=None, max_batch=1 << 21, device=None):
+    """Narrow-band threshold lattice, coarse to fine: (df [R^3] fp32 flat, +inf where never evaluated; info).
+
+    The lattice is extract_geometry's: R = `resolution` points per axis on the box [bound_min, bound_max], coordinates from
+    axis_tables (the dense sweep's torch.linspace tables, read by the kernels, so the points are that sweep's bit for bit),
+    flat index (i R + j) R + k.  The level is rounded to fp32 once (mesh.iso_marching_cubes_index's rule); a non-finite
+    level raises ValueError.  The levels run as udf_band's, with the block test of csrc/mesh_band.cu's table rule: a block
+    is culled when min(corner value) - L r >= tau, r half its diagonal in table coordinates, tau = level + L D (iso_cull).
+    If `query` is `lipschitz`-Lipschitz at the lattice points and gives a point the same bits in any batch, df equals the
+    dense lattice bit for bit wherever that is below tau, every +inf stands for a value >= tau, and the threshold marching
+    cubes of df at `level` (mesh.iso_mesh_band) is the dense one exactly (the argument is beside the kernels).
+    `query`: any callable points [P,3] fp32 -> [P] or [P,1].  info: udf_band's keys, with the same RuntimeWarning when
+    max_edge_slope exceeds `lipschitz`, plus tau (the threshold compared with, slack included), pad and spacing (the largest
+    step per axis)."""
+    from neuraludf_b200.mesh import _iso_level
+    level = _iso_level(level)
+    N = int(resolution)
+    if N < 2:
+        raise ValueError("resolution must be at least 2 (got %r)" % (resolution,))
+    lipschitz = float(lipschitz)
+    if not 0.0 < lipschitz < float("inf"):
+        raise ValueError("lipschitz must be positive and finite (got %r)" % (lipschitz,))
+    strides = _check_strides(default_strides(N) if strides is None else strides)
+    device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+    axes = axis_tables(bound_min, bound_max, N, device)
+    if any(x.dtype != torch.float32 for x in axes):
+        raise ValueError("the lattice tables must be float32 (torch's default dtype is %s)" % torch.get_default_dtype())
+    h, e = table_spacing(axes)
+    tau, pad = iso_cull(level, lipschitz, h, e)
+    df, info = _coarse_to_fine(
+        lambda pts: query(pts).detach().reshape(-1).float(), N, strides, device, max_batch,
+        lambda s: band_sublattice_box(axes, s),
+        lambda df, s, parent, parent_s, flags: band_block_test_box(df, axes, s, parent, parent_s, h, pad, lipschitz, tau,
+                                                                   flags),
+        lambda flags, s, t: band_points(flags, N, s, t, axes))
+    info.update(tau=tau, pad=pad, spacing=h)
+    if info["max_edge_slope"] > lipschitz:
+        warnings.warn("iso_band: a lattice edge has slope %.3f > lipschitz=%.3f: the field is not %.3f-Lipschitz, so a "
+                      "threshold mesh may miss cells" % (info["max_edge_slope"], lipschitz, lipschitz), RuntimeWarning,
                       stacklevel=2)
     return df, info
 

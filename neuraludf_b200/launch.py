@@ -7,7 +7,9 @@ mirrors before the runner is executed from the reference root; everything else t
 still resolves from the reference checkout (its `models/` directory is a namespace package).  `custom_mc` (the Cython
 MeshUDF marching cubes that extract_mesh.py imports) is bound to neuraludf_b200.mesh when the reference's own build cannot
 be imported by the running interpreter.  With NUDF_DEVICE_LOSS=1 in the environment, `loss.loss` and `loss.patch_metric`
-are bound to neuraludf_b200.loss (the colour loss on the device); without it the runner's own loss files run.
+are bound to neuraludf_b200.loss (the colour loss on the device); without it the runner's own loss files run.  With
+NUDF_BAND_MESH=1, `validate_mesh`'s `extract_geometry` (when PyMCubes cannot be imported) evaluates its lattice narrow-band
+(grid.iso_band: the same mesh when the UDF is 2-Lipschitz and batch-invariant); without it the whole lattice is queried.
 """
 import importlib
 import importlib.machinery

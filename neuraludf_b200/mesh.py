@@ -8,7 +8,8 @@ for the reference's `custom_mc._marching_cubes_lewiner.udf_mc_lewiner`, served t
 `launch.install_shadow_modules` when the reference's Cython build cannot be imported.  The kernels are in
 csrc/mesh_udf.cu (stages and deviations documented there); tests/proto/udf_mc.py is their NumPy restatement.
 `iso_marching_cubes_index` / `iso_marching_cubes` are threshold marching cubes on the same kernels (the runner's
-validate_mesh without PyMCubes; `python -m neuraludf_b200.mesh --threshold T`), restated in tests/proto/iso_mc.py.
+validate_mesh without PyMCubes; `python -m neuraludf_b200.mesh --threshold T`), restated in tests/proto/iso_mc.py;
+`iso_mesh_band` is the same with the lattice evaluated narrow-band (grid.iso_band; `--threshold T --band`).
 """
 import ctypes
 
@@ -152,6 +153,27 @@ def iso_marching_cubes_index(df, dims, level):
           "nudf_iso_vertices")
     info["vertex_keys"] = ukeys
     return verts, inv.reshape(-1, 3).to(torch.int64), info
+
+
+@torch.no_grad()
+def iso_mesh_band(query, bound_min, bound_max, resolution, level, lipschitz=2.0, strides=None, max_batch=1 << 21,
+                  device=None):
+    """Threshold marching cubes of extract_geometry's lattice (R = `resolution` points per axis on the box, torch.linspace
+    coordinates) at `level`, the lattice evaluated narrow-band (grid.iso_band): iso_marching_cubes_index's (fp64 verts [V,3]
+    in lattice-index units, int64 faces [F,3], info), with grid.iso_band's info under info["band"].
+
+    Exact when `query` is `lipschitz`-Lipschitz at the lattice points and gives a point the same bits in any batch:
+    iso_band's df then equals the dense lattice wherever that is below level + L D (D: the largest cell diagonal) and every
+    point left out is above the level, so a cell with a culled corner is inactive as its dense corners make it, and the
+    later stages read df only at the corners of active cells.  grid.iso_band warns when the lattice shows a slope above
+    `lipschitz`."""
+    from neuraludf_b200 import grid
+    R = int(resolution)
+    df, binfo = grid.iso_band(query, bound_min, bound_max, R, level, lipschitz=lipschitz, strides=strides,
+                              max_batch=max_batch, device=device)
+    verts, faces, info = iso_marching_cubes_index(df, (R, R, R), level)
+    info["band"] = binfo
+    return verts, faces, info
 
 
 def iso_marching_cubes(volume, isovalue):
@@ -387,6 +409,9 @@ def main(argv=None):
                          "object box of --cameras) instead of the MeshUDF pipeline: the mesh the runner's "
                          "validate_mesh(world_space=True) exports with --cameras; the runner passes --threshold 0.005")
     ap.add_argument("--dist_threshold_ratio", type=float, default=None, help="vertex filter in voxels (default 1)")
+    ap.add_argument("--band", action="store_true",
+                    help="with --threshold: evaluate the lattice narrow-band (grid.iso_band) and mesh it on the device, "
+                         "the same mesh when the udf is --lipschitz-Lipschitz")
     ap.add_argument("--lipschitz", type=float, default=None, help="Lipschitz bound of the band's culling test (default 2)")
     ap.add_argument("--scale", type=float, default=1.0, help="the conf's udf_network.scale")
     ap.add_argument("--dense", action="store_true", help="evaluate the whole lattice (udf_mesh) instead of the narrow band")
@@ -396,8 +421,11 @@ def main(argv=None):
                          "passes --dist_threshold_ratio 5")
     ap.add_argument("--out", required=True, help="output PLY")
     a = ap.parse_args(argv)
+    if a.band and a.threshold is None:
+        ap.error("--band needs --threshold (the MeshUDF lattice is evaluated narrow-band without it)")
     if a.threshold is not None:
-        for flag, given in (("--postprocess", a.postprocess), ("--dense", a.dense), ("--lipschitz", a.lipschitz is not None),
+        for flag, given in (("--postprocess", a.postprocess), ("--dense", a.dense),
+                            ("--lipschitz", a.lipschitz is not None and not a.band),
                             ("--dist_threshold_ratio", a.dist_threshold_ratio is not None)):
             if given:
                 ap.error("--threshold cannot be combined with %s" % flag)
@@ -408,10 +436,16 @@ def main(argv=None):
     ck = torch.load(a.ckpt, map_location="cpu", weights_only=True)
     net = udf_network_from_state(ck["udf_network_fine"] if "udf_network_fine" in ck else ck, a.scale).cuda()
     if a.threshold is not None:                   # exp_runner_blending.py:746-761, renderer.extract_geometry
-        from neuraludf_b200.models.udf_renderer_blending import extract_geometry
+        from neuraludf_b200.models.udf_renderer_blending import box_vertices, extract_geometry
         bmin, bmax, sm = threshold_box(a.cameras)
-        v, faces = extract_geometry(torch.tensor(bmin, dtype=torch.float32), torch.tensor(bmax, dtype=torch.float32),
-                                    a.resolution, a.threshold, lambda pts: net.udf_values(pts), torch.device("cuda"))
+        bmin, bmax = torch.tensor(bmin, dtype=torch.float32), torch.tensor(bmax, dtype=torch.float32)
+        if a.band:                                # extract_geometry's device path with NUDF_BAND_MESH=1
+            v, faces, _ = iso_mesh_band(lambda pts: net.udf_values(pts), bmin, bmax, a.resolution, a.threshold,
+                                        lipschitz=a.lipschitz, device=torch.device("cuda"))
+            v, faces = box_vertices(v.cpu().numpy(), a.resolution, bmin, bmax), faces.cpu().numpy()
+        else:
+            v, faces = extract_geometry(bmin, bmax, a.resolution, a.threshold, lambda pts: net.udf_values(pts),
+                                        torch.device("cuda"))
         if sm is not None:
             v = v * sm[0, 0] + sm[:3, 3][None]
         write_ply_mesh(a.out, v, faces)

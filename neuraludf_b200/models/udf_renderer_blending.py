@@ -16,6 +16,7 @@ gathers of pixel and homography-warped patch colours, masked-softmax fusion over
 differentiable ray weights of the CUDA compositing kernel; patch_projector.py / fields.color_blend keep the op-by-op form.
 """
 import itertools
+import os
 
 import numpy as np
 import torch
@@ -32,7 +33,8 @@ GRID_BLOCK = 64     # the reference queries dense grids in 64^3 blocks (:16-49);
 def _grid_query_device(bound_min, bound_max, resolution, query_func, device, channels):
     """Evaluate query_func on the resolution^3 lattice spanned by the bounds, block by block; returns a float32 tensor
     [R, R, R] (channels == 0) or [R, R, R, channels] on the device."""
-    axes = [torch.linspace(float(bound_min[a]), float(bound_max[a]), resolution, device=device) for a in range(3)]
+    from ..grid import axis_tables
+    axes = axis_tables(bound_min, bound_max, resolution, device)
     out = torch.zeros([resolution] * 3 + ([channels] if channels else []), dtype=torch.float32, device=device)
     starts = range(0, resolution, GRID_BLOCK)
     for i0, j0, k0 in itertools.product(starts, starts, starts):
@@ -63,7 +65,10 @@ def extract_gradient_fields(bound_min, bound_max, resolution, query_func, device
 def extract_geometry(bound_min, bound_max, resolution, threshold, query_func, device):
     """reference :52-63.  With PyMCubes importable, exactly the reference's path.  Without it, the lattice stays on the
     device and is meshed there (mesh.iso_marching_cubes_index: fp32 threshold, faces wound towards decreasing values, this
-    project's vertex numbering and ambiguous-cell triangulation); the vertices then take the reference's mapping below."""
+    project's vertex numbering and ambiguous-cell triangulation); the vertices then take the reference's mapping
+    (box_vertices).  With NUDF_BAND_MESH=1 in the environment (and no PyMCubes) the lattice is evaluated narrow-band
+    (mesh.iso_mesh_band, Lipschitz bound 2): the same mesh when query_func is 2-Lipschitz and gives a point the same bits
+    in any batch."""
     try:
         import mcubes
     except ImportError:
@@ -72,15 +77,23 @@ def extract_geometry(bound_min, bound_max, resolution, threshold, query_func, de
         u = extract_fields(bound_min, bound_max, resolution, query_func, device)
         vertices, triangles = mcubes.marching_cubes(u, threshold)
     else:
-        from ..mesh import iso_marching_cubes_index
+        from ..mesh import iso_marching_cubes_index, iso_mesh_band
         with torch.no_grad():
-            u = _grid_query_device(bound_min, bound_max, resolution, query_func, device, 0)
-            v, f, _ = iso_marching_cubes_index(u, u.shape, threshold)
+            if os.environ.get("NUDF_BAND_MESH") == "1":
+                v, f, _ = iso_mesh_band(query_func, bound_min, bound_max, resolution, threshold, device=device)
+            else:
+                u = _grid_query_device(bound_min, bound_max, resolution, query_func, device, 0)
+                v, f, _ = iso_marching_cubes_index(u, u.shape, threshold)
         vertices, triangles = v.cpu().numpy(), f.cpu().numpy()
+    return box_vertices(vertices, resolution, bound_min, bound_max), triangles
+
+
+def box_vertices(vertices, resolution, bound_min, bound_max):
+    """lattice-index vertices -> box coordinates, as the reference maps them (:59-62): v / (R - 1) * (b_max - b_min) + b_min,
+    the box difference in fp32"""
     b_max_np = bound_max.detach().cpu().numpy()
     b_min_np = bound_min.detach().cpu().numpy()
-    vertices = vertices / (resolution - 1.0) * (b_max_np - b_min_np)[None, :] + b_min_np[None, :]
-    return vertices, triangles
+    return vertices / (resolution - 1.0) * (b_max_np - b_min_np)[None, :] + b_min_np[None, :]
 
 
 def sample_pdf(bins, weights, n_samples, det=False):
