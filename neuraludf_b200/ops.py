@@ -545,21 +545,53 @@ def _make_cfg(N, S, O, sample_dist, cos_anneal_ratio, flip_saturation, sparse_sc
     return cfg
 
 
+def _composite_udf(udf, N, S):
+    """udf as the kernels read it: (a [P] tensor, P = N*S, element p at p * ld_udf; ld_udf).  Takes [P] (a strided column
+    view too), [P, 1] or [N, S]; raises ValueError for any other shape."""
+    P = N * S
+    if udf.dtype != torch.float32:
+        udf = udf.float()
+    if tuple(udf.shape) == (N, S):
+        udf = udf.reshape(P)                # a copy only when the rows are not evenly strided
+    elif tuple(udf.shape) == (P, 1):
+        udf = udf[:, 0]
+    if tuple(udf.shape) != (P,):
+        raise ValueError("composite: udf of shape %s; expected [%d], [%d, 1] or [%d, %d]" % (tuple(udf.shape), P, P, N, S))
+    return udf, (udf.stride(0) if P > 1 else 1)
+
+
+def _check_composite_rows(N, S, O, **ts):
+    """Every per-sample tensor has N*S rows, the background ones N*(S+O), rays_d N; vectors are 3 wide.  Checked before
+    any launch: the kernels index these by ray and sample with no bound of their own."""
+    rows = {"rays_d": N, "bg_alpha": N * (S + O), "bg_color": N * (S + O), "heads": 1}
+    width = {"grads": 3, "scb": 3, "sc": 3, "pts": 3, "rays_d": 3, "bg_color": 3, "heads": 3}
+    for name, t in ts.items():
+        if t is None:
+            continue
+        r, w = rows.get(name, N * S), width.get(name, 1)
+        if t.numel() != r * w or (w > 1 and t.shape[-1] != w):
+            raise ValueError("composite: %s of shape %s; expected %d rows%s (N = %d rays, S = %d samples, O = %d)" % (
+                name, tuple(t.shape), r, " of %d" % w if w > 1 else "", N, S, O))
+
+
 class _CompositeFunction(torch.autograd.Function):
-    """differentiable inputs: udf [P], grads [P,3], scb [P,3], sc [P,3], bg_alpha [N,S+O], bg_color [N,S+O,3], heads [3]"""
+    """differentiable inputs: udf [P] / [P,1] / [N,S], grads [P,3], scb [P,3], sc [P,3], bg_alpha [N,S+O],
+    bg_color [N,S+O,3], heads [3]"""
 
     @staticmethod
     def forward(ctx, udf, grads, scb, sc, bg_alpha, bg_color, heads, geom, cfg, want_diag):
-        lib = L.lib()
-        rays_d, pts, mid, dists = geom
         N, S, O = cfg.n_rays, cfg.n_samples, cfg.n_outside
+        udf_shape = udf.shape
+        udf, ld_udf = _composite_udf(udf, N, S)
+        geom = tuple(_f32c(t) for t in geom)
+        rays_d, pts, mid, dists = geom
+        _check_composite_rows(N, S, O, grads=grads, scb=scb, sc=sc, pts=pts, mid=mid, dists=dists, rays_d=rays_d,
+                              heads=heads, bg_alpha=bg_alpha, bg_color=bg_color)
+        lib = L.lib()
         dev = grads.device
-        if udf.dtype != torch.float32:
-            udf = udf.float()
-        ld_udf = udf.stride(0) if udf.dim() >= 1 and udf.numel() > 1 else 1
         grads, scb, sc, heads = _f32c(grads), _f32c(scb), _f32c(sc), _f32c(heads)
         bg_alpha, bg_color = _f32c(bg_alpha), _f32c(bg_color)
-        _require_cuda(udf, grads, scb, sc, heads, rays_d, pts, mid, dists)
+        _require_cuda(udf, grads, scb, sc, heads, rays_d, pts, mid, dists, bg_alpha, bg_color)
         f = lambda *shape: torch.empty(*shape, dtype=torch.float32, device=dev)
         outs = {"color_base": f(N, 3), "color": f(N, 3), "depth": f(N, 1), "normals": f(N, 3), "weights": f(N, S + O),
                 "weight_sum": f(N, 1), "weight_sum_fg_bg": f(N, 1), "ray_sums": f(N, 5)}
@@ -575,7 +607,7 @@ class _CompositeFunction(torch.autograd.Function):
                                                   L.ptr(dists), L.ptr(udf), ld_udf, L.ptr(grads), L.ptr(scb), L.ptr(sc),
                                                   L.ptr(bg_alpha), L.ptr(bg_color), ctypes.byref(ro), L.stream_ptr()),
                 "nudf_render_composite_forward")
-        ctx.cfg, ctx.geom, ctx.ld_udf = cfg, geom, ld_udf
+        ctx.cfg, ctx.geom, ctx.ld_udf, ctx.udf_shape = cfg, geom, ld_udf, udf_shape
         ctx.has_bg = bg_alpha is not None
         ctx.save_for_backward(udf, grads, scb, sc, bg_alpha, bg_color, heads)
         diff = ("color_base", "color", "depth", "weight_sum", "weight_sum_fg_bg", "ray_sums", "weights")
@@ -614,8 +646,8 @@ class _CompositeFunction(torch.autograd.Function):
                                                    L.ptr(udf_bar), L.ptr(grads_bar), L.ptr(scb_bar), L.ptr(sc_bar),
                                                    L.ptr(bga_bar), L.ptr(bgc_bar), L.ptr(scal), L.stream_ptr()),
                 "nudf_render_composite_backward")
-        # udf came in as a (possibly strided) [P] view
-        return (udf_bar.reshape(udf.shape), grads_bar, scb_bar, sc_bar, bga_bar, bgc_bar, scal.sum(dim=0),
+        # in the caller's shape: [P] (possibly a strided view), [P, 1] or [N, S]
+        return (udf_bar.reshape(ctx.udf_shape), grads_bar, scb_bar, sc_bar, bga_bar, bgc_bar, scal.sum(dim=0),
                 None, None, None)
 
 

@@ -239,7 +239,9 @@ def exclusive_cumprod(t):
 # a9: inverse-CDF sampling, models/udf_renderer_blending.py:66-104 (det=True only) ---------------
 # ----------------------------------------------------------------------------------------------
 
-def sample_pdf_det(bins, weights, n_samples, return_inds=False):
+def sample_pdf_det(bins, weights, n_samples, return_inds=False, trace=None):
+    """trace: a list that receives dict(weights, cdf, u, inds) of the call (the cdf the indices were searched in)."""
+    raw_weights = weights
     weights = weights + 1e-5
     pdf = weights / torch.sum(weights, -1, keepdim=True)
     cdf = torch.cumsum(pdf, -1)
@@ -256,6 +258,9 @@ def sample_pdf_det(bins, weights, n_samples, return_inds=False):
     denom = torch.where(denom < 1e-5, torch.ones_like(denom), denom)
     t = (u - c0) / denom
     samples = b0 + t * (b1 - b0)
+    if trace is not None:
+        trace.append(dict(weights=raw_weights.detach().clone(), cdf=cdf.detach().clone(), u=u[:1].clone(),
+                          inds=inds.clone()))
     if return_inds:
         return samples, inds
     return samples
@@ -269,7 +274,8 @@ def _append_last(t, value):
     return torch.cat([t, torch.full_like(t[..., :1], value)], dim=-1)
 
 
-def up_sample_unbias(o, d, z, udf, sample_dist, n_importance, inv_s, beta, gamma, return_inds=False):
+def up_sample_unbias(o, d, z, udf, sample_dist, n_importance, inv_s, beta, gamma, return_inds=False, trace=None):
+    """trace: as sample_pdf_det."""
     n_rays, n = z.shape
     pts = o[:, None, :] + d[:, None, :] * z[..., :, None]
     radius = torch.linalg.norm(pts, ord=2, dim=-1)
@@ -292,15 +298,15 @@ def up_sample_unbias(o, d, z, udf, sample_dist, n_importance, inv_s, beta, gamma
     a_minus = neus_alpha(-mid_udf, cos_val, dists, inv_s)
     alpha = a_plus * signs + a_minus * (1 - signs)
     weights = alpha * exclusive_cumprod(1.0 - alpha + 1e-7)
-    return sample_pdf_det(z, weights, n_importance, return_inds=return_inds)
+    return sample_pdf_det(z, weights, n_importance, return_inds=return_inds, trace=trace)
 
 
-def up_sample_no_occ_aware(o, d, z, udf, sample_dist, n_importance, beta, gamma, return_inds=False):
-    """:834-866 -- note the reference passes (inv_s, beta, gamma) but only beta/gamma are used."""
+def up_sample_no_occ_aware(o, d, z, udf, sample_dist, n_importance, beta, gamma, return_inds=False, trace=None):
+    """:834-866 -- note the reference passes (inv_s, beta, gamma) but only beta/gamma are used.  trace: as sample_pdf_det."""
     dists = _append_last(z[..., 1:] - z[..., :-1], sample_dist)
     raw_occ = logistic_density(udf, beta, gamma, 1.0)
     alpha_occ = 1.0 - torch.exp(-F.relu(raw_occ) * dists)
-    return sample_pdf_det(z, alpha_occ[:, :-1], n_importance, return_inds=return_inds)
+    return sample_pdf_det(z, alpha_occ[:, :-1], n_importance, return_inds=return_inds, trace=trace)
 
 
 def merge_z(z, new_z):
