@@ -299,7 +299,9 @@ int nudf_outside_points(const float* rays_o, const float* rays_d, const float* z
  *   px     [n_rays,2] pixel coordinates of each ray in the query image (patch centre)
  *   imgs   [V,3,H,W] source images;  logits [P, ld_logits]: blending logits, the first V columns are used
  *   c_pix  [P,3] blended pixel colour;  c_pat [P,(2h+1)^2,3] blended patch colours;  m_pat [P] 1 if any view sees the
- *   whole patch.  Backward: gradients w.r.t. the logits only ([P,V]); everything else is a constant of the graph. */
+ *   whole patch.  Backward: gradients w.r.t. the logits only ([P,V]); everything else is a constant of the graph.
+ *   Limits: 1 <= n_views <= 32, 0 <= h_patch <= 5 (patches of at most 11 x 11 = 121 pixels); otherwise -1 and
+ *   nudf_last_error(), nothing is launched. */
 typedef struct {
   int32_t n_rays, n_samples, n_views, height, width, h_patch;
 } nudf_blend_cfg;

@@ -3,8 +3,10 @@ reference's `models/patch_projector.py` (`PatchProjector.pixel_warp` :21-43, `.p
 `models/projector_utils.py` (`sample_ptsFeatures_from_featureMaps` :52-85).
 
 Status (DESIGN.md, SURVEY 8(f) rank 1): the renderer uses the fused kernel `ops.blend_views` (csrc/blend.cu) fed by
-`PatchProjector.homographies` (small batched 3x3 algebra in torch); `pixel_warp` / `patch_warp` below are the op-by-op
-form (`grid_sample`, `einsum`) kept as API mirrors of the reference and as the test reference of the fused kernel.
+`PatchProjector.homographies` (small batched 3x3 algebra in torch) for patches of up to 11 x 11 pixels (h_patch_size <= 5,
+which covers the fine-tuning conf's h_patch_size = 5) and for pixel-only blending at any patch size; `pixel_warp` /
+`patch_warp` below are the op-by-op form (`grid_sample`, `einsum`) kept as API mirrors of the reference, as the test
+reference of the fused kernel, and as the renderer's path for larger patches, `img_index` and more than 32 source views.
 Unlike the reference, `patch_warp` does not modify the caller's `uv` tensor in place.
 """
 import torch

@@ -13,7 +13,8 @@ Differences that are deliberate (DESIGN.md "boundary"):
     .detach() or for logging (exp_runner_blending.py:309-371, 641-668); `weights` is differentiable.
 Pixel / patch blending (fine-tuning stage, :431-480): one fused CUDA kernel per pass (csrc/blend.cu: projection, bilinear
 gathers of pixel and homography-warped patch colours, masked-softmax fusion over views), composited with the
-differentiable ray weights of the CUDA compositing kernel; patch_projector.py / fields.color_blend keep the op-by-op form.
+differentiable ray weights of the CUDA compositing kernel; patch_projector.py / fields.color_blend keep the op-by-op form,
+which runs only for patches larger than 11 x 11 (h_patch_size > 5), img_index or more than 32 source views.
 """
 import itertools
 import os
@@ -28,6 +29,8 @@ from .patch_projector import PatchProjector
 
 
 GRID_BLOCK = 64     # the reference queries dense grids in 64^3 blocks (:16-49); 262 144 points per kernel chain here
+FUSED_MAX_H_PATCH = 5   # largest patch half-size of the fused blending kernel (11 x 11 pixels, csrc/blend.cu)
+FUSED_MAX_VIEWS = 32    # largest number of source views of the fused blending kernel (one lane per view)
 
 
 def _grid_query_device(bound_min, bound_max, resolution, query_func, device, channels):
@@ -303,9 +306,11 @@ class UDFRendererBlending:
             gn = g3 / (torch.linalg.norm(g3, ord=2, dim=-1, keepdim=True) + 1e-5)
             cos = (rays_d[:, None, :] * gn).sum(-1, keepdim=True)
             normals = torch.where(cos == 0, torch.ones_like(cos), -torch.sign(cos)) * gn
-        if img_index is None and self.h_patch_size <= 3 and color_maps.shape[0] <= 32:
+        if (img_index is None and color_maps.shape[0] <= FUSED_MAX_VIEWS
+                and (rays_uv is None or self.h_patch_size <= FUSED_MAX_H_PATCH)):
             # fused kernel: projection + bilinear gathers + masked-softmax fusion per point (csrc/blend.cu); the small
-            # per-point homographies come from torch (3x3 algebra on [V, P] matrices, no gradient)
+            # per-point homographies come from torch (3x3 algebra on [V, P] matrices, no gradient).  Pixel blending does
+            # not depend on the patch size, so without uv the kernel runs with h_patch = 0 whatever h_patch_size is.
             n_views = color_maps.shape[0]
             proj = (intrinsics[:, :3, :3] @ w2cs[:, :3, :]).reshape(n_views, 12)
             hom, px = None, None
@@ -313,10 +318,11 @@ class UDFRendererBlending:
                 hom, px = self.patch_projector.homographies(p3, rays_uv, normals, color_maps.shape[2:], intrinsics[0],
                                                             intrinsics, query_c2w, torch.inverse(w2cs))
                 hom = hom.reshape(n_views, -1, 9)
+            h_patch = self.h_patch_size if rays_uv is not None else 0
             c_pix, c_pat, m_pat = ops.blend_views(blending_weights.reshape(batch_size * n_samples, -1), p3.reshape(-1, 3), proj,
-                                                  hom, px, color_maps, batch_size, n_samples, self.h_patch_size)
+                                                  hom, px, color_maps, batch_size, n_samples, h_patch)
         else:
-            # op-by-op path: img_index selection (never used by the runner), patches larger than 7 x 7, > 32 source views
+            # op-by-op path: img_index selection (never used by the runner), patches larger than 11 x 11, > 32 source views
             pix_col, pix_mask = self.patch_projector.pixel_warp(p3, color_maps, intrinsics, w2cs, img_wh=None)
             pat_col, pat_mask = None, None
             if rays_uv is not None:
