@@ -507,6 +507,16 @@ int nudf_mp_smooth_step(const double* verts_in, double* verts_out, const int64_t
                         const int64_t* rowptr, const int64_t* cols, double lambda, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * Connected components of a mesh's faces (neuraludf_b200/clean.py face_components; sizes and selection in torch)
+ * ------------------------------------------------------------------------------------------------------------ */
+/* keys [n_keys] ascending: edge keys lo * V + hi (nudf_mp_faces' edge codes >> 1); key_face[e] in [0, n_faces): the face
+ * of key slot e.  A key occurring exactly twice, from two different faces, joins those faces (trimesh face_adjacency).
+ * label[F] <- the smallest face index of each face's component; paired[F] <- 1 when the face is in at least one such pair.
+ * Three launches (init, hook, compress), no host synchronisation; the labels do not depend on scheduling. */
+int nudf_cc_label(const int64_t* keys, const int64_t* key_face, int64_t n_keys, int64_t n_faces, int64_t* label,
+                  uint8_t* paired, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------
  * Colour loss of the training step (replaces loss/loss.py ColorLoss with loss/patch_metric.py; neuraludf_b200/loss.py)
  * ------------------------------------------------------------------------------------------------------------
  * fp32, row-major, contiguous.  N rays, P = (2 h_patch + 1)^2 patch pixels (row-major, the patch's x fastest). */

@@ -12,10 +12,19 @@ NumPy.  The projection runs in one fixed fp64 order (`count_views`); NumPy's mat
 vertex whose projection lies within rounding of a half-integer pixel to the neighbouring pixel.
 
 Images are any H x W (the reference requires 1600 x 1200 and gives the same result there).  What trimesh does on load and
-export (merging vertices, dropping unreferenced ones) is not reproduced: the outputs are the script's arrays.  CLI:
+export (merging vertices, dropping unreferenced ones) is not reproduced: the outputs are the script's arrays.
+
+The script's clean_outliers (:158-191) is here too: `clean_outliers` merges as trimesh.load does, then keeps the largest
+connected piece of faces (`keep_largest`) or drops the pieces of fewer than faces_num faces (`remove_small_components`).
+The face labelling is CUDA (csrc/mesh_cc.cu); sizes, selection and compaction are torch.  tests/proto/mesh_cc.py restates
+it with scipy's connected components.  CLI:
 
     python -m neuraludf_b200.clean --mesh M.ply --dtu_dir D --scan N [--out_dir O] [--mask_kernel 11] [--minimal_vis 2]
-                                   [--imgs_idx I ...]
+                                   [--imgs_idx I ...] [--outliers {largest,faces} [--faces_num 500]]
+    python -m neuraludf_b200.clean --mesh M.ply --outliers {largest,faces} [--faces_num 500] [--out PATH]
+
+With --scan, --outliers also writes final_<scan>.ply, clean_outliers of the visual-hull result; clean_<scan>.ply and
+visualhull_<scan>.ply are the same as without it.  Without --dtu_dir / --scan, only clean_outliers runs, on --mesh.
 """
 import argparse
 import ctypes
@@ -32,6 +41,7 @@ from neuraludf_b200._lib import check, ptr
 # the script's main block and visual-hull constants (clean_dtu_mesh.py:95, 105, 198, 213-217)
 MASK_KERNEL, MINIMAL_VIS, HULL_KERNEL_EXTRA, HULL_BORDER, HULL_MAX_OUTSIDE = 11, 2, 20, 50, 5
 MAX_KERNEL = 255
+FACES_NUM = 500                 # clean_outliers' default (clean_dtu_mesh.py:180)
 
 
 def ellipse_element(k):
@@ -200,6 +210,114 @@ def clean_dtu_mesh(verts, faces, world_mats, masks, mask_kernel=MASK_KERNEL, min
     return tuple(stages)
 
 
+def _faces(faces, n_verts, dev):
+    f = torch.as_tensor(faces).to(dev).to(torch.int64).reshape(-1, 3).contiguous()
+    if f.numel() and (int(f.min()) < 0 or int(f.max()) >= n_verts):
+        raise ValueError("face index out of range")
+    return f
+
+
+def _label_faces(keys, key_face, n_faces):
+    """csrc/mesh_cc.cu on sorted edge keys and their faces: (label int64 [F], paired uint8 [F]); no host synchronisation"""
+    dev = keys.device
+    label = torch.empty(n_faces, dtype=torch.int64, device=dev)
+    paired = torch.empty(n_faces, dtype=torch.uint8, device=dev)
+    check(_lib.lib().nudf_cc_label(ptr(keys), ptr(key_face), keys.numel(), n_faces, ptr(label), ptr(paired),
+                                   _lib.stream_ptr()), "nudf_cc_label")
+    return label, paired
+
+
+def _edge_keys(verts, faces):
+    """(ascending edge keys lo * V + hi of every face slot, the face of each key): nudf_mp_faces' edge codes, sorted"""
+    from neuraludf_b200.mesh_post import _face_pass
+    if faces.shape[0] == 0:
+        e = torch.empty(0, dtype=torch.int64, device=faces.device)
+        return e, e
+    codes = _face_pass(verts, faces, None)[2]
+    keys, order = torch.sort(codes.reshape(-1) >> 1)
+    return keys, order // 3
+
+
+@torch.no_grad()
+def face_components(faces, verts=None):
+    """Connected components of the faces under trimesh's face_adjacency: (label int64 [F], the smallest face index of each
+    face's component; paired uint8 [F], 1 when the face shares an edge used by exactly two face slots with another face).
+    An edge used by one face, or by three or more, joins nothing, and a degenerate face (a, a, b) pairs only with itself,
+    which is dropped.  verts: the fp64 [V, 3] the faces index (default: zeros over max(faces) + 1 vertices; only the
+    vertex count matters)."""
+    dev = _device_of(faces, verts)
+    if verts is None:
+        f = torch.as_tensor(faces).to(dev)
+        verts = torch.zeros(int(f.max()) + 1 if f.numel() else 0, 3, dtype=torch.float64, device=dev)
+    verts = _points(verts, dev)
+    f = _faces(faces, verts.shape[0], dev)
+    keys, key_face = _edge_keys(verts, f)
+    return _label_faces(keys, key_face, f.shape[0])
+
+
+def _sizes(label, count):
+    """int64 [F]: at each root, the number of its component's faces where `count` (int64 0/1) is set; 0 elsewhere.  A
+    scatter-add rather than torch.bincount, which reads its input's maximum on the host."""
+    return torch.zeros_like(label).index_add_(0, label, count)
+
+
+def _largest(label):
+    """faces of the largest component: equal sizes go to the smallest face index (scipy's component order, np.argmax's
+    first maximum)"""
+    if label.numel() == 0:
+        return torch.zeros(0, dtype=torch.bool, device=label.device)
+    return label == torch.argmax(_sizes(label, torch.ones_like(label)))
+
+
+def _at_least(label, paired, faces_num):
+    """faces in a pair whose component, counted over the paired faces, has at least faces_num faces"""
+    p = paired.bool()
+    return p & (_sizes(label, p.to(torch.int64))[label] >= faces_num)
+
+
+def _submesh(verts, faces, keep):
+    """the kept faces in ascending index over the vertices they reference, in ascending index (trimesh submesh)"""
+    f = faces[keep]
+    used = torch.zeros(verts.shape[0], dtype=torch.bool, device=verts.device)
+    used[f.reshape(-1)] = True
+    rank = torch.cumsum(used.to(torch.int64), 0) - 1
+    return verts[used], rank[f]
+
+
+def _filter(verts, faces, keep_largest, faces_num):
+    dev = _device_of(verts, faces)
+    v = _points(verts, dev)
+    f = _faces(faces, v.shape[0], dev)
+    label, paired = _label_faces(*_edge_keys(v, f), f.shape[0])
+    return _submesh(v, f, _largest(label) if keep_largest else _at_least(label, paired, faces_num))
+
+
+@torch.no_grad()
+def keep_largest(verts, faces):
+    """trimesh's split(only_watertight=False) followed by the piece with the most faces (clean_outliers, keep_largest=True):
+    (fp64 verts, int64 faces).  Every face is a node, so an isolated face is a piece of one face; equal sizes go to the
+    piece holding the smallest face index.  The pieces' holes are not filled."""
+    return _filter(verts, faces, True, 0)
+
+
+@torch.no_grad()
+def remove_small_components(verts, faces, faces_num=FACES_NUM):
+    """What clean_mesh_by_faces_num means to do (the reference's indexing cannot run): keep the faces of every component of
+    face_adjacency with at least faces_num faces, counted over the faces in a pair; a face in no pair is dropped."""
+    return _filter(verts, faces, False, faces_num)
+
+
+@torch.no_grad()
+def clean_outliers(verts, faces, faces_num=FACES_NUM, keep_largest=True):
+    """clean_outliers of clean_dtu_mesh.py: the merge trimesh.load applies (non-finite faces dropped, vertices on one 1e-8
+    grid point merged, unreferenced ones dropped), then keep_largest (keep_largest=True) or remove_small_components."""
+    from neuraludf_b200.mesh_post import export_merge
+    dev = _device_of(verts, faces)
+    v = _points(verts, dev)
+    v, f = export_merge(v, _faces(faces, v.shape[0], dev))
+    return _filter(v, f, keep_largest, faces_num)
+
+
 def load_dtu_scan(dtu_dir, scan, imgs_idx=None):
     """(world_mats float64 [V, 4, 4], masks uint8 [V, H, W]) of views imgs_idx (default: all 49 views of scans below 83,
     64 above) of <dtu_dir>/scan<scan>: `world_mat_i` of cameras.npz and channel 0 of cv2.imread of the i-th file of
@@ -232,16 +350,37 @@ def main(argv=None):
     from neuraludf_b200.evaluate import read_ply, write_ply_mesh
     ap = argparse.ArgumentParser(prog="python -m neuraludf_b200.clean", description=__doc__.split("\n\n")[0])
     ap.add_argument("--mesh", required=True, help="mesh to clean, PLY in the scan's world coordinates")
-    ap.add_argument("--dtu_dir", required=True, help="directory holding scan<N>/cameras.npz and scan<N>/mask/*.png")
-    ap.add_argument("--scan", type=int, required=True)
+    ap.add_argument("--dtu_dir", default=None, help="directory holding scan<N>/cameras.npz and scan<N>/mask/*.png")
+    ap.add_argument("--scan", type=int, default=None)
     ap.add_argument("--out_dir", default=None, help="where clean_<scan>.ply and visualhull_<scan>.ply go (default: beside --mesh)")
     ap.add_argument("--mask_kernel", type=int, default=MASK_KERNEL)
     ap.add_argument("--minimal_vis", type=int, default=MINIMAL_VIS)
     ap.add_argument("--imgs_idx", type=int, nargs="*", default=None, help="views to use (default: all of the scan's)")
+    ap.add_argument("--outliers", choices=("largest", "faces"), default=None,
+                    help="clean_outliers after the visual-hull pass (written to final_<scan>.ply), or on --mesh alone without "
+                         "--dtu_dir / --scan: keep the largest piece, or drop the pieces of fewer than --faces_num faces")
+    ap.add_argument("--faces_num", type=int, default=FACES_NUM)
+    ap.add_argument("--out", default=None, help="output of --outliers on --mesh alone (default: final_<mesh name> beside it)")
     a = ap.parse_args(argv)
+    if (a.dtu_dir is None) != (a.scan is None):
+        ap.error("--dtu_dir and --scan go together")
+    if a.dtu_dir is None and a.outliers is None:
+        ap.error("--dtu_dir and --scan are required unless --outliers cleans --mesh alone")
+    if a.dtu_dir is not None and a.out is not None:
+        ap.error("--out is for --outliers on --mesh alone; with --dtu_dir the outputs go to --out_dir")
     verts, faces = read_ply(a.mesh)
     if faces is None:
         raise SystemExit("%s has no faces" % a.mesh)
+
+    def outliers(v, f, path):
+        v, f = clean_outliers(v, f, faces_num=a.faces_num, keep_largest=a.outliers == "largest")
+        write_ply_mesh(path, v, f)
+        print("%s: %d vertices, %d faces" % (path, v.shape[0], f.shape[0]))
+        return v, f
+
+    if a.dtu_dir is None:
+        head, tail = os.path.split(os.path.abspath(a.mesh))
+        return outliers(verts, faces, a.out if a.out is not None else os.path.join(head, "final_" + tail))
     mats, masks = load_dtu_scan(a.dtu_dir, a.scan, a.imgs_idx)
     out_dir = a.out_dir if a.out_dir is not None else os.path.dirname(os.path.abspath(a.mesh))
     os.makedirs(out_dir, exist_ok=True)
@@ -250,6 +389,9 @@ def main(argv=None):
         path = os.path.join(out_dir, "%s_%03d.ply" % (name, a.scan))
         write_ply_mesh(path, v, f)
         print("%s: %d vertices, %d faces" % (path, v.shape[0], f.shape[0]))
+    if a.outliers is not None:
+        v, f, _ = stages[1]
+        return stages + (outliers(v, f, os.path.join(out_dir, "final_%03d.ply" % a.scan)),)
     return stages
 
 
