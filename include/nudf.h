@@ -481,6 +481,54 @@ int nudf_nb_emit_box(const uint8_t* flags, int32_t n, int32_t s, int32_t t, cons
                      void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * Block-sparse narrow band (neuraludf_b200/grid.py udf_band_sparse drives the levels, mesh.py udf_mesh_sparse meshes it)
+ * ------------------------------------------------------------------------------------------------------------
+ * The N^3 lattice of the nudf_nb_* entry points held without an N^3 array.  The points of the stride-c lattice (0, c, 2 c,
+ * ... and N - 1 per axis; mc = ceil((N - 1) / c) + 1) live in the dense array coarse[mc^3], point (i, j, k) at
+ * (ci * mc + cj) * mc + ck with ci = i / c, or mc - 1 for i = N - 1.  Every other point lives in a brick of NUDF_BRICK^3
+ * points: brick (i / 8, j / 8, k / 8), numbered (bx * nbk + by) * nbk + bz (nbk = ceil(N / 8)), has slot dir[brick] (-1:
+ * none), and the point is bricks[slot * 512 + ((i % 8) * 8 + j % 8) * 8 + k % 8].  keys[slot] is the brick number of
+ * each slot, ascending.  A point of a brick without a slot reads +inf, as do the slots of the stride-c points inside
+ * bricks (they are read from coarse).  Storage positions (nudf_sb_flat): [0, mc^3) for coarse, mc^3 + slot * 512 + local
+ * for the bricks.  All pointers DEVICE; the descriptor itself is host memory. */
+#define NUDF_BRICK 8
+typedef struct nudf_brick_store {
+  int32_t n, c, mc, nbk;
+  int64_t n_bricks;
+  float* coarse;          /* [mc^3] */
+  int32_t* dir;           /* [nbk^3] */
+  float* bricks;          /* [n_bricks * 512] */
+  const int64_t* keys;    /* [n_bricks] */
+} nudf_brick_store;
+/* nudf_nb_block_test with the corner values read from the store */
+int nudf_sb_block_test(const nudf_brick_store* st, int32_t s, const uint8_t* parent_flags, int32_t parent_s, double voxel,
+                       double lipschitz, double tau, uint8_t* flags, uint32_t* max_slope, void* stream);
+/* marks[b] = 1 (marks: [nbk^3], zeroed by the caller) for every brick b that meets the closed box of a kept block of
+ * stride s (flags [ceil((N - 1) / s)^3], nudf_nb_block_test's); s must be a multiple of the store's c */
+int nudf_sb_mark(const nudf_brick_store* st, int32_t s, const uint8_t* flags, int32_t* marks, void* stream);
+/* writes vals[t] to lattice point idx[t] (flat); -1 when a point is neither on the stride-c lattice nor in a brick with a
+ * slot (nothing is written then) */
+int nudf_sb_store(const nudf_brick_store* st, const int64_t* idx, const float* vals, int64_t n, int32_t* missing, void* stream);
+/* out[t] = the value of lattice point idx[t] (flat) */
+int nudf_sb_gather(const nudf_brick_store* st, const int64_t* idx, int64_t n, float* out, void* stream);
+/* out[t] = the flat lattice index of storage position pos[t] */
+int nudf_sb_flat(const nudf_brick_store* st, const int64_t* pos, int64_t n, int64_t* out, void* stream);
+/* The MeshUDF marching cubes stages nudf_mc_active, _cell_signs, _links, _count, _emit and _vertices on the store's N^3
+ * lattice (n0 = n1 = n2 = N), the same arguments otherwise; nudf_mc_polarity reads no df and is shared. */
+int nudf_mcs_active(const nudf_brick_store* st, const int64_t* cand, int64_t n_cand, float avg_t, float max_t, uint8_t* flags,
+                    void* stream);
+int nudf_mcs_cell_signs(const nudf_brick_store* st, const int64_t* cells, int64_t n_cells, const int64_t* idx, int64_t n_idx,
+                        const float* normals, uint8_t* mask, void* stream);
+int nudf_mcs_links(const nudf_brick_store* st, const int64_t* cells, int64_t n_cells, const uint8_t* mask, int64_t* links,
+                   void* stream);
+int nudf_mcs_count(const nudf_brick_store* st, const int64_t* cells, int64_t n_cells, const uint8_t* mask, int32_t* counts,
+                   void* stream);
+int nudf_mcs_emit(const nudf_brick_store* st, const int64_t* cells, int64_t n_cells, const uint8_t* mask,
+                  const int64_t* offsets, int64_t* keys, void* stream);
+int nudf_mcs_vertices(const nudf_brick_store* st, const int64_t* cells, int64_t n_cells, const uint8_t* mask,
+                      const int64_t* keys, int64_t n_keys, float* verts, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------
  * Mesh post-processing (neuraludf_b200/mesh_post.py drives the steps; sorting, unique and compaction in torch)
  * ------------------------------------------------------------------------------------------------------------
  * verts: fp64 [V,3]; faces and edges: int64 rows.  All fp64 arithmetic is correctly rounded per operation with no

@@ -72,6 +72,16 @@ class RenderBar(ctypes.Structure):
                                         "ray_sums")]
 
 
+class BrickStore(ctypes.Structure):
+    """nudf_brick_store (include/nudf.h): the block-sparse narrow band's layout, device pointers"""
+    _fields_ = [("n", ctypes.c_int32), ("c", ctypes.c_int32), ("mc", ctypes.c_int32), ("nbk", ctypes.c_int32),
+                ("n_bricks", ctypes.c_int64), ("coarse", c_void_p), ("dir", c_void_p), ("bricks", c_void_p),
+                ("keys", c_void_p)]
+
+
+BRICK = 8   # NUDF_BRICK
+
+
 PATCH_TYPES = {"l1": 0, "ssd": 1, "ssim": 2, "ncc": 3}
 
 
@@ -216,6 +226,18 @@ _SIGNATURES = {
     "nudf_nb_block_test_box": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 2 + [c_void_p, ctypes.c_int32] + [c_void_p] * 3
                                + [ctypes.c_double] * 6 + [c_void_p] * 3),
     "nudf_nb_emit_box": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [c_void_p, ctypes.c_int64] + [c_void_p] * 7),
+    "nudf_sb_block_test": (ctypes.c_int, [c_void_p, ctypes.c_int32, c_void_p, ctypes.c_int32] + [ctypes.c_double] * 3
+                           + [c_void_p] * 3),
+    "nudf_sb_mark": (ctypes.c_int, [c_void_p, ctypes.c_int32] + [c_void_p] * 3),
+    "nudf_sb_store": (ctypes.c_int, [c_void_p] * 3 + [ctypes.c_int64] + [c_void_p] * 2),
+    "nudf_sb_gather": (ctypes.c_int, [c_void_p] * 2 + [ctypes.c_int64] + [c_void_p] * 2),
+    "nudf_sb_flat": (ctypes.c_int, [c_void_p] * 2 + [ctypes.c_int64] + [c_void_p] * 2),
+    "nudf_mcs_active": (ctypes.c_int, [c_void_p] * 2 + [ctypes.c_int64, ctypes.c_float, ctypes.c_float] + [c_void_p] * 2),
+    "nudf_mcs_cell_signs": (ctypes.c_int, [c_void_p] * 2 + [ctypes.c_int64, c_void_p, ctypes.c_int64] + [c_void_p] * 3),
+    "nudf_mcs_links": (ctypes.c_int, [c_void_p] * 2 + [ctypes.c_int64] + [c_void_p] * 3),
+    "nudf_mcs_count": (ctypes.c_int, [c_void_p] * 2 + [ctypes.c_int64] + [c_void_p] * 3),
+    "nudf_mcs_emit": (ctypes.c_int, [c_void_p] * 2 + [ctypes.c_int64] + [c_void_p] * 4),
+    "nudf_mcs_vertices": (ctypes.c_int, [c_void_p] * 2 + [ctypes.c_int64] + [c_void_p] * 2 + [ctypes.c_int64] + [c_void_p] * 2),
     "nudf_mp_faces": (ctypes.c_int, [c_void_p, ctypes.c_int64, c_void_p, ctypes.c_int64] + [c_void_p] * 6),
     "nudf_mp_hole_count": (ctypes.c_int, [c_void_p, ctypes.c_int64, c_void_p, c_void_p, ctypes.c_int64, c_void_p, c_void_p]),
     "nudf_mp_hole_emit": (ctypes.c_int, [c_void_p] * 3 + [ctypes.c_int64, c_void_p, c_void_p, ctypes.c_int64]

@@ -40,6 +40,7 @@
 
 #include "../../include/nudf.h"
 #include "common.cuh"
+#include "df_access.cuh"
 
 namespace nudf {
 namespace nb {
@@ -109,8 +110,9 @@ struct TableSpacing {
   __device__ __forceinline__ double edge(int a, int64_t e) const { return __dmul_rn((double)e, h[a]); }
 };
 
-template <class S>
-__global__ void k_block_test(const float* __restrict__ df, Lat B, const uint8_t* __restrict__ parent, int64_t ps, int64_t pnb,
+// A: the lattice reader (df_access.cuh): DenseDf for grid.udf_band / iso_band, BrickDf for grid.udf_band_sparse
+template <class A, class S>
+__global__ void k_block_test(A df, Lat B, const uint8_t* __restrict__ parent, int64_t ps, int64_t pnb,
                              S sp, double lip, double tau, uint8_t* __restrict__ flags, unsigned* __restrict__ max_slope) {
   const int64_t n = B.nb * B.nb * B.nb, N = B.N;
   const double thr = sp.thr(tau);
@@ -128,7 +130,7 @@ __global__ void k_block_test(const float* __restrict__ df, Lat B, const uint8_t*
         float u[8];
 #pragma unroll
         for (int c = 0; c < 8; ++c)
-          u[c] = df[((x0 + ((c >> 2) & 1) * ex) * N + (y0 + ((c >> 1) & 1) * ey)) * N + z0 + (c & 1) * ez];
+          u[c] = df(((x0 + ((c >> 2) & 1) * ex) * N + (y0 + ((c >> 1) & 1) * ey)) * N + z0 + (c & 1) * ez);
         bool nan = false;
         double mn = u[0];
 #pragma unroll
@@ -248,7 +250,7 @@ int nudf_nb_block_test(const float* df, int32_t n, int32_t s, const uint8_t* par
   NUDF_REQUIRE(lipschitz >= 0.0, "negative Lipschitz constant");
   const Lat B{n, s, cdiv(n - 1, s)};
   const int64_t pnb = parent_flags ? cdiv(n - 1, parent_s) : 0;
-  k_block_test<<<grid_for(B.nb * B.nb * B.nb), 256, 0, (cudaStream_t)stream>>>(df, B, parent_flags, parent_s, pnb,
+  k_block_test<<<grid_for(B.nb * B.nb * B.nb), 256, 0, (cudaStream_t)stream>>>(DenseDf{df}, B, parent_flags, parent_s, pnb,
                                                                                CubeSpacing{voxel}, lipschitz, tau, flags,
                                                                                max_slope);
   NUDF_LAUNCH_OK();
@@ -297,7 +299,7 @@ int nudf_nb_block_test_box(const float* df, int32_t n, int32_t s, const uint8_t*
   const Lat B{n, s, cdiv(n - 1, s)};
   const int64_t pnb = parent_flags ? cdiv(n - 1, parent_s) : 0;
   k_block_test<<<grid_for(B.nb * B.nb * B.nb), 256, 0, (cudaStream_t)stream>>>(
-      df, B, parent_flags, parent_s, pnb, TableSpacing{{ax, ay, az}, {hx, hy, hz}, pad}, lipschitz, tau, flags, max_slope);
+      DenseDf{df}, B, parent_flags, parent_s, pnb, TableSpacing{{ax, ay, az}, {hx, hy, hz}, pad}, lipschitz, tau, flags, max_slope);
   NUDF_LAUNCH_OK();
   return 0;
 }
@@ -310,6 +312,22 @@ int nudf_nb_emit_box(const uint8_t* flags, int32_t n, int32_t s, int32_t t, cons
   if (n_kept == 0) return 0;
   k_emit<<<grid_for(n_kept), 256, 0, (cudaStream_t)stream>>>(flags, Lat{n, s, cdiv(n - 1, s)}, t, kept, n_kept, offsets,
                                                             TableCoord{{ax, ay, az}}, idx, pts);
+  NUDF_LAUNCH_OK();
+  return 0;
+}
+
+int nudf_sb_block_test(const nudf_brick_store* st, int32_t s, const uint8_t* parent_flags, int32_t parent_s, double voxel,
+                       double lipschitz, double tau, uint8_t* flags, uint32_t* max_slope, void* stream) {
+  NUDF_REQUIRE(st && st->coarse && st->dir && (st->bricks || st->n_bricks == 0) && max_slope, "null pointer");
+  NUDF_REQUIRE(st->n >= 2 && s >= 1, "need N >= 2 and stride >= 1");
+  NUDF_REQUIRE(!parent_flags || (parent_s > s && parent_s % s == 0), "the parent stride must be a multiple of the stride");
+  NUDF_REQUIRE(lipschitz >= 0.0, "negative Lipschitz constant");
+  const int32_t n = st->n;
+  const Lat B{n, s, cdiv(n - 1, s)};
+  const int64_t pnb = parent_flags ? cdiv(n - 1, parent_s) : 0;
+  k_block_test<<<grid_for(B.nb * B.nb * B.nb), 256, 0, (cudaStream_t)stream>>>(brick_df(*st), B, parent_flags, parent_s, pnb,
+                                                                               CubeSpacing{voxel}, lipschitz, tau, flags,
+                                                                               max_slope);
   NUDF_LAUNCH_OK();
   return 0;
 }

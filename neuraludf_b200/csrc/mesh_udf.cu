@@ -20,12 +20,16 @@
 // candidates and normals, a lattice whose values equal the dense ones wherever those are <= max_t and are > max_t elsewhere
 // (+inf included: max <= max_t fails) meshes exactly like the dense one -- what grid.udf_band's narrow band relies on.
 // tests/proto/udf_mc.py restates every stage in NumPy with the same float32 operation order.
+// Every MeshUDF stage reads df through a lattice reader A (df_access.cuh): DenseDf, the flat array (nudf_mc_*), or
+// BrickDf, the block-sparse band of grid.udf_band_sparse (nudf_mcs_*).  The reader only replaces the load: both compute the
+// same values from the same corner values.
 // Threshold meshing (nudf_iso_*) runs stages 4-5 on v = fl32(f - level) instead of the pseudo-signed udf (the corner rules
 // UdfCorners / IsoCorners), with its own active-cell test and fp64 vertices; tests/proto/iso_mc.py restates it.
 #include <algorithm>
 
 #include "../../include/nudf.h"
 #include "common.cuh"
+#include "df_access.cuh"
 
 namespace nudf {
 namespace mc {
@@ -71,16 +75,17 @@ __device__ __forceinline__ int64_t find_sorted(const int64_t* __restrict__ a, in
   return (lo < n && a[lo] == key) ? lo : -1;
 }
 
-__global__ void k_active(const float* __restrict__ df, Dims D, const int64_t* __restrict__ cand, int64_t n, float avg_t,
+template <class A>
+__global__ void k_active(A df, Dims D, const int64_t* __restrict__ cand, int64_t n, float avg_t,
                          float max_t, uint8_t* __restrict__ flag) {
   for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < n; t += (int64_t)gridDim.x * blockDim.x) {
     const int64_t g = cand ? cand[t] : t;
     uint8_t on = 0;
     if (D.is_cell(g)) {
-      float s = df[g + D.coff(kLewinerOrder[0])], mx = s;
+      float s = df(g + D.coff(kLewinerOrder[0])), mx = s;
 #pragma unroll
       for (int q = 1; q < 8; ++q) {
-        const float v = df[g + D.coff(kLewinerOrder[q])];
+        const float v = df(g + D.coff(kLewinerOrder[q]));
         s = __fadd_rn(s, v);
         mx = fmaxf(mx, v);
       }
@@ -90,7 +95,8 @@ __global__ void k_active(const float* __restrict__ df, Dims D, const int64_t* __
   }
 }
 
-__global__ void k_signs(const float* __restrict__ df, Dims D, const int64_t* __restrict__ cells, int64_t n,
+template <class A>
+__global__ void k_signs(A df, Dims D, const int64_t* __restrict__ cells, int64_t n,
                         const int64_t* __restrict__ idx, int64_t n_idx, const float* __restrict__ nrm,
                         uint8_t* __restrict__ mask) {
   for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < n; t += (int64_t)gridDim.x * blockDim.x) {
@@ -100,7 +106,7 @@ __global__ void k_signs(const float* __restrict__ df, Dims D, const int64_t* __r
 #pragma unroll
     for (int c = 0; c < 8; ++c) {
       const int64_t p = g + D.coff(c);
-      u[c] = df[p];
+      u[c] = df(p);
       const int64_t row = idx ? find_sorted(idx, n_idx, p) : p;
 #pragma unroll
       for (int k = 0; k < 3; ++k) gv[c][k] = row >= 0 ? nrm[row * 3 + k] : 0.f;
@@ -120,7 +126,8 @@ __global__ void k_signs(const float* __restrict__ df, Dims D, const int64_t* __r
   }
 }
 
-__global__ void k_links(const float* __restrict__ df, Dims D, const int64_t* __restrict__ cells, int64_t n,
+template <class A>
+__global__ void k_links(A df, Dims D, const int64_t* __restrict__ cells, int64_t n,
                         const uint8_t* __restrict__ mask, int64_t* __restrict__ links) {
   for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < n; t += (int64_t)gridDim.x * blockDim.x) {
     const int64_t g = cells[t];
@@ -133,7 +140,7 @@ __global__ void k_links(const float* __restrict__ df, Dims D, const int64_t* __r
         const int bit = 4 >> ax, mn = mask[pos];
         int agree = 0, disagree = 0;
         for (int c = 0; c < 8; ++c) {
-          if (!(c & bit) || !(df[g + D.coff(c)] > 0.f)) continue;
+          if (!(c & bit) || !(df(g + D.coff(c)) > 0.f)) continue;
           if (((m >> c) & 1) == ((mn >> (c ^ bit)) & 1)) ++agree; else ++disagree;
         }
         if ((agree == 0) != (disagree == 0)) out = 2 * pos + (disagree ? 1 : 0);
@@ -197,15 +204,16 @@ __global__ void k_uf_final(const int64_t* __restrict__ par, const uint8_t* __res
 
 // Corner-value rules of the shared triangulation (cell_loops, loop_triangles): rule(D, t, g, v) writes the values v[8] of
 // cell g = cells[t]; corner c is positive when v[c] > 0.  Faces are wound towards v > 0, or with kDescent towards v <= 0.
+template <class A>
 struct UdfCorners {             // MeshUDF: the udf with the cell's pseudo-sign
-  const float* __restrict__ df;
+  A df;
   const uint8_t* __restrict__ mask;
   static constexpr bool kDescent = false;
   __device__ __forceinline__ void operator()(const Dims& D, int64_t t, int64_t g, float v[8]) const {
     const int m = mask[t];
 #pragma unroll
     for (int c = 0; c < 8; ++c) {
-      const float u = df[g + D.coff(c)];
+      const float u = df(g + D.coff(c));
       v[c] = ((m >> c) & 1) ? -u : u;
     }
   }
@@ -393,8 +401,9 @@ __device__ int centre_loop(const C& cv, const Dims& D, int64_t c, int64_t g, int
 }
 
 // lattice-index coordinates of the point on the edge (lower corner gk, axis ax): t = u_a / (u_a + u_b)
-__device__ __forceinline__ void edge_point(const float* __restrict__ df, const Dims& D, int64_t gk, int ax, float x[3]) {
-  const float ua = df[gk], ub = df[gk + D.stride(ax)];
+template <class A>
+__device__ __forceinline__ void edge_point(const A& df, const Dims& D, int64_t gk, int ax, float x[3]) {
+  const float ua = df(gk), ub = df(gk + D.stride(ax));
   const float tt = __fdiv_rn(ua, __fadd_rn(ua, ub));
   for (int k = 0; k < 3; ++k) {
     const float c = (float)D.coord(gk, k);
@@ -402,7 +411,8 @@ __device__ __forceinline__ void edge_point(const float* __restrict__ df, const D
   }
 }
 
-__global__ void k_vertices(const float* __restrict__ df, Dims D, const int64_t* __restrict__ cells,
+template <class A>
+__global__ void k_vertices(A df, Dims D, const int64_t* __restrict__ cells,
                            const uint8_t* __restrict__ mask, const int64_t* __restrict__ keys, int64_t n,
                            float* __restrict__ verts) {
   const int64_t centre0 = 3 * D.n0 * D.n1 * D.n2;
@@ -414,7 +424,7 @@ __global__ void k_vertices(const float* __restrict__ df, Dims D, const int64_t* 
     } else {                   // centre of a loop: the mean of its edge points, summed in canonical loop order
       const int64_t c = (key - centre0) >> 2, g = cells[c];
       int8_t cl[12];
-      const int len = centre_loop(UdfCorners{df, mask}, D, c, g, (int)((key - centre0) & 3), cl);
+      const int len = centre_loop(UdfCorners<A>{df, mask}, D, c, g, (int)((key - centre0) & 3), cl);
       float s[3] = {0.f, 0.f, 0.f}, y[3];
       for (int i = 0; i < len; ++i) {
         const int e = cl[i];
@@ -498,7 +508,7 @@ int nudf_mc_active(const float* df, int32_t n0, int32_t n1, int32_t n2, const in
   MC_DIMS_OK();
   NUDF_REQUIRE(df && flags && n_cand >= 0, "null pointer or negative count");
   if (n_cand == 0) return 0;
-  k_active<<<grid_for(n_cand), 256, 0, (cudaStream_t)stream>>>(df, dims(n0, n1, n2), cand, n_cand, avg_t, max_t, flags);
+  k_active<<<grid_for(n_cand), 256, 0, (cudaStream_t)stream>>>(DenseDf{df}, dims(n0, n1, n2), cand, n_cand, avg_t, max_t, flags);
   NUDF_LAUNCH_OK();
   return 0;
 }
@@ -508,7 +518,8 @@ int nudf_mc_cell_signs(const float* df, int32_t n0, int32_t n1, int32_t n2, cons
   MC_DIMS_OK();
   NUDF_REQUIRE(df && cells && normals && mask && n_cells >= 0, "null pointer or negative count");
   if (n_cells == 0) return 0;
-  k_signs<<<grid_for(n_cells), 128, 0, (cudaStream_t)stream>>>(df, dims(n0, n1, n2), cells, n_cells, idx, n_idx, normals, mask);
+  k_signs<<<grid_for(n_cells), 128, 0, (cudaStream_t)stream>>>(DenseDf{df}, dims(n0, n1, n2), cells, n_cells, idx, n_idx, normals,
+                                                               mask);
   NUDF_LAUNCH_OK();
   return 0;
 }
@@ -518,7 +529,7 @@ int nudf_mc_links(const float* df, int32_t n0, int32_t n1, int32_t n2, const int
   MC_DIMS_OK();
   NUDF_REQUIRE(df && cells && mask && links && n_cells >= 0, "null pointer or negative count");
   if (n_cells == 0) return 0;
-  k_links<<<grid_for(n_cells), 256, 0, (cudaStream_t)stream>>>(df, dims(n0, n1, n2), cells, n_cells, mask, links);
+  k_links<<<grid_for(n_cells), 256, 0, (cudaStream_t)stream>>>(DenseDf{df}, dims(n0, n1, n2), cells, n_cells, mask, links);
   NUDF_LAUNCH_OK();
   return 0;
 }
@@ -570,7 +581,8 @@ int nudf_mc_count(const float* df, int32_t n0, int32_t n1, int32_t n2, const int
   MC_DIMS_OK();
   NUDF_REQUIRE(df && cells && mask && counts && n_cells >= 0, "null pointer or negative count");
   if (n_cells == 0) return 0;
-  k_count<<<grid_for(n_cells), 128, 0, (cudaStream_t)stream>>>(UdfCorners{df, mask}, dims(n0, n1, n2), cells, n_cells, counts);
+  k_count<<<grid_for(n_cells), 128, 0, (cudaStream_t)stream>>>(UdfCorners<DenseDf>{DenseDf{df}, mask}, dims(n0, n1, n2), cells,
+                                                                n_cells, counts);
   NUDF_LAUNCH_OK();
   return 0;
 }
@@ -580,8 +592,8 @@ int nudf_mc_emit(const float* df, int32_t n0, int32_t n1, int32_t n2, const int6
   MC_DIMS_OK();
   NUDF_REQUIRE(df && cells && mask && offsets && keys && n_cells >= 0, "null pointer or negative count");
   if (n_cells == 0) return 0;
-  k_emit<<<grid_for(n_cells), 128, 0, (cudaStream_t)stream>>>(UdfCorners{df, mask}, dims(n0, n1, n2), cells, n_cells, offsets,
-                                                               keys);
+  k_emit<<<grid_for(n_cells), 128, 0, (cudaStream_t)stream>>>(UdfCorners<DenseDf>{DenseDf{df}, mask}, dims(n0, n1, n2), cells,
+                                                               n_cells, offsets, keys);
   NUDF_LAUNCH_OK();
   return 0;
 }
@@ -591,7 +603,8 @@ int nudf_mc_vertices(const float* df, int32_t n0, int32_t n1, int32_t n2, const 
   MC_DIMS_OK();
   NUDF_REQUIRE(df && cells && mask && keys && verts && n_cells >= 0 && n_keys >= 0, "null pointer or negative count");
   if (n_keys == 0) return 0;
-  k_vertices<<<grid_for(n_keys), 128, 0, (cudaStream_t)stream>>>(df, dims(n0, n1, n2), cells, mask, keys, n_keys, verts);
+  k_vertices<<<grid_for(n_keys), 128, 0, (cudaStream_t)stream>>>(DenseDf{df}, dims(n0, n1, n2), cells, mask, keys, n_keys,
+                                                                 verts);
   NUDF_LAUNCH_OK();
   return 0;
 }
@@ -638,6 +651,76 @@ int nudf_iso_vertices(const float* df, int32_t n0, int32_t n1, int32_t n2, float
   NUDF_REQUIRE(df && cells && keys && verts && n_cells >= 0 && n_keys >= 0, "null pointer or negative count");
   if (n_keys == 0) return 0;
   k_iso_vertices<<<grid_for(n_keys), 128, 0, (cudaStream_t)stream>>>(df, dims(n0, n1, n2), level, cells, keys, n_keys, verts);
+  NUDF_LAUNCH_OK();
+  return 0;
+}
+
+// ---- the same stages on the block-sparse band (nudf_brick_store) ----
+#define MCS_STORE_OK() NUDF_REQUIRE(st && st->n >= 2 && st->coarse && st->dir && (st->bricks || st->n_bricks == 0), \
+                                    "null or invalid brick store")
+
+int nudf_mcs_active(const nudf_brick_store* st, const int64_t* cand, int64_t n_cand, float avg_t, float max_t, uint8_t* flags,
+                    void* stream) {
+  MCS_STORE_OK();
+  NUDF_REQUIRE(flags && n_cand >= 0 && (cand || n_cand == 0), "null pointer or negative count");
+  if (n_cand == 0) return 0;
+  k_active<<<grid_for(n_cand), 256, 0, (cudaStream_t)stream>>>(brick_df(*st), dims(st->n, st->n, st->n), cand, n_cand, avg_t,
+                                                               max_t, flags);
+  NUDF_LAUNCH_OK();
+  return 0;
+}
+
+int nudf_mcs_cell_signs(const nudf_brick_store* st, const int64_t* cells, int64_t n_cells, const int64_t* idx, int64_t n_idx,
+                        const float* normals, uint8_t* mask, void* stream) {
+  MCS_STORE_OK();
+  NUDF_REQUIRE(cells && normals && mask && n_cells >= 0, "null pointer or negative count");
+  if (n_cells == 0) return 0;
+  k_signs<<<grid_for(n_cells), 128, 0, (cudaStream_t)stream>>>(brick_df(*st), dims(st->n, st->n, st->n), cells, n_cells, idx,
+                                                               n_idx, normals, mask);
+  NUDF_LAUNCH_OK();
+  return 0;
+}
+
+int nudf_mcs_links(const nudf_brick_store* st, const int64_t* cells, int64_t n_cells, const uint8_t* mask, int64_t* links,
+                   void* stream) {
+  MCS_STORE_OK();
+  NUDF_REQUIRE(cells && mask && links && n_cells >= 0, "null pointer or negative count");
+  if (n_cells == 0) return 0;
+  k_links<<<grid_for(n_cells), 256, 0, (cudaStream_t)stream>>>(brick_df(*st), dims(st->n, st->n, st->n), cells, n_cells, mask,
+                                                               links);
+  NUDF_LAUNCH_OK();
+  return 0;
+}
+
+int nudf_mcs_count(const nudf_brick_store* st, const int64_t* cells, int64_t n_cells, const uint8_t* mask, int32_t* counts,
+                   void* stream) {
+  MCS_STORE_OK();
+  NUDF_REQUIRE(cells && mask && counts && n_cells >= 0, "null pointer or negative count");
+  if (n_cells == 0) return 0;
+  k_count<<<grid_for(n_cells), 128, 0, (cudaStream_t)stream>>>(UdfCorners<BrickDf>{brick_df(*st), mask},
+                                                               dims(st->n, st->n, st->n), cells, n_cells, counts);
+  NUDF_LAUNCH_OK();
+  return 0;
+}
+
+int nudf_mcs_emit(const nudf_brick_store* st, const int64_t* cells, int64_t n_cells, const uint8_t* mask,
+                  const int64_t* offsets, int64_t* keys, void* stream) {
+  MCS_STORE_OK();
+  NUDF_REQUIRE(cells && mask && offsets && keys && n_cells >= 0, "null pointer or negative count");
+  if (n_cells == 0) return 0;
+  k_emit<<<grid_for(n_cells), 128, 0, (cudaStream_t)stream>>>(UdfCorners<BrickDf>{brick_df(*st), mask},
+                                                              dims(st->n, st->n, st->n), cells, n_cells, offsets, keys);
+  NUDF_LAUNCH_OK();
+  return 0;
+}
+
+int nudf_mcs_vertices(const nudf_brick_store* st, const int64_t* cells, int64_t n_cells, const uint8_t* mask,
+                      const int64_t* keys, int64_t n_keys, float* verts, void* stream) {
+  MCS_STORE_OK();
+  NUDF_REQUIRE(cells && mask && keys && verts && n_cells >= 0 && n_keys >= 0, "null pointer or negative count");
+  if (n_keys == 0) return 0;
+  k_vertices<<<grid_for(n_keys), 128, 0, (cudaStream_t)stream>>>(brick_df(*st), dims(st->n, st->n, st->n), cells, mask, keys,
+                                                                 n_keys, verts);
   NUDF_LAUNCH_OK();
   return 0;
 }

@@ -10,7 +10,10 @@ is handed over as the dense distance grid plus a SPARSE list of near-surface cel
 out of scope).  `udf_band` is the coarse-to-fine alternative to the dense sweep: it evaluates the lattice only where a
 Lipschitz bound cannot rule out udf < 2 voxels (kernels in csrc/mesh_band.cu).  `iso_band` does the same for the threshold
 lattice of validate_mesh (any box, torch.linspace coordinates): it evaluates every point a threshold mesh at `level` can
-read."""
+read.  `udf_band_sparse` runs udf_band's levels into a block-sparse store (SparseBand: a coarse dense array plus 8^3
+bricks, csrc/mesh_sparse.cu) instead of an N^3 array, and `near_surface_cells_sparse` selects the band from it: what
+mesh.udf_mesh_sparse meshes at 2048^3."""
+import ctypes
 import math
 import warnings
 
@@ -54,7 +57,13 @@ def near_surface_cells(udf_network, N, df_flat=None, max_batch=1 << 20, dist_vox
         df_flat = udf_grid(udf_network, N)
     voxel = 2.0 / (N - 1)
     idx = torch.nonzero(df_flat < dist_voxels * voxel).reshape(-1) + lo
-    normals = torch.empty(idx.numel(), 3, device=device)
+    return idx, _surface_normals(udf_network, N, idx, max_batch)
+
+
+def _surface_normals(udf_network, N, idx, max_batch):
+    """unit vectors towards the surface at the flat lattice indices idx (extract_mesh.py:77-98), batches of max_batch"""
+    voxel = 2.0 / (N - 1)
+    normals = torch.empty(idx.numel(), 3, device=idx.device)
     for head in range(0, idx.numel(), max_batch):
         sel = idx[head:head + max_batch]
         k = sel % N
@@ -64,7 +73,7 @@ def near_surface_cells(udf_network, N, df_flat=None, max_batch=1 << 20, dist_vox
         g = udf_network.gradient(pts)[:, 0]
         g = g / (torch.linalg.norm(g, ord=2, dim=-1, keepdim=True) + 1e-5)          # exp_runner_blending.py:767-771 (func_grad)
         normals[head:head + sel.numel()] = -F.normalize(g, dim=1)                    # extract_mesh.py:93
-    return idx, normals
+    return normals
 
 
 def default_strides(N):
@@ -241,6 +250,202 @@ def udf_band(udf_network, N, lipschitz=2.0, strides=None, max_batch=1 << 21):
                       "may miss points with udf < 2 voxels" % (info["max_edge_slope"], lipschitz, lipschitz), RuntimeWarning,
                       stacklevel=2)
     return df, info
+
+
+def sparse_coarse_stride(strides):
+    """the stride c of SparseBand's coarse array for a schedule: its smallest stride >= 8 (one brick edge), else its first"""
+    big = [s for s in strides if s >= _lib.BRICK]
+    return big[-1] if big else strides[0]
+
+
+class SparseBand:
+    """The block-sparse narrow-band lattice of udf_band_sparse (nudf_brick_store in include/nudf.h; the reader BrickDf in
+    csrc/df_access.cuh).  The points of the stride-c lattice (per axis 0, c, 2 c, ... and N - 1) are held in the dense
+    array `coarse` [mc^3], mc = ceil((N - 1) / c) + 1; every other point in an 8^3 brick: `dir` [nbk^3] int32
+    (nbk = ceil(N / 8)) gives each brick's slot in `bricks` [slots * 512] or -1, `keys` [slots] the brick number of each
+    slot, ascending.  A point never stored reads +inf, as in udf_band's df.  `values(idx)` reads flat lattice indices."""
+
+    def __init__(self, N, c, device):
+        self.N, self.c = int(N), int(c)
+        self.mc = -(-(self.N - 1) // self.c) + 1
+        self.nbk = -(-self.N // _lib.BRICK)
+        self.coarse = torch.full((self.mc ** 3,), float("inf"), device=device)
+        self.dir = torch.full((self.nbk ** 3,), -1, dtype=torch.int32, device=device)
+        self.bricks = torch.empty(0, device=device)
+        self.keys = torch.empty(0, dtype=torch.int64, device=device)
+        self._missing = torch.zeros(1, dtype=torch.int32, device=device)
+
+    @property
+    def device(self):
+        return self.coarse.device
+
+    @property
+    def n_bricks(self):
+        return self.keys.numel()
+
+    def desc(self):
+        """the nudf_brick_store descriptor (host struct of device pointers), by reference"""
+        d = _lib.BrickStore(self.N, self.c, self.mc, self.nbk, self.n_bricks, self.coarse.data_ptr(), self.dir.data_ptr(),
+                            self.bricks.data_ptr() if self.n_bricks else None,
+                            self.keys.data_ptr() if self.n_bricks else None)
+        self._d = d                               # kept alive until the next call
+        return ctypes.byref(d)
+
+    def nbytes(self):
+        """bytes held: coarse, dir, bricks (with keys)"""
+        return {"coarse": self.coarse.numel() * 4, "dir": self.dir.numel() * 4,
+                "bricks": self.bricks.numel() * 4 + self.keys.numel() * 8}
+
+    def allocate(self, flags, s):
+        """slots for every brick that meets the closed box of a kept block of stride s (flags: the block test's)"""
+        L = _lib.lib()
+        marks = torch.zeros(self.nbk ** 3, dtype=torch.int32, device=self.device)
+        check(L.nudf_sb_mark(self.desc(), s, ptr(flags), ptr(marks), _lib.stream_ptr()), "nudf_sb_mark")
+        keys = torch.nonzero(marks).reshape(-1)
+        del marks
+        self.dir.fill_(-1)
+        self.dir[keys] = torch.arange(keys.numel(), dtype=torch.int32, device=self.device)
+        self.keys = keys.contiguous()
+        self.bricks = torch.full((keys.numel() * _lib.BRICK ** 3,), float("inf"), device=self.device)
+
+    def store(self, idx, vals):
+        """write vals [P] fp32 at the flat lattice indices idx [P]; a point with no storage raises at check_stored()"""
+        vals = vals.reshape(-1).float().contiguous()
+        check(_lib.lib().nudf_sb_store(self.desc(), ptr(idx), ptr(vals), idx.numel(), ptr(self._missing),
+                                       _lib.stream_ptr()), "nudf_sb_store")
+
+    def check_stored(self):
+        if int(self._missing.item()):
+            raise RuntimeError("SparseBand: a value was stored outside the coarse lattice and every brick")
+
+    def values(self, idx):
+        """fp32 values at the flat lattice indices idx (int64 device tensor)"""
+        idx = idx.reshape(-1).to(torch.int64).contiguous()
+        out = torch.empty(idx.numel(), device=self.device)
+        check(_lib.lib().nudf_sb_gather(self.desc(), ptr(idx), idx.numel(), ptr(out), _lib.stream_ptr()), "nudf_sb_gather")
+        return out
+
+    def flat_index(self, pos):
+        """flat lattice indices of storage positions pos (int64: [0, mc^3) coarse, then mc^3 + slot * 512 + local)"""
+        out = torch.empty(pos.numel(), dtype=torch.int64, device=self.device)
+        check(_lib.lib().nudf_sb_flat(self.desc(), ptr(pos), pos.numel(), ptr(out), _lib.stream_ptr()), "nudf_sb_flat")
+        return out
+
+
+def _band_point_chunks(flags, N, s, t, max_batch):
+    """band_points' (idx, pts) in its order, cut between kept blocks into chunks of about max_batch points, so that a level
+    never holds all its points at once: yields (idx, pts) per chunk"""
+    L = _lib.lib()
+    st = _lib.stream_ptr()
+    kept = torch.nonzero(flags).reshape(-1)
+    n = kept.numel()
+    if n == 0:
+        return
+    counts = torch.empty(n, dtype=torch.int32, device=flags.device)
+    check(L.nudf_nb_count(ptr(flags), N, s, t, ptr(kept), n, ptr(counts), st), "nudf_nb_count")
+    csum = torch.cumsum(counts, 0, dtype=torch.int64)
+    total = int(csum[-1])
+    cuts = []
+    if total > max_batch:
+        cuts = torch.searchsorted(csum, torch.arange(max_batch, total, max_batch, device=flags.device), right=True).tolist()
+    bounds = sorted(set([0, n] + cuts))
+    head = 0
+    for a, b in zip(bounds, bounds[1:]):
+        end = int(csum[b - 1])
+        offsets = (csum[a:b] - counts[a:b] - head).contiguous()
+        idx = torch.empty(end - head, dtype=torch.int64, device=flags.device)
+        pts = torch.empty(end - head, 3, device=flags.device)
+        check(L.nudf_nb_emit(ptr(flags), N, s, t, ptr(kept[a:b]), b - a, ptr(offsets), 2.0 / (N - 1), ptr(idx), ptr(pts), st),
+              "nudf_nb_emit")
+        yield idx, pts
+        head = end
+
+
+@torch.no_grad()
+def udf_band_sparse(udf_network, N, lipschitz=2.0, strides=None, max_batch=1 << 21):
+    """udf_band's lattice without an N^3 array: (SparseBand, info).
+
+    The levels are udf_band's -- the same sub-lattice, block tests (nudf_sb_block_test: nudf_nb_block_test reading the
+    store), point emission and evaluation -- so the same RuntimeWarning when max_edge_slope exceeds `lipschitz`.  The
+    points of strides >= c (sparse_coarse_stride) go to the coarse array; after the block test at stride c, every brick
+    meeting a kept stride-c block is allocated, and the points of the finer strides, all inside those blocks, go to the
+    bricks.  A level is emitted and evaluated in chunks of about max_batch points.  If `udf_values` gives a point the
+    same bits in any batch, SparseBand.values equals udf_band's df at every lattice point, +inf included (DESIGN.md
+    section 1).  info: udf_band's keys, plus coarse_stride, bricks (slots allocated) and bytes (SparseBand.nbytes, and
+    the largest block-test flags array)."""
+    strides = _check_strides(default_strides(N) if strides is None else strides)
+    device = _device(udf_network)
+    L = _lib.lib()
+    voxel = 2.0 / (N - 1)
+    c = sparse_coarse_stride(strides)
+    band = SparseBand(N, c, device)
+    info = {"strides": strides, "points": [], "kept_blocks": [], "edge_slope": [], "coarse_stride": c}
+    events = []
+    flag_bytes = 0
+
+    def mark():
+        events.append(torch.cuda.Event(enable_timing=True))
+        events[-1].record()
+
+    def evaluate(idx, pts):
+        for head in range(0, idx.numel(), max_batch):
+            band.store(idx[head:head + max_batch], udf_network.udf_values(pts[head:head + max_batch]))
+        return int(idx.numel())
+
+    mark()
+    info["points"].append(evaluate(*band_sublattice(N, strides[0], device)))
+    mark()
+    parent = None
+    for k, s in enumerate(strides):
+        last = k + 1 == len(strides)
+        nb = -(-(N - 1) // s)
+        flags = None if last else torch.empty(nb ** 3, dtype=torch.uint8, device=device)
+        slope = torch.zeros(1, dtype=torch.int32, device=device)
+        check(L.nudf_sb_block_test(band.desc(), s, ptr(parent), strides[k - 1] if k else 0, voxel, float(lipschitz),
+                                   2.0 * voxel, ptr(flags), ptr(slope), _lib.stream_ptr()), "nudf_sb_block_test")
+        info["edge_slope"].append(float(slope.view(torch.float32)))
+        if last:
+            break
+        flag_bytes = max(flag_bytes, flags.numel())
+        if s == c:
+            band.allocate(flags, s)
+        n_points = 0
+        for idx, pts in _band_point_chunks(flags, N, s, strides[k + 1], max_batch):
+            n_points += evaluate(idx, pts)
+            del idx, pts
+        info["points"].append(n_points)
+        info["kept_blocks"].append(int(torch.count_nonzero(flags)))
+        mark()
+        parent = flags
+    del parent, flags
+    mark()
+    torch.cuda.synchronize(device)
+    band.check_stored()
+    ms = [a.elapsed_time(b) for a, b in zip(events, events[1:])]
+    info["level_ms"], info["slope_ms"] = ms[:-1], ms[-1]
+    info["max_edge_slope"] = max(info["edge_slope"])
+    info["bricks"] = band.n_bricks
+    info["bytes"] = dict(band.nbytes(), flags=flag_bytes)
+    if info["max_edge_slope"] > lipschitz:
+        warnings.warn("udf_band_sparse: a lattice edge has slope %.3f > lipschitz=%.3f: the field is not %.3f-Lipschitz, so "
+                      "the band may miss points with udf < 2 voxels" % (info["max_edge_slope"], lipschitz, lipschitz),
+                      RuntimeWarning, stacklevel=2)
+    return band, info
+
+
+@torch.no_grad()
+def near_surface_cells_sparse(udf_network, band, max_batch=1 << 20, dist_voxels=2.0):
+    """near_surface_cells on a SparseBand: (sorted flat lattice indices [M] int64, unit vectors towards the surface [M,3])
+    of the points with udf < dist_voxels * voxel, the same comparison as near_surface_cells' (fp32 values against the
+    threshold), over the coarse array and the bricks only.  Equal to near_surface_cells on udf_band's df when band equals
+    it (udf_band_sparse)."""
+    voxel = 2.0 / (band.N - 1)
+    thr = dist_voxels * voxel
+    pos = torch.cat([torch.nonzero(band.coarse < thr).reshape(-1),
+                     torch.nonzero(band.bricks < thr).reshape(-1) + band.coarse.numel()])
+    idx = torch.sort(band.flat_index(pos.contiguous())).values
+    del pos
+    return idx, _surface_normals(udf_network, band.N, idx, max_batch)
 
 
 def axis_tables(bound_min, bound_max, resolution, device):

@@ -10,6 +10,8 @@ csrc/mesh_udf.cu (stages and deviations documented there); tests/proto/udf_mc.py
 `iso_marching_cubes_index` / `iso_marching_cubes` are threshold marching cubes on the same kernels (the runner's
 validate_mesh without PyMCubes; `python -m neuraludf_b200.mesh --threshold T`), restated in tests/proto/iso_mc.py;
 `iso_mesh_band` is the same with the lattice evaluated narrow-band (grid.iso_band; `--threshold T --band`).
+`udf_mesh_sparse` is `udf_mesh_band` on the block-sparse band (grid.udf_band_sparse, `marching_cubes_sparse`): the same
+mesh with no N^3 array, for lattices up to 2048^3 (`--sparse`).
 """
 import ctypes
 
@@ -50,10 +52,33 @@ def marching_cubes_index(df, dims, normals, idx=None):
             raise ValueError("normals must have one row per idx entry")
     elif normals.shape[0] != df.numel():
         raise ValueError("dense normals must have one row per lattice point")
-    avg_t, max_t = thresholds(n2)
     n_cand = n0 * n1 * n2 if idx is None else idx.numel()
+    stages = {
+        "active": lambda avg_t, max_t, flags: check(L.nudf_mc_active(ptr(df), n0, n1, n2, ptr(idx), n_cand, avg_t, max_t,
+                                                                     ptr(flags), st), "nudf_mc_active"),
+        "signs": lambda cells, n, mask0: check(L.nudf_mc_cell_signs(ptr(df), n0, n1, n2, ptr(cells), n, ptr(idx),
+                                                                    0 if idx is None else idx.numel(), ptr(normals),
+                                                                    ptr(mask0), st), "nudf_mc_cell_signs"),
+        "links": lambda cells, n, mask0, links: check(L.nudf_mc_links(ptr(df), n0, n1, n2, ptr(cells), n, ptr(mask0),
+                                                                      ptr(links), st), "nudf_mc_links"),
+        "count": lambda cells, n, mask, counts: check(L.nudf_mc_count(ptr(df), n0, n1, n2, ptr(cells), n, ptr(mask),
+                                                                      ptr(counts), st), "nudf_mc_count"),
+        "emit": lambda cells, n, mask, offsets, keys: check(L.nudf_mc_emit(ptr(df), n0, n1, n2, ptr(cells), n, ptr(mask),
+                                                                           ptr(offsets), ptr(keys), st), "nudf_mc_emit"),
+        "vertices": lambda cells, n, mask, ukeys, verts: check(L.nudf_mc_vertices(ptr(df), n0, n1, n2, ptr(cells), n,
+                                                                                  ptr(mask), ptr(ukeys), ukeys.numel(),
+                                                                                  ptr(verts), st), "nudf_mc_vertices")}
+    return _mc_stages(stages, n2, n_cand, idx, dev)
+
+
+def _mc_stages(stages, n2, n_cand, idx, dev):
+    """the MeshUDF MC driver shared by marching_cubes_index and marching_cubes_sparse: `stages` launch the kernels on
+    their lattice (dense df or brick store); idx the sorted candidate indices (None: every cell)"""
+    L = _lib.lib()
+    st = _lib.stream_ptr()
+    avg_t, max_t = thresholds(n2)
     flags = torch.empty(n_cand, dtype=torch.uint8, device=dev)
-    check(L.nudf_mc_active(ptr(df), n0, n1, n2, ptr(idx), n_cand, avg_t, max_t, ptr(flags), st), "nudf_mc_active")
+    stages["active"](avg_t, max_t, flags)
     sel = torch.nonzero(flags).reshape(-1)
     cells = (sel if idx is None else idx[sel]).contiguous()
     n = cells.numel()
@@ -63,10 +88,9 @@ def marching_cubes_index(df, dims, normals, idx=None):
         info.update(face_keys=empty[1], mask=torch.zeros(0, dtype=torch.uint8, device=dev))
         return empty[0], empty[1], info
     mask0 = torch.empty(n, dtype=torch.uint8, device=dev)
-    check(L.nudf_mc_cell_signs(ptr(df), n0, n1, n2, ptr(cells), n, ptr(idx), 0 if idx is None else idx.numel(), ptr(normals),
-                               ptr(mask0), st), "nudf_mc_cell_signs")
+    stages["signs"](cells, n, mask0)
     links = torch.empty(n * 3, dtype=torch.int64, device=dev)
-    check(L.nudf_mc_links(ptr(df), n0, n1, n2, ptr(cells), n, ptr(mask0), ptr(links), st), "nudf_mc_links")
+    stages["links"](cells, n, mask0, links)
     parent = torch.empty(n, dtype=torch.int64, device=dev)
     hook = torch.empty(n, dtype=torch.int64, device=dev)
     flag = torch.empty(1, dtype=torch.int32, device=dev)
@@ -76,22 +100,51 @@ def marching_cubes_index(df, dims, normals, idx=None):
           "nudf_mc_polarity")
     info["polarity_rounds"], info["polarity_jumps"] = int(stats[0]), int(stats[1])
     counts = torch.empty(n, dtype=torch.int32, device=dev)
-    check(L.nudf_mc_count(ptr(df), n0, n1, n2, ptr(cells), n, ptr(mask), ptr(counts), st), "nudf_mc_count")
+    stages["count"](cells, n, mask, counts)
     csum = torch.cumsum(counts, 0, dtype=torch.int64)
     n_faces = int(csum[-1])
     offsets = (csum - counts).contiguous()
     keys = torch.empty(3 * n_faces, dtype=torch.int64, device=dev)
-    check(L.nudf_mc_emit(ptr(df), n0, n1, n2, ptr(cells), n, ptr(mask), ptr(offsets), ptr(keys), st), "nudf_mc_emit")
+    stages["emit"](cells, n, mask, offsets, keys)
     info.update(face_keys=keys.reshape(-1, 3), mask=mask)
     if n_faces == 0:
         return empty[0], empty[1], info
     ukeys, inv = torch.unique(keys, sorted=True, return_inverse=True)
     ukeys = ukeys.contiguous()
     verts = torch.empty(ukeys.numel(), 3, device=dev)
-    check(L.nudf_mc_vertices(ptr(df), n0, n1, n2, ptr(cells), n, ptr(mask), ptr(ukeys), ukeys.numel(), ptr(verts), st),
-          "nudf_mc_vertices")
+    stages["vertices"](cells, n, mask, ukeys, verts)
     info["vertex_keys"] = ukeys
     return verts, inv.reshape(-1, 3).to(torch.int64), info
+
+
+@torch.no_grad()
+def marching_cubes_sparse(band, normals, idx):
+    """marching_cubes_index on the N^3 lattice of a grid.SparseBand (every df read through the brick store,
+    nudf_mcs_*): the same (verts [V,3] fp32 in lattice-index units, faces [F,3] int64, info).  idx / normals: the sorted
+    flat candidate indices and their rows (grid.near_surface_cells_sparse); there is no dense form."""
+    L = _lib.lib()
+    st = _lib.stream_ptr()
+    dev = band.device
+    idx = idx.reshape(-1).to(torch.int64).contiguous()
+    normals = normals.reshape(-1, 3).float().contiguous()
+    if normals.shape[0] != idx.numel():
+        raise ValueError("normals must have one row per idx entry")
+    d = band.desc()
+    stages = {
+        "active": lambda avg_t, max_t, flags: check(L.nudf_mcs_active(d, ptr(idx), idx.numel(), avg_t, max_t, ptr(flags), st),
+                                                    "nudf_mcs_active"),
+        "signs": lambda cells, n, mask0: check(L.nudf_mcs_cell_signs(d, ptr(cells), n, ptr(idx), idx.numel(), ptr(normals),
+                                                                     ptr(mask0), st), "nudf_mcs_cell_signs"),
+        "links": lambda cells, n, mask0, links: check(L.nudf_mcs_links(d, ptr(cells), n, ptr(mask0), ptr(links), st),
+                                                      "nudf_mcs_links"),
+        "count": lambda cells, n, mask, counts: check(L.nudf_mcs_count(d, ptr(cells), n, ptr(mask), ptr(counts), st),
+                                                      "nudf_mcs_count"),
+        "emit": lambda cells, n, mask, offsets, keys: check(L.nudf_mcs_emit(d, ptr(cells), n, ptr(mask), ptr(offsets),
+                                                                            ptr(keys), st), "nudf_mcs_emit"),
+        "vertices": lambda cells, n, mask, ukeys, verts: check(L.nudf_mcs_vertices(d, ptr(cells), n, ptr(mask), ptr(ukeys),
+                                                                                   ukeys.numel(), ptr(verts), st),
+                                                               "nudf_mcs_vertices")}
+    return _mc_stages(stages, band.N, idx.numel(), idx, dev)
 
 
 def _iso_level(level):
@@ -240,13 +293,34 @@ def _mc_lattice(udf_network, N, df, lo, max_batch):
 
 def _mesh_lattice(udf_network, N, df, dist_threshold_ratio, lo, max_batch):
     """near-surface normals -> MC -> vertex filter of the lattice values df (whole x-planes from flat index lo)"""
-    voxel = 2.0 / (N - 1)
     verts, faces = _mc_lattice(udf_network, N, df, lo, max_batch)
+    return _vertex_filter(udf_network, N, verts, faces, dist_threshold_ratio, lo)
+
+
+def _mc_sparse(udf_network, band, max_batch):
+    """near-surface normals -> MC of a grid.SparseBand: (verts [V,3] fp32 in lattice-index units, faces [F,3] int64)"""
+    from neuraludf_b200 import grid
+    idx, normals = grid.near_surface_cells_sparse(udf_network, band, max_batch=max(max_batch // 2, 1))
+    verts, faces, _ = marching_cubes_sparse(band, normals, idx)
+    return verts, faces
+
+
+def _batched_values(udf_network, pts, max_batch):
+    """udf_values of pts [P,3] in batches of max_batch (None: one call), flat: the same bits when udf_values is batch-invariant"""
+    if max_batch is None:
+        return udf_network.udf_values(pts).reshape(-1)
+    return torch.cat([udf_network.udf_values(pts[h:h + max_batch]).reshape(-1) for h in range(0, pts.shape[0], max_batch)])
+
+
+def _vertex_filter(udf_network, N, verts, faces, dist_threshold_ratio, lo, max_batch=None):
+    """world coordinates and the vertex filter of extract_mesh.py:205-214 for an MC of whole x-planes from flat index lo;
+    the udf at the vertices in batches of max_batch (None: one call)"""
+    voxel = 2.0 / (N - 1)
     verts = verts * voxel - 1.0
     verts[:, 0] += (lo // (N * N)) * voxel
     if faces.shape[0] == 0:
         return verts, faces
-    vd = udf_network.udf_values(verts).reshape(-1)
+    vd = _batched_values(udf_network, verts, max_batch)
     keep = vd[faces].max(dim=1).values < voxel * dist_threshold_ratio
     return _compact(verts, faces[keep])
 
@@ -266,28 +340,52 @@ def udf_mesh_band(udf_network, N, dist_threshold_ratio=1.0, lipschitz=2.0, strid
 
 
 @torch.no_grad()
+def udf_mesh_sparse(udf_network, N, dist_threshold_ratio=1.0, lipschitz=2.0, strides=None, max_batch=1 << 21):
+    """`udf_mesh_band` on the block-sparse band (grid.udf_band_sparse, near_surface_cells_sparse, marching_cubes_sparse):
+    the same (verts, faces), with no array of N^3 elements.
+
+    Exact under udf_mesh_band's conditions: the store then reads udf_band's df at every lattice point (DESIGN.md section 1),
+    so every stage sees the same values.  The store is released before the vertex filter, which evaluates the vertices in
+    batches of max_batch (at 2048^3 a single batch of every vertex would need tens of GB of value-chain workspace)."""
+    from neuraludf_b200 import grid
+    band, _ = grid.udf_band_sparse(udf_network, N, lipschitz=lipschitz, strides=strides, max_batch=max_batch)
+    verts, faces = _mc_sparse(udf_network, band, max_batch)
+    del band
+    return _vertex_filter(udf_network, N, verts, faces, dist_threshold_ratio, 0, max_batch)
+
+
+@torch.no_grad()
 def udf_mesh_post(udf_network, N, dist_threshold_ratio=5.0, dense=False, lipschitz=2.0, strides=None, smooth_borders=True,
-                  max_batch=1 << 21):
+                  max_batch=1 << 21, sparse=False):
     """The mesh `Runner.extract_udf_mesh` exports, before its world transform and final merge: (fp64 verts [V,3], int64
     faces [F,3], info) on the device.
 
-    The lattice is evaluated narrow-band (`udf_mesh_band`'s, `lipschitz` / `strides`) or, with `dense`, whole (`udf_mesh`'s);
-    the normals and MC are theirs.  The vertices are then formed as the reference holds them, fp64(fp32 MC vertex) *
+    The lattice is evaluated narrow-band (`udf_mesh_band`'s, `lipschitz` / `strides`), with `sparse` narrow-band into the
+    block-sparse store (`udf_mesh_sparse`'s, the same mesh), or with `dense` whole (`udf_mesh`'s); the normals and MC are
+    theirs.  The vertices are then formed as the reference holds them, fp64(fp32 MC vertex) *
     fp64(voxel) - 1 in fp64, the vertex filter of extract_mesh.py:205-214 evaluates the udf at their fp32 rounding, and
     `mesh_post.postprocess` does the rest of get_mesh_udf_fast (extract_mesh.py:215-265; the runner passes
     `dist_threshold_ratio` 5 and `smooth_borders` True).  info: postprocess's, plus `mc` ((V, F) of the raw MC) and
     `filtered` (faces after the vertex filter)."""
     from neuraludf_b200 import grid, mesh_post
     voxel = 2.0 / (N - 1)
-    if dense:
-        df = grid.udf_grid(udf_network, N, max_batch=max_batch)
+    if dense and sparse:
+        raise ValueError("udf_mesh_post: dense and sparse exclude each other")
+    if sparse:
+        band, _ = grid.udf_band_sparse(udf_network, N, lipschitz=lipschitz, strides=strides, max_batch=max_batch)
+        verts, faces = _mc_sparse(udf_network, band, max_batch)
+        del band
     else:
-        df, _ = grid.udf_band(udf_network, N, lipschitz=lipschitz, strides=strides, max_batch=max_batch)
-    verts, faces = _mc_lattice(udf_network, N, df, 0, max_batch)
+        if dense:
+            df = grid.udf_grid(udf_network, N, max_batch=max_batch)
+        else:
+            df, _ = grid.udf_band(udf_network, N, lipschitz=lipschitz, strides=strides, max_batch=max_batch)
+        verts, faces = _mc_lattice(udf_network, N, df, 0, max_batch)
+        del df
     v64 = verts.double() * voxel - 1.0
     n_mc = faces.shape[0]
     if n_mc:
-        vd = udf_network.udf_values(v64.float()).reshape(-1)
+        vd = _batched_values(udf_network, v64.float(), max_batch if sparse else None)
         faces = faces[vd[faces].max(dim=1).values < voxel * dist_threshold_ratio]
     v, f, info = mesh_post.postprocess(v64, faces, smooth_borders=smooth_borders)
     info["mc"], info["filtered"] = (verts.shape[0], n_mc), int(faces.shape[0])
@@ -415,12 +513,17 @@ def main(argv=None):
     ap.add_argument("--lipschitz", type=float, default=None, help="Lipschitz bound of the band's culling test (default 2)")
     ap.add_argument("--scale", type=float, default=1.0, help="the conf's udf_network.scale")
     ap.add_argument("--dense", action="store_true", help="evaluate the whole lattice (udf_mesh) instead of the narrow band")
+    ap.add_argument("--sparse", action="store_true",
+                    help="hold the narrow band block-sparse (udf_mesh_sparse): the same mesh with no N^3 array, for "
+                         "--resolution up to 2048")
     ap.add_argument("--postprocess", action="store_true",
                     help="apply the runner's post-processing (merge, duplicate and degenerate faces, hole filling, border "
                          "smoothing, the final merge after --cameras): the mesh Runner.extract_udf_mesh writes; the runner "
                          "passes --dist_threshold_ratio 5")
     ap.add_argument("--out", required=True, help="output PLY")
     a = ap.parse_args(argv)
+    if a.sparse and (a.dense or a.threshold is not None):
+        ap.error("--sparse cannot be combined with %s" % ("--dense" if a.dense else "--threshold"))
     if a.band and a.threshold is None:
         ap.error("--band needs --threshold (the MeshUDF lattice is evaluated narrow-band without it)")
     if a.threshold is not None:
@@ -452,9 +555,12 @@ def main(argv=None):
         print("%s: %d vertices, %d faces" % (a.out, v.shape[0], faces.shape[0]))
         return v, np.asarray(faces)
     if a.postprocess:
-        verts, faces, _ = udf_mesh_post(net, a.resolution, a.dist_threshold_ratio, dense=a.dense, lipschitz=a.lipschitz)
+        verts, faces, _ = udf_mesh_post(net, a.resolution, a.dist_threshold_ratio, dense=a.dense, lipschitz=a.lipschitz,
+                                        sparse=a.sparse)
     elif a.dense:
         verts, faces = udf_mesh(net, a.resolution, a.dist_threshold_ratio)
+    elif a.sparse:
+        verts, faces = udf_mesh_sparse(net, a.resolution, a.dist_threshold_ratio, a.lipschitz)
     else:
         verts, faces = udf_mesh_band(net, a.resolution, a.dist_threshold_ratio, a.lipschitz)
     v = verts.double().cpu().numpy()
