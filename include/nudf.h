@@ -20,7 +20,7 @@ extern "C" {
 #endif
 
 #define NUDF_MAX_LAYERS 16
-#define NUDF_ABI_VERSION 4
+#define NUDF_ABI_VERSION 5
 /* bits of the device-side status word (nudf_render_out.status, `status` of the sampling entry points): set by the kernels,
  * never cleared by the library; the caller reads it at a host synchronisation point of its choice */
 #define NUDF_STATUS_NONFINITE_SAMPLES 1   /* sample_pdf / up_sample produced a non-finite sample position (:97-101, 265-269) */
@@ -331,20 +331,29 @@ int nudf_gen_rays_grid(const float* intrinsics_inv, const float* pose, int32_t W
 /* ------------------------------------------------------------------------------------------------------------
  * MeshUDF marching cubes (replaces custom_mc's udf_mc_lewiner; neuraludf_b200/mesh.py drives the stages)
  * ------------------------------------------------------------------------------------------------------------
- * df: DEVICE fp32 lattice [n0, n1, n2] (axis 0 slowest).  Cells are named by the flat index of their lower corner; every cell
- * list is sorted ascending.  Normals are unit vectors towards the surface: dense [n0*n1*n2, 3] (idx = NULL) or the sparse
- * rows of the sorted flat indices idx[n_idx] (grid.near_surface_cells); a corner without a row counts as the zero vector.
- * All buffers are caller-provided; nothing is allocated. */
-/* flags[t] = 1 when cell cand[t] (cand = NULL: cell t of the whole lattice) is active: mean corner udf < avg_t and max <= max_t */
-int nudf_mc_active(const float* df, int32_t n0, int32_t n1, int32_t n2, const int64_t* cand, int64_t n_cand, float avg_t,
-                   float max_t, uint8_t* flags, void* stream);
+ * The lattice [n0, n1, n2] (axis 0 slowest) is named by a nudf_lattice.  Cells are named by the flat index of their lower
+ * corner; every cell list is sorted ascending.  Normals are unit vectors towards the surface: dense [n0*n1*n2, 3]
+ * (idx = NULL) or the sparse rows of the sorted flat indices idx[n_idx] (grid.near_surface_cells); a corner without a row
+ * counts as the zero vector.  All buffers are caller-provided; nothing is allocated. */
+/* The lattice a MeshUDF or narrow-band kernel reads, flat index (i n1 + j) n2 + k (the descriptor is host memory, the
+ * pointers DEVICE): the fp32 array df, or the block-sparse band `store` (nudf_brick_store below; n0 = n1 = n2 = store->n).
+ * Exactly one of df and store is set; every dimension is >= 2. */
+typedef struct nudf_lattice {
+  int32_t n0, n1, n2;
+  const float* df;
+  const struct nudf_brick_store* store;
+} nudf_lattice;
+/* flags[t] = 1 when cell cand[t] is active: mean corner udf < avg_t and max <= max_t.  cand = NULL (a df lattice only):
+ * cell t of the whole lattice */
+int nudf_mc_active(const nudf_lattice* lat, const int64_t* cand, int64_t n_cand, float avg_t, float max_t, uint8_t* flags,
+                   void* stream);
 /* mask[t] bit c = corner c of cells[t] on the other pseudo-side than the cell's largest-udf corner (c = 4 a0 + 2 a1 + a2) */
-int nudf_mc_cell_signs(const float* df, int32_t n0, int32_t n1, int32_t n2, const int64_t* cells, int64_t n_cells,
-                       const int64_t* idx, int64_t n_idx, const float* normals, uint8_t* mask, void* stream);
+int nudf_mc_cell_signs(const nudf_lattice* lat, const int64_t* cells, int64_t n_cells, const int64_t* idx, int64_t n_idx,
+                       const float* normals, uint8_t* mask, void* stream);
 /* links[t*3+axis] = 2 * (position of the + axis neighbour in cells) + (1 when the shared corners with udf > 0 all disagree,
  * 0 when they all agree), or -1 (no active neighbour, mixed or no evidence) */
-int nudf_mc_links(const float* df, int32_t n0, int32_t n1, int32_t n2, const int64_t* cells, int64_t n_cells,
-                  const uint8_t* mask, int64_t* links, void* stream);
+int nudf_mc_links(const nudf_lattice* lat, const int64_t* cells, int64_t n_cells, const uint8_t* mask, int64_t* links,
+                  void* stream);
 /* one polarity per linked component (deterministic union-find with parity; the root cell's corner 0 ends positive):
  * mask_out = mask_in, complemented where the cell flips.  Workspace: parent_ws, hook_ws [n_cells] int64, flag_ws [1] int32.
  * Synchronises the stream (one host read of flag_ws per pass).  stats (HOST int32[2], may be NULL): hooking rounds,
@@ -354,16 +363,16 @@ int nudf_mc_polarity(const int64_t* links, int64_t n_cells, const uint8_t* mask_
 /* triangles per cell (<= 12): each crossing loop is triangulated with no chord lying in a cube face (every edge of a
  * closed surface is shared by exactly two triangles); a loop that admits no such triangulation is fanned around a centre
  * vertex of its own */
-int nudf_mc_count(const float* df, int32_t n0, int32_t n1, int32_t n2, const int64_t* cells, int64_t n_cells,
-                  const uint8_t* mask, int32_t* counts, void* stream);
+int nudf_mc_count(const nudf_lattice* lat, const int64_t* cells, int64_t n_cells, const uint8_t* mask, int32_t* counts,
+                  void* stream);
 /* keys[3 * (offsets[t] + i) + k] = key of vertex k of triangle i of cells[t]: 3 * corner + axis for a lattice-edge point,
  * 3 * n0 * n1 * n2 + 4 * t + l for the centre vertex of the cell's loop l; offsets = exclusive scan of the counts */
-int nudf_mc_emit(const float* df, int32_t n0, int32_t n1, int32_t n2, const int64_t* cells, int64_t n_cells,
-                 const uint8_t* mask, const int64_t* offsets, int64_t* keys, void* stream);
+int nudf_mc_emit(const nudf_lattice* lat, const int64_t* cells, int64_t n_cells, const uint8_t* mask, const int64_t* offsets,
+                 int64_t* keys, void* stream);
 /* verts[n_keys, 3]: lattice-index coordinates of the vertices of the keys: edge points at t = u_a / (u_a + u_b) from the
  * lower corner, loop centres at the mean of their edge points (cells / mask: those given to nudf_mc_emit) */
-int nudf_mc_vertices(const float* df, int32_t n0, int32_t n1, int32_t n2, const int64_t* cells, int64_t n_cells,
-                     const uint8_t* mask, const int64_t* keys, int64_t n_keys, float* verts, void* stream);
+int nudf_mc_vertices(const nudf_lattice* lat, const int64_t* cells, int64_t n_cells, const uint8_t* mask, const int64_t* keys,
+                     int64_t n_keys, float* verts, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Threshold marching cubes (replaces PyMCubes' marching_cubes in the runner's validate_mesh; neuraludf_b200/mesh.py's
@@ -444,46 +453,45 @@ int nudf_cl_vote(const double* points, int64_t n, const double* mats, int32_t n_
 /* ------------------------------------------------------------------------------------------------------------
  * Narrow-band lattice evaluation, coarse to fine (neuraludf_b200/grid.py udf_band drives the levels)
  * ------------------------------------------------------------------------------------------------------------
- * The N^3 lattice on [-1,1]^3, flat index (i * N + j) * N + k, voxel = 2 / (N - 1).  The stride-s lattice holds the
- * coordinates 0, s, 2 s, ... and N - 1 per axis; a block of stride s is the box [a, min(a + s, N - 1)] per axis (a a multiple
- * of s below N - 1), nb = ceil((N - 1) / s) per axis, numbered (bx * nb + by) * nb + bz.  Coordinates are fp32
- * fl(fl(i * fl32(voxel)) - 1), as grid.lattice_points makes them.  Caller-provided buffers only. */
+ * The N^3 lattice, flat index (i * N + j) * N + k.  The stride-s lattice holds the coordinates 0, s, 2 s, ... and N - 1 per
+ * axis; a block of stride s is the box [a, min(a + s, N - 1)] per axis (a a multiple of s below N - 1),
+ * nb = ceil((N - 1) / s) per axis, numbered (bx * nb + by) * nb + bz.  The coordinates and the block test's spacing rule
+ * are named by a nudf_band_coords.  Caller-provided buffers only. */
+/* The band lattice's coordinates (host memory).  Cube (ax[0..2] NULL): [-1,1]^3, point i at fl(fl(i * fl32(voxel)) - 1)
+ * per axis, as grid.lattice_points makes them.  Table (ax[0..2] all set): three DEVICE fp32 tables [N] (any box; grid.iso_band
+ * passes the torch.linspace tables of the dense threshold sweep), point (i, j, k) at (ax[0][i], ax[1][j], ax[2][k]);
+ * h[a] >= 0 the largest step of table a, pad >= 0 (the block test's only). */
+typedef struct nudf_band_coords {
+  double voxel;
+  const float* ax[3];
+  double h[3];
+  double pad;
+} nudf_band_coords;
 /* idx / pts [m^3] (m = ceil((N - 1) / s) + 1): the stride-s lattice in (x, y, z) lexicographic order */
-int nudf_nb_sublattice(int32_t n, int32_t s, double voxel, int64_t* idx, float* pts, void* stream);
-/* flags[nb^3] (may be NULL) = 1 for the kept blocks of stride s: candidates (every block when parent_flags is NULL, else the
- * blocks inside a kept block of stride parent_s) with a NaN corner or min(corner df) - lipschitz r < tau in fp64, r = half
- * the box diagonal, with slack (r + 1e-6 relative + 1e-6, tau + 1e-6 relative) against rounding.  Candidates' corners must
- * have been evaluated.  max_slope (DEVICE uint32[1], fp32 bits, zeroed by the caller) is raised to the largest
- * |du| / (edge length) over the candidates' box edges with finite ends */
-int nudf_nb_block_test(const float* df, int32_t n, int32_t s, const uint8_t* parent_flags, int32_t parent_s, double voxel,
-                       double lipschitz, double tau, uint8_t* flags, uint32_t* max_slope, void* stream);
+int nudf_nb_sublattice(int32_t n, int32_t s, const nudf_band_coords* co, int64_t* idx, float* pts, void* stream);
+/* flags[nb^3] (may be NULL) = 1 for the kept blocks of stride s on the cubic lattice `lat` (N = n0 = n1 = n2): candidates
+ * (every block when parent_flags is NULL, else the blocks inside a kept block of stride parent_s) with a NaN corner or
+ * min(corner df) - lipschitz r < tau in fp64, r = half the box diagonal.  Cube: r in voxels, with slack
+ * (r + 1e-6 relative + 1e-6, tau + 1e-6 relative) against rounding; edge slopes |du| / (e_a voxel).  Table (a df lattice
+ * only): r from the block's table-coordinate box (fp64, |ax[hi] - ax[lo]| per axis), enlarged by 1e-6 relative plus pad,
+ * and tau used as given (the caller's slack included); edge slopes |du| / (e_a h_a).  Candidates' corners must have been
+ * evaluated.  max_slope (DEVICE uint32[1], fp32 bits, zeroed by the caller) is raised to the largest |du| / (edge length)
+ * over the candidates' box edges with finite ends */
+int nudf_nb_block_test(const nudf_lattice* lat, int32_t s, const uint8_t* parent_flags, int32_t parent_s,
+                       const nudf_band_coords* co, double lipschitz, double tau, uint8_t* flags, uint32_t* max_slope,
+                       void* stream);
 /* counts[i] = the points block kept[i] of stride s emits: the stride-t lattice (t divides s) in its closed box, less the
  * stride-s lattice, less the points that a lower-numbered kept block (flags) also holds.  kept: ascending block numbers */
 int nudf_nb_count(const uint8_t* flags, int32_t n, int32_t s, int32_t t, const int64_t* kept, int64_t n_kept,
                   int32_t* counts, void* stream);
 /* idx / pts[offsets[i] ...] = those points of block kept[i] in (x, y, z) lexicographic order; offsets = exclusive scan */
 int nudf_nb_emit(const uint8_t* flags, int32_t n, int32_t s, int32_t t, const int64_t* kept, int64_t n_kept,
-                 const int64_t* offsets, double voxel, int64_t* idx, float* pts, void* stream);
-/* The same stages on the lattice of three DEVICE fp32 axis tables ax, ay, az [N] (any box; grid.iso_band passes the
- * torch.linspace tables of the dense threshold sweep): point (i, j, k) is (ax[i], ay[j], az[k]).  nudf_nb_count is shared. */
-/* nudf_nb_sublattice with the table coordinates */
-int nudf_nb_sublattice_box(int32_t n, int32_t s, const float* ax, const float* ay, const float* az, int64_t* idx, float* pts,
-                           void* stream);
-/* nudf_nb_block_test with r = half the diagonal of the block's table-coordinate box (fp64, |ax[hi] - ax[lo]| per axis),
- * enlarged by 1e-6 relative plus pad (>= 0), and tau used as given (the caller's slack included); edge slopes
- * |du| / (e_a h_a), h_a >= 0 the largest step of table a */
-int nudf_nb_block_test_box(const float* df, int32_t n, int32_t s, const uint8_t* parent_flags, int32_t parent_s,
-                           const float* ax, const float* ay, const float* az, double hx, double hy, double hz, double pad,
-                           double lipschitz, double tau, uint8_t* flags, uint32_t* max_slope, void* stream);
-/* nudf_nb_emit with the table coordinates */
-int nudf_nb_emit_box(const uint8_t* flags, int32_t n, int32_t s, int32_t t, const int64_t* kept, int64_t n_kept,
-                     const int64_t* offsets, const float* ax, const float* ay, const float* az, int64_t* idx, float* pts,
-                     void* stream);
+                 const int64_t* offsets, const nudf_band_coords* co, int64_t* idx, float* pts, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Block-sparse narrow band (neuraludf_b200/grid.py udf_band_sparse drives the levels, mesh.py udf_mesh_sparse meshes it)
  * ------------------------------------------------------------------------------------------------------------
- * The N^3 lattice of the nudf_nb_* entry points held without an N^3 array.  The points of the stride-c lattice (0, c, 2 c,
+ * The N^3 lattice of the nudf_nb_* entry points held without an N^3 array (a nudf_lattice with `store` set).  The points of the stride-c lattice (0, c, 2 c,
  * ... and N - 1 per axis; mc = ceil((N - 1) / c) + 1) live in the dense array coarse[mc^3], point (i, j, k) at
  * (ci * mc + cj) * mc + ck with ci = i / c, or mc - 1 for i = N - 1.  Every other point lives in a brick of NUDF_BRICK^3
  * points: brick (i / 8, j / 8, k / 8), numbered (bx * nbk + by) * nbk + bz (nbk = ceil(N / 8)), has slot dir[brick] (-1:
@@ -500,9 +508,6 @@ typedef struct nudf_brick_store {
   float* bricks;          /* [n_bricks * 512] */
   const int64_t* keys;    /* [n_bricks] */
 } nudf_brick_store;
-/* nudf_nb_block_test with the corner values read from the store */
-int nudf_sb_block_test(const nudf_brick_store* st, int32_t s, const uint8_t* parent_flags, int32_t parent_s, double voxel,
-                       double lipschitz, double tau, uint8_t* flags, uint32_t* max_slope, void* stream);
 /* marks[b] = 1 (marks: [nbk^3], zeroed by the caller) for every brick b that meets the closed box of a kept block of
  * stride s (flags [ceil((N - 1) / s)^3], nudf_nb_block_test's); s must be a multiple of the store's c */
 int nudf_sb_mark(const nudf_brick_store* st, int32_t s, const uint8_t* flags, int32_t* marks, void* stream);
@@ -513,20 +518,6 @@ int nudf_sb_store(const nudf_brick_store* st, const int64_t* idx, const float* v
 int nudf_sb_gather(const nudf_brick_store* st, const int64_t* idx, int64_t n, float* out, void* stream);
 /* out[t] = the flat lattice index of storage position pos[t] */
 int nudf_sb_flat(const nudf_brick_store* st, const int64_t* pos, int64_t n, int64_t* out, void* stream);
-/* The MeshUDF marching cubes stages nudf_mc_active, _cell_signs, _links, _count, _emit and _vertices on the store's N^3
- * lattice (n0 = n1 = n2 = N), the same arguments otherwise; nudf_mc_polarity reads no df and is shared. */
-int nudf_mcs_active(const nudf_brick_store* st, const int64_t* cand, int64_t n_cand, float avg_t, float max_t, uint8_t* flags,
-                    void* stream);
-int nudf_mcs_cell_signs(const nudf_brick_store* st, const int64_t* cells, int64_t n_cells, const int64_t* idx, int64_t n_idx,
-                        const float* normals, uint8_t* mask, void* stream);
-int nudf_mcs_links(const nudf_brick_store* st, const int64_t* cells, int64_t n_cells, const uint8_t* mask, int64_t* links,
-                   void* stream);
-int nudf_mcs_count(const nudf_brick_store* st, const int64_t* cells, int64_t n_cells, const uint8_t* mask, int32_t* counts,
-                   void* stream);
-int nudf_mcs_emit(const nudf_brick_store* st, const int64_t* cells, int64_t n_cells, const uint8_t* mask,
-                  const int64_t* offsets, int64_t* keys, void* stream);
-int nudf_mcs_vertices(const nudf_brick_store* st, const int64_t* cells, int64_t n_cells, const uint8_t* mask,
-                      const int64_t* keys, int64_t n_keys, float* verts, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Mesh post-processing (neuraludf_b200/mesh_post.py drives the steps; sorting, unique and compaction in torch)

@@ -82,6 +82,18 @@ class BrickStore(ctypes.Structure):
 BRICK = 8   # NUDF_BRICK
 
 
+class Lattice(ctypes.Structure):
+    """nudf_lattice (include/nudf.h): the lattice a kernel reads, the fp32 array df or a brick store (exactly one set)"""
+    _fields_ = [("n0", ctypes.c_int32), ("n1", ctypes.c_int32), ("n2", ctypes.c_int32), ("df", c_void_p),
+                ("store", ctypes.POINTER(BrickStore))]
+
+
+class BandCoords(ctypes.Structure):
+    """nudf_band_coords (include/nudf.h): the band lattice's cube coordinates (voxel), or its three fp32 tables with their
+    largest steps h and the block test's pad"""
+    _fields_ = [("voxel", ctypes.c_double), ("ax", c_void_p * 3), ("h", ctypes.c_double * 3), ("pad", ctypes.c_double)]
+
+
 PATCH_TYPES = {"l1": 0, "ssd": 1, "ssim": 2, "ncc": 3}
 
 
@@ -177,18 +189,13 @@ _SIGNATURES = {
     "nudf_gen_rays_grid": (ctypes.c_int, [c_void_p] * 2 + [ctypes.c_int32] * 4 + [c_void_p] * 5),
     "nudf_outside_points": (ctypes.c_int, [c_void_p, c_void_p, c_void_p, ctypes.c_int32, ctypes.c_int32, ctypes.c_int32,
                                            ctypes.c_float, c_void_p, c_void_p, c_void_p]),
-    "nudf_mc_active": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [c_void_p, ctypes.c_int64, ctypes.c_float,
-                                                                          ctypes.c_float, c_void_p, c_void_p]),
-    "nudf_mc_cell_signs": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [c_void_p, ctypes.c_int64, c_void_p,
-                                                                              ctypes.c_int64, c_void_p, c_void_p, c_void_p]),
-    "nudf_mc_links": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [c_void_p, ctypes.c_int64, c_void_p, c_void_p,
-                                                                         c_void_p]),
+    "nudf_mc_active": (ctypes.c_int, [c_void_p] * 2 + [ctypes.c_int64, ctypes.c_float, ctypes.c_float] + [c_void_p] * 2),
+    "nudf_mc_cell_signs": (ctypes.c_int, [c_void_p] * 2 + [ctypes.c_int64, c_void_p, ctypes.c_int64] + [c_void_p] * 3),
+    "nudf_mc_links": (ctypes.c_int, [c_void_p] * 2 + [ctypes.c_int64] + [c_void_p] * 3),
     "nudf_mc_polarity": (ctypes.c_int, [c_void_p, ctypes.c_int64] + [c_void_p] * 7),
-    "nudf_mc_count": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [c_void_p, ctypes.c_int64, c_void_p, c_void_p,
-                                                                         c_void_p]),
-    "nudf_mc_emit": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [c_void_p, ctypes.c_int64] + [c_void_p] * 4),
-    "nudf_mc_vertices": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [c_void_p, ctypes.c_int64, c_void_p, c_void_p,
-                                                                            ctypes.c_int64, c_void_p, c_void_p]),
+    "nudf_mc_count": (ctypes.c_int, [c_void_p] * 2 + [ctypes.c_int64] + [c_void_p] * 3),
+    "nudf_mc_emit": (ctypes.c_int, [c_void_p] * 2 + [ctypes.c_int64] + [c_void_p] * 4),
+    "nudf_mc_vertices": (ctypes.c_int, [c_void_p] * 2 + [ctypes.c_int64] + [c_void_p] * 2 + [ctypes.c_int64] + [c_void_p] * 2),
     "nudf_iso_active": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [ctypes.c_float, c_void_p, c_void_p]),
     "nudf_iso_count": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [ctypes.c_float, c_void_p, ctypes.c_int64, c_void_p,
                                                                           c_void_p]),
@@ -216,28 +223,15 @@ _SIGNATURES = {
                        + [c_void_p] * 2),
     "nudf_cl_vote": (ctypes.c_int, [c_void_p, ctypes.c_int64, c_void_p, ctypes.c_int32, c_void_p] + [ctypes.c_int32] * 3
                      + [c_void_p] * 2),
-    "nudf_nb_sublattice": (ctypes.c_int, [ctypes.c_int32] * 2 + [ctypes.c_double] + [c_void_p] * 3),
-    "nudf_nb_block_test": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 2 + [c_void_p, ctypes.c_int32] + [ctypes.c_double] * 3
+    "nudf_nb_sublattice": (ctypes.c_int, [ctypes.c_int32] * 2 + [c_void_p] * 4),
+    "nudf_nb_block_test": (ctypes.c_int, [c_void_p, ctypes.c_int32, c_void_p, ctypes.c_int32, c_void_p] + [ctypes.c_double] * 2
                            + [c_void_p] * 3),
     "nudf_nb_count": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [c_void_p, ctypes.c_int64] + [c_void_p] * 2),
-    "nudf_nb_emit": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [c_void_p, ctypes.c_int64, c_void_p, ctypes.c_double]
-                     + [c_void_p] * 3),
-    "nudf_nb_sublattice_box": (ctypes.c_int, [ctypes.c_int32] * 2 + [c_void_p] * 6),
-    "nudf_nb_block_test_box": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 2 + [c_void_p, ctypes.c_int32] + [c_void_p] * 3
-                               + [ctypes.c_double] * 6 + [c_void_p] * 3),
-    "nudf_nb_emit_box": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [c_void_p, ctypes.c_int64] + [c_void_p] * 7),
-    "nudf_sb_block_test": (ctypes.c_int, [c_void_p, ctypes.c_int32, c_void_p, ctypes.c_int32] + [ctypes.c_double] * 3
-                           + [c_void_p] * 3),
+    "nudf_nb_emit": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [c_void_p, ctypes.c_int64] + [c_void_p] * 5),
     "nudf_sb_mark": (ctypes.c_int, [c_void_p, ctypes.c_int32] + [c_void_p] * 3),
     "nudf_sb_store": (ctypes.c_int, [c_void_p] * 3 + [ctypes.c_int64] + [c_void_p] * 2),
     "nudf_sb_gather": (ctypes.c_int, [c_void_p] * 2 + [ctypes.c_int64] + [c_void_p] * 2),
     "nudf_sb_flat": (ctypes.c_int, [c_void_p] * 2 + [ctypes.c_int64] + [c_void_p] * 2),
-    "nudf_mcs_active": (ctypes.c_int, [c_void_p] * 2 + [ctypes.c_int64, ctypes.c_float, ctypes.c_float] + [c_void_p] * 2),
-    "nudf_mcs_cell_signs": (ctypes.c_int, [c_void_p] * 2 + [ctypes.c_int64, c_void_p, ctypes.c_int64] + [c_void_p] * 3),
-    "nudf_mcs_links": (ctypes.c_int, [c_void_p] * 2 + [ctypes.c_int64] + [c_void_p] * 3),
-    "nudf_mcs_count": (ctypes.c_int, [c_void_p] * 2 + [ctypes.c_int64] + [c_void_p] * 3),
-    "nudf_mcs_emit": (ctypes.c_int, [c_void_p] * 2 + [ctypes.c_int64] + [c_void_p] * 4),
-    "nudf_mcs_vertices": (ctypes.c_int, [c_void_p] * 2 + [ctypes.c_int64] + [c_void_p] * 2 + [ctypes.c_int64] + [c_void_p] * 2),
     "nudf_mp_faces": (ctypes.c_int, [c_void_p, ctypes.c_int64, c_void_p, ctypes.c_int64] + [c_void_p] * 6),
     "nudf_mp_hole_count": (ctypes.c_int, [c_void_p, ctypes.c_int64, c_void_p, c_void_p, ctypes.c_int64, c_void_p, c_void_p]),
     "nudf_mp_hole_emit": (ctypes.c_int, [c_void_p] * 3 + [ctypes.c_int64, c_void_p, c_void_p, ctypes.c_int64]
@@ -266,7 +260,7 @@ def lib():
             fn = getattr(L, name)
             fn.restype = res
             fn.argtypes = args
-        if L.nudf_abi_version() != 4:
+        if L.nudf_abi_version() != 5:
             raise RuntimeError("libnudf.so ABI version mismatch")
         _lib = L
     return _lib

@@ -5,11 +5,14 @@
 //             stride-c lattice (per axis 0, c, 2 c, ... and N - 1) in a dense coarse array [mc^3], every other point in an
 //             8^3 brick found through a dense directory over the ceil(N / 8)^3 bricks; a point whose brick has no slot
 //             reads +inf, as an unevaluated point of the dense band does.
+// with_lattice picks the reader a nudf_lattice descriptor names, so that every entry point taking one launches the same
+// kernel instantiations for both forms.
 #pragma once
 #include <math.h>
 #include <stdint.h>
 
 #include "../../include/nudf.h"
+#include "common.cuh"
 
 namespace nudf {
 
@@ -52,6 +55,19 @@ struct BrickDf {
 
 inline BrickDf brick_df(const nudf_brick_store& s) {
   return BrickDf{s.n, s.c, s.mc, s.nbk, s.coarse, s.dir, s.bricks};
+}
+
+// Checks the descriptor, then returns launch(DenseDf) or launch(BrickDf) for the lattice it names (-1: invalid).
+template <class F>
+inline int with_lattice(const nudf_lattice* lat, F&& launch) {
+  NUDF_REQUIRE(lat, "null lattice");
+  NUDF_REQUIRE(lat->n0 >= 2 && lat->n1 >= 2 && lat->n2 >= 2, "lattice dimensions must be at least 2");
+  NUDF_REQUIRE(!lat->df != !lat->store, "exactly one of df and store must be set");
+  if (lat->df) return launch(DenseDf{lat->df});
+  const nudf_brick_store* st = lat->store;
+  NUDF_REQUIRE(st->n >= 2 && st->coarse && st->dir && (st->bricks || st->n_bricks == 0), "null or invalid brick store");
+  NUDF_REQUIRE(lat->n0 == st->n && lat->n1 == st->n && lat->n2 == st->n, "the lattice dimensions must be the store's n");
+  return launch(brick_df(*st));
 }
 
 }  // namespace nudf

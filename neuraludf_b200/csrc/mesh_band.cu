@@ -37,6 +37,7 @@
 // so it is inactive in both lattices.  The threshold marching cubes (nudf_iso_*) reads df only at the corners of active
 // cells, so it gives the same active cells, faces, vertex keys and fp64 vertices on both.
 #include <algorithm>
+#include <type_traits>
 
 #include "../../include/nudf.h"
 #include "common.cuh"
@@ -110,7 +111,8 @@ struct TableSpacing {
   __device__ __forceinline__ double edge(int a, int64_t e) const { return __dmul_rn((double)e, h[a]); }
 };
 
-// A: the lattice reader (df_access.cuh): DenseDf for grid.udf_band / iso_band, BrickDf for grid.udf_band_sparse
+// A: the lattice reader (df_access.cuh): DenseDf for grid.udf_band / iso_band, BrickDf for grid.udf_band_sparse (cube
+// spacing only)
 template <class A, class S>
 __global__ void k_block_test(A df, Lat B, const uint8_t* __restrict__ parent, int64_t ps, int64_t pnb,
                              S sp, double lip, double tau, uint8_t* __restrict__ flags, unsigned* __restrict__ max_slope) {
@@ -233,28 +235,59 @@ static inline unsigned grid_for(int64_t n, int per_block = 256) {
 using namespace nudf;
 using namespace nudf::nb;
 
-int nudf_nb_sublattice(int32_t n, int32_t s, double voxel, int64_t* idx, float* pts, void* stream) {
-  NUDF_REQUIRE(idx && pts, "null pointer");
-  NUDF_REQUIRE(n >= 2 && s >= 1, "need N >= 2 and stride >= 1");
-  const int64_t m = cdiv(n - 1, s) + 1;
-  k_sublattice<<<grid_for(m * m * m), 256, 0, (cudaStream_t)stream>>>(n, s, m, CubeCoord{(float)voxel}, idx, pts);
-  NUDF_LAUNCH_OK();
+static inline bool is_table(const nudf_band_coords& co) { return co.ax[0] || co.ax[1] || co.ax[2]; }
+
+static int check_coords(const nudf_band_coords* co) {
+  NUDF_REQUIRE(co && (!is_table(*co) || (co->ax[0] && co->ax[1] && co->ax[2])), "null pointer");
+  NUDF_REQUIRE(!is_table(*co) || (co->h[0] >= 0.0 && co->h[1] >= 0.0 && co->h[2] >= 0.0 && co->pad >= 0.0),
+               "negative spacing or pad");
   return 0;
 }
 
-int nudf_nb_block_test(const float* df, int32_t n, int32_t s, const uint8_t* parent_flags, int32_t parent_s, double voxel,
-                       double lipschitz, double tau, uint8_t* flags, uint32_t* max_slope, void* stream) {
-  NUDF_REQUIRE(df && max_slope, "null pointer");
-  NUDF_REQUIRE(n >= 2 && s >= 1, "need N >= 2 and stride >= 1");
-  NUDF_REQUIRE(!parent_flags || (parent_s > s && parent_s % s == 0), "the parent stride must be a multiple of the stride");
-  NUDF_REQUIRE(lipschitz >= 0.0, "negative Lipschitz constant");
-  const Lat B{n, s, cdiv(n - 1, s)};
-  const int64_t pnb = parent_flags ? cdiv(n - 1, parent_s) : 0;
-  k_block_test<<<grid_for(B.nb * B.nb * B.nb), 256, 0, (cudaStream_t)stream>>>(DenseDf{df}, B, parent_flags, parent_s, pnb,
-                                                                               CubeSpacing{voxel}, lipschitz, tau, flags,
-                                                                               max_slope);
-  NUDF_LAUNCH_OK();
-  return 0;
+// Checks the descriptor, then returns launch(TableCoord) or launch(CubeCoord) (-1: invalid).
+template <class F>
+static int with_coords(const nudf_band_coords* co, F&& launch) {
+  if (check_coords(co)) return -1;
+  if (is_table(*co)) return launch(TableCoord{{co->ax[0], co->ax[1], co->ax[2]}});
+  return launch(CubeCoord{(float)co->voxel});
+}
+
+int nudf_nb_sublattice(int32_t n, int32_t s, const nudf_band_coords* co, int64_t* idx, float* pts, void* stream) {
+  return with_coords(co, [&](auto cr) {
+    NUDF_REQUIRE(idx && pts, "null pointer");
+    NUDF_REQUIRE(n >= 2 && s >= 1, "need N >= 2 and stride >= 1");
+    const int64_t m = cdiv(n - 1, s) + 1;
+    k_sublattice<<<grid_for(m * m * m), 256, 0, (cudaStream_t)stream>>>(n, s, m, cr, idx, pts);
+    NUDF_LAUNCH_OK();
+    return 0;
+  });
+}
+
+int nudf_nb_block_test(const nudf_lattice* lat, int32_t s, const uint8_t* parent_flags, int32_t parent_s,
+                       const nudf_band_coords* co, double lipschitz, double tau, uint8_t* flags, uint32_t* max_slope,
+                       void* stream) {
+  // the spacing rule follows the coordinates; the table form reads a dense lattice only
+  if (check_coords(co)) return -1;
+  NUDF_REQUIRE(!(is_table(*co) && lat && lat->store), "the table coordinates need a dense lattice");
+  return with_lattice(lat, [&](auto df) {
+    NUDF_REQUIRE(max_slope, "null pointer");
+    NUDF_REQUIRE(lat->n0 == lat->n1 && lat->n1 == lat->n2, "the band lattice must be cubic");
+    NUDF_REQUIRE(s >= 1, "need stride >= 1");
+    NUDF_REQUIRE(!parent_flags || (parent_s > s && parent_s % s == 0), "the parent stride must be a multiple of the stride");
+    NUDF_REQUIRE(lipschitz >= 0.0, "negative Lipschitz constant");
+    const int32_t n = lat->n0;
+    const Lat B{n, s, cdiv(n - 1, s)};
+    const int64_t pnb = parent_flags ? cdiv(n - 1, parent_s) : 0;
+    auto launch = [&](auto sp) {
+      k_block_test<<<grid_for(B.nb * B.nb * B.nb), 256, 0, (cudaStream_t)stream>>>(df, B, parent_flags, parent_s, pnb, sp,
+                                                                                   lipschitz, tau, flags, max_slope);
+      NUDF_LAUNCH_OK();
+      return 0;
+    };
+    if constexpr (std::is_same<decltype(df), DenseDf>::value)
+      if (is_table(*co)) return launch(TableSpacing{{co->ax[0], co->ax[1], co->ax[2]}, {co->h[0], co->h[1], co->h[2]}, co->pad});
+    return launch(CubeSpacing{co->voxel});
+  });
 }
 
 int nudf_nb_count(const uint8_t* flags, int32_t n, int32_t s, int32_t t, const int64_t* kept, int64_t n_kept,
@@ -268,66 +301,14 @@ int nudf_nb_count(const uint8_t* flags, int32_t n, int32_t s, int32_t t, const i
 }
 
 int nudf_nb_emit(const uint8_t* flags, int32_t n, int32_t s, int32_t t, const int64_t* kept, int64_t n_kept,
-                 const int64_t* offsets, double voxel, int64_t* idx, float* pts, void* stream) {
-  NUDF_REQUIRE(flags && (n_kept == 0 || (kept && offsets && idx && pts)), "null pointer");
-  NUDF_REQUIRE(n >= 2 && t >= 1 && s > t && s % t == 0, "the stride must be a multiple of the next stride");
-  if (n_kept == 0) return 0;
-  k_emit<<<grid_for(n_kept), 256, 0, (cudaStream_t)stream>>>(flags, Lat{n, s, cdiv(n - 1, s)}, t, kept, n_kept, offsets,
-                                                            CubeCoord{(float)voxel}, idx, pts);
-  NUDF_LAUNCH_OK();
-  return 0;
-}
-
-int nudf_nb_sublattice_box(int32_t n, int32_t s, const float* ax, const float* ay, const float* az, int64_t* idx, float* pts,
-                           void* stream) {
-  NUDF_REQUIRE(idx && pts && ax && ay && az, "null pointer");
-  NUDF_REQUIRE(n >= 2 && s >= 1, "need N >= 2 and stride >= 1");
-  const int64_t m = cdiv(n - 1, s) + 1;
-  k_sublattice<<<grid_for(m * m * m), 256, 0, (cudaStream_t)stream>>>(n, s, m, TableCoord{{ax, ay, az}}, idx, pts);
-  NUDF_LAUNCH_OK();
-  return 0;
-}
-
-int nudf_nb_block_test_box(const float* df, int32_t n, int32_t s, const uint8_t* parent_flags, int32_t parent_s,
-                           const float* ax, const float* ay, const float* az, double hx, double hy, double hz, double pad,
-                           double lipschitz, double tau, uint8_t* flags, uint32_t* max_slope, void* stream) {
-  NUDF_REQUIRE(df && max_slope && ax && ay && az, "null pointer");
-  NUDF_REQUIRE(n >= 2 && s >= 1, "need N >= 2 and stride >= 1");
-  NUDF_REQUIRE(!parent_flags || (parent_s > s && parent_s % s == 0), "the parent stride must be a multiple of the stride");
-  NUDF_REQUIRE(lipschitz >= 0.0, "negative Lipschitz constant");
-  NUDF_REQUIRE(hx >= 0.0 && hy >= 0.0 && hz >= 0.0 && pad >= 0.0, "negative spacing or pad");
-  const Lat B{n, s, cdiv(n - 1, s)};
-  const int64_t pnb = parent_flags ? cdiv(n - 1, parent_s) : 0;
-  k_block_test<<<grid_for(B.nb * B.nb * B.nb), 256, 0, (cudaStream_t)stream>>>(
-      DenseDf{df}, B, parent_flags, parent_s, pnb, TableSpacing{{ax, ay, az}, {hx, hy, hz}, pad}, lipschitz, tau, flags, max_slope);
-  NUDF_LAUNCH_OK();
-  return 0;
-}
-
-int nudf_nb_emit_box(const uint8_t* flags, int32_t n, int32_t s, int32_t t, const int64_t* kept, int64_t n_kept,
-                     const int64_t* offsets, const float* ax, const float* ay, const float* az, int64_t* idx, float* pts,
-                     void* stream) {
-  NUDF_REQUIRE(flags && ax && ay && az && (n_kept == 0 || (kept && offsets && idx && pts)), "null pointer");
-  NUDF_REQUIRE(n >= 2 && t >= 1 && s > t && s % t == 0, "the stride must be a multiple of the next stride");
-  if (n_kept == 0) return 0;
-  k_emit<<<grid_for(n_kept), 256, 0, (cudaStream_t)stream>>>(flags, Lat{n, s, cdiv(n - 1, s)}, t, kept, n_kept, offsets,
-                                                            TableCoord{{ax, ay, az}}, idx, pts);
-  NUDF_LAUNCH_OK();
-  return 0;
-}
-
-int nudf_sb_block_test(const nudf_brick_store* st, int32_t s, const uint8_t* parent_flags, int32_t parent_s, double voxel,
-                       double lipschitz, double tau, uint8_t* flags, uint32_t* max_slope, void* stream) {
-  NUDF_REQUIRE(st && st->coarse && st->dir && (st->bricks || st->n_bricks == 0) && max_slope, "null pointer");
-  NUDF_REQUIRE(st->n >= 2 && s >= 1, "need N >= 2 and stride >= 1");
-  NUDF_REQUIRE(!parent_flags || (parent_s > s && parent_s % s == 0), "the parent stride must be a multiple of the stride");
-  NUDF_REQUIRE(lipschitz >= 0.0, "negative Lipschitz constant");
-  const int32_t n = st->n;
-  const Lat B{n, s, cdiv(n - 1, s)};
-  const int64_t pnb = parent_flags ? cdiv(n - 1, parent_s) : 0;
-  k_block_test<<<grid_for(B.nb * B.nb * B.nb), 256, 0, (cudaStream_t)stream>>>(brick_df(*st), B, parent_flags, parent_s, pnb,
-                                                                               CubeSpacing{voxel}, lipschitz, tau, flags,
-                                                                               max_slope);
-  NUDF_LAUNCH_OK();
-  return 0;
+                 const int64_t* offsets, const nudf_band_coords* co, int64_t* idx, float* pts, void* stream) {
+  return with_coords(co, [&](auto cr) {
+    NUDF_REQUIRE(flags && (n_kept == 0 || (kept && offsets && idx && pts)), "null pointer");
+    NUDF_REQUIRE(n >= 2 && t >= 1 && s > t && s % t == 0, "the stride must be a multiple of the next stride");
+    if (n_kept == 0) return 0;
+    k_emit<<<grid_for(n_kept), 256, 0, (cudaStream_t)stream>>>(flags, Lat{n, s, cdiv(n - 1, s)}, t, kept, n_kept, offsets, cr,
+                                                              idx, pts);
+    NUDF_LAUNCH_OK();
+    return 0;
+  });
 }

@@ -20,9 +20,9 @@
 // candidates and normals, a lattice whose values equal the dense ones wherever those are <= max_t and are > max_t elsewhere
 // (+inf included: max <= max_t fails) meshes exactly like the dense one -- what grid.udf_band's narrow band relies on.
 // tests/proto/udf_mc.py restates every stage in NumPy with the same float32 operation order.
-// Every MeshUDF stage reads df through a lattice reader A (df_access.cuh): DenseDf, the flat array (nudf_mc_*), or
-// BrickDf, the block-sparse band of grid.udf_band_sparse (nudf_mcs_*).  The reader only replaces the load: both compute the
-// same values from the same corner values.
+// Every MeshUDF stage reads df through a lattice reader A (df_access.cuh): DenseDf, the flat array, or BrickDf, the
+// block-sparse band of grid.udf_band_sparse, as the nudf_lattice given to nudf_mc_* names.  The reader only replaces the
+// load: both compute the same values from the same corner values.
 // Threshold meshing (nudf_iso_*) runs stages 4-5 on v = fl32(f - level) instead of the pseudo-signed udf (the corner rules
 // UdfCorners / IsoCorners), with its own active-cell test and fp64 vertices; tests/proto/iso_mc.py restates it.
 #include <algorithm>
@@ -494,6 +494,7 @@ __global__ void k_iso_vertices(const float* __restrict__ df, Dims D, float level
 
 static inline unsigned grid_for(int64_t n) { return (unsigned)std::min<int64_t>(std::max<int64_t>(cdiv(n, 256), 1), 65535ll * 8); }
 static inline Dims dims(int32_t n0, int32_t n1, int32_t n2) { return Dims{n0, n1, n2}; }
+static inline Dims dims(const nudf_lattice& l) { return Dims{l.n0, l.n1, l.n2}; }
 
 }  // namespace mc
 }  // namespace nudf
@@ -503,35 +504,37 @@ using namespace nudf::mc;
 
 #define MC_DIMS_OK() NUDF_REQUIRE(n0 >= 2 && n1 >= 2 && n2 >= 2, "lattice dimensions must be at least 2")
 
-int nudf_mc_active(const float* df, int32_t n0, int32_t n1, int32_t n2, const int64_t* cand, int64_t n_cand, float avg_t,
-                   float max_t, uint8_t* flags, void* stream) {
-  MC_DIMS_OK();
-  NUDF_REQUIRE(df && flags && n_cand >= 0, "null pointer or negative count");
-  if (n_cand == 0) return 0;
-  k_active<<<grid_for(n_cand), 256, 0, (cudaStream_t)stream>>>(DenseDf{df}, dims(n0, n1, n2), cand, n_cand, avg_t, max_t, flags);
-  NUDF_LAUNCH_OK();
-  return 0;
+int nudf_mc_active(const nudf_lattice* lat, const int64_t* cand, int64_t n_cand, float avg_t, float max_t, uint8_t* flags,
+                   void* stream) {
+  return with_lattice(lat, [&](auto df) {
+    NUDF_REQUIRE(flags && n_cand >= 0 && (cand || lat->df || n_cand == 0), "null pointer or negative count");
+    if (n_cand == 0) return 0;
+    k_active<<<grid_for(n_cand), 256, 0, (cudaStream_t)stream>>>(df, dims(*lat), cand, n_cand, avg_t, max_t, flags);
+    NUDF_LAUNCH_OK();
+    return 0;
+  });
 }
 
-int nudf_mc_cell_signs(const float* df, int32_t n0, int32_t n1, int32_t n2, const int64_t* cells, int64_t n_cells,
-                       const int64_t* idx, int64_t n_idx, const float* normals, uint8_t* mask, void* stream) {
-  MC_DIMS_OK();
-  NUDF_REQUIRE(df && cells && normals && mask && n_cells >= 0, "null pointer or negative count");
-  if (n_cells == 0) return 0;
-  k_signs<<<grid_for(n_cells), 128, 0, (cudaStream_t)stream>>>(DenseDf{df}, dims(n0, n1, n2), cells, n_cells, idx, n_idx, normals,
-                                                               mask);
-  NUDF_LAUNCH_OK();
-  return 0;
+int nudf_mc_cell_signs(const nudf_lattice* lat, const int64_t* cells, int64_t n_cells, const int64_t* idx, int64_t n_idx,
+                       const float* normals, uint8_t* mask, void* stream) {
+  return with_lattice(lat, [&](auto df) {
+    NUDF_REQUIRE(cells && normals && mask && n_cells >= 0, "null pointer or negative count");
+    if (n_cells == 0) return 0;
+    k_signs<<<grid_for(n_cells), 128, 0, (cudaStream_t)stream>>>(df, dims(*lat), cells, n_cells, idx, n_idx, normals, mask);
+    NUDF_LAUNCH_OK();
+    return 0;
+  });
 }
 
-int nudf_mc_links(const float* df, int32_t n0, int32_t n1, int32_t n2, const int64_t* cells, int64_t n_cells,
-                  const uint8_t* mask, int64_t* links, void* stream) {
-  MC_DIMS_OK();
-  NUDF_REQUIRE(df && cells && mask && links && n_cells >= 0, "null pointer or negative count");
-  if (n_cells == 0) return 0;
-  k_links<<<grid_for(n_cells), 256, 0, (cudaStream_t)stream>>>(DenseDf{df}, dims(n0, n1, n2), cells, n_cells, mask, links);
-  NUDF_LAUNCH_OK();
-  return 0;
+int nudf_mc_links(const nudf_lattice* lat, const int64_t* cells, int64_t n_cells, const uint8_t* mask, int64_t* links,
+                  void* stream) {
+  return with_lattice(lat, [&](auto df) {
+    NUDF_REQUIRE(cells && mask && links && n_cells >= 0, "null pointer or negative count");
+    if (n_cells == 0) return 0;
+    k_links<<<grid_for(n_cells), 256, 0, (cudaStream_t)stream>>>(df, dims(*lat), cells, n_cells, mask, links);
+    NUDF_LAUNCH_OK();
+    return 0;
+  });
 }
 
 int nudf_mc_polarity(const int64_t* links, int64_t n_cells, const uint8_t* mask_in, int64_t* parent_ws, int64_t* hook_ws,
@@ -576,37 +579,39 @@ int nudf_mc_polarity(const int64_t* links, int64_t n_cells, const uint8_t* mask_
   return 0;
 }
 
-int nudf_mc_count(const float* df, int32_t n0, int32_t n1, int32_t n2, const int64_t* cells, int64_t n_cells,
-                  const uint8_t* mask, int32_t* counts, void* stream) {
-  MC_DIMS_OK();
-  NUDF_REQUIRE(df && cells && mask && counts && n_cells >= 0, "null pointer or negative count");
-  if (n_cells == 0) return 0;
-  k_count<<<grid_for(n_cells), 128, 0, (cudaStream_t)stream>>>(UdfCorners<DenseDf>{DenseDf{df}, mask}, dims(n0, n1, n2), cells,
-                                                                n_cells, counts);
-  NUDF_LAUNCH_OK();
-  return 0;
+int nudf_mc_count(const nudf_lattice* lat, const int64_t* cells, int64_t n_cells, const uint8_t* mask, int32_t* counts,
+                  void* stream) {
+  return with_lattice(lat, [&](auto df) {
+    NUDF_REQUIRE(cells && mask && counts && n_cells >= 0, "null pointer or negative count");
+    if (n_cells == 0) return 0;
+    k_count<<<grid_for(n_cells), 128, 0, (cudaStream_t)stream>>>(UdfCorners<decltype(df)>{df, mask}, dims(*lat), cells,
+                                                                  n_cells, counts);
+    NUDF_LAUNCH_OK();
+    return 0;
+  });
 }
 
-int nudf_mc_emit(const float* df, int32_t n0, int32_t n1, int32_t n2, const int64_t* cells, int64_t n_cells,
-                 const uint8_t* mask, const int64_t* offsets, int64_t* keys, void* stream) {
-  MC_DIMS_OK();
-  NUDF_REQUIRE(df && cells && mask && offsets && keys && n_cells >= 0, "null pointer or negative count");
-  if (n_cells == 0) return 0;
-  k_emit<<<grid_for(n_cells), 128, 0, (cudaStream_t)stream>>>(UdfCorners<DenseDf>{DenseDf{df}, mask}, dims(n0, n1, n2), cells,
-                                                               n_cells, offsets, keys);
-  NUDF_LAUNCH_OK();
-  return 0;
+int nudf_mc_emit(const nudf_lattice* lat, const int64_t* cells, int64_t n_cells, const uint8_t* mask, const int64_t* offsets,
+                 int64_t* keys, void* stream) {
+  return with_lattice(lat, [&](auto df) {
+    NUDF_REQUIRE(cells && mask && offsets && keys && n_cells >= 0, "null pointer or negative count");
+    if (n_cells == 0) return 0;
+    k_emit<<<grid_for(n_cells), 128, 0, (cudaStream_t)stream>>>(UdfCorners<decltype(df)>{df, mask}, dims(*lat), cells,
+                                                                 n_cells, offsets, keys);
+    NUDF_LAUNCH_OK();
+    return 0;
+  });
 }
 
-int nudf_mc_vertices(const float* df, int32_t n0, int32_t n1, int32_t n2, const int64_t* cells, int64_t n_cells,
-                     const uint8_t* mask, const int64_t* keys, int64_t n_keys, float* verts, void* stream) {
-  MC_DIMS_OK();
-  NUDF_REQUIRE(df && cells && mask && keys && verts && n_cells >= 0 && n_keys >= 0, "null pointer or negative count");
-  if (n_keys == 0) return 0;
-  k_vertices<<<grid_for(n_keys), 128, 0, (cudaStream_t)stream>>>(DenseDf{df}, dims(n0, n1, n2), cells, mask, keys, n_keys,
-                                                                 verts);
-  NUDF_LAUNCH_OK();
-  return 0;
+int nudf_mc_vertices(const nudf_lattice* lat, const int64_t* cells, int64_t n_cells, const uint8_t* mask, const int64_t* keys,
+                     int64_t n_keys, float* verts, void* stream) {
+  return with_lattice(lat, [&](auto df) {
+    NUDF_REQUIRE(cells && mask && keys && verts && n_cells >= 0 && n_keys >= 0, "null pointer or negative count");
+    if (n_keys == 0) return 0;
+    k_vertices<<<grid_for(n_keys), 128, 0, (cudaStream_t)stream>>>(df, dims(*lat), cells, mask, keys, n_keys, verts);
+    NUDF_LAUNCH_OK();
+    return 0;
+  });
 }
 
 #define ISO_LEVEL_OK() NUDF_REQUIRE(level == level && level - level == 0.f, "level must be finite")
@@ -651,76 +656,6 @@ int nudf_iso_vertices(const float* df, int32_t n0, int32_t n1, int32_t n2, float
   NUDF_REQUIRE(df && cells && keys && verts && n_cells >= 0 && n_keys >= 0, "null pointer or negative count");
   if (n_keys == 0) return 0;
   k_iso_vertices<<<grid_for(n_keys), 128, 0, (cudaStream_t)stream>>>(df, dims(n0, n1, n2), level, cells, keys, n_keys, verts);
-  NUDF_LAUNCH_OK();
-  return 0;
-}
-
-// ---- the same stages on the block-sparse band (nudf_brick_store) ----
-#define MCS_STORE_OK() NUDF_REQUIRE(st && st->n >= 2 && st->coarse && st->dir && (st->bricks || st->n_bricks == 0), \
-                                    "null or invalid brick store")
-
-int nudf_mcs_active(const nudf_brick_store* st, const int64_t* cand, int64_t n_cand, float avg_t, float max_t, uint8_t* flags,
-                    void* stream) {
-  MCS_STORE_OK();
-  NUDF_REQUIRE(flags && n_cand >= 0 && (cand || n_cand == 0), "null pointer or negative count");
-  if (n_cand == 0) return 0;
-  k_active<<<grid_for(n_cand), 256, 0, (cudaStream_t)stream>>>(brick_df(*st), dims(st->n, st->n, st->n), cand, n_cand, avg_t,
-                                                               max_t, flags);
-  NUDF_LAUNCH_OK();
-  return 0;
-}
-
-int nudf_mcs_cell_signs(const nudf_brick_store* st, const int64_t* cells, int64_t n_cells, const int64_t* idx, int64_t n_idx,
-                        const float* normals, uint8_t* mask, void* stream) {
-  MCS_STORE_OK();
-  NUDF_REQUIRE(cells && normals && mask && n_cells >= 0, "null pointer or negative count");
-  if (n_cells == 0) return 0;
-  k_signs<<<grid_for(n_cells), 128, 0, (cudaStream_t)stream>>>(brick_df(*st), dims(st->n, st->n, st->n), cells, n_cells, idx,
-                                                               n_idx, normals, mask);
-  NUDF_LAUNCH_OK();
-  return 0;
-}
-
-int nudf_mcs_links(const nudf_brick_store* st, const int64_t* cells, int64_t n_cells, const uint8_t* mask, int64_t* links,
-                   void* stream) {
-  MCS_STORE_OK();
-  NUDF_REQUIRE(cells && mask && links && n_cells >= 0, "null pointer or negative count");
-  if (n_cells == 0) return 0;
-  k_links<<<grid_for(n_cells), 256, 0, (cudaStream_t)stream>>>(brick_df(*st), dims(st->n, st->n, st->n), cells, n_cells, mask,
-                                                               links);
-  NUDF_LAUNCH_OK();
-  return 0;
-}
-
-int nudf_mcs_count(const nudf_brick_store* st, const int64_t* cells, int64_t n_cells, const uint8_t* mask, int32_t* counts,
-                   void* stream) {
-  MCS_STORE_OK();
-  NUDF_REQUIRE(cells && mask && counts && n_cells >= 0, "null pointer or negative count");
-  if (n_cells == 0) return 0;
-  k_count<<<grid_for(n_cells), 128, 0, (cudaStream_t)stream>>>(UdfCorners<BrickDf>{brick_df(*st), mask},
-                                                               dims(st->n, st->n, st->n), cells, n_cells, counts);
-  NUDF_LAUNCH_OK();
-  return 0;
-}
-
-int nudf_mcs_emit(const nudf_brick_store* st, const int64_t* cells, int64_t n_cells, const uint8_t* mask,
-                  const int64_t* offsets, int64_t* keys, void* stream) {
-  MCS_STORE_OK();
-  NUDF_REQUIRE(cells && mask && offsets && keys && n_cells >= 0, "null pointer or negative count");
-  if (n_cells == 0) return 0;
-  k_emit<<<grid_for(n_cells), 128, 0, (cudaStream_t)stream>>>(UdfCorners<BrickDf>{brick_df(*st), mask},
-                                                              dims(st->n, st->n, st->n), cells, n_cells, offsets, keys);
-  NUDF_LAUNCH_OK();
-  return 0;
-}
-
-int nudf_mcs_vertices(const nudf_brick_store* st, const int64_t* cells, int64_t n_cells, const uint8_t* mask,
-                      const int64_t* keys, int64_t n_keys, float* verts, void* stream) {
-  MCS_STORE_OK();
-  NUDF_REQUIRE(cells && mask && keys && verts && n_cells >= 0 && n_keys >= 0, "null pointer or negative count");
-  if (n_keys == 0) return 0;
-  k_vertices<<<grid_for(n_keys), 128, 0, (cudaStream_t)stream>>>(brick_df(*st), dims(st->n, st->n, st->n), cells, mask, keys,
-                                                                 n_keys, verts);
   NUDF_LAUNCH_OK();
   return 0;
 }

@@ -27,8 +27,12 @@ from neuraludf_b200._lib import check, ptr
 def lattice_points(head, count, N, device):
     """points `head .. head+count-1` of the N^3 lattice on [-1,1]^3 in the reference's order (x slowest, z fastest;
     extract_mesh.py:38-51), generated on the device"""
+    return _index_points(torch.arange(head, head + count, device=device, dtype=torch.int64), N)
+
+
+def _index_points(idx, N):
+    """fp32 points [P,3] of the flat lattice indices idx on the N^3 lattice on [-1,1]^3"""
     voxel = 2.0 / (N - 1)
-    idx = torch.arange(head, head + count, device=device, dtype=torch.int64)
     k = idx % N
     j = torch.div(idx, N, rounding_mode="floor") % N
     i = torch.div(torch.div(idx, N, rounding_mode="floor"), N, rounding_mode="floor") % N
@@ -62,15 +66,10 @@ def near_surface_cells(udf_network, N, df_flat=None, max_batch=1 << 20, dist_vox
 
 def _surface_normals(udf_network, N, idx, max_batch):
     """unit vectors towards the surface at the flat lattice indices idx (extract_mesh.py:77-98), batches of max_batch"""
-    voxel = 2.0 / (N - 1)
     normals = torch.empty(idx.numel(), 3, device=idx.device)
     for head in range(0, idx.numel(), max_batch):
         sel = idx[head:head + max_batch]
-        k = sel % N
-        j = torch.div(sel, N, rounding_mode="floor") % N
-        i = torch.div(torch.div(sel, N, rounding_mode="floor"), N, rounding_mode="floor") % N
-        pts = torch.stack([i.float() * voxel - 1.0, j.float() * voxel - 1.0, k.float() * voxel - 1.0], dim=-1)
-        g = udf_network.gradient(pts)[:, 0]
+        g = udf_network.gradient(_index_points(sel, N))[:, 0]
         g = g / (torch.linalg.norm(g, ord=2, dim=-1, keepdim=True) + 1e-5)          # exp_runner_blending.py:767-771 (func_grad)
         normals[head:head + sel.numel()] = -F.normalize(g, dim=1)                    # extract_mesh.py:93
     return normals
@@ -104,26 +103,61 @@ def _device(udf_network):
         return torch.device("cuda", torch.cuda.current_device())
 
 
-def band_sublattice(N, s, device):
-    """(flat indices [m^3] int64, points [m^3,3] fp32) of the stride-s lattice: 0, s, 2 s, ... and N - 1 per axis"""
-    L = _lib.lib()
+def _coords(N, axes=None, spacing=None, pad=0.0):
+    """the nudf_band_coords of the N^3 band lattice, by reference: the cube [-1,1]^3 (axes None) or the fp32 tables `axes`
+    (three contiguous [N] device tensors) with their largest steps `spacing` and the block test's `pad`"""
+    if axes is None:
+        return ctypes.byref(_lib.BandCoords(voxel=2.0 / (N - 1)))
+    if len(axes) != 3 or any(x.dtype != torch.float32 or x.shape != (N,) or not x.is_contiguous() for x in axes):
+        raise ValueError("axes must be three contiguous float32 tables of %d coordinates" % N)
+    return ctypes.byref(_lib.BandCoords(0.0, (ctypes.c_void_p * 3)(*(x.data_ptr() for x in axes)),
+                                        (ctypes.c_double * 3)(*(float(h) for h in spacing or (0.0, 0.0, 0.0))), float(pad)))
+
+
+def band_sublattice(N, s, device, axes=None):
+    """(flat indices [m^3] int64, points [m^3,3] fp32) of the stride-s lattice: 0, s, 2 s, ... and N - 1 per axis;
+    coordinates on [-1,1]^3, or from the three fp32 tables `axes` (iso_band)"""
     m = -(-(N - 1) // s) + 1
     idx = torch.empty(m ** 3, dtype=torch.int64, device=device)
     pts = torch.empty(m ** 3, 3, device=device)
-    check(L.nudf_nb_sublattice(N, s, 2.0 / (N - 1), ptr(idx), ptr(pts), _lib.stream_ptr()), "nudf_nb_sublattice")
+    check(_lib.lib().nudf_nb_sublattice(N, s, _coords(N, axes), ptr(idx), ptr(pts), _lib.stream_ptr()), "nudf_nb_sublattice")
     return idx, pts
 
 
-def band_block_test(df, N, s, parent=None, parent_s=0, lipschitz=2.0, dist_voxels=2.0, flags=True):
+class _DenseLattice:
+    """The N^3 lattice as one flat fp32 array `df`, +inf where never stored: the store of udf_band and iso_band."""
+
+    def __init__(self, df, N):
+        self.df, self.N = df, N
+
+    @property
+    def device(self):
+        return self.df.device
+
+    def lattice(self):
+        """the nudf_lattice descriptor, by reference"""
+        return ctypes.byref(_lib.Lattice(self.N, self.N, self.N, self.df.data_ptr(), None))
+
+    def store(self, idx, vals):
+        self.df[idx] = vals
+
+    def level_kept(self, flags, s):
+        pass
+
+
+def band_block_test(df, N, s, parent=None, parent_s=0, lipschitz=2.0, tau=None, flags=True, axes=None, spacing=None, pad=0.0):
     """(kept flags [nb^3] uint8 or None, largest edge slope) of the blocks of stride s (csrc/mesh_band.cu): candidates are every
-    block, or those inside a kept block of `parent` (stride parent_s)"""
-    L = _lib.lib()
-    voxel = 2.0 / (N - 1)
+    block, or those inside a kept block of `parent` (stride parent_s).  df: the flat fp32 lattice, or a store with lattice()
+    (SparseBand).  On [-1,1]^3 the threshold `tau` defaults to 2 voxels; with the fp32 tables `axes` the table rule: r from
+    the block's table coordinates plus `pad`, `tau` as given, edge slopes over `spacing` (the largest step per axis)."""
+    lat = _DenseLattice(df, N).lattice() if torch.is_tensor(df) else df.lattice()
+    device = df.device
     nb = -(-(N - 1) // s)
-    out = torch.empty(nb ** 3, dtype=torch.uint8, device=df.device) if flags else None
-    slope = torch.zeros(1, dtype=torch.int32, device=df.device)
-    check(L.nudf_nb_block_test(ptr(df), N, s, ptr(parent), parent_s, voxel, float(lipschitz), dist_voxels * voxel, ptr(out),
-                               ptr(slope), _lib.stream_ptr()), "nudf_nb_block_test")
+    out = torch.empty(nb ** 3, dtype=torch.uint8, device=device) if flags else None
+    slope = torch.zeros(1, dtype=torch.int32, device=device)
+    tau = 2.0 * (2.0 / (N - 1)) if tau is None else tau
+    check(_lib.lib().nudf_nb_block_test(lat, s, ptr(parent), parent_s, _coords(N, axes, spacing, pad), float(lipschitz),
+                                        float(tau), ptr(out), ptr(slope), _lib.stream_ptr()), "nudf_nb_block_test")
     return out, float(slope.view(torch.float32))
 
 
@@ -131,63 +165,45 @@ def band_points(flags, N, s, t, axes=None):
     """(flat indices [M] int64, points [M,3] fp32, kept block count): the stride-t points that the kept blocks of stride s
     emit, each point once (the lowest-numbered kept block holding it), blocks ascending, each in lexicographic order;
     coordinates on [-1,1]^3, or from the three fp32 tables `axes` (iso_band)"""
+    (out,) = _band_chunks(flags, N, s, t, axes)
+    return out
+
+
+def _band_chunks(flags, N, s, t, axes=None, chunk=None):
+    """band_points in its order, cut between kept blocks into chunks of about `chunk` points (None: one chunk), so that a
+    level need not hold all its points at once: yields (idx, pts, kept blocks) per chunk, at least one"""
     L = _lib.lib()
     st = _lib.stream_ptr()
+    co = _coords(N, axes)
     kept = torch.nonzero(flags).reshape(-1)
     n = kept.numel()
     counts = torch.empty(n, dtype=torch.int32, device=flags.device)
     check(L.nudf_nb_count(ptr(flags), N, s, t, ptr(kept), n, ptr(counts), st), "nudf_nb_count")
     csum = torch.cumsum(counts, 0, dtype=torch.int64)
-    total = int(csum[-1]) if n else 0
-    offsets = (csum - counts).contiguous()
-    idx = torch.empty(total, dtype=torch.int64, device=flags.device)
-    pts = torch.empty(total, 3, device=flags.device)
-    if axes is None:
-        check(L.nudf_nb_emit(ptr(flags), N, s, t, ptr(kept), n, ptr(offsets), 2.0 / (N - 1), ptr(idx), ptr(pts), st),
+    total = int(csum[-1]) if chunk is not None and n else 0
+    cuts = []
+    if chunk is not None and total > chunk:
+        cuts = torch.searchsorted(csum, torch.arange(chunk, total, chunk, device=flags.device), right=True).tolist()
+    bounds = [0] + sorted(set(cuts) - {0, n}) + [n]
+    head = 0
+    for a, b in zip(bounds, bounds[1:]):
+        end = int(csum[b - 1]) if b else 0
+        offsets = (csum[a:b] - counts[a:b] - head).contiguous()
+        idx = torch.empty(end - head, dtype=torch.int64, device=flags.device)
+        pts = torch.empty(end - head, 3, device=flags.device)
+        check(L.nudf_nb_emit(ptr(flags), N, s, t, ptr(kept[a:b]), b - a, ptr(offsets), co, ptr(idx), ptr(pts), st),
               "nudf_nb_emit")
-    else:
-        check(L.nudf_nb_emit_box(ptr(flags), N, s, t, ptr(kept), n, ptr(offsets), *_table_ptrs(axes, N), ptr(idx), ptr(pts),
-                                 st), "nudf_nb_emit_box")
-    return idx, pts, n
+        if b == n:                          # the level's block lists are not held while its last chunk is evaluated
+            del kept, counts, csum, offsets
+        yield idx, pts, b - a
+        head = end
 
 
-def _table_ptrs(axes, N):
-    if len(axes) != 3 or any(x.dtype != torch.float32 or x.shape != (N,) or not x.is_contiguous() for x in axes):
-        raise ValueError("axes must be three contiguous float32 tables of %d coordinates" % N)
-    return [ptr(x) for x in axes]
-
-
-def band_sublattice_box(axes, s):
-    """band_sublattice with the coordinates of the fp32 tables `axes` (three [N] device tensors)"""
-    L = _lib.lib()
-    N = axes[0].numel()
-    m = -(-(N - 1) // s) + 1
-    idx = torch.empty(m ** 3, dtype=torch.int64, device=axes[0].device)
-    pts = torch.empty(m ** 3, 3, device=axes[0].device)
-    check(L.nudf_nb_sublattice_box(N, s, *_table_ptrs(axes, N), ptr(idx), ptr(pts), _lib.stream_ptr()),
-          "nudf_nb_sublattice_box")
-    return idx, pts
-
-
-def band_block_test_box(df, axes, s, parent, parent_s, spacing, pad, lipschitz, tau, flags=True):
-    """band_block_test on the lattice of the tables `axes` (csrc/mesh_band.cu's table rule): r from the block's table
-    coordinates plus `pad`, `tau` as given, edge slopes over `spacing` (the largest step per axis)"""
-    L = _lib.lib()
-    N = axes[0].numel()
-    nb = -(-(N - 1) // s)
-    out = torch.empty(nb ** 3, dtype=torch.uint8, device=df.device) if flags else None
-    slope = torch.zeros(1, dtype=torch.int32, device=df.device)
-    check(L.nudf_nb_block_test_box(ptr(df), N, s, ptr(parent), parent_s, *_table_ptrs(axes, N), *(float(x) for x in spacing),
-                                   float(pad), float(lipschitz), float(tau), ptr(out), ptr(slope), _lib.stream_ptr()),
-          "nudf_nb_block_test_box")
-    return out, float(slope.view(torch.float32))
-
-
-def _coarse_to_fine(values, N, strides, device, max_batch, sublattice, block_test, points):
-    """The level loop of udf_band and iso_band: (df [N^3] fp32 flat, +inf where never evaluated; info without
-    max_edge_slope).  values(pts [P,3]) -> [P] fp32; sublattice(s) -> (idx, pts); block_test(df, s, parent, parent_s,
-    flags) -> (flags or None, slope); points(flags, s, t) -> (idx, pts, kept blocks)."""
-    df = torch.full((N ** 3,), float("inf"), device=device)
+def _coarse_to_fine(store, values, N, strides, lipschitz, tau, max_batch, chunk=None, axes=None, spacing=None, pad=0.0):
+    """The level loop of udf_band, iso_band and udf_band_sparse: fills `store` (store(idx, vals), lattice(), device and
+    level_kept(flags, s), called after each block test that hands flags on) and returns info without the wrappers' own keys.
+    values(pts [P,3]) -> [P] fp32, called in batches of max_batch; each level is emitted in chunks of about `chunk` points
+    (None: whole); coordinates and block test as band_block_test's."""
     info = {"strides": strides, "points": [], "kept_blocks": [], "edge_slope": []}
     events = []
 
@@ -197,33 +213,46 @@ def _coarse_to_fine(values, N, strides, device, max_batch, sublattice, block_tes
 
     def evaluate(idx, pts):
         for head in range(0, idx.numel(), max_batch):
-            df[idx[head:head + max_batch]] = values(pts[head:head + max_batch])
-        info["points"].append(int(idx.numel()))
+            store.store(idx[head:head + max_batch], values(pts[head:head + max_batch]))
+        return int(idx.numel())
 
     mark()
-    evaluate(*sublattice(strides[0]))
+    info["points"].append(evaluate(*band_sublattice(N, strides[0], store.device, axes)))
     mark()
     parent = None
     for k, s in enumerate(strides):
         last = k + 1 == len(strides)
-        flags, slope = block_test(df, s, parent, strides[k - 1] if k else 0, not last)
+        flags, slope = band_block_test(store, N, s, parent, strides[k - 1] if k else 0, lipschitz, tau, not last, axes,
+                                       spacing, pad)
         info["edge_slope"].append(slope)
         if last:
             break
-        idx, pts, n_kept = points(flags, s, strides[k + 1])
+        store.level_kept(flags, s)
+        n_points = n_kept = 0
+        for idx, pts, n in _band_chunks(flags, N, s, strides[k + 1], axes, chunk):
+            n_points += evaluate(idx, pts)
+            n_kept += n
+            del idx, pts
+        info["points"].append(n_points)
         info["kept_blocks"].append(n_kept)
-        evaluate(idx, pts)
-        del idx, pts
         mark()
         parent = flags
+    del parent, flags
     mark()
-    torch.cuda.synchronize(device)
+    torch.cuda.synchronize(store.device)
     ms = [a.elapsed_time(b) for a, b in zip(events, events[1:])]
     # level 0: the stride-strides[0] lattice; level k: block test at strides[k-1], emission and evaluation of strides[k]
     # points; slope_ms: the slope pass over the finest level
     info["level_ms"], info["slope_ms"] = ms[:-1], ms[-1]
     info["max_edge_slope"] = max(info["edge_slope"])
-    return df, info
+    return info
+
+
+def _warn_slope(info, lipschitz, what, miss):
+    """the RuntimeWarning of the band builders when a lattice edge is steeper than `lipschitz`"""
+    if info["max_edge_slope"] > lipschitz:
+        warnings.warn("%s: a lattice edge has slope %.3f > lipschitz=%.3f: the field is not %.3f-Lipschitz, so %s"
+                      % (what, info["max_edge_slope"], lipschitz, lipschitz, miss), RuntimeWarning, stacklevel=3)
 
 
 @torch.no_grad()
@@ -239,17 +268,11 @@ def udf_band(udf_network, N, lipschitz=2.0, strides=None, max_batch=1 << 21):
     `max_edge_slope` -- a lower bound on the field's Lipschitz constant: a RuntimeWarning is issued when it exceeds
     `lipschitz` -- and level_ms (CUDA events)."""
     strides = _check_strides(default_strides(N) if strides is None else strides)
-    device = _device(udf_network)
-    df, info = _coarse_to_fine(
-        lambda pts: udf_network.udf_values(pts).reshape(-1), N, strides, device, max_batch,
-        lambda s: band_sublattice(N, s, device),
-        lambda df, s, parent, parent_s, flags: band_block_test(df, N, s, parent, parent_s, lipschitz, flags=flags),
-        lambda flags, s, t: band_points(flags, N, s, t))
-    if info["max_edge_slope"] > lipschitz:
-        warnings.warn("udf_band: a lattice edge has slope %.3f > lipschitz=%.3f: the field is not %.3f-Lipschitz, so the band "
-                      "may miss points with udf < 2 voxels" % (info["max_edge_slope"], lipschitz, lipschitz), RuntimeWarning,
-                      stacklevel=2)
-    return df, info
+    lattice = _DenseLattice(torch.full((N ** 3,), float("inf"), device=_device(udf_network)), N)
+    info = _coarse_to_fine(lattice, lambda pts: udf_network.udf_values(pts).reshape(-1), N, strides, lipschitz,
+                           2.0 * (2.0 / (N - 1)), max_batch)
+    _warn_slope(info, lipschitz, "udf_band", "the band may miss points with udf < 2 voxels")
+    return lattice.df, info
 
 
 def sparse_coarse_stride(strides):
@@ -283,13 +306,16 @@ class SparseBand:
     def n_bricks(self):
         return self.keys.numel()
 
-    def desc(self):
-        """the nudf_brick_store descriptor (host struct of device pointers), by reference"""
-        d = _lib.BrickStore(self.N, self.c, self.mc, self.nbk, self.n_bricks, self.coarse.data_ptr(), self.dir.data_ptr(),
-                            self.bricks.data_ptr() if self.n_bricks else None,
-                            self.keys.data_ptr() if self.n_bricks else None)
-        self._d = d                               # kept alive until the next call
-        return ctypes.byref(d)
+    def _desc(self):
+        """the nudf_brick_store descriptor (host struct of device pointers), kept alive until the next call"""
+        self._d = _lib.BrickStore(self.N, self.c, self.mc, self.nbk, self.n_bricks, self.coarse.data_ptr(),
+                                  self.dir.data_ptr(), self.bricks.data_ptr() if self.n_bricks else None,
+                                  self.keys.data_ptr() if self.n_bricks else None)
+        return self._d
+
+    def lattice(self):
+        """the nudf_lattice descriptor naming the store, by reference"""
+        return ctypes.byref(_lib.Lattice(self.N, self.N, self.N, None, ctypes.pointer(self._desc())))
 
     def nbytes(self):
         """bytes held: coarse, dir, bricks (with keys)"""
@@ -300,7 +326,7 @@ class SparseBand:
         """slots for every brick that meets the closed box of a kept block of stride s (flags: the block test's)"""
         L = _lib.lib()
         marks = torch.zeros(self.nbk ** 3, dtype=torch.int32, device=self.device)
-        check(L.nudf_sb_mark(self.desc(), s, ptr(flags), ptr(marks), _lib.stream_ptr()), "nudf_sb_mark")
+        check(L.nudf_sb_mark(ctypes.byref(self._desc()), s, ptr(flags), ptr(marks), _lib.stream_ptr()), "nudf_sb_mark")
         keys = torch.nonzero(marks).reshape(-1)
         del marks
         self.dir.fill_(-1)
@@ -308,10 +334,15 @@ class SparseBand:
         self.keys = keys.contiguous()
         self.bricks = torch.full((keys.numel() * _lib.BRICK ** 3,), float("inf"), device=self.device)
 
+    def level_kept(self, flags, s):
+        """udf_band_sparse's levels: the bricks are allocated after the block test at stride c"""
+        if s == self.c:
+            self.allocate(flags, s)
+
     def store(self, idx, vals):
         """write vals [P] fp32 at the flat lattice indices idx [P]; a point with no storage raises at check_stored()"""
         vals = vals.reshape(-1).float().contiguous()
-        check(_lib.lib().nudf_sb_store(self.desc(), ptr(idx), ptr(vals), idx.numel(), ptr(self._missing),
+        check(_lib.lib().nudf_sb_store(ctypes.byref(self._desc()), ptr(idx), ptr(vals), idx.numel(), ptr(self._missing),
                                        _lib.stream_ptr()), "nudf_sb_store")
 
     def check_stored(self):
@@ -322,114 +353,39 @@ class SparseBand:
         """fp32 values at the flat lattice indices idx (int64 device tensor)"""
         idx = idx.reshape(-1).to(torch.int64).contiguous()
         out = torch.empty(idx.numel(), device=self.device)
-        check(_lib.lib().nudf_sb_gather(self.desc(), ptr(idx), idx.numel(), ptr(out), _lib.stream_ptr()), "nudf_sb_gather")
+        check(_lib.lib().nudf_sb_gather(ctypes.byref(self._desc()), ptr(idx), idx.numel(), ptr(out), _lib.stream_ptr()),
+              "nudf_sb_gather")
         return out
 
     def flat_index(self, pos):
         """flat lattice indices of storage positions pos (int64: [0, mc^3) coarse, then mc^3 + slot * 512 + local)"""
         out = torch.empty(pos.numel(), dtype=torch.int64, device=self.device)
-        check(_lib.lib().nudf_sb_flat(self.desc(), ptr(pos), pos.numel(), ptr(out), _lib.stream_ptr()), "nudf_sb_flat")
+        check(_lib.lib().nudf_sb_flat(ctypes.byref(self._desc()), ptr(pos), pos.numel(), ptr(out), _lib.stream_ptr()),
+              "nudf_sb_flat")
         return out
-
-
-def _band_point_chunks(flags, N, s, t, max_batch):
-    """band_points' (idx, pts) in its order, cut between kept blocks into chunks of about max_batch points, so that a level
-    never holds all its points at once: yields (idx, pts) per chunk"""
-    L = _lib.lib()
-    st = _lib.stream_ptr()
-    kept = torch.nonzero(flags).reshape(-1)
-    n = kept.numel()
-    if n == 0:
-        return
-    counts = torch.empty(n, dtype=torch.int32, device=flags.device)
-    check(L.nudf_nb_count(ptr(flags), N, s, t, ptr(kept), n, ptr(counts), st), "nudf_nb_count")
-    csum = torch.cumsum(counts, 0, dtype=torch.int64)
-    total = int(csum[-1])
-    cuts = []
-    if total > max_batch:
-        cuts = torch.searchsorted(csum, torch.arange(max_batch, total, max_batch, device=flags.device), right=True).tolist()
-    bounds = sorted(set([0, n] + cuts))
-    head = 0
-    for a, b in zip(bounds, bounds[1:]):
-        end = int(csum[b - 1])
-        offsets = (csum[a:b] - counts[a:b] - head).contiguous()
-        idx = torch.empty(end - head, dtype=torch.int64, device=flags.device)
-        pts = torch.empty(end - head, 3, device=flags.device)
-        check(L.nudf_nb_emit(ptr(flags), N, s, t, ptr(kept[a:b]), b - a, ptr(offsets), 2.0 / (N - 1), ptr(idx), ptr(pts), st),
-              "nudf_nb_emit")
-        yield idx, pts
-        head = end
 
 
 @torch.no_grad()
 def udf_band_sparse(udf_network, N, lipschitz=2.0, strides=None, max_batch=1 << 21):
     """udf_band's lattice without an N^3 array: (SparseBand, info).
 
-    The levels are udf_band's -- the same sub-lattice, block tests (nudf_sb_block_test: nudf_nb_block_test reading the
-    store), point emission and evaluation -- so the same RuntimeWarning when max_edge_slope exceeds `lipschitz`.  The
-    points of strides >= c (sparse_coarse_stride) go to the coarse array; after the block test at stride c, every brick
-    meeting a kept stride-c block is allocated, and the points of the finer strides, all inside those blocks, go to the
-    bricks.  A level is emitted and evaluated in chunks of about max_batch points.  If `udf_values` gives a point the
-    same bits in any batch, SparseBand.values equals udf_band's df at every lattice point, +inf included (DESIGN.md
-    section 1).  info: udf_band's keys, plus coarse_stride, bricks (slots allocated) and bytes (SparseBand.nbytes, and
-    the largest block-test flags array)."""
+    The levels are udf_band's -- the same sub-lattice, block tests (reading the store), point emission and evaluation --
+    so the same RuntimeWarning when max_edge_slope exceeds `lipschitz`.  The points of strides >= c
+    (sparse_coarse_stride) go to the coarse array; after the block test at stride c, every brick meeting a kept stride-c
+    block is allocated, and the points of the finer strides, all inside those blocks, go to the bricks.  A level is
+    emitted and evaluated in chunks of about max_batch points.  If `udf_values` gives a point the same bits in any batch,
+    SparseBand.values equals udf_band's df at every lattice point, +inf included (DESIGN.md section 1).  info: udf_band's
+    keys, plus coarse_stride, bricks (slots allocated) and bytes (SparseBand.nbytes, and the largest block-test flags
+    array)."""
     strides = _check_strides(default_strides(N) if strides is None else strides)
-    device = _device(udf_network)
-    L = _lib.lib()
-    voxel = 2.0 / (N - 1)
     c = sparse_coarse_stride(strides)
-    band = SparseBand(N, c, device)
-    info = {"strides": strides, "points": [], "kept_blocks": [], "edge_slope": [], "coarse_stride": c}
-    events = []
-    flag_bytes = 0
-
-    def mark():
-        events.append(torch.cuda.Event(enable_timing=True))
-        events[-1].record()
-
-    def evaluate(idx, pts):
-        for head in range(0, idx.numel(), max_batch):
-            band.store(idx[head:head + max_batch], udf_network.udf_values(pts[head:head + max_batch]))
-        return int(idx.numel())
-
-    mark()
-    info["points"].append(evaluate(*band_sublattice(N, strides[0], device)))
-    mark()
-    parent = None
-    for k, s in enumerate(strides):
-        last = k + 1 == len(strides)
-        nb = -(-(N - 1) // s)
-        flags = None if last else torch.empty(nb ** 3, dtype=torch.uint8, device=device)
-        slope = torch.zeros(1, dtype=torch.int32, device=device)
-        check(L.nudf_sb_block_test(band.desc(), s, ptr(parent), strides[k - 1] if k else 0, voxel, float(lipschitz),
-                                   2.0 * voxel, ptr(flags), ptr(slope), _lib.stream_ptr()), "nudf_sb_block_test")
-        info["edge_slope"].append(float(slope.view(torch.float32)))
-        if last:
-            break
-        flag_bytes = max(flag_bytes, flags.numel())
-        if s == c:
-            band.allocate(flags, s)
-        n_points = 0
-        for idx, pts in _band_point_chunks(flags, N, s, strides[k + 1], max_batch):
-            n_points += evaluate(idx, pts)
-            del idx, pts
-        info["points"].append(n_points)
-        info["kept_blocks"].append(int(torch.count_nonzero(flags)))
-        mark()
-        parent = flags
-    del parent, flags
-    mark()
-    torch.cuda.synchronize(device)
+    band = SparseBand(N, c, _device(udf_network))
+    info = _coarse_to_fine(band, lambda pts: udf_network.udf_values(pts).reshape(-1), N, strides, lipschitz,
+                           2.0 * (2.0 / (N - 1)), max_batch, chunk=max_batch)
     band.check_stored()
-    ms = [a.elapsed_time(b) for a, b in zip(events, events[1:])]
-    info["level_ms"], info["slope_ms"] = ms[:-1], ms[-1]
-    info["max_edge_slope"] = max(info["edge_slope"])
-    info["bricks"] = band.n_bricks
-    info["bytes"] = dict(band.nbytes(), flags=flag_bytes)
-    if info["max_edge_slope"] > lipschitz:
-        warnings.warn("udf_band_sparse: a lattice edge has slope %.3f > lipschitz=%.3f: the field is not %.3f-Lipschitz, so "
-                      "the band may miss points with udf < 2 voxels" % (info["max_edge_slope"], lipschitz, lipschitz),
-                      RuntimeWarning, stacklevel=2)
+    info.update(coarse_stride=c, bricks=band.n_bricks,
+                bytes=dict(band.nbytes(), flags=max([(-(-(N - 1) // s)) ** 3 for s in strides[:-1]], default=0)))
+    _warn_slope(info, lipschitz, "udf_band_sparse", "the band may miss points with udf < 2 voxels")
     return band, info
 
 
@@ -511,18 +467,12 @@ def iso_band(query, bound_min, bound_max, resolution, level, lipschitz=2.0, stri
         raise ValueError("the lattice tables must be float32 (torch's default dtype is %s)" % torch.get_default_dtype())
     h, e = table_spacing(axes)
     tau, pad = iso_cull(level, lipschitz, h, e)
-    df, info = _coarse_to_fine(
-        lambda pts: query(pts).detach().reshape(-1).float(), N, strides, device, max_batch,
-        lambda s: band_sublattice_box(axes, s),
-        lambda df, s, parent, parent_s, flags: band_block_test_box(df, axes, s, parent, parent_s, h, pad, lipschitz, tau,
-                                                                   flags),
-        lambda flags, s, t: band_points(flags, N, s, t, axes))
+    lattice = _DenseLattice(torch.full((N ** 3,), float("inf"), device=device), N)
+    info = _coarse_to_fine(lattice, lambda pts: query(pts).detach().reshape(-1).float(), N, strides, lipschitz, tau,
+                           max_batch, axes=axes, spacing=h, pad=pad)
     info.update(tau=tau, pad=pad, spacing=h)
-    if info["max_edge_slope"] > lipschitz:
-        warnings.warn("iso_band: a lattice edge has slope %.3f > lipschitz=%.3f: the field is not %.3f-Lipschitz, so a "
-                      "threshold mesh may miss cells" % (info["max_edge_slope"], lipschitz, lipschitz), RuntimeWarning,
-                      stacklevel=2)
-    return df, info
+    _warn_slope(info, lipschitz, "iso_band", "a threshold mesh may miss cells")
+    return lattice.df, info
 
 
 @torch.no_grad()

@@ -36,8 +36,6 @@ def marching_cubes_index(df, dims, normals, idx=None):
     of the sorted flat indices `idx`.  info: `active` (sorted active cells), `face_keys` [F,3] (vertex keys: lattice edges,
     then loop centres), `mask` (final per-cell pseudo-sign masks), `polarity_rounds` / `polarity_jumps` (union-find
     hooking rounds / pointer-jumping passes).  Faces are wound towards the positive pseudo-side (the reference's 'descent' winding)."""
-    L = _lib.lib()
-    st = _lib.stream_ptr()
     n0, n1, n2 = (int(d) for d in dims)
     dev = df.device
     if dev.type != "cuda":
@@ -52,33 +50,19 @@ def marching_cubes_index(df, dims, normals, idx=None):
             raise ValueError("normals must have one row per idx entry")
     elif normals.shape[0] != df.numel():
         raise ValueError("dense normals must have one row per lattice point")
-    n_cand = n0 * n1 * n2 if idx is None else idx.numel()
-    stages = {
-        "active": lambda avg_t, max_t, flags: check(L.nudf_mc_active(ptr(df), n0, n1, n2, ptr(idx), n_cand, avg_t, max_t,
-                                                                     ptr(flags), st), "nudf_mc_active"),
-        "signs": lambda cells, n, mask0: check(L.nudf_mc_cell_signs(ptr(df), n0, n1, n2, ptr(cells), n, ptr(idx),
-                                                                    0 if idx is None else idx.numel(), ptr(normals),
-                                                                    ptr(mask0), st), "nudf_mc_cell_signs"),
-        "links": lambda cells, n, mask0, links: check(L.nudf_mc_links(ptr(df), n0, n1, n2, ptr(cells), n, ptr(mask0),
-                                                                      ptr(links), st), "nudf_mc_links"),
-        "count": lambda cells, n, mask, counts: check(L.nudf_mc_count(ptr(df), n0, n1, n2, ptr(cells), n, ptr(mask),
-                                                                      ptr(counts), st), "nudf_mc_count"),
-        "emit": lambda cells, n, mask, offsets, keys: check(L.nudf_mc_emit(ptr(df), n0, n1, n2, ptr(cells), n, ptr(mask),
-                                                                           ptr(offsets), ptr(keys), st), "nudf_mc_emit"),
-        "vertices": lambda cells, n, mask, ukeys, verts: check(L.nudf_mc_vertices(ptr(df), n0, n1, n2, ptr(cells), n,
-                                                                                  ptr(mask), ptr(ukeys), ukeys.numel(),
-                                                                                  ptr(verts), st), "nudf_mc_vertices")}
-    return _mc_stages(stages, n2, n_cand, idx, dev)
+    lat = _lib.Lattice(n0, n1, n2, df.data_ptr(), None)
+    return _mc_stages(ctypes.byref(lat), n2, n0 * n1 * n2 if idx is None else idx.numel(), idx, normals, dev)
 
 
-def _mc_stages(stages, n2, n_cand, idx, dev):
-    """the MeshUDF MC driver shared by marching_cubes_index and marching_cubes_sparse: `stages` launch the kernels on
-    their lattice (dense df or brick store); idx the sorted candidate indices (None: every cell)"""
+def _mc_stages(lat, n2, n_cand, idx, normals, dev):
+    """the MeshUDF MC driver of marching_cubes_index and marching_cubes_sparse on the lattice descriptor `lat` (dense df or
+    brick store); idx the sorted candidate indices (None: every cell) and normals their rows"""
     L = _lib.lib()
     st = _lib.stream_ptr()
+    n_idx = 0 if idx is None else idx.numel()
     avg_t, max_t = thresholds(n2)
     flags = torch.empty(n_cand, dtype=torch.uint8, device=dev)
-    stages["active"](avg_t, max_t, flags)
+    check(L.nudf_mc_active(lat, ptr(idx), n_cand, avg_t, max_t, ptr(flags), st), "nudf_mc_active")
     sel = torch.nonzero(flags).reshape(-1)
     cells = (sel if idx is None else idx[sel]).contiguous()
     n = cells.numel()
@@ -88,9 +72,9 @@ def _mc_stages(stages, n2, n_cand, idx, dev):
         info.update(face_keys=empty[1], mask=torch.zeros(0, dtype=torch.uint8, device=dev))
         return empty[0], empty[1], info
     mask0 = torch.empty(n, dtype=torch.uint8, device=dev)
-    stages["signs"](cells, n, mask0)
+    check(L.nudf_mc_cell_signs(lat, ptr(cells), n, ptr(idx), n_idx, ptr(normals), ptr(mask0), st), "nudf_mc_cell_signs")
     links = torch.empty(n * 3, dtype=torch.int64, device=dev)
-    stages["links"](cells, n, mask0, links)
+    check(L.nudf_mc_links(lat, ptr(cells), n, ptr(mask0), ptr(links), st), "nudf_mc_links")
     parent = torch.empty(n, dtype=torch.int64, device=dev)
     hook = torch.empty(n, dtype=torch.int64, device=dev)
     flag = torch.empty(1, dtype=torch.int32, device=dev)
@@ -100,51 +84,33 @@ def _mc_stages(stages, n2, n_cand, idx, dev):
           "nudf_mc_polarity")
     info["polarity_rounds"], info["polarity_jumps"] = int(stats[0]), int(stats[1])
     counts = torch.empty(n, dtype=torch.int32, device=dev)
-    stages["count"](cells, n, mask, counts)
+    check(L.nudf_mc_count(lat, ptr(cells), n, ptr(mask), ptr(counts), st), "nudf_mc_count")
     csum = torch.cumsum(counts, 0, dtype=torch.int64)
     n_faces = int(csum[-1])
     offsets = (csum - counts).contiguous()
     keys = torch.empty(3 * n_faces, dtype=torch.int64, device=dev)
-    stages["emit"](cells, n, mask, offsets, keys)
+    check(L.nudf_mc_emit(lat, ptr(cells), n, ptr(mask), ptr(offsets), ptr(keys), st), "nudf_mc_emit")
     info.update(face_keys=keys.reshape(-1, 3), mask=mask)
     if n_faces == 0:
         return empty[0], empty[1], info
     ukeys, inv = torch.unique(keys, sorted=True, return_inverse=True)
     ukeys = ukeys.contiguous()
     verts = torch.empty(ukeys.numel(), 3, device=dev)
-    stages["vertices"](cells, n, mask, ukeys, verts)
+    check(L.nudf_mc_vertices(lat, ptr(cells), n, ptr(mask), ptr(ukeys), ukeys.numel(), ptr(verts), st), "nudf_mc_vertices")
     info["vertex_keys"] = ukeys
     return verts, inv.reshape(-1, 3).to(torch.int64), info
 
 
 @torch.no_grad()
 def marching_cubes_sparse(band, normals, idx):
-    """marching_cubes_index on the N^3 lattice of a grid.SparseBand (every df read through the brick store,
-    nudf_mcs_*): the same (verts [V,3] fp32 in lattice-index units, faces [F,3] int64, info).  idx / normals: the sorted
-    flat candidate indices and their rows (grid.near_surface_cells_sparse); there is no dense form."""
-    L = _lib.lib()
-    st = _lib.stream_ptr()
-    dev = band.device
+    """marching_cubes_index on the N^3 lattice of a grid.SparseBand (every df read through the brick store): the same
+    (verts [V,3] fp32 in lattice-index units, faces [F,3] int64, info).  idx / normals: the sorted flat candidate indices
+    and their rows (grid.near_surface_cells_sparse); there is no dense form."""
     idx = idx.reshape(-1).to(torch.int64).contiguous()
     normals = normals.reshape(-1, 3).float().contiguous()
     if normals.shape[0] != idx.numel():
         raise ValueError("normals must have one row per idx entry")
-    d = band.desc()
-    stages = {
-        "active": lambda avg_t, max_t, flags: check(L.nudf_mcs_active(d, ptr(idx), idx.numel(), avg_t, max_t, ptr(flags), st),
-                                                    "nudf_mcs_active"),
-        "signs": lambda cells, n, mask0: check(L.nudf_mcs_cell_signs(d, ptr(cells), n, ptr(idx), idx.numel(), ptr(normals),
-                                                                     ptr(mask0), st), "nudf_mcs_cell_signs"),
-        "links": lambda cells, n, mask0, links: check(L.nudf_mcs_links(d, ptr(cells), n, ptr(mask0), ptr(links), st),
-                                                      "nudf_mcs_links"),
-        "count": lambda cells, n, mask, counts: check(L.nudf_mcs_count(d, ptr(cells), n, ptr(mask), ptr(counts), st),
-                                                      "nudf_mcs_count"),
-        "emit": lambda cells, n, mask, offsets, keys: check(L.nudf_mcs_emit(d, ptr(cells), n, ptr(mask), ptr(offsets),
-                                                                            ptr(keys), st), "nudf_mcs_emit"),
-        "vertices": lambda cells, n, mask, ukeys, verts: check(L.nudf_mcs_vertices(d, ptr(cells), n, ptr(mask), ptr(ukeys),
-                                                                                   ukeys.numel(), ptr(verts), st),
-                                                               "nudf_mcs_vertices")}
-    return _mc_stages(stages, band.N, idx.numel(), idx, dev)
+    return _mc_stages(band.lattice(), band.N, idx.numel(), idx, normals, band.device)
 
 
 def _iso_level(level):
@@ -273,12 +239,10 @@ def udf_mesh(udf_network, N, dist_threshold_ratio=1.0, lo=0, hi=None, max_batch=
     can mesh disjoint slabs -- adjacent slabs must share one plane for the cells between them to be meshed.  Faces with a
     vertex whose udf is at or above voxel * dist_threshold_ratio are dropped (extract_mesh.py:205-214) and unused vertices
     removed."""
-    from neuraludf_b200 import grid
     hi = N ** 3 if hi is None else hi
     if lo % (N * N) or hi % (N * N) or not 0 <= lo < hi <= N ** 3:
         raise ValueError("lo / hi must select whole x-planes of the N^3 lattice")
-    df = grid.udf_grid(udf_network, N, max_batch=max_batch, lo=lo, hi=hi)
-    return _mesh_lattice(udf_network, N, df, dist_threshold_ratio, lo, max_batch)
+    return _udf_mesh(udf_network, N, "dense", dist_threshold_ratio, max_batch=max_batch, lo=lo, hi=hi)
 
 
 def _mc_lattice(udf_network, N, df, lo, max_batch):
@@ -291,18 +255,32 @@ def _mc_lattice(udf_network, N, df, lo, max_batch):
     return verts, faces
 
 
-def _mesh_lattice(udf_network, N, df, dist_threshold_ratio, lo, max_batch):
-    """near-surface normals -> MC -> vertex filter of the lattice values df (whole x-planes from flat index lo)"""
-    verts, faces = _mc_lattice(udf_network, N, df, lo, max_batch)
-    return _vertex_filter(udf_network, N, verts, faces, dist_threshold_ratio, lo)
-
-
-def _mc_sparse(udf_network, band, max_batch):
-    """near-surface normals -> MC of a grid.SparseBand: (verts [V,3] fp32 in lattice-index units, faces [F,3] int64)"""
+def _udf_mc(udf_network, N, lattice, lipschitz=2.0, strides=None, max_batch=1 << 21, lo=0, hi=None):
+    """The raw MeshUDF MC of the N^3 lattice evaluated `lattice`: "dense" (grid.udf_grid of the slab [lo, hi)), "band"
+    (grid.udf_band) or "sparse" (grid.udf_band_sparse): (verts [V,3] fp32 in the slab's lattice-index units, faces [F,3]
+    int64).  The lattice is released on return."""
     from neuraludf_b200 import grid
-    idx, normals = grid.near_surface_cells_sparse(udf_network, band, max_batch=max(max_batch // 2, 1))
-    verts, faces, _ = marching_cubes_sparse(band, normals, idx)
-    return verts, faces
+    if lattice == "sparse":
+        band, _ = grid.udf_band_sparse(udf_network, N, lipschitz=lipschitz, strides=strides, max_batch=max_batch)
+        idx, normals = grid.near_surface_cells_sparse(udf_network, band, max_batch=max(max_batch // 2, 1))
+        verts, faces, _ = marching_cubes_sparse(band, normals, idx)
+        return verts, faces
+    if lattice == "dense":
+        df = grid.udf_grid(udf_network, N, max_batch=max_batch, lo=lo, hi=hi)
+    else:
+        df, _ = grid.udf_band(udf_network, N, lipschitz=lipschitz, strides=strides, max_batch=max_batch)
+    return _mc_lattice(udf_network, N, df, lo, max_batch)
+
+
+def _udf_mesh(udf_network, N, lattice, dist_threshold_ratio, lipschitz=2.0, strides=None, max_batch=1 << 21, lo=0, hi=None):
+    """_udf_mc's MC with the vertex filter: udf_mesh, udf_mesh_band or udf_mesh_sparse as `lattice` names it"""
+    verts, faces = _udf_mc(udf_network, N, lattice, lipschitz, strides, max_batch, lo, hi)
+    return _vertex_filter(udf_network, N, verts, faces, dist_threshold_ratio, lo, max_batch if lattice == "sparse" else None)
+
+
+def _lattice_kind(dense, sparse):
+    """the lattice _udf_mc evaluates for udf_mesh_post's / the CLI's dense and sparse switches"""
+    return "dense" if dense else ("sparse" if sparse else "band")
 
 
 def _batched_values(udf_network, pts, max_batch):
@@ -334,9 +312,7 @@ def udf_mesh_band(udf_network, N, dist_threshold_ratio=1.0, lipschitz=2.0, strid
     the same points and normals, an unevaluated (+inf) corner fails the MC's active-cell test (max <= 1.74 voxel) exactly
     as its dense value >= 2 voxels does, and the later MC stages read df only at the corners of active cells
     (csrc/mesh_udf.cu).  grid.udf_band warns when the lattice shows a slope above `lipschitz`."""
-    from neuraludf_b200 import grid
-    df, _ = grid.udf_band(udf_network, N, lipschitz=lipschitz, strides=strides, max_batch=max_batch)
-    return _mesh_lattice(udf_network, N, df, dist_threshold_ratio, 0, max_batch)
+    return _udf_mesh(udf_network, N, "band", dist_threshold_ratio, lipschitz, strides, max_batch)
 
 
 @torch.no_grad()
@@ -347,11 +323,7 @@ def udf_mesh_sparse(udf_network, N, dist_threshold_ratio=1.0, lipschitz=2.0, str
     Exact under udf_mesh_band's conditions: the store then reads udf_band's df at every lattice point (DESIGN.md section 1),
     so every stage sees the same values.  The store is released before the vertex filter, which evaluates the vertices in
     batches of max_batch (at 2048^3 a single batch of every vertex would need tens of GB of value-chain workspace)."""
-    from neuraludf_b200 import grid
-    band, _ = grid.udf_band_sparse(udf_network, N, lipschitz=lipschitz, strides=strides, max_batch=max_batch)
-    verts, faces = _mc_sparse(udf_network, band, max_batch)
-    del band
-    return _vertex_filter(udf_network, N, verts, faces, dist_threshold_ratio, 0, max_batch)
+    return _udf_mesh(udf_network, N, "sparse", dist_threshold_ratio, lipschitz, strides, max_batch)
 
 
 @torch.no_grad()
@@ -367,21 +339,11 @@ def udf_mesh_post(udf_network, N, dist_threshold_ratio=5.0, dense=False, lipschi
     `mesh_post.postprocess` does the rest of get_mesh_udf_fast (extract_mesh.py:215-265; the runner passes
     `dist_threshold_ratio` 5 and `smooth_borders` True).  info: postprocess's, plus `mc` ((V, F) of the raw MC) and
     `filtered` (faces after the vertex filter)."""
-    from neuraludf_b200 import grid, mesh_post
+    from neuraludf_b200 import mesh_post
     voxel = 2.0 / (N - 1)
     if dense and sparse:
         raise ValueError("udf_mesh_post: dense and sparse exclude each other")
-    if sparse:
-        band, _ = grid.udf_band_sparse(udf_network, N, lipschitz=lipschitz, strides=strides, max_batch=max_batch)
-        verts, faces = _mc_sparse(udf_network, band, max_batch)
-        del band
-    else:
-        if dense:
-            df = grid.udf_grid(udf_network, N, max_batch=max_batch)
-        else:
-            df, _ = grid.udf_band(udf_network, N, lipschitz=lipschitz, strides=strides, max_batch=max_batch)
-        verts, faces = _mc_lattice(udf_network, N, df, 0, max_batch)
-        del df
+    verts, faces = _udf_mc(udf_network, N, _lattice_kind(dense, sparse), lipschitz, strides, max_batch)
     v64 = verts.double() * voxel - 1.0
     n_mc = faces.shape[0]
     if n_mc:
@@ -557,12 +519,8 @@ def main(argv=None):
     if a.postprocess:
         verts, faces, _ = udf_mesh_post(net, a.resolution, a.dist_threshold_ratio, dense=a.dense, lipschitz=a.lipschitz,
                                         sparse=a.sparse)
-    elif a.dense:
-        verts, faces = udf_mesh(net, a.resolution, a.dist_threshold_ratio)
-    elif a.sparse:
-        verts, faces = udf_mesh_sparse(net, a.resolution, a.dist_threshold_ratio, a.lipschitz)
     else:
-        verts, faces = udf_mesh_band(net, a.resolution, a.dist_threshold_ratio, a.lipschitz)
+        verts, faces = _udf_mesh(net, a.resolution, _lattice_kind(a.dense, a.sparse), a.dist_threshold_ratio, a.lipschitz)
     v = verts.double().cpu().numpy()
     if a.cameras is not None:                     # exp_runner_blending.py:792-794, with the dataset's fp32 scale_mat_0
         sm = np.load(a.cameras)["scale_mat_0"].astype(np.float32)

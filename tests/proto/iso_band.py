@@ -1,4 +1,4 @@
-"""NumPy restatement of the narrow-band kernels' table form (csrc/mesh_band.cu: nudf_nb_*_box) and of grid.iso_band's
+"""NumPy restatement of the narrow-band kernels' table form (csrc/mesh_band.cu: nudf_nb_*, tables) and of grid.iso_band's
 level chain: the lattice of three fp32 axis tables on any box, the fp64 block test of the table spacing rule (same operation
 order and slack as the kernel and grid.iso_cull), and point emission (udf_band.emit's order, coordinates from the tables)."""
 import math

@@ -15,7 +15,7 @@ def _header_functions():
     return sorted(set(re.findall(r"\b(nudf_[a-z0-9_]+)\s*\(", txt)))
 
 
-def test_library_exports_every_declared_symbol():
+def test_library_exports_the_declared_abi():
     from neuraludf_b200 import _lib
     assert os.path.exists(_lib.LIB_PATH), "libnudf.so missing: run `python -m neuraludf_b200.build`"
     L = _lib.lib()
@@ -24,7 +24,7 @@ def test_library_exports_every_declared_symbol():
     for name in declared:
         assert hasattr(L, name), "libnudf.so does not export %s" % name
     assert sorted(_lib.exported_symbols()) == declared, "python binding and include/nudf.h disagree"
-    assert L.nudf_abi_version() == 4
+    assert L.nudf_abi_version() == 5
 
 
 def test_descriptor_validation_runs_without_gpu():
@@ -45,6 +45,27 @@ def test_descriptor_validation_runs_without_gpu():
     # fp32 folded weights (>= 524 544 floats) followed by the bf16 hi/lo tensor-engine images of every layer
     assert 524544 <= n < 8 * 1024 * 1024
     assert L.nudf_udf_ctx_floats(ctypes.byref(d), 1024, 1) > L.nudf_udf_ctx_floats(ctypes.byref(d), 1024, 0) > 0
+
+
+def test_lattice_descriptor_validation_runs_without_gpu():
+    from neuraludf_b200 import _lib
+    import ctypes
+    L = _lib.lib()
+    store = _lib.BrickStore(4, 1, 4, 1, 0, 1, 1, None, None)
+    for lat, what in ((_lib.Lattice(4, 4, 4, 1, ctypes.pointer(store)), b"exactly one of df and store"),
+                      (_lib.Lattice(4, 4, 4, None, None), b"exactly one of df and store"),
+                      (_lib.Lattice(4, 4, 1, 1, None), b"at least 2"),
+                      (_lib.Lattice(4, 4, 5, None, ctypes.pointer(store)), b"the store's n")):
+        assert L.nudf_mc_links(ctypes.byref(lat), None, 0, None, None, None) == -1
+        assert what in L.nudf_last_error()
+    tables = _lib.BandCoords(0.0, (ctypes.c_void_p * 3)(1, 1, 1))
+    lat = _lib.Lattice(4, 4, 4, None, ctypes.pointer(store))
+    assert L.nudf_nb_block_test(ctypes.byref(lat), 1, None, 0, ctypes.byref(tables), 2.0, 0.1, None, 1, None) == -1
+    assert b"dense lattice" in L.nudf_last_error()
+    lat = _lib.Lattice(4, 4, 5, 1, None)
+    assert L.nudf_nb_block_test(ctypes.byref(lat), 1, None, 0, ctypes.byref(_lib.BandCoords(0.5)), 2.0, 0.1, None, 1,
+                                None) == -1
+    assert b"cubic" in L.nudf_last_error()
 
 
 @pytest.mark.skipif(torch.cuda.is_available(), reason="checks the no-GPU behaviour")

@@ -59,7 +59,7 @@ def boxes(tmp_path_factory):
 
 @pytest.mark.parametrize("N,strides,name", [(50, [6, 3, 1], "cylinder"), (65, [8, 4, 2, 1], "sphere"),
                                             (33, [16, 4, 1], "patch"), (97, [8, 2, 1], "plane")])
-def test_box_kernels_match_restatement(N, strides, name):
+def test_table_kernels_match_restatement(N, strides, name):
     dev = _dev()
     from neuraludf_b200 import grid
     axes = grid.axis_tables(*_box(*BOX), N, dev)
@@ -75,14 +75,14 @@ def test_box_kernels_match_restatement(N, strides, name):
     assert tau == tau_np
     ud = torch.from_numpy(u).to(dev)
     df = torch.full((N ** 3,), float("inf"), device=dev)
-    idx, pts = grid.band_sublattice_box(axes, strides[0])
+    idx, pts = grid.band_sublattice(N, strides[0], dev, axes)
     assert np.array_equal(idx.cpu().numpy(), levels[0])
     assert np.array_equal(pts.cpu().numpy(), I.points(ax, levels[0]))      # bit for bit
     df[idx] = ud[idx]
     parent = None
     for k, s in enumerate(strides[:-1]):
         ps = strides[k - 1] if k else 0
-        flags, slope = grid.band_block_test_box(df, axes, s, parent, ps, h, pad, 2.0, tau)
+        flags, slope = grid.band_block_test(df, N, s, parent, ps, 2.0, tau, axes=axes, spacing=h, pad=pad)
         assert np.array_equal(flags.cpu().numpy(), flags_np[k])
         _, slope_np = I.block_test(df.cpu().numpy(), ax, s, None if parent is None else parent.cpu().numpy(), ps, h, pad,
                                    2.0, tau)
