@@ -19,6 +19,7 @@ namespace cl {
 
 constexpr int kRejectThreads = 1024;
 constexpr int kMaxRays = 16384;             // keys of the rejection CTA live in shared memory (64 KB)
+constexpr size_t kRejectStaticSmem = kRejectThreads / 32 * sizeof(double);   // reject_kernel's block_sum buffer
 constexpr double C1 = 0.01 * 0.01, C2 = 0.03 * 0.03;
 
 __device__ __forceinline__ double warp_sum(double v) {
@@ -159,7 +160,7 @@ __device__ __forceinline__ double block_sum(double v, double* red) {
 __global__ void __launch_bounds__(kRejectThreads) reject_kernel(nudf_color_loss_args a, float* __restrict__ losses,
                                                                  uint8_t* __restrict__ kept, float* __restrict__ ws) {
   extern __shared__ uint32_t keys[];
-  __shared__ double red[kRejectThreads / 32];
+  __shared__ double red[kRejectStaticSmem / sizeof(double)];
   const int N = a.n_rays, tid = threadIdx.x;
   const float* err = ws;
   const bool patch = a.patch_colors != nullptr;
@@ -355,8 +356,9 @@ int nudf_color_loss_forward(const nudf_color_loss_args* args, float* losses, uin
   NUDF_REQUIRE(losses && ws && (kept || !args->patch_colors), "null pointer");
   NUDF_REQUIRE(ws_aligned(ws), "ws must be 8-byte aligned");
   const size_t smem = args->patch_colors ? (size_t)args->n_rays * 4 : 0;
-  // the opt-in above 48 KB is a per-device attribute of the kernel: set it on the current device whenever it is needed
-  if (smem > 48 * 1024)
+  // without the opt-in a block gets 48 KB of static and dynamic shared memory together (N = 12225 .. 12288 already needs
+  // it); the opt-in is a per-device attribute of the kernel: set it on the current device whenever it is needed
+  if (smem + kRejectStaticSmem > 48 * 1024)
     NUDF_CUDA_OK(cudaFuncSetAttribute(reject_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   LaunchTimer lt_(FAM_RAY, (cudaStream_t)stream);
   ray_kernel<<<warp_blocks(args->n_rays), 256, 0, (cudaStream_t)stream>>>(*args, ws);

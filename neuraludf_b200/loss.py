@@ -19,8 +19,10 @@ computes (loss.py:29-45, 59-84, 105-133; patch_metric.py:21-66):
     color_patch_loss * color_patch_weight.  A term whose input is None stays the Python float 0.0.
 
 Deviations: equal keys of the rejection order are taken in ray order (the reference's `torch.sort` is unstable and may
-exclude any of them; the loss and its gradients do not depend on which, when the tied errors are equal); NaN ranks largest
-as there; the per-ray moments and formulas are evaluated in fp64 and rounded to fp32 once per ray; no gradient flows to `gt_color` /
+exclude any of them -- unmasked rays too when the tie is at 0, so there even how many masked rays it excludes is undecided;
+the loss and its gradients do not depend on which, when the tied errors are equal); NaN ranks largest as there; the
+per-ray moments and formulas are evaluated in fp64 and rounded to fp32 once per ray; a bool `pixel_mask`'s count + 1e-4
+is formed in fp64 (the reference forms it in fp32: a relative difference below 2^-24); no gradient flows to `gt_color` /
 `gt_patch_colors`.  Inputs must be fp32 CUDA tensors (masks: any float / bool tensor for `pixel_mask`, bool for
 `patch_mask`); anything else raises -- there is no fallback.
 

@@ -107,8 +107,9 @@ def make_inputs(name, seed, spec=None):
     return x
 
 
-def run(mod, spec, x, dtype):
-    """the reference's five scalars, kept mask and gradients for inputs x (spec: a CASES tuple)"""
+def run(mod, spec, x, dtype, bars=None):
+    """the reference's five scalars, kept mask and gradients for inputs x (spec: a CASES tuple; absent inputs are passed
+    as None).  The gradients are of `loss`, or of sum_i bars[i] * losses[i] over the five scalars when bars is given."""
     N, h, ptype, w, *_ = spec
     loss_fn = mod.ColorLoss(*w, pixel_loss_type="l1", patch_loss_type=ptype, h_patch_size=h)
     if dtype == torch.float64:
@@ -124,12 +125,15 @@ def run(mod, spec, x, dtype):
     rec = _Recorder()
     mod.torch = rec
     try:
-        out = loss_fn(t["color_base"], t["color"], t["gt_color"], t.get("color_pixel"), t.get("pixel_mask"),
+        out = loss_fn(t.get("color_base"), t.get("color"), t.get("gt_color"), t.get("color_pixel"), t.get("pixel_mask"),
                       t.get("patch_colors"), t.get("gt_patch_colors"), t.get("patch_mask"))
     finally:
         mod.torch = torch
-    out["loss"].backward()
     keys = ["loss", "color_base_loss", "color_loss", "color_pixel_loss", "color_patch_loss"]
+    if bars is None:
+        out["loss"].backward()
+    else:
+        sum(b * out[k] for b, k in zip(bars, keys) if torch.is_tensor(out[k])).backward()
     losses = np.array([float(out[k]) for k in keys], np.float64)
     kept = None
     if "patch_colors" in t:

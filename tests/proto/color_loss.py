@@ -2,7 +2,10 @@
 reference's ColorLoss (loss/loss.py, loss/patch_metric.py) and its hand-derived backward.  The kernels follow it step by
 step: per-ray Gaussian-window moments, the per-ray error, the rejection order (error * mask descending, NaN largest, equal
 keys in ray order), and per-pixel gradients of the form w_p (k0 + 2 x_p k1 + y_p k2) (SSIM) or
-w_p (k1 (x_p - mu1) + k0 ((y_p - mu2) - U)) (NCC)."""
+w_p (k1 (x_p - mu1) + k0 ((y_p - mu2) - U)) (NCC).
+
+`forward` and `backward` also run in fp32 (`dtype=np.float32`): the same formulas with fp32 arrays, the rounding noise an
+fp32 evaluation of the loss has, which the device tests take as their yardstick."""
 import numpy as np
 
 PATCH_TYPES = ["l1", "ssd", "ssim", "ncc"]
@@ -51,61 +54,76 @@ def order_rank(key):
 
 def kept_mask(err, mask):
     """rays left after excluding the first int(0.3f * count) of the descending order of err * mask (loss.py:78-82)"""
-    key = err * mask.astype(np.float64)
+    key = err * mask.astype(err.dtype)
     k = int(np.float32(0.3) * np.float32(mask.sum()))
     return mask & (order_rank(key) >= k)
 
 
-def denominators(fx):
-    """L1-sum denominators of the three pixel terms: mask.sum() + 1e-4 (a bool mask's count + 1e-4 is fp32), or N * 3"""
-    n = fx["gt_color"].shape[0]
+def n_rays(fx):
+    return next(fx[k].shape[0] for k in ("gt_color", "patch_colors") if k in fx)
+
+
+def _count_den(mask, dt):
+    """mask.sum() + 1e-4: a bool mask's sum is an integer tensor, so torch forms count + 1e-4 in fp32 whatever the
+    precision of the predictions; a float mask's in its own precision"""
+    if mask.dtype == bool:
+        return float(np.float32(np.float32(mask.sum()) + np.float32(1e-4)))
+    return float(mask.astype(dt).sum() + dt.type(1e-4))
+
+
+def denominators(fx, dtype=np.float64):
+    """L1-sum denominators of the three pixel terms: mask.sum() + 1e-4, or N * 3"""
+    n, dt = n_rays(fx), np.dtype(dtype)
     pm, qm = fx.get("pixel_mask"), fx.get("patch_mask")
-    d = float(pm.astype(np.float64).sum() + 1e-4) if pm is not None else 3.0 * n
-    dq = float(np.float32(np.float32(qm.sum()) + np.float32(1e-4))) if qm is not None else 3.0 * n
+    d = _count_den(pm, dt) if pm is not None else 3.0 * n
+    dq = _count_den(qm, dt) if qm is not None else 3.0 * n
     return [d, d, dq]
 
 
-def forward(fx):
+def forward(fx, dtype=np.float64):
     """fx: dict of the golden's inputs (absent terms missing).  Returns losses [5], kept [N] or None, err [N] or None."""
-    w = fx["weights"]
+    dt = np.dtype(dtype)
+    w = np.asarray(fx["weights"], np.float64).astype(dt)
     ptype = PATCH_TYPES[int(fx["patch_type"])]
-    den = denominators(fx)
-    gt = fx["gt_color"].astype(np.float64)
-    terms = [np.abs(fx[t].astype(np.float64) - gt).sum() / den[i] if t in fx else 0.0 for i, t in enumerate(TERMS)]
+    den = denominators(fx, dt)
+    gt = fx["gt_color"].astype(dt) if "gt_color" in fx else None
+    terms = [np.abs(fx[t].astype(dt) - gt).sum() / den[i] if t in fx else 0.0 for i, t in enumerate(TERMS)]
     kept = err = None
     patch = 0.0
     if "patch_colors" in fx:
-        err = patch_errors(ptype, fx["patch_colors"].astype(np.float64), fx["gt_patch_colors"].astype(np.float64),
-                           window(int(fx["h"])))
+        err = patch_errors(ptype, fx["patch_colors"].astype(dt), fx["gt_patch_colors"].astype(dt),
+                           window(int(fx["h"])).astype(dt))
         kept = kept_mask(err, fx["patch_mask"].reshape(-1))
         patch = err[kept].mean() if kept.any() else np.nan
     total = (terms[0] * w[0] + terms[1] * w[1] + terms[2] * w[2]) / (w[0] + w[1] + w[2]) + patch * w[3]
     return np.array([total] + terms + [patch], np.float64), kept, err
 
 
-def backward(fx, bars=(1.0, 0.0, 0.0, 0.0, 0.0)):
+def backward(fx, bars=(1.0, 0.0, 0.0, 0.0, 0.0), dtype=np.float64):
     """gradients of sum_i bars[i] * losses[i] w.r.t. each present prediction, {'d_<name>': array}"""
-    w = fx["weights"]
+    dt = np.dtype(dtype)
+    w = np.asarray(fx["weights"], np.float64).astype(dt)
+    bars = np.asarray(bars, np.float64).astype(dt)
     ws = w[0] + w[1] + w[2]
-    den = denominators(fx)
-    gt = fx["gt_color"].astype(np.float64)
+    den = denominators(fx, dt)
+    gt = fx["gt_color"].astype(dt) if "gt_color" in fx else None
     out = {}
     for i, t in enumerate(TERMS):
         if t in fx:
-            out["d_" + t] = np.sign(fx[t].astype(np.float64) - gt) * ((bars[1 + i] + bars[0] * w[i] / ws) / den[i])
+            out["d_" + t] = np.sign(fx[t].astype(dt) - gt) * ((bars[1 + i] + bars[0] * w[i] / ws) / den[i])
     if "patch_colors" not in fx:
         return out
     ptype = PATCH_TYPES[int(fx["patch_type"])]
-    x, y = fx["patch_colors"].astype(np.float64), fx["gt_patch_colors"].astype(np.float64)
-    _, kept, _ = forward(fx)
-    g = np.where(kept, (bars[4] + bars[0] * w[3]) / max(int(kept.sum()), 1), 0.0)[:, None, None]   # d loss / d error
+    x, y = fx["patch_colors"].astype(dt), fx["gt_patch_colors"].astype(dt)
+    _, kept, _ = forward(fx, dt)
+    g = np.where(kept, (bars[4] + bars[0] * w[3]) / max(int(kept.sum()), 1), 0.0).astype(dt)[:, None, None]   # d / d error
     if ptype == "l1":
         out["d_patch_colors"] = g * np.sign(x - y) / 3
         return out
     if ptype == "ssd":
         out["d_patch_colors"] = g * 2 * (x - y) / 3
         return out
-    wp = window(int(fx["h"]))[None, :, None]
+    wp = window(int(fx["h"])).astype(dt)[None, :, None]
     mu1, mu2, xx, yy, xy = _moments(x, y, wp[0, :, 0])
     g = g[:, :, 0]
     if ptype == "ssim":

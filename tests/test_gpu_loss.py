@@ -1,6 +1,7 @@
 """The device colour loss (neuraludf_b200/loss.py, csrc/color_loss.cu) against the reference's ColorLoss: the goldens of
 oracle/make_golden_loss.py, the unmodified loss/loss.py on fresh inputs at the runner's shapes, determinism, no host
-synchronisation, CUDA-graph replay, and the unmodified runner's fine-tuning steps under NUDF_DEVICE_LOSS=1."""
+synchronisation, CUDA-graph replay, and the unmodified runner's fine-tuning steps under NUDF_DEVICE_LOSS=1.
+Away from those shapes (patch sizes, ray counts, rejection edges, term subsets, degenerate patches): test_gpu_loss_shapes.py."""
 import os
 import re
 import subprocess
