@@ -7,6 +7,8 @@
 // the operand allows it); weight slices arrive by cp.async.bulk on an mbarrier.  The accumulators go
 // through shared memory to the fused epilogue functor (4 consecutive columns of a row per call: coalesced).  WN = 256 for
 // 2-plane layers wider than 128 columns, so that each activation row block is read from HBM and split into planes once.
+// 3-plane layers on such operands run gemm_w3_tma_kernel instead: persistent, a producer warpgroup feeding two consumer
+// warpgroups through mbarriers, the epilogue applied from the accumulator fragments.
 #pragma once
 #include <cuda.h>
 #include <cudaTypedefs.h>
@@ -60,19 +62,19 @@ __device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
   __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
   return *reinterpret_cast<uint32_t*>(&v);
 }
-// split 4 consecutive values into NP bf16 planes (packed pairs)
+// split 4 consecutive values into NP bf16 planes (packed pairs): plane p holds bf16_rn of what the planes before it
+// left, r -= plane.  One paired conversion per two values and plane; the plane's values are read back from its bits.
 template <int NP>
 __device__ __forceinline__ void split4(const float x[4], uint2 planes[NP]) {
   float r[4] = {x[0], x[1], x[2], x[3]};
 #pragma unroll
   for (int p = 0; p < NP; ++p) {
-    float h[4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      h[j] = __bfloat162float(__float2bfloat16_rn(r[j]));
-      r[j] -= h[j];
-    }
-    planes[p] = make_uint2(pack_bf16(h[0], h[1]), pack_bf16(h[2], h[3]));
+    const uint32_t a = pack_bf16(r[0], r[1]), b = pack_bf16(r[2], r[3]);
+    planes[p] = make_uint2(a, b);
+    r[0] -= __uint_as_float(a << 16);
+    r[1] -= __uint_as_float(a & 0xffff0000u);
+    r[2] -= __uint_as_float(b << 16);
+    r[3] -= __uint_as_float(b & 0xffff0000u);
   }
 }
 // ---- weight image --------------------------------------------------------------------------------------------------
@@ -132,6 +134,9 @@ __device__ __forceinline__ uint8_t* align1024(uint8_t* p) {
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
 }
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
@@ -182,6 +187,10 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
 __device__ __forceinline__ uint64_t make_desc_mn(uint32_t smem_addr) {
   return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)(4096 >> 4) << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
 }
+// the threads of one warpgroup (named barrier 1; 0 is __syncthreads)
+__device__ __forceinline__ void wg_bar_sync() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
+template <uint32_t R> __device__ __forceinline__ void reg_dealloc() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <uint32_t R> __device__ __forceinline__ void reg_alloc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
@@ -485,8 +494,9 @@ __device__ __forceinline__ void store_block_t(const float4 (&v)[8][2], int r0, i
 // in place: each reads its 8 float4 (store_a's mapping: a warp reads 512 contiguous bytes), a CTA barrier, then the
 // hi / lo K-major SW128 planes go over the same 32 KB.  A slot is refilled as soon as the barrier after the wgmma group
 // that read it has passed.  The planes and the products are the register path's, so both give the same bits.
-// Otherwise all threads stage each slice through registers (stage_a_direct): the loads of slice ks + 1 are issued after
-// the wgmma group of slice ks, then split into the free stage.
+// Otherwise all threads stage each slice through registers (stage_a_direct; 3-plane layers come here only with operands
+// gemm_w3_tma_kernel cannot take): the loads of slice ks + 1 are issued after the wgmma group of slice ks, then split
+// into the free stage.
 // ---------------------------------------------------------------------------------------------------------------
 template <int NP, int WN, class Epi, bool RING>
 __global__ void __launch_bounds__(THREADS, 1)
@@ -646,6 +656,201 @@ gemm_w_kernel(const float* __restrict__ A, int64_t lda, int64_t M, int N, int K,
   else acc_to_smem<WN>(acc, acc_s, wg, tid & 127);
   __syncthreads();
   tile_epilogue<WN>(acc_s, m0, M, n0, N, epi, tid);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// 3-plane layers on an operand that allows a 2-D tensor map (a row stride that is a multiple of 4 floats and a
+// 16-byte-aligned base): C[M x N] = epi( A[M x K] * B^T ) with the register path's planes, products and sums, so both
+// paths give the same bits.  Persistent: min(tiles, SMs) CTAs take the [128 x 128] tiles t = blockIdx.x + i * gridDim.x
+// (column tile fastest, so the two column tiles of a row block run at the same time and the second read of its
+// activations hits L2).  Three warpgroups and no CTA barrier after the set-up:
+// * Producer (warpgroup 0, 40 registers).  One thread issues the 2-D TMA copies of each 64-wide K slice as four
+//   [32 rows x 64 k] fp32 boxes into four landing quarters, each on its own mbarrier (rows past M and columns past K
+//   arrive as zeros; a quarter that starts past M is not copied and splits as zeros), and the weight slice's three
+//   plane copies into the stage.  The warpgroup splits each landed quarter with split4<3> in store_a's mapping into the
+//   stage's K-major SWIZZLE_128B planes; once every thread has split its part of a quarter (an async proxy fence and a
+//   warpgroup barrier), the quarter is refilled with the next slice's rows, which may belong to the CTA's next tile.
+//   After the fourth quarter: an arrival on the stage's "full" barrier (128 arrivals plus the weight bytes).
+// * Two consumers (warpgroups 1 and 2, 232 registers), each owning 64 rows of the tile.  Per slice: wait "full", issue
+//   mma_slice<3> (the five correction products into an accumulator zeroed at the slice) and the four hi * hi steps
+//   into fresh registers, add corrections, hh0 .. hh3 into tot in that order, and arrive on the stage's "empty"
+//   barrier (256 arrivals) once the last group has completed.  The consumers drift apart: one's adds overlap the other's
+//   products.  After the tile's last slice each consumer applies the epilogue functor to its own 64 rows straight
+//   from the fragment: lane pairs swap one float2 so that each thread holds 4 consecutive columns of one row.
+// Weight rows past the image tile (N = 217 -> 224 rows) and stage contents left by an earlier slice or tile reach only
+// accumulator columns >= N, which are never passed to the epilogue.
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int W3_THREADS = 384;
+constexpr int W3_QROWS = 32;                                   // rows of one landing quarter
+constexpr uint32_t W3_QUARTER = W3_QROWS * BK * 4;             // 8 KB
+constexpr int W3_NQ = BM / W3_QROWS;
+constexpr uint32_t W3_A_STAGE = 3 * A_HALF_BYTES;              // 48 KB: hi, mid, lo planes of a [128 x 64] slice
+constexpr uint32_t W3_STAGE = W3_A_STAGE + 3 * b_plane_bytes(BN);   // + the weight slice's three planes: 96 KB
+constexpr uint32_t W3_LAND = W3_NQ * W3_QUARTER;               // 32 KB: one fp32 slice
+constexpr int W3_PRODUCER_REGS = 40, W3_CONSUMER_REGS = 232;
+static_assert(W3_LAND == W_SLOT, "the landing quarters hold one fp32 slice");
+static_assert(W3_PRODUCER_REGS + 2 * W3_CONSUMER_REGS <= 65536 / 128, "register file of one SM");
+static_assert(BM * 16 / 128 / W3_NQ == 4, "four float4 per producer thread and quarter");
+
+template <class Epi>
+__global__ void __launch_bounds__(W3_THREADS, 1)
+gemm_w3_tma_kernel(const float* __restrict__ A, int64_t M, int N, int K, const uint16_t* __restrict__ img, Epi epi,
+                   const __grid_constant__ CUtensorMap amap) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = align1024(smem_raw);
+  uint8_t* land = smem + 2 * W3_STAGE;
+  uint64_t* full = reinterpret_cast<uint64_t*>(land + W3_LAND);
+  uint64_t* empty = full + 2;
+  uint64_t* landed = empty + 2;
+  const int tid = threadIdx.x, wg = tid >> 7;
+  const int n_ct = (N + BN - 1) / BN;
+  const int tiles = (int)((M + BM - 1) / BM) * n_ct;
+  const int n_slices = pad64(K) / 64;
+  constexpr uint32_t B_PLANE = b_plane_bytes(BN);
+  if (tid == 0) {
+    mbar_init(&full[0], 129);
+    mbar_init(&full[1], 129);
+    mbar_init(&empty[0], 256);
+    mbar_init(&empty[1], 256);
+    for (int q = 0; q < W3_NQ; ++q) mbar_init(&landed[q], 1);
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (wg == 0) {
+    reg_dealloc<W3_PRODUCER_REGS>();
+    auto issue_quarter = [&](int t, int ks, int q) {         // one thread: rows 32q.. of slice ks of tile t
+      const int64_t r0 = (int64_t)(t / n_ct) * BM + q * W3_QROWS;
+      if (r0 < M) {
+        mbar_arrive_expect_tx(&landed[q], W3_QUARTER);
+        tma_load_2d(land + q * W3_QUARTER, &amap, ks * BK, (int)r0, &landed[q]);
+      } else {
+        mbar_arrive(&landed[q]);
+      }
+    };
+    if (tid == 0 && (int)blockIdx.x < tiles)
+      for (int q = 0; q < W3_NQ; ++q) issue_quarter(blockIdx.x, 0, q);
+    const int c = tid & 15, rsub = tid >> 4;                  // store_a's mapping for 128 threads
+    uint32_t g = 0;                                           // slices of this CTA so far
+    for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
+      const int64_t m0 = (int64_t)(t / n_ct) * BM;
+      const int tn = t % n_ct;                                // image tile = column tile (3 planes: 128 rows)
+      const int rows_t = tile_rows(N, tn, 3);
+      const uint16_t* img_t = img + tile_offset(N, K, tn, 3);
+      for (int ks = 0; ks < n_slices; ++ks, ++g) {
+        int t1 = t, ks1 = ks + 1;                             // the slice after this one
+        if (ks1 == n_slices) { ks1 = 0; t1 += gridDim.x; }
+        const int s = g & 1;
+        uint8_t* st = smem + s * W3_STAGE;
+        mbar_wait(&empty[s], ((g >> 1) & 1) ^ 1);
+        if (tid == 0) {
+          const uint32_t wb = (uint32_t)rows_t * 128u;
+          mbar_arrive_expect_tx(&full[s], 3 * wb);
+          for (int p = 0; p < 3; ++p) bulk_g2s(st + W3_A_STAGE + p * B_PLANE, img_t + ((int64_t)ks * 3 + p) * rows_t * 64, wb, &full[s]);
+        }
+#pragma unroll 1
+        for (int q = 0; q < W3_NQ; ++q) {
+          float4 v[4];
+          if (m0 + q * W3_QROWS < M) {
+            mbar_wait(&landed[q], g & 1);
+            const float4* f = reinterpret_cast<const float4*>(land + q * W3_QUARTER) + rsub * (BK / 4) + c;
+#pragma unroll
+            for (int pass = 0; pass < 4; ++pass) v[pass] = f[pass * 8 * (BK / 4)];
+          } else {
+#pragma unroll
+            for (int pass = 0; pass < 4; ++pass) v[pass] = make_float4(0.f, 0.f, 0.f, 0.f);
+          }
+#pragma unroll
+          for (int pass = 0; pass < 4; ++pass) {
+            const float x[4] = {v[pass].x, v[pass].y, v[pass].z, v[pass].w};
+            uint2 pl[3];
+            split4<3>(x, pl);
+            const uint32_t off = sw128((uint32_t)(q * W3_QROWS + pass * 8 + rsub), (uint32_t)(c * 4));
+#pragma unroll
+            for (int p = 0; p < 3; ++p) *reinterpret_cast<uint2*>(st + p * A_HALF_BYTES + off) = pl[p];
+          }
+          // The refill is an async-proxy write over the quarter: every thread's reads of it must have returned (their
+          // values are split and stored by now) and be ordered before it.  A barrier alone does not wait for loads in
+          // flight, and refilling right after it let the TMA overwrite rows that were still being read.
+          fence_proxy_async();
+          wg_bar_sync();
+          if (tid == 0 && t1 < tiles) issue_quarter(t1, ks1, q);
+        }
+        fence_proxy_async();
+        mbar_arrive(&full[s]);
+      }
+    }
+  } else {
+    reg_alloc<W3_CONSUMER_REGS>();
+    const int cw = wg - 1, wtid = tid & 127, lane = tid & 31;
+    float acc[64], acc2[64], tot[64];
+    auto hi_hi = [&](float (&d)[64], uint32_t a, uint32_t b, int j) {
+      wg_fence();
+      wgmma_128_fresh(d, make_desc(a + 32u * j), make_desc(b + 32u * j));
+      wg_commit();
+    };
+    auto add_unbiased = [&](float (&d)[64]) {                 // after the wait that completes d
+      fence_operand(d);
+#pragma unroll
+      for (int q = 0; q < 64; ++q) tot[q] += unbias_rz(d[q]);
+    };
+    uint32_t g = 0;
+    for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
+      const int64_t m0 = (int64_t)(t / n_ct) * BM;
+      const int n0 = (t % n_ct) * BN;
+#pragma unroll
+      for (int q = 0; q < 64; ++q) tot[q] = 0.f;
+      for (int ks = 0; ks < n_slices; ++ks, ++g) {
+        const int s = g & 1;
+        mbar_wait(&full[s], (g >> 1) & 1);
+        const uint32_t a = smem_u32(smem + s * W3_STAGE) + cw * (64 * 128), b = smem_u32(smem + s * W3_STAGE + W3_A_STAGE);
+        wg_fence();
+        mma_slice<3, BN>(acc, a, A_HALF_BYTES, b, B_PLANE, true);
+        wg_commit();
+        hi_hi(acc2, a, b, 0);
+        wg_wait_but_one();
+        fence_operand(acc);
+#pragma unroll
+        for (int q = 0; q < 64; ++q) tot[q] += acc[q];          // corrections
+        hi_hi(acc, a, b, 1);
+        wg_wait_but_one();
+        add_unbiased(acc2);                                     // hh0
+        hi_hi(acc2, a, b, 2);
+        wg_wait_but_one();
+        add_unbiased(acc);                                      // hh1
+        hi_hi(acc, a, b, 3);
+        wg_wait_but_one();
+        add_unbiased(acc2);                                     // hh2
+        wg_wait_all();
+        mbar_arrive(&empty[s]);                                 // every group that read stage s has completed
+        add_unbiased(acc);                                      // hh3
+      }
+      // fragment rows r, r + 8, columns 8j + 2(lane & 3) + {0, 1}: the even lane of a pair takes row r, the odd one row
+      // r + 8, of the pair's 4 columns 8j + 4((lane & 3) >> 1) + {0 .. 3}
+      const bool odd = lane & 1;
+      const int64_t row = m0 + 64 * cw + 16 * (wtid >> 5) + (lane >> 2) + (odd ? 8 : 0);
+      const int cbase = n0 + 4 * ((lane & 3) >> 1);
+      // column groups whose epilogue loads are in flight together: as many as the registers of the free accumulators hold
+      constexpr int EPI_G = sizeof(typename Epi::Aux) <= 4 * sizeof(float) ? 8 : 4;
+#pragma unroll
+      for (int j0 = 0; j0 < 16; j0 += EPI_G) {
+        typename Epi::Aux aux[EPI_G];
+#pragma unroll
+        for (int i = 0; i < EPI_G; ++i) {
+          const int col = cbase + 8 * (j0 + i);
+          if (row < M && col < N) epi.load(row, col, N - col < 4 ? N - col : 4, aux[i]);
+        }
+#pragma unroll
+        for (int i = 0; i < EPI_G; ++i) {
+          const int j = j0 + i, col = cbase + 8 * j;
+          const float s0 = odd ? tot[4 * j] : tot[4 * j + 2], s1 = odd ? tot[4 * j + 1] : tot[4 * j + 3];
+          const float r0 = __shfl_xor_sync(0xffffffffu, s0, 1), r1 = __shfl_xor_sync(0xffffffffu, s1, 1);
+          const float x[4] = {odd ? r0 : tot[4 * j], odd ? r1 : tot[4 * j + 1], odd ? tot[4 * j + 2] : r0, odd ? tot[4 * j + 3] : r1};
+          if (row < M && col < N) epi.apply(row, col, x, N - col < 4 ? N - col : 4, aux[i]);
+        }
+      }
+    }
+  }
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -894,13 +1099,36 @@ static inline int gemm_w_launch(const float* A, int64_t lda, int64_t M, int N, i
   NUDF_LAUNCH_OK();
   return 0;
 }
-// The activation path follows from the operand: 2-plane layers take the ring when the row stride is a multiple of 4
-// floats and the base is 16-byte aligned (a 2-D tensor map needs both; every operand the networks pass has them), the
-// register path otherwise.  3-plane layers always take the register path.
+// gemm_w3_tma_kernel: 2 stages of the A and weight planes, the 4 landing quarters and 8 mbarriers; the epilogue runs
+// from registers, so no accumulator tile has to fit beside them
+constexpr size_t W3_SMEM = 2 * (size_t)W3_STAGE + W3_LAND + 8 * sizeof(uint64_t) + 1024;
+static_assert(W3_SMEM <= 227 * 1024, "one CTA per SM");
+
+template <class Epi>
+static inline int gemm_w3_tma_launch(const float* A, int64_t lda, int64_t M, int N, int K, const uint16_t* img, const Epi& epi, cudaStream_t st) {
+  static bool attr_set = false;   // per template instantiation
+  if (!attr_set) {
+    NUDF_CUDA_OK(cudaFuncSetAttribute(gemm_w3_tma_kernel<Epi>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)W3_SMEM));
+    attr_set = true;
+  }
+  CUtensorMap amap{};
+  if (int rc = tensor_map_2d(&amap, A, lda, K, M, BK, W3_QROWS)) return rc;
+  const int64_t tiles = cdiv(M, BM) * cdiv(N, BN);
+  const unsigned grid = (unsigned)(tiles < sm_count() ? tiles : sm_count());
+  LaunchTimer lt_(epi_family<Epi>::value, st);
+  gemm_w3_tma_kernel<Epi><<<grid, W3_THREADS, W3_SMEM, st>>>(A, M, N, K, img, epi, amap);
+  NUDF_LAUNCH_OK();
+  return 0;
+}
+// The activation path follows from the operand: when the row stride is a multiple of 4 floats and the base is 16-byte
+// aligned (a 2-D tensor map needs both; every operand the networks pass has them), 2-plane layers take the ring and
+// 3-plane layers gemm_w3_tma_kernel; any other operand takes the register path.
 template <int NP, int WN, class Epi>
 static inline int gemm_w_path(const float* A, int64_t lda, int64_t M, int N, int K, const uint16_t* img, const Epi& epi, cudaStream_t st) {
-  if constexpr (NP == 2)
-    if (K > 0 && (lda & 3) == 0 && aligned16(A)) return gemm_w_launch<2, WN, Epi, true>(A, lda, M, N, K, img, epi, st);
+  if (K > 0 && (lda & 3) == 0 && aligned16(A)) {
+    if constexpr (NP == 2) return gemm_w_launch<2, WN, Epi, true>(A, lda, M, N, K, img, epi, st);
+    else return gemm_w3_tma_launch<Epi>(A, lda, M, N, K, img, epi, st);
+  }
   return gemm_w_launch<NP, WN, Epi, false>(A, lda, M, N, K, img, epi, st);
 }
 // The output width per CTA follows from the shape: 256 columns for 2-plane layers wider than 128 (one read and split of
