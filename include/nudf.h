@@ -546,6 +546,23 @@ int nudf_mp_smooth_step(const double* verts_in, double* verts_out, const int64_t
                         const int64_t* rowptr, const int64_t* cols, double lambda, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * Gradient branch of get_mesh_udf_fast (neuraludf_b200/extract_mesh.py drives the steps; the CSR sort in torch)
+ * ------------------------------------------------------------------------------------------------------------
+ * Every fp64 / fp32 operation is correctly rounded on its own, no contraction (acos aside). */
+/* normals[V,3] fp32 <- the angle-weighted vertex normals of the fp64 mesh (verts [V,3], faces [F,3]): per face the unit
+ * normal of (v1 - v0) x (v2 - v0) times the angle at each corner (face_terms: workspace of 9 F doubles), summed per vertex
+ * over incidences [3F] = corner * F + face in the CSR order of rowptr [V+1] (the caller sorts them by (vertex, corner,
+ * face)), divided by max(|sum|, 1e-300) and rounded to fp32.  A vertex without faces gets 0.  Two launches. */
+int nudf_mg_vertex_normals(const double* verts, int64_t n_verts, const int64_t* faces, int64_t n_faces, const int64_t* rowptr,
+                           const int64_t* incidences, double* face_terms, float* normals, void* stream);
+/* fp32 verts / normals [V,3].  s1 == s2 == NULL: probes [2V,3] <- verts + eps n, then verts - eps n.  Otherwise (s1, s2 [V]:
+ * the udf at those probes): new_verts [V,3] <- (v - (eps s1) n) + (eps s2) n, and next_indices [7V] <- the flat index of
+ * trunc((x + 1) / fl32(2 / (n_mc - 1))) per axis and its six neighbours clamped to [0, n_mc - 1] along one axis (+x, +y,
+ * +z, -x, -y, -z), block-major; a NaN or out-of-range quotient gives INT64_MIN, the index arithmetic wraps.  One launch. */
+int nudf_mg_refine(const float* verts, const float* normals, int64_t n_verts, float eps, const float* s1, const float* s2,
+                   int32_t n_mc, float* probes, float* new_verts, int64_t* next_indices, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------
  * Connected components of a mesh's faces (neuraludf_b200/clean.py face_components; sizes and selection in torch)
  * ------------------------------------------------------------------------------------------------------------ */
 /* keys [n_keys] ascending: edge keys lo * V + hi (nudf_mp_faces' edge codes >> 1); key_face[e] in [0, n_faces): the face

@@ -237,6 +237,9 @@ _SIGNATURES = {
     "nudf_mp_hole_emit": (ctypes.c_int, [c_void_p] * 3 + [ctypes.c_int64, c_void_p, c_void_p, ctypes.c_int64]
                           + [c_void_p] * 3),
     "nudf_mp_smooth_step": (ctypes.c_int, [c_void_p] * 3 + [ctypes.c_int64, c_void_p, c_void_p, ctypes.c_double, c_void_p]),
+    "nudf_mg_vertex_normals": (ctypes.c_int, [c_void_p, ctypes.c_int64, c_void_p, ctypes.c_int64] + [c_void_p] * 5),
+    "nudf_mg_refine": (ctypes.c_int, [c_void_p, c_void_p, ctypes.c_int64, ctypes.c_float, c_void_p, c_void_p, ctypes.c_int32]
+                       + [c_void_p] * 4),
     "nudf_cc_label": (ctypes.c_int, [c_void_p, c_void_p, ctypes.c_int64, ctypes.c_int64] + [c_void_p] * 3),
     "nudf_color_loss_forward": (ctypes.c_int, [c_void_p] * 5),
     "nudf_color_loss_backward": (ctypes.c_int, [c_void_p] * 9),

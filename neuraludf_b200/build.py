@@ -8,7 +8,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libnudf.so")
 SOURCES = ["capi.cu", "udf_net.cu", "mlp_nets.cu", "ray_kernels.cu", "sampling.cu", "gemm_tc.cu", "blend.cu", "raygen.cu",
            "mesh_udf.cu", "eval_pc.cu", "mesh_clean.cu", "mesh_band.cu", "mesh_sparse.cu",
-           "mesh_post.cu", "mesh_cc.cu", "color_loss.cu"]
+           "mesh_post.cu", "mesh_cc.cu", "color_loss.cu", "mesh_grad.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 

@@ -43,7 +43,7 @@ def _index_points(idx, N):
 def udf_grid(udf_network, N, max_batch=1 << 21, lo=0, hi=None):
     """udf at the lattice points [lo, hi) (default: all N^3) as a flat device tensor -- one fused-chain launch per batch,
     no host round trips.  Slab partitioning for multi-GPU sweeps: give each rank its own [lo, hi)."""
-    device = next(udf_network.parameters()).device
+    device = _device(udf_network)
     hi = N ** 3 if hi is None else hi
     out = torch.empty(hi - lo, device=device)
     for head in range(lo, hi, max_batch):
@@ -56,7 +56,6 @@ def udf_grid(udf_network, N, max_batch=1 << 21, lo=0, hi=None):
 def near_surface_cells(udf_network, N, df_flat=None, max_batch=1 << 20, dist_voxels=2.0, lo=0):
     """(flat lattice indices [M] int64, unit vectors pointing towards the surface [M,3]) of the cells with
     udf < dist_voxels * voxel (extract_mesh.py:77-98): compaction and gradient evaluation stay on the device."""
-    device = next(udf_network.parameters()).device
     if df_flat is None:
         df_flat = udf_grid(udf_network, N)
     voxel = 2.0 / (N - 1)
@@ -64,14 +63,22 @@ def near_surface_cells(udf_network, N, df_flat=None, max_batch=1 << 20, dist_vox
     return idx, _surface_normals(udf_network, N, idx, max_batch)
 
 
+def _runner_normals(udf_network, pts):
+    """unit vectors towards the surface at pts from a UDF network's gradient, normalised as the runner's func_grad does"""
+    g = udf_network.gradient(pts)[:, 0]
+    g = g / (torch.linalg.norm(g, ord=2, dim=-1, keepdim=True) + 1e-5)              # exp_runner_blending.py:767-771 (func_grad)
+    return -F.normalize(g, dim=1)                                                    # extract_mesh.py:93
+
+
 def _surface_normals(udf_network, N, idx, max_batch):
-    """unit vectors towards the surface at the flat lattice indices idx (extract_mesh.py:77-98), batches of max_batch"""
+    """unit vectors towards the surface at the flat lattice indices idx (extract_mesh.py:77-98), batches of max_batch: the
+    field's own `surface_normals(points)` when it has one (extract_mesh.CallerField: a caller's func_grad), else the UDF
+    network's runner-normalised gradient"""
+    at = getattr(udf_network, "surface_normals", None) or (lambda pts: _runner_normals(udf_network, pts))
     normals = torch.empty(idx.numel(), 3, device=idx.device)
     for head in range(0, idx.numel(), max_batch):
         sel = idx[head:head + max_batch]
-        g = udf_network.gradient(_index_points(sel, N))[:, 0]
-        g = g / (torch.linalg.norm(g, ord=2, dim=-1, keepdim=True) + 1e-5)          # exp_runner_blending.py:767-771 (func_grad)
-        normals[head:head + sel.numel()] = -F.normalize(g, dim=1)                    # extract_mesh.py:93
+        normals[head:head + sel.numel()] = at(_index_points(sel, N))
     return normals
 
 

@@ -10,6 +10,9 @@ be imported by the running interpreter.  With NUDF_DEVICE_LOSS=1 in the environm
 are bound to neuraludf_b200.loss (the colour loss on the device); without it the runner's own loss files run.  With
 NUDF_BAND_MESH=1, `validate_mesh`'s `extract_geometry` (when PyMCubes cannot be imported) evaluates its lattice narrow-band
 (grid.iso_band: the same mesh when the UDF is 2-Lipschitz and batch-invariant); without it the whole lattice is queried.
+With NUDF_DEVICE_MESH=1, `extract_mesh` (the runner's get_mesh_udf_fast) is bound to neuraludf_b200.extract_mesh: the
+lattice, MC, post-processing and gradient branch of extract_udf_mesh on the device, with no N^3 host array (NUDF_BAND_MESH=1
+then evaluates its lattice narrow-band too); without it the runner's own extract_mesh.py runs.
 """
 import importlib
 import importlib.machinery
@@ -38,6 +41,9 @@ def install_shadow_modules(reference_root=None):
     _install_custom_mc(reference_root)
     if os.environ.get("NUDF_DEVICE_LOSS") == "1":
         _install_device_loss(reference_root)
+    if os.environ.get("NUDF_DEVICE_MESH") == "1":
+        from neuraludf_b200 import extract_mesh
+        sys.modules["extract_mesh"] = extract_mesh
     return pkg
 
 

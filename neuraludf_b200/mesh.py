@@ -245,31 +245,44 @@ def udf_mesh(udf_network, N, dist_threshold_ratio=1.0, lo=0, hi=None, max_batch=
     return _udf_mesh(udf_network, N, "dense", dist_threshold_ratio, max_batch=max_batch, lo=lo, hi=hi)
 
 
-def _mc_lattice(udf_network, N, df, lo, max_batch):
+def _no_mark(stage):
+    pass
+
+
+def _mc_lattice(udf_network, N, df, lo, max_batch, mark=_no_mark):
     """near-surface normals -> MC of the lattice values df (whole x-planes from flat index lo): (verts [V,3] fp32 in the
-    slab's lattice-index units, faces [F,3] int64)"""
+    slab's lattice-index units, faces [F,3] int64); mark(stage) is called after the normals and after the MC"""
     from neuraludf_b200 import grid
     planes = df.numel() // (N * N)
     idx, normals = grid.near_surface_cells(udf_network, N, df, max_batch=max(max_batch // 2, 1), lo=lo)
+    mark("normals")
     verts, faces, _ = marching_cubes_index(df, (planes, N, N), normals, idx - lo)
+    mark("mc")
     return verts, faces
 
 
-def _udf_mc(udf_network, N, lattice, lipschitz=2.0, strides=None, max_batch=1 << 21, lo=0, hi=None):
+def _udf_mc(udf_network, N, lattice, lipschitz=2.0, strides=None, max_batch=1 << 21, lo=0, hi=None, mark=_no_mark):
     """The raw MeshUDF MC of the N^3 lattice evaluated `lattice`: "dense" (grid.udf_grid of the slab [lo, hi)), "band"
     (grid.udf_band) or "sparse" (grid.udf_band_sparse): (verts [V,3] fp32 in the slab's lattice-index units, faces [F,3]
-    int64).  The lattice is released on return."""
+    int64).  Negative lattice values are set to 0 (extract_mesh.py:196; a UDF network gives none) after the normals'
+    selection, which reads them unchanged either way (< 2 voxels).  The lattice is released on return.  mark(stage) is
+    called after the lattice, the normals and the MC."""
     from neuraludf_b200 import grid
     if lattice == "sparse":
         band, _ = grid.udf_band_sparse(udf_network, N, lipschitz=lipschitz, strides=strides, max_batch=max_batch)
+        mark("lattice")
         idx, normals = grid.near_surface_cells_sparse(udf_network, band, max_batch=max(max_batch // 2, 1))
+        mark("normals")
         verts, faces, _ = marching_cubes_sparse(band, normals, idx)
+        mark("mc")
         return verts, faces
     if lattice == "dense":
         df = grid.udf_grid(udf_network, N, max_batch=max_batch, lo=lo, hi=hi)
     else:
         df, _ = grid.udf_band(udf_network, N, lipschitz=lipschitz, strides=strides, max_batch=max_batch)
-    return _mc_lattice(udf_network, N, df, lo, max_batch)
+    df.masked_fill_(df < 0, 0.0)
+    mark("lattice")
+    return _mc_lattice(udf_network, N, df, lo, max_batch, mark)
 
 
 def _udf_mesh(udf_network, N, lattice, dist_threshold_ratio, lipschitz=2.0, strides=None, max_batch=1 << 21, lo=0, hi=None):
@@ -337,20 +350,46 @@ def udf_mesh_post(udf_network, N, dist_threshold_ratio=5.0, dense=False, lipschi
     theirs.  The vertices are then formed as the reference holds them, fp64(fp32 MC vertex) *
     fp64(voxel) - 1 in fp64, the vertex filter of extract_mesh.py:205-214 evaluates the udf at their fp32 rounding, and
     `mesh_post.postprocess` does the rest of get_mesh_udf_fast (extract_mesh.py:215-265; the runner passes
-    `dist_threshold_ratio` 5 and `smooth_borders` True).  info: postprocess's, plus `mc` ((V, F) of the raw MC) and
-    `filtered` (faces after the vertex filter)."""
-    from neuraludf_b200 import mesh_post
-    voxel = 2.0 / (N - 1)
+    `dist_threshold_ratio` 5 and `smooth_borders` True).  info: postprocess's, plus `mc` ((V, F) of the raw MC),
+    `filtered` (faces after the vertex filter) and `stage_ms` (_mesh_post's)."""
     if dense and sparse:
         raise ValueError("udf_mesh_post: dense and sparse exclude each other")
-    verts, faces = _udf_mc(udf_network, N, _lattice_kind(dense, sparse), lipschitz, strides, max_batch)
+    return _mesh_post(udf_network, N, _lattice_kind(dense, sparse), dist_threshold_ratio, smooth_borders, lipschitz, strides,
+                      max_batch)
+
+
+def _mesh_post(field, N, lattice, dist_threshold_ratio, smooth_borders, lipschitz=2.0, strides=None, max_batch=1 << 21):
+    """get_mesh_udf_fast up to its gradient branch (extract_mesh.py:194-265) on `field`, the lattice evaluated as _udf_mc's
+    `lattice` names it: (fp64 verts [V,3], int64 faces [F,3], info) on the device.  `field` is a UDF network (its
+    udf_values and runner-normalised gradient: udf_mesh_post) or anything with udf_values(points [P,3]) -> [P] and
+    surface_normals(points) -> unit vectors towards the surface [P,3] (extract_mesh.CallerField).
+
+    The vertices are formed as the reference holds them, fp64(fp32 MC vertex) * fp64(voxel) - 1 in fp64; the vertex filter
+    evaluates the field at their fp32 rounding in one call (in batches of max_batch on the sparse lattice) and keeps the
+    faces whose vertices are all below voxel * dist_threshold_ratio; mesh_post.postprocess does the rest.  info:
+    postprocess's, plus `mc` ((V, F) of the raw MC), `filtered` (faces after the vertex filter) and `stage_ms` (CUDA-event
+    milliseconds of the lattice, normals, mc, filter and post stages)."""
+    from neuraludf_b200 import mesh_post
+    voxel = 2.0 / (N - 1)
+    events = [("start", torch.cuda.Event(enable_timing=True))]
+    events[0][1].record()
+
+    def mark(stage):
+        events.append((stage, torch.cuda.Event(enable_timing=True)))
+        events[-1][1].record()
+
+    verts, faces = _udf_mc(field, N, lattice, lipschitz, strides, max_batch, mark=mark)
     v64 = verts.double() * voxel - 1.0
     n_mc = faces.shape[0]
     if n_mc:
-        vd = _batched_values(udf_network, v64.float(), max_batch if sparse else None)
+        vd = _batched_values(field, v64.float(), max_batch if lattice == "sparse" else None)
         faces = faces[vd[faces].max(dim=1).values < voxel * dist_threshold_ratio]
+    mark("filter")
     v, f, info = mesh_post.postprocess(v64, faces, smooth_borders=smooth_borders)
+    mark("post")
     info["mc"], info["filtered"] = (verts.shape[0], n_mc), int(faces.shape[0])
+    torch.cuda.synchronize(v.device)
+    info["stage_ms"] = {b[0]: a[1].elapsed_time(b[1]) for a, b in zip(events, events[1:])}
     return v, f, info
 
 

@@ -151,6 +151,13 @@ def hole_faces(verts, codes):
     return out
 
 
+def has_border(verts, faces):
+    """whether the mesh has an edge used by one face (an empty mesh has none)"""
+    if faces.shape[0] == 0:
+        return False
+    return boundary(_codes(verts, faces), verts.shape[0])[0].shape[0] > 0
+
+
 def smooth_border_vertices(verts, codes, steps=SMOOTH_STEPS, lam=SMOOTH_LAMBDA):
     """(verts, border vertex count): `steps` Jacobi steps over the border vertices (csrc/mesh_post.cu smoothing)"""
     V = verts.shape[0]
