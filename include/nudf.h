@@ -87,7 +87,9 @@ typedef struct nudf_udf_desc {
 int64_t nudf_udf_folded_floats(const nudf_udf_desc* d);
 /* folds weight-norm once per optimiser step (replaces torch._weight_norm inside every nn.Linear call) */
 int nudf_udf_fold_weights(const nudf_udf_desc* d, float* wfold, void* stream);
-/* floats of the activation context saved by forward for `P` points (with_grad: also the reverse-sweep tensors) */
+/* floats of the activation context saved by forward for `P` points (with_grad: also the reverse-sweep tensors).
+ * The ctx, scratch and work buffers of every network below need 16-byte-aligned bases: the layouts keep each block's
+ * rows in whole 16-byte units from there, as the tensor-core kernels read them through 2-D tensor maps. */
 int64_t nudf_udf_ctx_floats(const nudf_udf_desc* d, int64_t P, int with_grad);
 /* floats of the scratch needed by backward */
 int64_t nudf_udf_scratch_floats(const nudf_udf_desc* d, int64_t P);
@@ -134,6 +136,7 @@ typedef struct nudf_color_desc {
 
 int64_t nudf_color_folded_floats(const nudf_color_desc* d);
 int nudf_color_fold_weights(const nudf_color_desc* d, float* wfold, void* stream);
+/* ctx and scratch: 16-byte-aligned bases */
 int64_t nudf_color_ctx_floats(const nudf_color_desc* d, int64_t P);
 int64_t nudf_color_scratch_floats(const nudf_color_desc* d, int64_t P);
 /* color_base[P,3], color[P,3], blend[P,n_blend] <- forward(points, view_dirs, feature_vectors) (fields.py:452-495).
@@ -171,6 +174,7 @@ typedef struct nudf_nerf_desc {
  * to forward/backward (NULL = exact-fp32 engine) */
 int64_t nudf_nerf_image_floats(const nudf_nerf_desc* d);
 int nudf_nerf_prepare(const nudf_nerf_desc* d, float* wimg, void* stream);
+/* ctx and scratch: 16-byte-aligned bases */
 int64_t nudf_nerf_ctx_floats(const nudf_nerf_desc* d, int64_t P);
 int64_t nudf_nerf_scratch_floats(const nudf_nerf_desc* d, int64_t P);
 /* sigma[P], rgb[P,3] <- NeRF.forward(pts4, view_dirs) (fields.py:599-628; no sigmoid on rgb) */

@@ -1,14 +1,16 @@
 // Tensor-core GEMM engine for sm_90a (wgmma) with an fp32-grade split-bf16 operand scheme:
 //   D = sum over K slices of A_hi*B_hi + A_hi*B_lo + A_lo*B_hi  (2 planes, ~4e-6 vs fp64), or with 3 planes hi/mid/lo the 6
 //   products of weight >= 2^-16 (fp32-grade); x = hi + lo, hi = bf16(x), lo = bf16(x - hi) (SURVEY.md section 0, fact 3).
-// One CTA = 2 warpgroups, a 128 x WN output tile, a 2-stage shared-memory ring over 64-wide K slices: warpgroup w issues
-// wgmma.m64n{WN}k16 for rows 64w.. (K-major SWIZZLE_128B operands, fp32 accumulators in registers) while all threads stage
-// the next activation slice as bf16 planes (2-plane layers from a ring of TMA-copied fp32 slices, split in place, when
-// the operand allows it); weight slices arrive by cp.async.bulk on an mbarrier.  The accumulators go
-// through shared memory to the fused epilogue functor (4 consecutive columns of a row per call: coalesced).  WN = 256 for
-// 2-plane layers wider than 128 columns, so that each activation row block is read from HBM and split into planes once.
-// 3-plane layers on such operands run gemm_w3_tma_kernel instead: persistent, a producer warpgroup feeding two consumer
-// warpgroups through mbarriers, the epilogue applied from the accumulator fragments.
+// Weights arrive as pre-split plane images by cp.async.bulk; activations arrive as fp32 by TMA (2-D tensor maps) and are
+// split into K-major SWIZZLE_128B bf16 planes in shared memory.  One kernel per job:
+// * gemm_w_kernel, 2-plane layers: 2 warpgroups, a 128 x WN output tile (WN = 256 for layers wider than 128 columns, so
+//   that each activation row block is read from HBM and split once), a ring of fp32 activation slices split in place.
+//   The accumulators go through shared memory to the fused epilogue functor (4 consecutive columns of a row per call).
+// * gemm_w3_tma_kernel, 3-plane layers: persistent, a producer warpgroup feeding two consumer warpgroups through
+//   mbarriers, the epilogue applied from the accumulator fragments.
+// * gemm_tn_kernel, weight gradients: a ring of fp32 slices of both operands split into MN-major planes, split-K over
+//   the points.
+// Every activation operand has a row stride of whole 16-byte units and a 16-byte-aligned base (check_tma_operand).
 #pragma once
 #include <cuda.h>
 #include <cudaTypedefs.h>
@@ -24,7 +26,6 @@ constexpr int BN = 128;        // output columns per CTA of gemm_tn_kernel and o
 constexpr int BK = 64;
 constexpr int THREADS = 256;   // 2 warpgroups: MMA issue, operand staging and epilogue
 constexpr int A_HALF_BYTES = BM * BK * 2;   // 16 KB: one plane of a [128 x 64] operand slice
-constexpr int B_HALF_BYTES = BN * BK * 2;
 __host__ __device__ constexpr int b_plane_bytes(int wn) { return wn * BK * 2; }   // one plane of a [wn x 64] weight slice
 __host__ __device__ constexpr int acc_ld(int wn) { return wn + 4; }   // floats per row of the accumulator tile in smem
 
@@ -36,7 +37,7 @@ __host__ __device__ inline uint32_t sw128(uint32_t row, uint32_t k) {
   return (row >> 3) * 1024u + (row & 7u) * 128u + ((((k >> 3) ^ (row & 7u)) & 7u) << 4) + ((k & 7u) << 1);
 }
 
-// gemm_tn_kernel's ring path: slices of TN_PS points, fp32 operand blocks as they lie in HBM ([point][128 columns]) in a
+// gemm_tn_kernel: slices of TN_PS points, fp32 operand blocks as they lie in HBM ([point][128 columns]) in a
 // TN_RING-deep ring, and a double-buffered stage of bf16 planes (hi, lo of A, then of B)
 constexpr int TN_PS = 32;
 constexpr int TN_RING = 4;
@@ -44,7 +45,7 @@ constexpr uint32_t TN_F32_OPND = TN_PS * BM * 4;            // 16 KB: one operan
 constexpr uint32_t TN_F32_STAGE = 2 * TN_F32_OPND;          // A, then B
 constexpr uint32_t TN_PLANE = BM * TN_PS * 2;               // 8 KB: one bf16 plane of one operand
 constexpr uint32_t TN_PLANE_STAGE = 4 * TN_PLANE;
-struct TnMaps { CUtensorMap a, b; };                         // the ring path's 2-D tensor maps of A and B
+struct TnMaps { CUtensorMap a, b; };                         // gemm_tn_kernel's 2-D tensor maps of A and B
 // byte offset of element (mn, k) inside a [128 x 32] bf16 MN-major SWIZZLE_128B plane (base 1024-aligned): two 64-wide
 // MN blocks of 4 KB, each four 1 KB atoms of 8 points x 128 B; the 16-byte chunk index is XOR-ed with the point's row
 // in its atom, as the hardware's 128B swizzle does with address bits 4-6 and 7-9
@@ -52,7 +53,7 @@ __host__ __device__ inline uint32_t sw128_mn(uint32_t mn, uint32_t k) {
   return (mn >> 6) * 4096u + (k >> 3) * 1024u + (k & 7u) * 128u + ((((mn >> 3) ^ k) & 7u) << 4) + ((mn & 7u) << 1);
 }
 
-// gemm_w_kernel's ring path (2 planes): slots of one fp32 [128 x 64] activation slice as it lies in HBM, each split in
+// gemm_w_kernel (2 planes): slots of one fp32 [128 x 64] activation slice as it lies in HBM, each split in
 // place into its hi and lo planes; W_RING(WN) slots beside the two weight stages
 constexpr uint32_t W_SLOT = BM * BK * 4;                     // 32 KB
 static_assert(W_SLOT == 2 * A_HALF_BYTES, "a slot holds exactly the two bf16 planes of its slice");
@@ -283,8 +284,8 @@ __device__ __forceinline__ void wgmma_256(float (&d)[128], uint64_t da, uint64_t
 
 // The wgmma group of one 64-wide K slice, smallest products first; plane p at +p * stride, 32 B per 16-wide K step.
 // With 3 planes only the five correction products (lo * hi, hi * lo, mid * mid, mid * hi, hi * mid: ~2^-8 of the result's
-// scale, so the tensor core's truncation of each wgmma result to fp32 costs ~2^-32 of it); gemm_w_kernel issues each hi * hi
-// step into fresh accumulators and adds them up in fp32 with round-to-nearest.
+// scale, so the tensor core's truncation of each wgmma result to fp32 costs ~2^-32 of it); gemm_w3_tma_kernel issues each
+// hi * hi step into fresh accumulators and adds them up in fp32 with round-to-nearest.
 // WN (128 or 256) is the width of the weight slice and of the accumulator fragment.
 template <int WN>
 __device__ __forceinline__ void wgmma_n(float (&d)[WN / 2], uint64_t da, uint64_t db, uint32_t accumulate) {
@@ -310,7 +311,7 @@ __device__ __forceinline__ void mma_slice(float (&d)[WN / 2], uint32_t a, uint32
     }
   }
 }
-// The wgmma group of one TN_PS-point slice of gemm_tn_kernel's ring path: MN-major planes (lo at +TN_PLANE), 2 KB per
+// The wgmma group of one TN_PS-point slice of gemm_tn_kernel: MN-major planes (lo at +TN_PLANE), 2 KB per
 // 16-point step, the products of each step in mma_slice<2>'s order
 __device__ __forceinline__ void mma_slice_mn(float (&d)[64], uint32_t a, uint32_t b, bool zero_first) {
 #pragma unroll
@@ -375,295 +376,123 @@ __device__ __forceinline__ void tile_epilogue(const float* acc_s, int64_t m0, in
   }
 }
 
-template <int NT>   // NT = number of producer threads (128 or 256); fetches this thread's part of a [128 x 64] fp32 slice
-__device__ __forceinline__ void fetch_a(const float* __restrict__ A, int64_t lda, int64_t m0, int64_t M, int k0, int K, int tid,
-                                        bool vec_ok, float4 (&v)[BM * 16 / NT]) {
-  const int c = tid & 15;            // float4 chunk along k
-  const int rsub = tid >> 4;         // 0 .. NT/16-1
-  const int k = k0 + c * 4;
-#pragma unroll
-  for (int pass = 0; pass < BM * 16 / NT; ++pass) {
-    const int64_t row = m0 + pass * (NT / 16) + rsub;
-    v[pass] = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (row < M) {
-      const float* p = A + row * lda + k;
-      if (vec_ok && k + 3 < K) {
-        v[pass] = *reinterpret_cast<const float4*>(p);
-      } else {
-        if (k + 0 < K) v[pass].x = p[0];
-        if (k + 1 < K) v[pass].y = p[1];
-        if (k + 2 < K) v[pass].z = p[2];
-        if (k + 3 < K) v[pass].w = p[3];
-      }
-    }
-  }
-}
-// splits the fetched values into NP bf16 planes and writes them into the K-major SW128 stage (16 KB per plane)
-template <int NP, int NT>
-__device__ __forceinline__ void store_a(const float4 (&v)[BM * 16 / NT], uint8_t* sa, int tid) {
+// splits this thread's 8 float4 of a [128 x 64] fp32 slice into hi / lo bf16 planes and writes them into the K-major SW128
+// stage (16 KB per plane); thread t holds rows 16 pass + t / 16, columns 4 (t % 16) .. + 3
+__device__ __forceinline__ void store_a(const float4 (&v)[BM * 16 / THREADS], uint8_t* sa, int tid) {
   const int c = tid & 15;
   const int rsub = tid >> 4;
 #pragma unroll
-  for (int pass = 0; pass < BM * 16 / NT; ++pass) {
+  for (int pass = 0; pass < BM * 16 / THREADS; ++pass) {
     const float x[4] = {v[pass].x, v[pass].y, v[pass].z, v[pass].w};
-    uint2 pl[NP];
-    split4<NP>(x, pl);
-    const uint32_t off = sw128((uint32_t)(pass * (NT / 16) + rsub), (uint32_t)(c * 4));
+    uint2 pl[2];
+    split4<2>(x, pl);
+    const uint32_t off = sw128((uint32_t)(pass * (THREADS / 16) + rsub), (uint32_t)(c * 4));
 #pragma unroll
-    for (int p = 0; p < NP; ++p) *reinterpret_cast<uint2*>(sa + p * A_HALF_BYTES + off) = pl[p];
-  }
-}
-// Stage a [128 x 64] slice of row-major fp32 A (K contiguous) as NP bf16 planes.  All global loads of a thread are issued
-// before the first conversion so that the whole 32 KB slice is in flight.
-template <int NP, int NT>
-__device__ __forceinline__ void stage_a_direct(const float* __restrict__ A, int64_t lda, int64_t m0, int64_t M, int k0, int K,
-                                               uint8_t* sa, int tid, bool vec_ok) {
-  float4 v[BM * 16 / NT];
-  fetch_a<NT>(A, lda, m0, M, k0, K, tid, vec_ok, v);
-  store_a<NP, NT>(v, sa, tid);
-}
-
-// One warp stages a [32 rows x 64 k] block of the K-major tile  T(r, k) = X[(k0 + k) * ld + m0 + r]  as 2 bf16 planes
-// (on-the-fly transpose; the contraction index k runs over points).  Lane l owns the m-quad (l & 7) and, in iteration q,
-// the k pair 4q + (l >> 3): every warp-level load covers 4 rows of X x 128 contiguous bytes (4 L1 wavefronts instead of
-// the 32 of a lane-per-row mapping).  Two steps, so that the 16 loads of a lane stay in flight while the tensor cores work
-// on the previous slice: fetch_block_t loads the block into registers, store_block_t splits them into the stage.
-// Tile rows are padded to 16 and blocks cover 32: both skip the quads beyond the tile.
-__device__ __forceinline__ void fetch_block_t(const float* __restrict__ X, int64_t ld, int m0, int m_total, int r0, int rows,
-                                              int64_t k0, int64_t k_end, int lane, bool vec_ok, float4 (&v)[8][2]) {
-  const int mq = lane & 7, kq = lane >> 3;
-  if (r0 + 4 * mq >= rows) return;
-  const int m = m0 + r0 + 4 * mq;
-#pragma unroll
-  for (int q = 0; q < 8; ++q) {
-#pragma unroll
-    for (int kk = 0; kk < 2; ++kk) {
-      const int64_t k = k0 + 2 * (4 * q + kq) + kk;
-      v[q][kk] = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (k < k_end) {
-        const float* p = X + k * ld + m;
-        if (vec_ok && m + 3 < m_total) {
-          v[q][kk] = *reinterpret_cast<const float4*>(p);
-        } else {
-          if (m + 0 < m_total) v[q][kk].x = p[0];
-          if (m + 1 < m_total) v[q][kk].y = p[1];
-          if (m + 2 < m_total) v[q][kk].z = p[2];
-          if (m + 3 < m_total) v[q][kk].w = p[3];
-        }
-      }
-    }
-  }
-}
-template <bool CSUM = false>
-__device__ __forceinline__ void store_block_t(const float4 (&v)[8][2], int r0, int rows, uint8_t* s_hi, uint8_t* s_lo, int lane,
-                                              float* csum = nullptr) {
-  const int mq = lane & 7, kq = lane >> 3;
-  if (r0 + 4 * mq >= rows) return;
-  if (CSUM) {                             // per-lane partial column sums of X (bias gradients), fp32
-#pragma unroll
-    for (int q = 0; q < 8; ++q) {
-      csum[0] += v[q][0].x + v[q][1].x; csum[1] += v[q][0].y + v[q][1].y;
-      csum[2] += v[q][0].z + v[q][1].z; csum[3] += v[q][0].w + v[q][1].w;
-    }
-  }
-#pragma unroll
-  for (int q = 0; q < 8; ++q) {
-    const float x0[4] = {v[q][0].x, v[q][0].y, v[q][0].z, v[q][0].w};
-    const float x1[4] = {v[q][1].x, v[q][1].y, v[q][1].z, v[q][1].w};
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const float h0 = __bfloat162float(__float2bfloat16_rn(x0[j])), h1 = __bfloat162float(__float2bfloat16_rn(x1[j]));
-      const uint32_t off = sw128((uint32_t)(r0 + 4 * mq + j), (uint32_t)(2 * (4 * q + kq)));
-      *reinterpret_cast<uint32_t*>(s_hi + off) = pack_bf16(h0, h1);
-      *reinterpret_cast<uint32_t*>(s_lo + off) = pack_bf16(x0[j] - h0, x1[j] - h1);
-    }
+    for (int p = 0; p < 2; ++p) *reinterpret_cast<uint2*>(sa + p * A_HALF_BYTES + off) = pl[p];
   }
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// C[M x N] = epi( A[M x K] * B^T ),  B given as a pre-split NP-plane weight image, WN output columns per CTA.
+// 2-plane layers: C[M x N] = epi( A[M x K] * B^T ),  B given as a pre-split 2-plane weight image, WN output columns per CTA.
 // 1-D grid of ceil(M/128) * ceil(N/WN) CTAs with the column tile fastest: the column tiles of a row block run back to
 // back, so that a second read of its activations hits L2.  Weight rows beyond the image tile (N = 217 -> 224 rows) leave
 // stale shared memory in the last rows of the slice; they only feed columns >= N, which the epilogue never passes on.
-// Weight slices arrive by cp.async.bulk into two stages on mbarriers.  The activation slices take one of two paths:
-//
-// RING (2 planes; a row stride that is a multiple of 4 floats and a 16-byte-aligned base, as a 2-D tensor map needs):
-// one thread issues a 2-D TMA copy per 64-wide K slice (a [128 rows x 64 k] fp32 box, 32 KB; rows past M and columns
-// past K arrive as zeros, padding columns of the row stride are never read) into a w_ring(WN)-deep ring of slots on
-// mbarriers, all of them before the main loop.  While the wgmma group of slice ks runs, all threads split slice ks + 1
+// Weight slices arrive by cp.async.bulk into two stages on mbarriers.  The activations reach shared memory as they lie in
+// HBM: one thread issues a 2-D TMA copy per 64-wide K slice (a [128 rows x 64 k] fp32 box, 32 KB; rows past M and
+// columns past K arrive as zeros, padding columns of the row stride are never read) into a w_ring(WN)-deep ring of slots
+// on mbarriers, all of them before the main loop.  While the wgmma group of slice ks runs, all threads split slice ks + 1
 // in place: each reads its 8 float4 (store_a's mapping: a warp reads 512 contiguous bytes), a CTA barrier, then the
 // hi / lo K-major SW128 planes go over the same 32 KB.  A slot is refilled as soon as the barrier after the wgmma group
-// that read it has passed.  The planes and the products are the register path's, so both give the same bits.
-// Otherwise all threads stage each slice through registers (stage_a_direct; 3-plane layers come here only with operands
-// gemm_w3_tma_kernel cannot take): the loads of slice ks + 1 are issued after the wgmma group of slice ks, then split
-// into the free stage.
+// that read it has passed.  With K = 0 no copy is issued and the epilogue sees zero accumulators.
 // ---------------------------------------------------------------------------------------------------------------
-template <int NP, int WN, class Epi, bool RING>
+template <int WN, class Epi>
 __global__ void __launch_bounds__(THREADS, 1)
-gemm_w_kernel(const float* __restrict__ A, int64_t lda, int64_t M, int N, int K, const uint16_t* __restrict__ img, Epi epi,
-              const __grid_constant__ CUtensorMap amap) {
-  static_assert(WN == 128 || (WN == 256 && NP == 2), "WN = 256 only with 2 planes (3 planes need 2 x WN/2 accumulators)");
-  static_assert(!RING || NP == 2, "the ring path splits a slot into 2 planes in place");
+gemm_w_kernel(int64_t M, int N, int K, const uint16_t* __restrict__ img, Epi epi, const __grid_constant__ CUtensorMap amap) {
+  static_assert(WN == 128 || WN == 256, "a 128- or 256-column weight slice");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = align1024(smem_raw);
   const int tid = threadIdx.x, wg = tid >> 7;
   const int n_ct = (N + WN - 1) / WN;
   const int n0 = (int)(blockIdx.x % (unsigned)n_ct) * WN;
   const int64_t m0 = (int64_t)(blockIdx.x / (unsigned)n_ct) * BM;
-  const int t = n0 / nt_of(NP);                             // image tile of this CTA's columns
-  const int rows_t = tile_rows(N, t, NP);
-  const int row_in_tile = n0 - t * nt_of(NP);
+  const int t = n0 / nt_of(2);                              // image tile of this CTA's columns
+  const int rows_t = tile_rows(N, t, 2);
+  const int row_in_tile = n0 - t * nt_of(2);
   int rows_h = rows_t - row_in_tile; rows_h = rows_h < WN ? rows_h : WN;   // weight rows of this CTA (multiple of 16)
   const int n_slices = pad64(K) / 64;
   constexpr uint32_t B_PLANE = b_plane_bytes(WN);
-  const uint16_t* img_t = img + tile_offset(N, K, t, NP) + (int64_t)row_in_tile * 64;
-  // 3 planes: the corrections of each K slice and each 16-wide hi * hi step in fresh registers, summed in fp32 with
-  // round-to-nearest.  The tensor core truncates a wgmma result toward zero; every hi * hi result is a single truncation of
-  // 16 full-size products, so adding half an ulp of it (with its sign) leaves an unbiased error.  Without that the bias of
-  // the 16 truncations per output (K = 256) adds up coherently over the points of a parameter-gradient sum.
-  // The hi * hi steps alternate between acc2 and acc, so that step j + 1 is in flight while step j is added; tot still
-  // takes the corrections, hh0, hh1, hh2, hh3 in that order.
-  constexpr int NACC = WN / 2, NTOT = NP == 3 ? 64 : 1;
-  float acc[NACC], tot[NTOT], acc2[NTOT];
+  const uint16_t* img_t = img + tile_offset(N, K, t, 2) + (int64_t)row_in_tile * 64;
+  constexpr int NACC = WN / 2;
+  float acc[NACC];
 #pragma unroll
   for (int q = 0; q < NACC; ++q) acc[q] = 0.f;
-#pragma unroll
-  for (int q = 0; q < NTOT; ++q) tot[q] = 0.f;
 
-  if constexpr (RING) {
-    // [w_ring(WN) activation slots][2 weight stages of 2 planes][a barrier per slot][a barrier per weight stage]
-    constexpr int NR = w_ring(WN);
-    constexpr uint32_t W_STAGE = 2 * B_PLANE;
-    uint8_t* wst = smem + NR * W_SLOT;
-    uint64_t* afull = reinterpret_cast<uint64_t*>(wst + 2 * W_STAGE);
-    uint64_t* wfull = afull + NR;
-    auto issue_a = [&](int i) {                             // one thread: activation slice i into slot i % NR
-      const int r = i % NR;
-      mbar_arrive_expect_tx(&afull[r], W_SLOT);
-      tma_load_2d(smem + r * W_SLOT, &amap, i * BK, (int)m0, &afull[r]);
-    };
-    auto issue_w = [&](int ks) {                            // one thread: weight slice ks into stage ks & 1
-      uint8_t* st = wst + (ks & 1) * W_STAGE;
-      const uint32_t wb = (uint32_t)rows_h * 128u;
-      mbar_arrive_expect_tx(&wfull[ks & 1], 2 * wb);
-      for (int p = 0; p < 2; ++p) bulk_g2s(st + p * B_PLANE, img_t + ((int64_t)ks * 2 + p) * rows_t * 64, wb, &wfull[ks & 1]);
-    };
-    auto split = [&](int i) {                               // slice i, once landed, into hi / lo planes over its slot
-      uint8_t* slot = smem + (i % NR) * W_SLOT;
-      mbar_wait(&afull[i % NR], (uint32_t)((i / NR) & 1));
-      float4 v[BM * 16 / THREADS];
-      const float4* f = reinterpret_cast<const float4*>(slot) + (tid >> 4) * (BK / 4) + (tid & 15);
+  // [w_ring(WN) activation slots][2 weight stages of 2 planes][a barrier per slot][a barrier per weight stage]
+  constexpr int NR = w_ring(WN);
+  constexpr uint32_t W_STAGE = 2 * B_PLANE;
+  uint8_t* wst = smem + NR * W_SLOT;
+  uint64_t* afull = reinterpret_cast<uint64_t*>(wst + 2 * W_STAGE);
+  uint64_t* wfull = afull + NR;
+  auto issue_a = [&](int i) {                               // one thread: activation slice i into slot i % NR
+    const int r = i % NR;
+    mbar_arrive_expect_tx(&afull[r], W_SLOT);
+    tma_load_2d(smem + r * W_SLOT, &amap, i * BK, (int)m0, &afull[r]);
+  };
+  auto issue_w = [&](int ks) {                              // one thread: weight slice ks into stage ks & 1
+    uint8_t* st = wst + (ks & 1) * W_STAGE;
+    const uint32_t wb = (uint32_t)rows_h * 128u;
+    mbar_arrive_expect_tx(&wfull[ks & 1], 2 * wb);
+    for (int p = 0; p < 2; ++p) bulk_g2s(st + p * B_PLANE, img_t + ((int64_t)ks * 2 + p) * rows_t * 64, wb, &wfull[ks & 1]);
+  };
+  auto split = [&](int i) {                                 // slice i, once landed, into hi / lo planes over its slot
+    uint8_t* slot = smem + (i % NR) * W_SLOT;
+    mbar_wait(&afull[i % NR], (uint32_t)((i / NR) & 1));
+    float4 v[BM * 16 / THREADS];
+    const float4* f = reinterpret_cast<const float4*>(slot) + (tid >> 4) * (BK / 4) + (tid & 15);
 #pragma unroll
-      for (int pass = 0; pass < BM * 16 / THREADS; ++pass) v[pass] = f[pass * (THREADS / 16) * (BK / 4)];
-      __syncthreads();                                      // every read of the slot before the first plane store
-      store_a<2, THREADS>(v, slot, tid);
-    };
-    if (tid == 0) {
-      for (int r = 0; r < NR; ++r) mbar_init(&afull[r], 1);
-      mbar_init(&wfull[0], 1);
-      mbar_init(&wfull[1], 1);
-      fence_barrier_init();
-      if (n_slices > 0) issue_w(0);
-      for (int i = 0; i < NR && i < n_slices; ++i) issue_a(i);
-    }
-    __syncthreads();
-    if (n_slices > 0) {
-      split(0);
-      fence_proxy_async();
-    }
-    __syncthreads();
-    for (int ks = 0; ks < n_slices; ++ks) {
-      const int s = ks & 1;
-      if (tid == 0 && ks + 1 < n_slices) issue_w(ks + 1);   // stage s ^ 1 was released by the wait + barrier of ks - 1
-      mbar_wait(&wfull[s], (uint32_t)((ks >> 1) & 1));
-      const uint32_t sa = smem_u32(smem + (ks % NR) * W_SLOT), sb = smem_u32(wst + s * W_STAGE);
-      wg_fence();
-      mma_slice<2, WN>(acc, sa + wg * (64 * 128), A_HALF_BYTES, sb, B_PLANE, ks == 0);
-      wg_commit();
-      if (ks + 1 < n_slices) split(ks + 1);
-      wg_wait_all();
-      fence_proxy_async();
-      __syncthreads();
-      if (tid == 0 && ks + NR < n_slices) issue_a(ks + NR);  // slot ks % NR: the group that read it has completed
-    }
-  } else {
-    const uint32_t a_bytes = NP * A_HALF_BYTES, stage_bytes = a_bytes + NP * B_PLANE;
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + 2 * stage_bytes);
-    const bool vec_ok = ((lda & 3) == 0) && aligned16(A);
-
-    auto issue_copies = [&](int ks) {                       // one thread: weight slice ks
-      uint8_t* st = smem + (ks & 1) * stage_bytes;
-      const uint32_t wb = (uint32_t)rows_h * 128u;
-      mbar_arrive_expect_tx(&full[ks & 1], NP * wb);
-      for (int p = 0; p < NP; ++p) bulk_g2s(st + a_bytes + p * B_PLANE, img_t + ((int64_t)ks * NP + p) * rows_t * 64, wb, &full[ks & 1]);
-    };
-    if (tid == 0) {
-      mbar_init(&full[0], 1);
-      mbar_init(&full[1], 1);
-      fence_barrier_init();
-    }
-    __syncthreads();
-    if (n_slices > 0) {
-      if (tid == 0) issue_copies(0);
-      stage_a_direct<NP, THREADS>(A, lda, m0, M, 0, K, smem, tid, vec_ok);
-      fence_proxy_async();
-    }
-    __syncthreads();
-    for (int ks = 0; ks < n_slices; ++ks) {
-      const int s = ks & 1;
-      if (tid == 0 && ks + 1 < n_slices) issue_copies(ks + 1);   // stage s ^ 1 was released by the wait + barrier of ks - 1
-      mbar_wait(&full[s], (uint32_t)((ks >> 1) & 1));
-      const uint32_t st = smem_u32(smem + s * stage_bytes);
-      wg_fence();
-      mma_slice<NP, WN>(acc, st + wg * (64 * 128), A_HALF_BYTES, st + a_bytes, B_PLANE, NP == 3 || ks == 0);
-      wg_commit();
-      if (ks + 1 < n_slices) stage_a_direct<NP, THREADS>(A, lda, m0, M, (ks + 1) * BK, K, smem + (s ^ 1) * stage_bytes, tid, vec_ok);
-      wg_wait_all();
-      if constexpr (NP == 3) {
-        static_assert(BK / 16 == 4, "four hi * hi steps per K slice");
-        auto hi_hi = [&](float (&d)[64], int j) {
-          wg_fence();
-          wgmma_128_fresh(d, make_desc(st + wg * (64 * 128) + 32u * j), make_desc(st + a_bytes + 32u * j));
-          wg_commit();
-        };
-        auto add_unbiased = [&](float (&d)[64]) {            // after the wait that completes d
-          fence_operand(d);
-#pragma unroll
-          for (int q = 0; q < 64; ++q) tot[q] += unbias_rz(d[q]);
-        };
-        hi_hi(acc2, 0);
-        fence_operand(acc);
-#pragma unroll
-        for (int q = 0; q < 64; ++q) tot[q] += acc[q];        // corrections
-        hi_hi(acc, 1);
-        wg_wait_but_one();
-        add_unbiased(acc2);                                   // hh0
-        hi_hi(acc2, 2);
-        wg_wait_but_one();
-        add_unbiased(acc);                                    // hh1
-        hi_hi(acc, 3);
-        wg_wait_but_one();
-        add_unbiased(acc2);                                   // hh2
-        wg_wait_all();
-        add_unbiased(acc);                                    // hh3
-      }
-      fence_proxy_async();
-      __syncthreads();
-    }
+    for (int pass = 0; pass < BM * 16 / THREADS; ++pass) v[pass] = f[pass * (THREADS / 16) * (BK / 4)];
+    __syncthreads();                                        // every read of the slot before the first plane store
+    store_a(v, slot, tid);
+  };
+  if (tid == 0) {
+    for (int r = 0; r < NR; ++r) mbar_init(&afull[r], 1);
+    mbar_init(&wfull[0], 1);
+    mbar_init(&wfull[1], 1);
+    fence_barrier_init();
+    if (n_slices > 0) issue_w(0);
+    for (int i = 0; i < NR && i < n_slices; ++i) issue_a(i);
   }
-  float* acc_s = reinterpret_cast<float*>(smem);              // the operand stages are free by now: every copy has landed
-  if constexpr (NP == 3) acc_to_smem<WN>(tot, acc_s, wg, tid & 127);
-  else acc_to_smem<WN>(acc, acc_s, wg, tid & 127);
+  __syncthreads();
+  if (n_slices > 0) {
+    split(0);
+    fence_proxy_async();
+  }
+  __syncthreads();
+  for (int ks = 0; ks < n_slices; ++ks) {
+    const int s = ks & 1;
+    if (tid == 0 && ks + 1 < n_slices) issue_w(ks + 1);     // stage s ^ 1 was released by the wait + barrier of ks - 1
+    mbar_wait(&wfull[s], (uint32_t)((ks >> 1) & 1));
+    const uint32_t sa = smem_u32(smem + (ks % NR) * W_SLOT), sb = smem_u32(wst + s * W_STAGE);
+    wg_fence();
+    mma_slice<2, WN>(acc, sa + wg * (64 * 128), A_HALF_BYTES, sb, B_PLANE, ks == 0);
+    wg_commit();
+    if (ks + 1 < n_slices) split(ks + 1);
+    wg_wait_all();
+    fence_proxy_async();
+    __syncthreads();
+    if (tid == 0 && ks + NR < n_slices) issue_a(ks + NR);  // slot ks % NR: the group that read it has completed
+  }
+  float* acc_s = reinterpret_cast<float*>(smem);              // the slots and stages are free by now: every copy has landed
+  acc_to_smem<WN>(acc, acc_s, wg, tid & 127);
   __syncthreads();
   tile_epilogue<WN>(acc_s, m0, M, n0, N, epi, tid);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// 3-plane layers on an operand that allows a 2-D tensor map (a row stride that is a multiple of 4 floats and a
-// 16-byte-aligned base): C[M x N] = epi( A[M x K] * B^T ) with the register path's planes, products and sums, so both
-// paths give the same bits.  Persistent: min(tiles, SMs) CTAs take the [128 x 128] tiles t = blockIdx.x + i * gridDim.x
-// (column tile fastest, so the two column tiles of a row block run at the same time and the second read of its
-// activations hits L2).  Three warpgroups and no CTA barrier after the set-up:
+// 3-plane layers: C[M x N] = epi( A[M x K] * B^T ), B given as a pre-split 3-plane weight image, K > 0.  Persistent:
+// min(tiles, SMs) CTAs take the [128 x 128] tiles t = blockIdx.x + i * gridDim.x (column tile fastest, so the two column
+// tiles of a row block run at the same time and the second read of its activations hits L2).  Three warpgroups and no
+// CTA barrier after the set-up:
 // * Producer (warpgroup 0, 40 registers).  One thread issues the 2-D TMA copies of each 64-wide K slice as four
 //   [32 rows x 64 k] fp32 boxes into four landing quarters, each on its own mbarrier (rows past M and columns past K
 //   arrive as zeros; a quarter that starts past M is not copied and splits as zeros), and the weight slice's three
@@ -674,8 +503,10 @@ gemm_w_kernel(const float* __restrict__ A, int64_t lda, int64_t M, int N, int K,
 // * Two consumers (warpgroups 1 and 2, 232 registers), each owning 64 rows of the tile.  Per slice: wait "full", issue
 //   mma_slice<3> (the five correction products into an accumulator zeroed at the slice) and the four hi * hi steps
 //   into fresh registers, add corrections, hh0 .. hh3 into tot in that order, and arrive on the stage's "empty"
-//   barrier (256 arrivals) once the last group has completed.  The consumers drift apart: one's adds overlap the other's
-//   products.  After the tile's last slice each consumer applies the epilogue functor to its own 64 rows straight
+//   barrier (256 arrivals) once the last group has completed.  The tensor core truncates a wgmma result toward zero;
+//   every hi * hi result is a single truncation of 16 full-size products, so adding half an ulp of it (with its sign)
+//   leaves an unbiased error.  Without that the bias of the 16 truncations per output (K = 256) adds up coherently over
+//   the points of a parameter-gradient sum.  The consumers drift apart: one's adds overlap the other's products.  After the tile's last slice each consumer applies the epilogue functor to its own 64 rows straight
 //   from the fragment: lane pairs swap one float2 so that each thread holds 4 consecutive columns of one row.
 // Weight rows past the image tile (N = 217 -> 224 rows) and stage contents left by an earlier slice or tile reach only
 // accumulator columns >= N, which are never passed to the epilogue.
@@ -857,26 +688,22 @@ gemm_w3_tma_kernel(const float* __restrict__ A, int64_t M, int N, int K, const u
 // C[M x N] += A[K x M]^T B[K x N]  (weight gradients; contraction over points, split over gridDim.z), row-major operands.
 // grid = (ceil(M/128), ceil(N/128), splits).  Epi is the caller's epilogue with one split, EpiSplitStore into the split-K
 // workspace with several.  colsum (optional): colsum[m] += sum_k A[k, m], the bias gradient, from the fp32 values the A
-// stagers read anyway; one writer per column and split (cs_ws: [split][M], or the output itself with one split).
-// Both paths keep each column's sum in the same order: per k-quarter partials (points 8q + 2kq, 8q + 2kq + 1 of each
-// 64 points, pairs added first, in point order), then (q0 + q1) + (q2 + q3).
+// split reads anyway; one writer per column and split (cs_ws: [split][M], or the output itself with one split).  Each
+// column's sum has a fixed order: per k-quarter partials (points 8q + 2kq, 8q + 2kq + 1 of each 64 points, pairs added
+// first, in point order), then (q0 + q1) + (q2 + q3).
 //
-// RING (row strides a multiple of 4 floats and 16-byte-aligned bases, as 2-D tensor maps need): the operands reach
-// shared memory as they lie in HBM.  One thread issues a 2-D TMA copy per operand and slice (a [TN_PS points x 128
-// columns] fp32 box, 16 KB; columns past M / N and points past K arrive as zeros) into a TN_RING-deep ring on an
-// mbarrier, and refills a stage as soon as the barrier after its split has passed: up to TN_RING - 1 slices are in
-// flight per CTA beyond the one being split, in no registers.  While the wgmma group of slice i runs, all threads split
-// slice i + 1 into the free MN-major plane stage (warps 0-3 A, warps 4-7 B; warp w takes k-quarter kq = w & 3 of each 8
-// points, lane l columns 4l..4l+3), and the wgmma reads both operands with its transpose flags set.  Points of the
+// The operands reach shared memory as they lie in HBM.  One thread issues a 2-D TMA copy per operand and slice (a
+// [TN_PS points x 128 columns] fp32 box, 16 KB; columns past M / N and points past K arrive as zeros) into a TN_RING-deep
+// ring on an mbarrier, and refills a stage as soon as the barrier after its split has passed: up to TN_RING - 1 slices
+// are in flight per CTA beyond the one being split, in no registers.  While the wgmma group of slice i runs, all threads
+// split slice i + 1 into the free MN-major plane stage (warps 0-3 A, warps 4-7 B; warp w takes k-quarter kq = w & 3 of
+// each 8 points, lane l columns 4l..4l+3), and the wgmma reads both operands with its transpose flags set.  Points of the
 // last slice past the chunk end (the next chunk's) are split as zeros.
-// Otherwise warps 0-3 stage the [128 x 64] A^T slice, warps 4-7 the B^T slice (fetch_block_t / store_block_t), K-major.
-// Slice i + 1 waits in registers while the tensor cores work on slice i: iteration i issues the wgmma group of slice i,
-// splits slice i + 1 into the free stage, issues the loads of slice i + 2, then waits for the group.
 // ---------------------------------------------------------------------------------------------------------------
-template <class Epi, bool RING>
+template <class Epi>
 __global__ void __launch_bounds__(THREADS, 1)
-gemm_tn_kernel(const float* __restrict__ A, int64_t lda, const float* __restrict__ B, int64_t ldb, int M, int N, int64_t K, int64_t k_chunk,
-               Epi epi, float* __restrict__ colsum, float* __restrict__ cs_ws, const __grid_constant__ TnMaps maps) {
+gemm_tn_kernel(int M, int N, int64_t K, int64_t k_chunk, Epi epi, float* __restrict__ colsum, float* __restrict__ cs_ws,
+               const __grid_constant__ TnMaps maps) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = align1024(smem_raw);
   const int tid = threadIdx.x, wg = tid >> 7, warp = tid >> 5, lane = tid & 31;
@@ -890,146 +717,85 @@ gemm_tn_kernel(const float* __restrict__ A, int64_t lda, const float* __restrict
   float acc[64];
 #pragma unroll
   for (int q = 0; q < 64; ++q) acc[q] = 0.f;
-  if constexpr (RING) {
-    uint8_t* ring = smem;
-    uint8_t* planes = smem + TN_RING * TN_F32_STAGE;
-    float* cs_part = reinterpret_cast<float*>(planes + 2 * TN_PLANE_STAGE);   // [4 k-quarters][128 columns]
-    uint64_t* full = reinterpret_cast<uint64_t*>(cs_part + 4 * BM);
-    const int n_sl = (int)((ke - kb + TN_PS - 1) / TN_PS);
-    const int opnd = warp >> 2, kq = warp & 3;
+  uint8_t* ring = smem;
+  uint8_t* planes = smem + TN_RING * TN_F32_STAGE;
+  float* cs_part = reinterpret_cast<float*>(planes + 2 * TN_PLANE_STAGE);   // [4 k-quarters][128 columns]
+  uint64_t* full = reinterpret_cast<uint64_t*>(cs_part + 4 * BM);
+  const int n_sl = (int)((ke - kb + TN_PS - 1) / TN_PS);
+  const int opnd = warp >> 2, kq = warp & 3;
 
-    auto issue = [&](int i) {                               // one thread: slice i into ring stage i % TN_RING
-      const int r = i % TN_RING;
-      const int k0 = (int)(kb + (int64_t)i * TN_PS);
-      uint8_t* st = ring + r * TN_F32_STAGE;
-      mbar_arrive_expect_tx(&full[r], TN_F32_STAGE);
-      tma_load_2d(st, &maps.a, m0, k0, &full[r]);
-      tma_load_2d(st + TN_F32_OPND, &maps.b, n0, k0, &full[r]);
-    };
-    // slice i from the ring into the plane stage dst.  Shared-memory traffic without bank conflicts: a warp's float4
-    // reads cover one point's 512 contiguous bytes, and each half-warp's 8-byte plane stores cover all 8 16-byte chunks
-    // of one 128-byte swizzled row (64 columns of one point), i.e. all 32 banks once.
-    auto split = [&](int i, uint8_t* dst) {
-      const int r = i % TN_RING;
-      mbar_wait(&full[r], (uint32_t)((i / TN_RING) & 1));
-      const float* f = reinterpret_cast<const float*>(ring + r * TN_F32_STAGE + opnd * TN_F32_OPND) + 4 * lane;
-      uint8_t* hi = dst + opnd * 2 * TN_PLANE;
-      const int64_t k0 = kb + (int64_t)i * TN_PS;
+  auto issue = [&](int i) {                               // one thread: slice i into ring stage i % TN_RING
+    const int r = i % TN_RING;
+    const int k0 = (int)(kb + (int64_t)i * TN_PS);
+    uint8_t* st = ring + r * TN_F32_STAGE;
+    mbar_arrive_expect_tx(&full[r], TN_F32_STAGE);
+    tma_load_2d(st, &maps.a, m0, k0, &full[r]);
+    tma_load_2d(st + TN_F32_OPND, &maps.b, n0, k0, &full[r]);
+  };
+  // slice i from the ring into the plane stage dst.  Shared-memory traffic without bank conflicts: a warp's float4
+  // reads cover one point's 512 contiguous bytes, and each half-warp's 8-byte plane stores cover all 8 16-byte chunks
+  // of one 128-byte swizzled row (64 columns of one point), i.e. all 32 banks once.
+  auto split = [&](int i, uint8_t* dst) {
+    const int r = i % TN_RING;
+    mbar_wait(&full[r], (uint32_t)((i / TN_RING) & 1));
+    const float* f = reinterpret_cast<const float*>(ring + r * TN_F32_STAGE + opnd * TN_F32_OPND) + 4 * lane;
+    uint8_t* hi = dst + opnd * 2 * TN_PLANE;
+    const int64_t k0 = kb + (int64_t)i * TN_PS;
 #pragma unroll
-      for (int q = 0; q < TN_PS / 8; ++q) {
-        float4 v[2];
+    for (int q = 0; q < TN_PS / 8; ++q) {
+      float4 v[2];
 #pragma unroll
-        for (int kk = 0; kk < 2; ++kk) {
-          const int p = 8 * q + 2 * kq + kk;
-          v[kk] = k0 + p < ke ? *reinterpret_cast<const float4*>(f + p * BM) : make_float4(0.f, 0.f, 0.f, 0.f);
-        }
-        if (opnd == 0 && do_csum) {
-          csum[0] += v[0].x + v[1].x; csum[1] += v[0].y + v[1].y;
-          csum[2] += v[0].z + v[1].z; csum[3] += v[0].w + v[1].w;
-        }
-#pragma unroll
-        for (int kk = 0; kk < 2; ++kk) {
-          const float x[4] = {v[kk].x, v[kk].y, v[kk].z, v[kk].w};
-          uint2 pl[2];
-          split4<2>(x, pl);
-          const uint32_t off = sw128_mn(4u * lane, (uint32_t)(8 * q + 2 * kq + kk));
-          *reinterpret_cast<uint2*>(hi + off) = pl[0];
-          *reinterpret_cast<uint2*>(hi + TN_PLANE + off) = pl[1];
-        }
+      for (int kk = 0; kk < 2; ++kk) {
+        const int p = 8 * q + 2 * kq + kk;
+        v[kk] = k0 + p < ke ? *reinterpret_cast<const float4*>(f + p * BM) : make_float4(0.f, 0.f, 0.f, 0.f);
       }
-    };
-    if (tid == 0) {
-      for (int r = 0; r < TN_RING; ++r) mbar_init(&full[r], 1);
-      fence_barrier_init();
-      for (int i = 0; i < TN_RING && i < n_sl; ++i) issue(i);
-    }
-    __syncthreads();
-    split(0, planes);
-    fence_proxy_async();
-    __syncthreads();
-    if (tid == 0 && TN_RING < n_sl) issue(TN_RING);         // slice 0's ring stage is split
-    for (int i = 0; i < n_sl; ++i) {
-      const int s = i & 1;
-      const uint32_t st = smem_u32(planes + s * TN_PLANE_STAGE);
-      wg_fence();
-      mma_slice_mn(acc, st + wg * 4096u, st + 2 * TN_PLANE, i == 0);
-      wg_commit();
-      if (i + 1 < n_sl) split(i + 1, planes + (s ^ 1) * TN_PLANE_STAGE);   // released by the wait + barrier of i - 1
-      wg_wait_all();
-      fence_proxy_async();
-      __syncthreads();
-      if (tid == 0 && i + 1 + TN_RING < n_sl) issue(i + 1 + TN_RING);     // slice i + 1's ring stage is split
-    }
-    if (do_csum && opnd == 0)
-#pragma unroll
-      for (int j = 0; j < 4; ++j) cs_part[kq * BM + 4 * lane + j] = csum[j];
-  } else {
-    int rows_b = N - n0; rows_b = pad16(rows_b < BN ? rows_b : BN);
-    const int n_sl = (int)((ke - kb + BK - 1) / BK);
-    constexpr uint32_t stage_bytes = 2u * A_HALF_BYTES + 2u * B_HALF_BYTES;
-    const bool a_vec = ((lda & 3) == 0) && aligned16(A) && ((m0 & 3) == 0);
-    const bool b_vec = ((ldb & 3) == 0) && aligned16(B);
-    const bool b_warp = warp >= 4 && 32 * (warp - 4) < rows_b;
-    float4 v[8][2];                                         // this thread's part of the next K slice
-
-    auto fetch = [&](int i) {                               // K slice i into v
-      const int64_t k0 = kb + (int64_t)i * BK;
-      if (warp < 4) fetch_block_t(A, lda, m0, M, 32 * warp, BM, k0, ke, lane, a_vec, v);
-      else if (b_warp) fetch_block_t(B, ldb, n0, N, 32 * (warp - 4), rows_b, k0, ke, lane, b_vec, v);
-    };
-    auto store = [&](uint8_t* st) {                         // v into stage st
-      if (warp < 4) {
-        if (do_csum) store_block_t<true>(v, 32 * warp, BM, st, st + A_HALF_BYTES, lane, csum);
-        else store_block_t(v, 32 * warp, BM, st, st + A_HALF_BYTES, lane);
-      } else if (b_warp) {
-        store_block_t(v, 32 * (warp - 4), rows_b, st + 2 * A_HALF_BYTES, st + 2 * A_HALF_BYTES + B_HALF_BYTES, lane);
+      if (opnd == 0 && do_csum) {
+        csum[0] += v[0].x + v[1].x; csum[1] += v[0].y + v[1].y;
+        csum[2] += v[0].z + v[1].z; csum[3] += v[0].w + v[1].w;
       }
-    };
-    fetch(0);
-    store(smem);
-    if (n_sl > 1) fetch(1);
-    fence_proxy_async();
-    __syncthreads();
-    for (int i = 0; i < n_sl; ++i) {
-      const int s = i & 1;
-      const uint32_t st = smem_u32(smem + s * stage_bytes);
-      wg_fence();
-      mma_slice<2, BN>(acc, st + wg * (64 * 128), A_HALF_BYTES, st + 2 * A_HALF_BYTES, B_HALF_BYTES, i == 0);
-      wg_commit();
-      if (i + 1 < n_sl) {
-        store(smem + (s ^ 1) * stage_bytes);                // stage s ^ 1 was released by the wait + barrier of i - 1
-        if (i + 2 < n_sl) fetch(i + 2);
-      }
-      wg_wait_all();
-      fence_proxy_async();
-      __syncthreads();
-    }
-    if (do_csum && warp < 4) {                              // lanes (mq, kq): reduce over the 4 kq lanes
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        csum[j] += __shfl_xor_sync(0xffffffffu, csum[j], 8);
-        csum[j] += __shfl_xor_sync(0xffffffffu, csum[j], 16);
+      for (int kk = 0; kk < 2; ++kk) {
+        const float x[4] = {v[kk].x, v[kk].y, v[kk].z, v[kk].w};
+        uint2 pl[2];
+        split4<2>(x, pl);
+        const uint32_t off = sw128_mn(4u * lane, (uint32_t)(8 * q + 2 * kq + kk));
+        *reinterpret_cast<uint2*>(hi + off) = pl[0];
+        *reinterpret_cast<uint2*>(hi + TN_PLANE + off) = pl[1];
       }
-      const int m = m0 + 32 * warp + 4 * (lane & 7);
-      if ((lane >> 3) == 0)
-#pragma unroll
-        for (int j = 0; j < 4; ++j)
-          if (m + j < M) {
-            if (cs_ws != nullptr) cs_ws[(int64_t)blockIdx.z * M + m + j] = csum[j];
-            else colsum[m + j] += csum[j];
-          }
     }
+  };
+  if (tid == 0) {
+    for (int r = 0; r < TN_RING; ++r) mbar_init(&full[r], 1);
+    fence_barrier_init();
+    for (int i = 0; i < TN_RING && i < n_sl; ++i) issue(i);
   }
-  float* acc_s = reinterpret_cast<float*>(smem);            // the operand stages (or the ring: every copy has landed)
+  __syncthreads();
+  split(0, planes);
+  fence_proxy_async();
+  __syncthreads();
+  if (tid == 0 && TN_RING < n_sl) issue(TN_RING);         // slice 0's ring stage is split
+  for (int i = 0; i < n_sl; ++i) {
+    const int s = i & 1;
+    const uint32_t st = smem_u32(planes + s * TN_PLANE_STAGE);
+    wg_fence();
+    mma_slice_mn(acc, st + wg * 4096u, st + 2 * TN_PLANE, i == 0);
+    wg_commit();
+    if (i + 1 < n_sl) split(i + 1, planes + (s ^ 1) * TN_PLANE_STAGE);   // released by the wait + barrier of i - 1
+    wg_wait_all();
+    fence_proxy_async();
+    __syncthreads();
+    if (tid == 0 && i + 1 + TN_RING < n_sl) issue(i + 1 + TN_RING);     // slice i + 1's ring stage is split
+  }
+  if (do_csum && opnd == 0)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) cs_part[kq * BM + 4 * lane + j] = csum[j];
+  float* acc_s = reinterpret_cast<float*>(smem);            // the ring: every copy has landed
   acc_to_smem<BN>(acc, acc_s, wg, tid & 127);
   __syncthreads();
-  if constexpr (RING) {
-    const float* cs_part = reinterpret_cast<const float*>(smem + TN_RING * TN_F32_STAGE + 2 * TN_PLANE_STAGE);
-    if (do_csum && tid < BM && m0 + tid < M) {
-      const float c = (cs_part[tid] + cs_part[BM + tid]) + (cs_part[2 * BM + tid] + cs_part[3 * BM + tid]);
-      if (cs_ws != nullptr) cs_ws[(int64_t)blockIdx.z * M + m0 + tid] = c;
-      else colsum[m0 + tid] += c;
-    }
+  if (do_csum && tid < BM && m0 + tid < M) {
+    const float c = (cs_part[tid] + cs_part[BM + tid]) + (cs_part[2 * BM + tid] + cs_part[3 * BM + tid]);
+    if (cs_ws != nullptr) cs_ws[(int64_t)blockIdx.z * M + m0 + tid] = c;
+    else colsum[m0 + tid] += c;
   }
   tile_epilogue<BN>(acc_s, m0, M, n0, N, epi, tid);
 }
@@ -1071,31 +837,38 @@ static inline int tensor_map_2d(CUtensorMap* map, const float* X, int64_t ld, in
   }
   return 0;
 }
-// 2 stages x NP planes of the A and weight slices; the [128 x acc_ld(WN)] fp32 accumulator tile reuses them
-constexpr size_t w_smem_bytes(int np, int wn) { return 2 * (size_t)np * (A_HALF_BYTES + b_plane_bytes(wn)) + 2 * sizeof(uint64_t) + 1024; }
-static_assert(BM * acc_ld(2 * BN) * sizeof(float) <= 2 * 2 * (size_t)(A_HALF_BYTES + b_plane_bytes(2 * BN)), "accumulator tile");
-// the ring path: w_ring(wn) fp32 slots, 2 weight stages of 2 planes, a barrier per slot and per stage; the accumulator
+// An activation operand of the tensor-core kernels is read through a 2-D tensor map, which needs a row stride of whole
+// 16-byte units and a 16-byte-aligned base.  The networks' layouts guarantee both (udf_net.cu, mlp_nets.cu); the
+// stand-alone entry points repack an operand that lacks them (gemm_tc.cu).
+static inline bool tma_operand_ok(const float* X, int64_t ld) { return (ld & 3) == 0 && aligned16(X); }
+static inline int check_tma_operand(const float* X, int64_t ld) {
+  if (tma_operand_ok(X, ld)) return 0;
+  nudf::set_error("tensor-core operand at %p with row stride %lld floats: needs a stride of a multiple of 4 floats and a "
+                  "16-byte-aligned base", (const void*)X, (long long)ld);
+  return -1;
+}
+
+// gemm_w_kernel: w_ring(wn) fp32 slots, 2 weight stages of 2 planes, a barrier per slot and per stage; the accumulator
 // tile reuses the slots and stages
 constexpr size_t w_ring_operand_bytes(int wn) { return (size_t)w_ring(wn) * W_SLOT + 2 * 2 * (size_t)b_plane_bytes(wn); }
 constexpr size_t w_ring_smem_bytes(int wn) { return w_ring_operand_bytes(wn) + (w_ring(wn) + 2) * sizeof(uint64_t) + 1024; }
 static_assert(w_ring_smem_bytes(BN) <= 227 * 1024 && w_ring_smem_bytes(2 * BN) <= 227 * 1024, "one CTA per SM");
-static_assert(BM * acc_ld(BN) * sizeof(float) <= w_ring_operand_bytes(BN), "accumulator tile in the ring path's stages");
-static_assert(BM * acc_ld(2 * BN) * sizeof(float) <= w_ring_operand_bytes(2 * BN), "accumulator tile in the ring path's stages");
+static_assert(BM * acc_ld(BN) * sizeof(float) <= w_ring_operand_bytes(BN), "accumulator tile in the slots and stages");
+static_assert(BM * acc_ld(2 * BN) * sizeof(float) <= w_ring_operand_bytes(2 * BN), "accumulator tile in the slots and stages");
 
-template <int NP, int WN, class Epi, bool RING>
+template <int WN, class Epi>
 static inline int gemm_w_launch(const float* A, int64_t lda, int64_t M, int N, int K, const uint16_t* img, const Epi& epi, cudaStream_t st) {
-  constexpr size_t smem = RING ? w_ring_smem_bytes(WN) : w_smem_bytes(NP, WN);
+  constexpr size_t smem = w_ring_smem_bytes(WN);
   static bool attr_set = false;   // per template instantiation
   if (!attr_set) {
-    NUDF_CUDA_OK(cudaFuncSetAttribute(gemm_w_kernel<NP, WN, Epi, RING>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    NUDF_CUDA_OK(cudaFuncSetAttribute(gemm_w_kernel<WN, Epi>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr_set = true;
   }
   CUtensorMap amap{};
-  if constexpr (RING)
-    if (int rc = tensor_map_2d(&amap, A, lda, K, M, BK, BM)) return rc;
+  if (int rc = tensor_map_2d(&amap, A, lda, K > 0 ? K : 1, M, BK, BM)) return rc;   // K = 0: a map no copy reads
   const unsigned grid = (unsigned)(cdiv(M, BM) * cdiv(N, WN));
   LaunchTimer lt_(epi_family<Epi>::value, st);
-  gemm_w_kernel<NP, WN, Epi, RING><<<grid, THREADS, smem, st>>>(A, lda, M, N, K, img, epi, amap);
+  gemm_w_kernel<WN, Epi><<<grid, THREADS, smem, st>>>(M, N, K, img, epi, amap);
   NUDF_LAUNCH_OK();
   return 0;
 }
@@ -1120,25 +893,19 @@ static inline int gemm_w3_tma_launch(const float* A, int64_t lda, int64_t M, int
   NUDF_LAUNCH_OK();
   return 0;
 }
-// The activation path follows from the operand: when the row stride is a multiple of 4 floats and the base is 16-byte
-// aligned (a 2-D tensor map needs both; every operand the networks pass has them), 2-plane layers take the ring and
-// 3-plane layers gemm_w3_tma_kernel; any other operand takes the register path.
-template <int NP, int WN, class Epi>
-static inline int gemm_w_path(const float* A, int64_t lda, int64_t M, int N, int K, const uint16_t* img, const Epi& epi, cudaStream_t st) {
-  if (K > 0 && (lda & 3) == 0 && aligned16(A)) {
-    if constexpr (NP == 2) return gemm_w_launch<2, WN, Epi, true>(A, lda, M, N, K, img, epi, st);
-    else return gemm_w3_tma_launch<Epi>(A, lda, M, N, K, img, epi, st);
-  }
-  return gemm_w_launch<NP, WN, Epi, false>(A, lda, M, N, K, img, epi, st);
-}
-// The output width per CTA follows from the shape: 256 columns for 2-plane layers wider than 128 (one read and split of
-// each activation row block instead of two), 128 otherwise (3 planes, and 2-plane layers of at most 128 columns).
+// 2-plane layers run gemm_w_kernel, 256 columns per CTA when wider than 128 (one read and split of each activation row
+// block instead of two), 128 otherwise; 3-plane layers run gemm_w3_tma_kernel, which needs K > 0.
 template <int NP, class Epi>
 static inline int gemm_w(const float* A, int64_t lda, int64_t M, int N, int K, const uint16_t* img, const Epi& epi, cudaStream_t st) {
   if (M <= 0 || N <= 0) return 0;
-  if constexpr (NP == 2)
-    if (N > BN) return gemm_w_path<2, 2 * BN, Epi>(A, lda, M, N, K, img, epi, st);
-  return gemm_w_path<NP, BN, Epi>(A, lda, M, N, K, img, epi, st);
+  if (int rc = check_tma_operand(A, lda)) return rc;
+  if constexpr (NP == 3) {
+    NUDF_REQUIRE(K > 0, "3-plane layers need K > 0");
+    return gemm_w3_tma_launch<Epi>(A, lda, M, N, K, img, epi, st);
+  } else {
+    if (N > BN) return gemm_w_launch<2 * BN, Epi>(A, lda, M, N, K, img, epi, st);
+    return gemm_w_launch<BN, Epi>(A, lda, M, N, K, img, epi, st);
+  }
 }
 
 // The split of a weight-gradient contraction over its points (split-K), from the shape alone: the same inputs give the
@@ -1155,27 +922,23 @@ static inline int64_t tn_k_chunk(int M, int N, int64_t K) {
   return round_up(cdiv(K, splits), BK);
 }
 
-constexpr size_t TN_SMEM = 2 * (size_t)(2 * A_HALF_BYTES + 2 * B_HALF_BYTES) + 2 * sizeof(uint64_t) + 1024;
-// the ring path: the fp32 ring, 2 plane stages, the k-quarter column-sum partials and one mbarrier per ring stage
+// the fp32 ring, 2 plane stages, the k-quarter column-sum partials and one mbarrier per ring stage
 constexpr size_t TN_RING_SMEM = (size_t)TN_RING * TN_F32_STAGE + 2 * TN_PLANE_STAGE + 4 * BM * sizeof(float) + TN_RING * sizeof(uint64_t) + 1024;
 static_assert(BM * acc_ld(BN) * sizeof(float) <= (size_t)TN_RING * TN_F32_STAGE, "accumulator tile in the ring");
 static_assert(TN_RING_SMEM <= 227 * 1024, "one CTA per SM");
 
-template <class Epi, bool RING>
+template <class Epi>
 static inline int gemm_tn_launch(dim3 grid, const float* A, int64_t lda, const float* B, int64_t ldb, int M, int N, int64_t K,
                                  int64_t k_chunk, const Epi& epi, float* colsum, float* cs_ws, cudaStream_t st) {
-  constexpr size_t smem = RING ? TN_RING_SMEM : TN_SMEM;
   static bool attr_set = false;   // per template instantiation
   if (!attr_set) {
-    NUDF_CUDA_OK(cudaFuncSetAttribute(gemm_tn_kernel<Epi, RING>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    NUDF_CUDA_OK(cudaFuncSetAttribute(gemm_tn_kernel<Epi>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TN_RING_SMEM));
     attr_set = true;
   }
   TnMaps maps{};
-  if constexpr (RING) {
-    if (int rc = tensor_map_2d(&maps.a, A, lda, M, K, BM, TN_PS)) return rc;
-    if (int rc = tensor_map_2d(&maps.b, B, ldb, N, K, BN, TN_PS)) return rc;
-  }
-  gemm_tn_kernel<Epi, RING><<<grid, THREADS, smem, st>>>(A, lda, B, ldb, M, N, K, k_chunk, epi, colsum, cs_ws, maps);
+  if (int rc = tensor_map_2d(&maps.a, A, lda, M, K, BM, TN_PS)) return rc;
+  if (int rc = tensor_map_2d(&maps.b, B, ldb, N, K, BN, TN_PS)) return rc;
+  gemm_tn_kernel<Epi><<<grid, THREADS, TN_RING_SMEM, st>>>(M, N, K, k_chunk, epi, colsum, cs_ws, maps);
   NUDF_LAUNCH_OK();
   return 0;
 }
@@ -1184,24 +947,19 @@ template <class Epi>
 static inline int gemm_tn(const float* A, int64_t lda, const float* B, int64_t ldb, int M, int N, int64_t K, const Epi& epi,
                           cudaStream_t st, float* colsum_a = nullptr) {
   if (M <= 0 || N <= 0 || K <= 0) return 0;
+  if (int rc = check_tma_operand(A, lda)) return rc;
+  if (int rc = check_tma_operand(B, ldb)) return rc;
   const int64_t k_chunk = tn_k_chunk(M, N, K);
   const int splits = (int)cdiv(K, k_chunk);
   dim3 grid((unsigned)cdiv(M, BM), (unsigned)cdiv(N, BN), (unsigned)splits);
   LaunchTimer lt_(FAM_TC_WGRAD, st);
-  // the ring path's tensor maps need row strides of whole 16-byte units and 16-byte-aligned bases
-  const bool ring = (lda & 3) == 0 && (ldb & 3) == 0 && aligned16(A) && aligned16(B);
-  if (splits == 1) {
-    if (ring) return gemm_tn_launch<Epi, true>(grid, A, lda, B, ldb, M, N, K, k_chunk, epi, colsum_a, nullptr, st);
-    return gemm_tn_launch<Epi, false>(grid, A, lda, B, ldb, M, N, K, k_chunk, epi, colsum_a, nullptr, st);
-  }
+  if (splits == 1) return gemm_tn_launch(grid, A, lda, B, ldb, M, N, K, k_chunk, epi, colsum_a, nullptr, st);
   // deterministic split-K (gemm_simt.cuh): partial tiles and column sums go to the workspace, summed in split order
   float* ws = split_workspace(st);
   if (ws == nullptr) return -2;
   float* cs = ws + (int64_t)splits * M * N;
   const EpiSplitStore e{ws, (int64_t)M * N, N};
-  if (int rc = ring ? gemm_tn_launch<EpiSplitStore, true>(grid, A, lda, B, ldb, M, N, K, k_chunk, e, colsum_a, cs, st)
-                    : gemm_tn_launch<EpiSplitStore, false>(grid, A, lda, B, ldb, M, N, K, k_chunk, e, colsum_a, cs, st))
-    return rc;
+  if (int rc = gemm_tn_launch(grid, A, lda, B, ldb, M, N, K, k_chunk, e, colsum_a, cs, st)) return rc;
   if (int rc = splitk_reduce(ws, splits, M, N, epi, st)) return rc;
   return colsum_a != nullptr ? vec_reduce(cs, splits, M, colsum_a, st) : 0;
 }

@@ -238,7 +238,7 @@ struct ColorPlan {
   int n_lin, F, H, d_out, n_blend, Lv, d_view;
   DenseLayer stack[2][NUDF_MAX_LAYERS];        // [BASE] and [MAIN], n_lin layers each
   int64_t w_total, b_total, img_total;
-  int ld_xb, ld_xm, ld_ym, c_cb, c_hid;
+  int ld_xb, ld_xm, ld_ym, ld_h, c_cb, c_hid;   // ld_h: row stride of the hidden activations and their gradients
 };
 
 // wfold (optional): the folded buffer the layers' weights and images are read from
@@ -269,6 +269,7 @@ static int color_plan(const nudf_color_desc* d, ColorPlan* p, const float* wfold
   p->ld_xb = (int)round_up(3 + p->F, 4);
   p->ld_xm = (int)round_up(p->stack[MAIN][0].n_in, 4);
   p->ld_ym = (int)round_up(p->d_out + p->n_blend, 4);
+  p->ld_h = (int)round_up(p->H, 4);
   p->c_cb = p->d_view; p->c_hid = p->d_view + p->d_out;
   return 0;
 }
@@ -277,9 +278,9 @@ struct ColorCtx { int64_t xb, hb[NUDF_MAX_LAYERS], xm, hm[NUDF_MAX_LAYERS], ym, 
 static void color_ctx_layout(const ColorPlan& p, int64_t P, ColorCtx* c) {
   Bump b;
   c->xb = b.take(P * p.ld_xb);
-  for (int l = 1; l <= p.n_lin - 2; ++l) c->hb[l] = b.take(P * p.H);   // outputs of base layers 0..n_lin-3
+  for (int l = 1; l <= p.n_lin - 2; ++l) c->hb[l] = b.take(P * p.ld_h);   // outputs of base layers 0..n_lin-3
   c->xm = b.take(P * p.ld_xm);
-  for (int l = 1; l <= p.n_lin - 1; ++l) c->hm[l] = b.take(P * p.H);   // outputs of main layers 0..n_lin-2
+  for (int l = 1; l <= p.n_lin - 1; ++l) c->hm[l] = b.take(P * p.ld_h);   // outputs of main layers 0..n_lin-2
   c->ym = b.take(P * p.ld_ym);
   c->cs = b.take(P * 4);
   c->total = b.off;
@@ -287,7 +288,7 @@ static void color_ctx_layout(const ColorPlan& p, int64_t P, ColorCtx* c) {
 struct ColorScratch { int64_t buf[2], dym, dyb, dcbx, total; };
 static void color_scratch_layout(const ColorPlan& p, int64_t P, ColorScratch* s) {
   Bump b;
-  s->buf[0] = b.take(P * p.H); s->buf[1] = b.take(P * p.H);
+  s->buf[0] = b.take(P * p.ld_h); s->buf[1] = b.take(P * p.ld_h);
   s->dym = b.take(P * p.ld_ym); s->dyb = b.take(P * 4); s->dcbx = b.take(P * 4);
   s->total = b.off;
 }
@@ -362,6 +363,7 @@ int nudf_color_forward(const nudf_color_desc* d, const float* wfold, const float
   if (int rc = color_plan(d, &p, wfold)) return rc;
   if (P <= 0) return 0;
   NUDF_REQUIRE(wfold && pts && dirs && feat && ctx, "null pointer");
+  NUDF_REQUIRE(aligned16(ctx), "ctx must be 16-byte aligned");
   NUDF_REQUIRE(ld_feat >= p.F, "ld_feat too small");
   cudaStream_t st = (cudaStream_t)stream;
   const int spr = samples_per_ray > 0 ? samples_per_ray : 1;
@@ -377,10 +379,10 @@ int nudf_color_forward(const nudf_color_desc* d, const float* wfold, const float
   // base stack
   for (int l = 0; l < nl; ++l) {
     const float* X = l == 0 ? xb : (l == nl - 1 ? xm + p.c_hid : ctx + c.hb[l]);
-    int64_t ldx = l == 0 ? p.ld_xb : (l == nl - 1 ? p.ld_xm : p.H);
+    int64_t ldx = l == 0 ? p.ld_xb : (l == nl - 1 ? p.ld_xm : p.ld_h);
     EpiAct e;
     e.bias = p.stack[BASE][l].bias; e.post_scale = 1.0f;
-    if (l < nl - 2) { e.C = ctx + c.hb[l + 1]; e.ldc = p.H; e.act = ACT_RELU; }
+    if (l < nl - 2) { e.C = ctx + c.hb[l + 1]; e.ldc = p.ld_h; e.act = ACT_RELU; }
     else if (l == nl - 2) { e.C = xm + p.c_hid; e.ldc = p.ld_xm; e.act = ACT_RELU; }      // x_hidden (fields.py:472-473)
     else { e.C = xm + p.c_cb; e.ldc = p.ld_xm; e.act = ACT_SIGMOID; }                      // color_base (:475-476)
     if (int rc = color_layer_forward(p.stack[BASE][l], X, ldx, P, e, st)) return rc;
@@ -392,10 +394,10 @@ int nudf_color_forward(const nudf_color_desc* d, const float* wfold, const float
   // main stack
   for (int l = 0; l < nl; ++l) {
     const float* X = l == 0 ? xm : ctx + c.hm[l];
-    int64_t ldx = l == 0 ? p.ld_xm : p.H;
+    int64_t ldx = l == 0 ? p.ld_xm : p.ld_h;
     EpiAct e;
     e.bias = p.stack[MAIN][l].bias; e.post_scale = 1.0f;
-    if (l < nl - 1) { e.C = ctx + c.hm[l + 1]; e.ldc = p.H; e.act = ACT_RELU; }
+    if (l < nl - 1) { e.C = ctx + c.hm[l + 1]; e.ldc = p.ld_h; e.act = ACT_RELU; }
     else { e.C = ctx + c.ym; e.ldc = p.ld_ym; e.act = ACT_NONE; }
     if (int rc = color_layer_forward(p.stack[MAIN][l], X, ldx, P, e, st)) return rc;
   }
@@ -411,6 +413,7 @@ int nudf_color_backward(const nudf_color_desc* d, const float* wfold, int64_t P,
   ColorPlan p;
   if (int rc = color_plan(d, &p, wfold)) return rc;
   NUDF_REQUIRE(wfold && ctx_c && scratch && dwfold && dbias, "null pointer");
+  NUDF_REQUIRE(aligned16(ctx_c) && aligned16(scratch), "ctx and scratch must be 16-byte aligned");
   cudaStream_t st = (cudaStream_t)stream;
   NUDF_CUDA_OK(cudaMemsetAsync(dwfold, 0, sizeof(float) * p.w_total, st));
   NUDF_CUDA_OK(cudaMemsetAsync(dbias, 0, sizeof(float) * p.b_total, st));
@@ -432,17 +435,17 @@ int nudf_color_backward(const nudf_color_desc* d, const float* wfold, int64_t P,
   for (int l = nl - 1; l >= 0; --l) {
     const DenseLayer& L = p.stack[MAIN][l];
     const float* X = l == 0 ? xm : ctx + c.hm[l];
-    int64_t ldx = l == 0 ? p.ld_xm : p.H;
+    int64_t ldx = l == 0 ? p.ld_xm : p.ld_h;
     if (int rc = wgrad(L, dz, ldz, X, ldx, P, dwfold + L.w_off, dbias + L.b_off, st)) return rc;
     float* out = scratch + s.buf[flip];
     if (l >= 1) {
-      EpiReluBwd e{0, p.H, ctx + c.hm[l], p.H, out, p.H, 0};
+      EpiReluBwd e{0, p.H, ctx + c.hm[l], p.ld_h, out, p.ld_h, 0};
       if (int rc = layer_nn(L, dz, ldz, P, e, TC_COLOR, st)) return rc;
     } else {
-      EpiColorMainIn e{p.c_cb, p.c_hid, L.n_in, scratch + s.dcbx, 4, xm + p.c_hid, p.ld_xm, out, p.H};
+      EpiColorMainIn e{p.c_cb, p.c_hid, L.n_in, scratch + s.dcbx, 4, xm + p.c_hid, p.ld_xm, out, p.ld_h};
       if (int rc = layer_nn(L, dz, ldz, P, e, TC_COLOR, st)) return rc;
     }
-    dz = out; ldz = p.H; flip ^= 1;
+    dz = out; ldz = p.ld_h; flip ^= 1;
   }
   // dz now = masked d(pre-activation of base layer nl-2) coming through the main stack, living in buf[flip^1]
   float* dzb = const_cast<float*>(dz);
@@ -454,18 +457,18 @@ int nudf_color_backward(const nudf_color_desc* d, const float* wfold, int64_t P,
   {
     const DenseLayer& L = p.stack[BASE][nl - 1];       // colour_base head: K = d_out <= 4, no image, the FFMA kernel
     if (int rc = wgrad(L, dyb, 4, xm + p.c_hid, p.ld_xm, P, dwfold + L.w_off, dbias + L.b_off, st)) return rc;
-    EpiReluBwd e{0, p.H, xm + p.c_hid, p.ld_xm, dzb, p.H, 1};
+    EpiReluBwd e{0, p.H, xm + p.c_hid, p.ld_xm, dzb, p.ld_h, 1};
     if (int rc = layer_nn(L, dyb, 4, P, e, TC_COLOR, st)) return rc;
   }
-  dz = dzb; ldz = p.H;
+  dz = dzb; ldz = p.ld_h;
   for (int l = nl - 2; l >= 0; --l) {
     const DenseLayer& L = p.stack[BASE][l];
     const float* X = l == 0 ? ctx + c.xb : ctx + c.hb[l];
-    int64_t ldx = l == 0 ? p.ld_xb : p.H;
+    int64_t ldx = l == 0 ? p.ld_xb : p.ld_h;
     if (int rc = wgrad(L, dz, ldz, X, ldx, P, dwfold + L.w_off, dbias + L.b_off, st)) return rc;
     if (l >= 1) {
       float* out = scratch + s.buf[flip];
-      EpiReluBwd e{0, p.H, ctx + c.hb[l], p.H, out, p.H, 0};
+      EpiReluBwd e{0, p.H, ctx + c.hb[l], p.ld_h, out, p.ld_h, 0};
       if (int rc = layer_nn(L, dz, ldz, P, e, TC_COLOR, st)) return rc;
       dz = out; flip ^= 1;
     } else if (dfeat) {
@@ -501,6 +504,7 @@ namespace nudf {
 enum { VIEWS = 0, FEATURE = 1, ALPHA = 2, RGB = 3 };
 struct NerfPlan {
   int D, W, d_in, L, Lv, skip, ch, chv, ld_f, ld_x5;
+  int ld_w, ld_v;   // row strides of the W-wide hidden activations (and gradients) and of the W / 2-wide views layer
   // the D pts layers, then [D + VIEWS .. D + RGB]: the order of nudf_nerf_backward's dparams (weight, bias) pairs
   DenseLayer layer[NUDF_MAX_LAYERS + 4];
   int64_t img_total;
@@ -516,6 +520,8 @@ static int nerf_plan(const nudf_nerf_desc* d, NerfPlan* p, const float* wimg = n
   p->chv = 3 * (1 + 2 * p->Lv);
   p->ld_f = (int)round_up(p->W + p->chv, 4);
   p->ld_x5 = (int)round_up(p->W + p->ch, 4);
+  p->ld_w = (int)round_up(p->W, 4);
+  p->ld_v = (int)round_up(p->W / 2, 4);
   int64_t io = 0;
   auto set = [&](int i, const float* W, const float* b, int n_out, int n_in, int want) {
     DenseLayer& L = p->layer[i];
@@ -541,28 +547,28 @@ struct NerfCtx { int64_t e, h[NUDF_MAX_LAYERS], f, hv, total; };
 static void nerf_ctx_layout(const NerfPlan& p, int64_t P, NerfCtx* c) {
   Bump b;
   c->e = b.take(P * round_up(p.ch, 4));
-  for (int i = 0; i < p.D; ++i) c->h[i] = b.take(P * (i == p.skip ? p.ld_x5 : p.W));
+  for (int i = 0; i < p.D; ++i) c->h[i] = b.take(P * (i == p.skip ? p.ld_x5 : p.ld_w));
   c->f = b.take(P * p.ld_f);
-  c->hv = b.take(P * (p.W / 2));
+  c->hv = b.take(P * p.ld_v);
   c->total = b.off;
 }
 struct NerfScratch { int64_t buf[2], dzv, total; };
 static void nerf_scratch_layout(const NerfPlan& p, int64_t P, NerfScratch* s) {
   Bump b;
-  s->buf[0] = b.take(P * p.W); s->buf[1] = b.take(P * p.W);
-  s->dzv = b.take(P * (p.W / 2));
+  s->buf[0] = b.take(P * p.ld_w); s->buf[1] = b.take(P * p.ld_w);
+  s->dzv = b.take(P * p.ld_v);
   s->total = b.off;
 }
 // layer-i output location
 static inline float* nerf_h(const NerfPlan& p, float* ctx, const NerfCtx& c, int i, int64_t* ld) {
   if (i == p.skip) { *ld = p.ld_x5; return ctx + c.h[i] + p.ch; }
-  *ld = p.W; return ctx + c.h[i];
+  *ld = p.ld_w; return ctx + c.h[i];
 }
 // layer-i input location
 static inline const float* nerf_x(const NerfPlan& p, float* ctx, const NerfCtx& c, int i, int64_t* ld) {
   if (i == 0) { *ld = round_up(p.ch, 4); return ctx + c.e; }
   if (i - 1 == p.skip) { *ld = p.ld_x5; return ctx + c.h[i - 1]; }
-  *ld = p.W; return ctx + c.h[i - 1];
+  *ld = p.ld_w; return ctx + c.h[i - 1];
 }
 }  // namespace nudf
 
@@ -606,6 +612,7 @@ int nudf_nerf_forward(const nudf_nerf_desc* d, const float* wimg, const float* p
   if (int rc = nerf_plan(d, &p, wimg)) return rc;
   if (P <= 0) return 0;
   NUDF_REQUIRE(pts && dirs && sigma && rgb && ctx, "null pointer");
+  NUDF_REQUIRE(aligned16(ctx), "ctx must be 16-byte aligned");
   cudaStream_t st = (cudaStream_t)stream;
   const int spr = samples_per_ray > 0 ? samples_per_ray : 1;
   NerfCtx c;
@@ -635,12 +642,12 @@ int nudf_nerf_forward(const nudf_nerf_desc* d, const float* wimg, const float* p
     if (int rc = layer_nt(head[FEATURE], Hl, ldl, P, e, TC_RELU_FWD, st)) return rc;
   }
   {
-    EpiAct e{ctx + c.hv, p.W / 2, head[VIEWS].bias, ACT_RELU, 1.0f};
+    EpiAct e{ctx + c.hv, p.ld_v, head[VIEWS].bias, ACT_RELU, 1.0f};
     if (int rc = layer_nt(head[VIEWS], ctx + c.f, p.ld_f, P, e, TC_RELU_FWD, st)) return rc;
   }
   {
     EpiAct e{rgb, 3, head[RGB].bias, ACT_NONE, 1.0f};
-    if (int rc = layer_nt(head[RGB], ctx + c.hv, p.W / 2, P, e, TC_RELU_FWD, st)) return rc;
+    if (int rc = layer_nt(head[RGB], ctx + c.hv, p.ld_v, P, e, TC_RELU_FWD, st)) return rc;
   }
   return 0;
 }
@@ -650,8 +657,9 @@ int nudf_nerf_backward(const nudf_nerf_desc* d, const float* wimg, int64_t P, co
   NerfPlan p;
   if (int rc = nerf_plan(d, &p, wimg)) return rc;
   NUDF_REQUIRE(sigma_bar && rgb_bar && ctx_c && scratch && dparams, "null pointer");
+  NUDF_REQUIRE(aligned16(ctx_c) && aligned16(scratch), "ctx and scratch must be 16-byte aligned");
   cudaStream_t st = (cudaStream_t)stream;
-  const int D = p.D, W = p.W, W2 = p.W / 2;
+  const int D = p.D, W = p.W, W2 = p.W / 2, ld_w = p.ld_w, ld_v = p.ld_v;
   for (int i = 0; i < D + 4; ++i) {                        // dparams[2 i], [2 i + 1] = weight and bias gradient of layer i
     NUDF_CUDA_OK(cudaMemsetAsync(dparams[2 * i], 0, sizeof(float) * p.layer[i].n_out * p.layer[i].n_in, st));
     NUDF_CUDA_OK(cudaMemsetAsync(dparams[2 * i + 1], 0, sizeof(float) * p.layer[i].n_out, st));
@@ -665,43 +673,43 @@ int nudf_nerf_backward(const nudf_nerf_desc* d, const float* wimg, int64_t P, co
   const DenseLayer* head = p.layer + D;
   float* const* dhead = dparams + 2 * D;
   // rgb head
-  if (int rc = wgrad(head[RGB], rgb_bar, 3, ctx + c.hv, W2, P, dhead[2 * RGB], dhead[2 * RGB + 1], st)) return rc;
+  if (int rc = wgrad(head[RGB], rgb_bar, 3, ctx + c.hv, ld_v, P, dhead[2 * RGB], dhead[2 * RGB + 1], st)) return rc;
   float* dzv = scratch + s.dzv;
   {
-    EpiReluBwd e{0, W2, ctx + c.hv, W2, dzv, W2, 0};
+    EpiReluBwd e{0, W2, ctx + c.hv, ld_v, dzv, ld_v, 0};
     if (int rc = layer_nn(head[RGB], rgb_bar, 3, P, e, TC_NERF, st)) return rc;
   }
   // views layer
-  if (int rc = wgrad(head[VIEWS], dzv, W2, ctx + c.f, p.ld_f, P, dhead[2 * VIEWS], dhead[2 * VIEWS + 1], st)) return rc;
+  if (int rc = wgrad(head[VIEWS], dzv, ld_v, ctx + c.f, p.ld_f, P, dhead[2 * VIEWS], dhead[2 * VIEWS + 1], st)) return rc;
   float* dfeat = scratch + s.buf[0];
   {
-    EpiReluBwd e{0, W, nullptr, 0, dfeat, W, 0};
-    if (int rc = layer_nn(head[VIEWS], dzv, W2, P, e, TC_NERF, st)) return rc;
+    EpiReluBwd e{0, W, nullptr, 0, dfeat, ld_w, 0};
+    if (int rc = layer_nn(head[VIEWS], dzv, ld_v, P, e, TC_NERF, st)) return rc;
   }
   // feature + alpha heads -> dZ of the last pts layer
   int64_t ldl;
   const float* Hl = nerf_h(p, ctx, c, D - 1, &ldl);
-  if (int rc = wgrad(head[FEATURE], dfeat, W, Hl, ldl, P, dhead[2 * FEATURE], dhead[2 * FEATURE + 1], st)) return rc;
+  if (int rc = wgrad(head[FEATURE], dfeat, ld_w, Hl, ldl, P, dhead[2 * FEATURE], dhead[2 * FEATURE + 1], st)) return rc;
   if (int rc = wgrad(head[ALPHA], sigma_bar, 1, Hl, ldl, P, dhead[2 * ALPHA], dhead[2 * ALPHA + 1], st)) return rc;
   float* dz = scratch + s.buf[1];
   {
-    EpiReluBwd e0{0, W, nullptr, 0, dz, W, 0};
+    EpiReluBwd e0{0, W, nullptr, 0, dz, ld_w, 0};
     if (int rc = layer_nn(head[ALPHA], sigma_bar, 1, P, e0, TC_NERF, st)) return rc;
-    EpiReluBwd e1{0, W, Hl, ldl, dz, W, 1};
-    if (int rc = layer_nn(head[FEATURE], dfeat, W, P, e1, TC_NERF, st)) return rc;
+    EpiReluBwd e1{0, W, Hl, ldl, dz, ld_w, 1};
+    if (int rc = layer_nn(head[FEATURE], dfeat, ld_w, P, e1, TC_NERF, st)) return rc;
   }
   int flip = 0;  // dz lives in buf[1]; next output goes to buf[0]
   for (int i = D - 1; i >= 0; --i) {
     int64_t ldx;
     const float* X = nerf_x(p, ctx, c, i, &ldx);
-    if (int rc = wgrad(p.layer[i], dz, W, X, ldx, P, dparams[2 * i], dparams[2 * i + 1], st)) return rc;
+    if (int rc = wgrad(p.layer[i], dz, ld_w, X, ldx, P, dparams[2 * i], dparams[2 * i + 1], st)) return rc;
     if (i == 0) break;
     float* out = scratch + s.buf[flip];
     int64_t ldh;
     const float* Hprev = nerf_h(p, ctx, c, i - 1, &ldh);
     int col_lo = (i - 1 == p.skip) ? p.ch : 0;
-    EpiReluBwd e{col_lo, col_lo + W, Hprev, ldh, out, W, 0};
-    if (int rc = layer_nn(p.layer[i], dz, W, P, e, TC_NERF, st)) return rc;
+    EpiReluBwd e{col_lo, col_lo + W, Hprev, ldh, out, ld_w, 0};
+    if (int rc = layer_nn(p.layer[i], dz, ld_w, P, e, TC_NERF, st)) return rc;
     dz = out; flip ^= 1;
   }
   return 0;

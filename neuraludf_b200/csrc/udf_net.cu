@@ -415,6 +415,7 @@ static int udf_forward_impl(const nudf_udf_desc* d, const float* wfold, const fl
   if (int rc = make_plan(d, &p, wfold)) return rc;
   if (P <= 0) return 0;
   NUDF_REQUIRE(wfold && pts && ctx, "null pointer");
+  NUDF_REQUIRE(aligned16(ctx), "ctx must be 16-byte aligned");
   cudaStream_t st = (cudaStream_t)stream;
   UdfCtx c;
   ctx_layout(p, P, grad != nullptr, &c);
@@ -448,6 +449,7 @@ int nudf_udf_value(const nudf_udf_desc* d, const float* wfold, const float* pts,
   NUDF_REQUIRE(wfold && pts && udf, "null pointer");
   cudaStream_t st = (cudaStream_t)stream;
   NUDF_REQUIRE(work != nullptr, "null pointer (work)");
+  NUDF_REQUIRE(aligned16(work), "work must be 16-byte aligned");
   UdfCtx c;
   ctx_layout(p, P, 0, &c);
   // value-only: of the last layer only row 0 (the udf head), through the same kernel as the full forward
@@ -486,6 +488,7 @@ static int udf_backward_impl(const nudf_udf_desc* d, const float* wfold, const f
   NUDF_CUDA_OK(cudaMemsetAsync(dbias, 0, sizeof(float) * p.b_total, st));
   if (P <= 0) return 0;
   NUDF_REQUIRE(pts && ctx_c && scratch, "null pointer");
+  NUDF_REQUIRE(aligned16(ctx_c) && aligned16(scratch), "ctx and scratch must be 16-byte aligned");
   float* ctx = const_cast<float*>(ctx_c);  // read-only use
   UdfCtx c;
   ctx_layout(p, P, 1, &c);

@@ -45,6 +45,15 @@ def test_descriptor_validation_runs_without_gpu():
     # fp32 folded weights (>= 524 544 floats) followed by the bf16 hi/lo tensor-engine images of every layer
     assert 524544 <= n < 8 * 1024 * 1024
     assert L.nudf_udf_ctx_floats(ctypes.byref(d), 1024, 1) > L.nudf_udf_ctx_floats(ctypes.byref(d), 1024, 0) > 0
+    # the activation context must start 16-byte aligned: refused before any device work (the pointers are never read)
+    assert L.nudf_udf_forward(ctypes.byref(d), 4096, 4096, 128, None, 0, None, 4100, None) == -1
+    assert b"16-byte aligned" in L.nudf_last_error()
+    assert L.nudf_udf_value(ctypes.byref(d), 4096, 4096, 128, 8192, 4100, None) == -1
+    assert b"16-byte aligned" in L.nudf_last_error()
+    n = _lib.NerfDesc()
+    n.D, n.W, n.d_in, n.multires, n.multires_view, n.skip = 8, 256, 4, 10, 4, 4
+    assert L.nudf_nerf_forward(ctypes.byref(n), None, 4096, 4096, 1, 128, 4096, 4096, 4100, None) == -1
+    assert b"16-byte aligned" in L.nudf_last_error()
 
 
 def test_lattice_descriptor_validation_runs_without_gpu():

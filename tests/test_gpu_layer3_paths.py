@@ -1,9 +1,9 @@
-"""GPU tests of the two activation paths of the 3-plane tensor-core layer (nudf_dense_forward_tc, planes = 3).  A row
-stride that is a multiple of 4 floats with a 16-byte-aligned base takes the persistent TMA-fed kernel (producer
-warpgroup splitting 2-D TMA boxes into planes, two consumer warpgroups, epilogue from registers); any other operand
-takes the register-staged kernel.  Both split the same bf16 planes, issue the same products and add them in the same
-order, so they must give the same bits: the meshing paths rely on a point getting the same bits in any batch, and a
-batch offset can change an operand's alignment.  Each is also checked against fp64."""
+"""GPU tests of the 3-plane tensor-core layer (nudf_dense_forward_tc, planes = 3) on operands on and off alignment.  The
+persistent kernel (a producer warpgroup splitting 2-D TMA boxes into planes, two consumer warpgroups, epilogue from
+registers) reads activations through a tensor map (a row stride that is a multiple of 4 floats and a 16-byte-aligned
+base); nudf_dense_forward_tc copies any other operand into an aligned temporary first.  The padding columns are never
+read, so an operand off alignment must give the bits of the aligned one: the meshing paths rely on a point getting the
+same bits in any batch, and a batch offset can change an operand's alignment.  Each is also checked against fp64."""
 import pytest
 import torch
 
@@ -60,11 +60,10 @@ def _image(W, N, K, transposed):
 @pytest.mark.parametrize("transposed", [0, 1])
 @pytest.mark.parametrize("N,K", SHAPES)
 @pytest.mark.parametrize("P", POINTS)
-def test_layer3_tma_matches_register_path(P, N, K, transposed, act):
-    """The row stride rounded up to 4 floats with NaN in the padding columns: the TMA path, whose tensor map must stop
-    at K (a ragged last K slice arrives zero-filled) and at P (a ragged last row block, landing quarters past P split as
-    zeros).  The same values one float into a buffer take the register path, and the two results must be the same
-    bits, on every call."""
+def test_layer3_offset_operand_matches_aligned(P, N, K, transposed, act):
+    """The row stride rounded up to 4 floats with NaN in the padding columns: the kernel's tensor map must stop at K (a
+    ragged last K slice arrives zero-filled) and at P (a ragged last row block, landing quarters past P split as zeros).
+    The same values one float into a buffer are repacked, and the two results must be the same bits, on every call."""
     g = torch.Generator(device=DEV).manual_seed(P * 7 + N * 3 + K + transposed + 11 * act)
     W = torch.randn(N, K, generator=g, device=DEV) / K ** 0.5
     b = torch.randn(N, generator=g, device=DEV)
@@ -73,16 +72,35 @@ def test_layer3_tma_matches_register_path(P, N, K, transposed, act):
     X = _operand(P, K, _ld4(K), 0, g)
     X1 = _operand(P, K, _ld4(K), 1, g)
     X1[:, :K] = X[:, :K]
-    tma = _layer(X, img, b, N, K, P, act)
-    regs = _layer(X1, img, b, N, K, P, act)
-    assert torch.isfinite(tma).all()
-    assert torch.equal(tma, regs)
-    assert torch.equal(tma, _layer(X, img, b, N, K, P, act))
+    aligned = _layer(X, img, b, N, K, P, act)
+    offset = _layer(X1, img, b, N, K, P, act)
+    assert torch.isfinite(aligned).all()
+    assert torch.equal(aligned, offset)
+    assert torch.equal(aligned, _layer(X, img, b, N, K, P, act))
     ref = X[:, :K].double() @ W.double().t() + b.double()
     if act == ACT_SOFTPLUS100:
         ref = torch.nn.functional.softplus(ref, beta=100.0)
     tag = "layer3[%d,%d,%d,t%d,a%d]" % (P, N, K, transposed, act)
-    for name, Y in (("tma", tma), ("regs", regs)):
+    for name, Y in (("aligned", aligned), ("offset", offset)):
         e = err_inf(Y, ref) / scale_inf(ref)
         report("%s.%s" % (tag, name), rel=e)
         assert e < BOUND, (name, e)
+
+
+@pytest.mark.parametrize("act", [ACT_NONE, ACT_SOFTPLUS100])
+@pytest.mark.parametrize("offset", [0, 1])
+@pytest.mark.parametrize("N", [256, 128])
+def test_layer3_k0_gives_act_bias(N, offset, act):
+    """K = 0: no copy and no product, the epilogue on zero accumulators gives act(bias) on every row, for an operand on
+    or off alignment."""
+    P = 1000
+    g = torch.Generator(device=DEV).manual_seed(N + offset + 11 * act)
+    b = torch.randn(N, generator=g, device=DEV)
+    img = torch.zeros(8, dtype=torch.int16, device=DEV)     # the image of a K = 0 layer is empty and never read
+    Y = _layer(_operand(P, 0, 4, offset, g), img, b, N, 0, P, act)
+    assert torch.equal(Y, Y[:1].expand(P, N))
+    if act == ACT_NONE:
+        assert torch.equal(Y[0], b)
+    else:
+        ref = torch.nn.functional.softplus(b.double(), beta=100.0)
+        assert (Y[0].double() - ref).abs().max().item() < 1e-6

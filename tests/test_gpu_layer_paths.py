@@ -1,8 +1,8 @@
-"""GPU tests of the two activation paths of the 2-plane tensor-core layer kernel (nudf_dense_forward_tc, planes = 2).
-A row stride that is a multiple of 4 floats with a 16-byte-aligned base takes the ring path (2-D TMA boxes into fp32
-slots, split in place into K-major planes); any other operand takes the register-staged path.  Both split the same bf16
-values and issue the same products in the same order, so they must give the same bits; each is also checked against
-fp64."""
+"""GPU tests of the 2-plane tensor-core layer kernel (nudf_dense_forward_tc, planes = 2) on operands on and off
+alignment.  The kernel reads activations through a 2-D tensor map (a row stride that is a multiple of 4 floats and a
+16-byte-aligned base); nudf_dense_forward_tc copies any other operand into an aligned temporary first.  The kernel never
+reads the padding columns, so an operand off alignment must give the bits of the aligned one; each is also checked
+against fp64."""
 import pytest
 import torch
 
@@ -54,11 +54,10 @@ def _image(W, N, K, transposed):
 @pytest.mark.parametrize("transposed", [0, 1])
 @pytest.mark.parametrize("N,K", SHAPES)
 @pytest.mark.parametrize("P", [65499, 1000, 40])
-def test_layer_ring_matches_register_path(P, N, K, transposed):
-    """The row stride rounded up to 4 floats with NaN in the padding columns: the ring path, whose tensor map must stop
-    at K (a ragged last K slice arrives zero-filled) and at P (a ragged last row block).  The same values one float into
-    a buffer take the register-staged path, and the two results must be the same bits.  P = 40 is one partial row
-    block."""
+def test_layer_offset_operand_matches_aligned(P, N, K, transposed):
+    """The row stride rounded up to 4 floats with NaN in the padding columns: the kernel's tensor map must stop at K (a
+    ragged last K slice arrives zero-filled) and at P (a ragged last row block).  The same values one float into a
+    buffer are repacked, and the two results must be the same bits.  P = 40 is one partial row block."""
     g = torch.Generator(device=DEV).manual_seed(P * 7 + N * 3 + K + transposed)
     W = torch.randn(N, K, generator=g, device=DEV) / K ** 0.5
     b = torch.randn(N, generator=g, device=DEV)
@@ -67,14 +66,27 @@ def test_layer_ring_matches_register_path(P, N, K, transposed):
     X = _operand(P, K, _ld4(K), 0, g)
     X1 = _operand(P, K, _ld4(K), 1, g)
     X1[:, :K] = X[:, :K]
-    ring = _layer(X, img, b, N, K, P)
-    regs = _layer(X1, img, b, N, K, P)
-    assert torch.isfinite(ring).all()
-    assert torch.equal(ring, regs)
-    assert torch.equal(ring, _layer(X, img, b, N, K, P))
+    aligned = _layer(X, img, b, N, K, P)
+    offset = _layer(X1, img, b, N, K, P)
+    assert torch.isfinite(aligned).all()
+    assert torch.equal(aligned, offset)
+    assert torch.equal(aligned, _layer(X, img, b, N, K, P))
     ref = X[:, :K].double() @ W.double().t() + b.double()
     tag = "layer[%d,%d,%d,t%d]" % (P, N, K, transposed)
-    for name, Y in (("ring", ring), ("regs", regs)):
+    for name, Y in (("aligned", aligned), ("offset", offset)):
         e = err_inf(Y, ref) / scale_inf(ref)
         report("%s.%s" % (tag, name), rel=e)
         assert e < BOUND, (name, e)
+
+
+@pytest.mark.parametrize("offset", [0, 1])
+@pytest.mark.parametrize("N", [256, 128])
+def test_layer_k0_gives_bias(N, offset):
+    """K = 0: no copy and no product, the epilogue on zero accumulators gives the bias on every row, for an operand on
+    or off alignment."""
+    P = 1000
+    g = torch.Generator(device=DEV).manual_seed(N + offset)
+    b = torch.randn(N, generator=g, device=DEV)
+    img = torch.zeros(8, dtype=torch.int16, device=DEV)     # the image of a K = 0 layer is empty and never read
+    Y = _layer(_operand(P, 0, 4, offset, g), img, b, N, 0, P)
+    assert torch.equal(Y, b.expand(P, N))

@@ -1,7 +1,8 @@
-"""GPU tests of the two operand paths of the tensor-core weight-gradient contraction (nudf_wgrad, engine 1).
-Row strides that are a multiple of 4 floats with 16-byte-aligned bases take the ring path (2-D TMA boxes into an fp32
-ring, MN-major planes); any other operand takes the register-staged path.  Both split the same bf16 values and issue the same 16-point
-steps in the same order, so they must give the same bits; each is also checked against fp64."""
+"""GPU tests of the tensor-core weight-gradient contraction (nudf_wgrad, engine 1) on operands on and off alignment.
+The kernel reads both operands through 2-D tensor maps (row strides that are a multiple of 4 floats and 16-byte-aligned
+bases; an fp32 ring split into MN-major planes); nudf_wgrad copies any other operand into an aligned temporary first.
+The padding columns are never read, so operands off alignment must give the bits of aligned ones; each is also checked
+against fp64."""
 import pytest
 import torch
 
@@ -50,11 +51,10 @@ def _vs_fp64(dW, dZ, X, n_out, n_in, tag, P):
 
 @pytest.mark.parametrize("n_out,n_in", SHAPES)
 @pytest.mark.parametrize("P", [65499, 1000, 40])
-def test_wgrad_bulk_matches_register_path(P, n_out, n_in):
-    """Strides rounded up to 4 floats with NaN in the padding columns: the ring path, whose tensor maps must stop at
-    the width (a ragged last column tile arrives zero-filled).  The same values one float into a buffer take the
-    register-staged path, and the two results must be the same bits.  P = 40 is a single split of one full and one
-    8-point slice."""
+def test_wgrad_offset_operands_match_aligned(P, n_out, n_in):
+    """Strides rounded up to 4 floats with NaN in the padding columns: the kernel's tensor maps must stop at the width
+    (a ragged last column tile arrives zero-filled).  The same values one float into a buffer are repacked, and the two
+    results must be the same bits.  P = 40 is a single split of one full and one 8-point slice."""
     g = torch.Generator(device=DEV).manual_seed(P * 5 + n_out + n_in)
     ldz, ldx = _ld4(n_out), _ld4(n_in)
     dZ = _operand(P, n_out, ldz, 0, g)
@@ -63,18 +63,18 @@ def test_wgrad_bulk_matches_register_path(P, n_out, n_in):
     X1 = _operand(P, n_in, ldx, 1, g)
     dZ1[:, :n_out] = dZ[:, :n_out]
     X1[:, :n_in] = X[:, :n_in]
-    bulk = _wgrad(dZ, X, n_out, n_in, P)
-    regs = _wgrad(dZ1, X1, n_out, n_in, P)
-    assert torch.isfinite(bulk).all()
-    assert torch.equal(bulk, regs)
-    assert torch.equal(bulk, _wgrad(dZ, X, n_out, n_in, P))
-    _vs_fp64(bulk, dZ, X, n_out, n_in, "bulk", P)
+    aligned = _wgrad(dZ, X, n_out, n_in, P)
+    offset = _wgrad(dZ1, X1, n_out, n_in, P)
+    assert torch.isfinite(aligned).all()
+    assert torch.equal(aligned, offset)
+    assert torch.equal(aligned, _wgrad(dZ, X, n_out, n_in, P))
+    _vs_fp64(aligned, dZ, X, n_out, n_in, "aligned", P)
 
 
 @pytest.mark.parametrize("P", [65499, 40])
 @pytest.mark.parametrize("misaligned", ["dZ", "X"])
 def test_wgrad_misaligned_base_vs_fp64(P, misaligned):
-    """Row strides a multiple of 4, but one base pointer one float past a 16-byte boundary: the register-staged path."""
+    """Row strides a multiple of 4, but one base pointer one float past a 16-byte boundary: that operand is repacked."""
     n_out, n_in = 256, 256
     g = torch.Generator(device=DEV).manual_seed(P + (misaligned == "X"))
     dZ = _operand(P, n_out, n_out, 1 if misaligned == "dZ" else 0, g)

@@ -1,13 +1,11 @@
 """Per-layer timing of the tensor-core layer kernel (Y = X W^T + b) through nudf_dense_forward_tc at the C2 step's
-point count: the 2-plane layer at 256 x 256 and 128 x 128 and the 3-plane layer at 256 x 256 on both activation paths,
-and the 3-plane layer at 128 x 128 and 256 x 39 (the UDF network's first layer) on the TMA path.  One JSON line.
+point count: the 2-plane layer at 256 x 256 and 128 x 128, and the 3-plane layer at 256 x 256, 128 x 128 and 256 x 39
+(the UDF network's first layer).  One JSON line.
 
     python tools/layer_tile_bench.py [--points 65536] [--rounds 5] [--iters 50]
 
-The 256 x 256 layers run on two operands holding the same values: `ring` / `tma` is an activation with a row stride of
-whole 16-byte units and a 16-byte-aligned base (the TMA-fed path, as the networks' operands), `regs` the same
-activation one float into its buffer (the register-staged path).  A row stride is K rounded up to 4 floats.  Each
-figure is the median over the rounds of the CUDA-event time of `iters` back-to-back calls, with the min and max beside
+Each activation has a row stride of K rounded up to 4 floats and a 16-byte-aligned base, as the networks' operands
+have: the kernels read it through a tensor map, with no repack.  Each figure is the median over the rounds of the CUDA-event time of `iters` back-to-back calls, with the min and max beside
 it; the layers alternate within each round.  The achieved bandwidth counts the bytes the layer needs, from
 the shapes: the fp32 activations read once, the fp32 output written once, the bias and the weight image read once.
 Compare two builds of the library by running this in separate processes with NUDF_LIB_PATH pointing at each; the
@@ -54,10 +52,9 @@ def main():
     st = L.stream_ptr()
     calls = {}    # name -> (bytes, flops, fn)
 
-    def add(name, N, K, planes, offset):
+    def add(name, N, K, planes):
         ld = (K + 3) // 4 * 4
-        buf = torch.zeros(P * ld + offset, device=dev)
-        X = buf[offset:].view(P, ld)
+        X = torch.zeros(P, ld, device=dev)
         X[:, :K] = torch.randn(P, K, generator=g).to(dev)
         W = (torch.randn(N, K, generator=g) / K ** 0.5).to(dev)
         b = torch.randn(N, generator=g).to(dev)
@@ -69,12 +66,10 @@ def main():
         calls[name] = (4 * P * K + 4 * P * N + 4 * N + 2 * img.numel(), 2.0 * P * N * K, fn, (X, W, b, Y, img))
 
     for n in (256, 128):
-        add("planes2_%dx%d_ring" % (n, n), n, n, 2, 0)
-        add("planes2_%dx%d_regs" % (n, n), n, n, 2, 1)
-    add("planes3_256x256_tma", 256, 256, 3, 0)
-    add("planes3_256x256_regs", 256, 256, 3, 1)
-    add("planes3_128x128_tma", 128, 128, 3, 0)
-    add("planes3_256x39_tma", 256, 39, 3, 0)
+        add("planes2_%dx%d_ring" % (n, n), n, n, 2)
+    add("planes3_256x256_tma", 256, 256, 3)
+    add("planes3_128x128_tma", 128, 128, 3)
+    add("planes3_256x39_tma", 256, 39, 3)
     runs = {name: [] for name in calls}
     for _, _, fn, _ in calls.values():
         fn()
