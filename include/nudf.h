@@ -397,6 +397,23 @@ int nudf_iso_emit(const float* df, int32_t n0, int32_t n1, int32_t n2, float lev
  * fp32 v, no contraction), loop centres at the mean of their loop's edge points summed in loop order */
 int nudf_iso_vertices(const float* df, int32_t n0, int32_t n1, int32_t n2, float level, const int64_t* cells, int64_t n_cells,
                       const int64_t* keys, int64_t n_keys, double* verts, void* stream);
+/* The same stages on a nudf_lattice (the flat array or a brick store; the nudf_iso_* above are their df form, the same
+ * kernels).  The active cells without a scan of every cell: the storage positions (df: the flat indices; a store: coarse,
+ * then the brick slots, as nudf_sb_flat numbers them) are taken in n_seg = ceil(positions / NUDF_ISO_SEG) segments.  Each
+ * position holding a lattice point with v <= 0 emits the active cells (as nudf_iso_active defines them) of which it is the
+ * lowest corner with v <= 0: counts[seg] = the segment's cells; cells[offsets[seg] ...] = them, in position order
+ * (offsets = exclusive scan of the counts).  Sorted, they are nonzero(nudf_iso_active) of the lattice's values, with no
+ * condition on the field: every active cell has a corner with v <= 0, which is finite and so stored. */
+#define NUDF_ISO_SEG 256
+int nudf_iso_lat_cells_count(const nudf_lattice* lat, float level, int64_t n_seg, int32_t* counts, void* stream);
+int nudf_iso_lat_cells_emit(const nudf_lattice* lat, float level, int64_t n_seg, const int64_t* offsets, int64_t* cells,
+                            void* stream);
+int nudf_iso_lat_count(const nudf_lattice* lat, float level, const int64_t* cells, int64_t n_cells, int32_t* counts,
+                       void* stream);
+int nudf_iso_lat_emit(const nudf_lattice* lat, float level, const int64_t* cells, int64_t n_cells, const int64_t* offsets,
+                      int64_t* keys, void* stream);
+int nudf_iso_lat_vertices(const nudf_lattice* lat, float level, const int64_t* cells, int64_t n_cells, const int64_t* keys,
+                          int64_t n_keys, double* verts, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Point-cloud evaluation (the DTU / DeepFashion3D Chamfer protocols; neuraludf_b200/evaluate.py drives the stages)
@@ -484,6 +501,11 @@ int nudf_nb_sublattice(int32_t n, int32_t s, const nudf_band_coords* co, int64_t
 int nudf_nb_block_test(const nudf_lattice* lat, int32_t s, const uint8_t* parent_flags, int32_t parent_s,
                        const nudf_band_coords* co, double lipschitz, double tau, uint8_t* flags, uint32_t* max_slope,
                        void* stream);
+/* nudf_nb_block_test on any lattice with either coordinate form: the table form on a brick store too
+ * (grid.iso_band_sparse), the same test on the same corner values */
+int nudf_nb_lat_block_test(const nudf_lattice* lat, int32_t s, const uint8_t* parent_flags, int32_t parent_s,
+                           const nudf_band_coords* co, double lipschitz, double tau, uint8_t* flags, uint32_t* max_slope,
+                           void* stream);
 /* counts[i] = the points block kept[i] of stride s emits: the stride-t lattice (t divides s) in its closed box, less the
  * stride-s lattice, less the points that a lower-numbered kept block (flags) also holds.  kept: ascending block numbers */
 int nudf_nb_count(const uint8_t* flags, int32_t n, int32_t s, int32_t t, const int64_t* kept, int64_t n_kept,

@@ -80,6 +80,7 @@ class BrickStore(ctypes.Structure):
 
 
 BRICK = 8   # NUDF_BRICK
+ISO_SEG = 256   # NUDF_ISO_SEG
 
 
 class Lattice(ctypes.Structure):
@@ -223,9 +224,17 @@ _SIGNATURES = {
                        + [c_void_p] * 2),
     "nudf_cl_vote": (ctypes.c_int, [c_void_p, ctypes.c_int64, c_void_p, ctypes.c_int32, c_void_p] + [ctypes.c_int32] * 3
                      + [c_void_p] * 2),
+    "nudf_iso_lat_cells_count": (ctypes.c_int, [c_void_p, ctypes.c_float, ctypes.c_int64, c_void_p, c_void_p]),
+    "nudf_iso_lat_cells_emit": (ctypes.c_int, [c_void_p, ctypes.c_float, ctypes.c_int64] + [c_void_p] * 3),
+    "nudf_iso_lat_count": (ctypes.c_int, [c_void_p, ctypes.c_float, c_void_p, ctypes.c_int64, c_void_p, c_void_p]),
+    "nudf_iso_lat_emit": (ctypes.c_int, [c_void_p, ctypes.c_float, c_void_p, ctypes.c_int64] + [c_void_p] * 3),
+    "nudf_iso_lat_vertices": (ctypes.c_int, [c_void_p, ctypes.c_float, c_void_p, ctypes.c_int64, c_void_p, ctypes.c_int64,
+                                             c_void_p, c_void_p]),
     "nudf_nb_sublattice": (ctypes.c_int, [ctypes.c_int32] * 2 + [c_void_p] * 4),
     "nudf_nb_block_test": (ctypes.c_int, [c_void_p, ctypes.c_int32, c_void_p, ctypes.c_int32, c_void_p] + [ctypes.c_double] * 2
                            + [c_void_p] * 3),
+    "nudf_nb_lat_block_test": (ctypes.c_int, [c_void_p, ctypes.c_int32, c_void_p, ctypes.c_int32, c_void_p]
+                               + [ctypes.c_double] * 2 + [c_void_p] * 3),
     "nudf_nb_count": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [c_void_p, ctypes.c_int64] + [c_void_p] * 2),
     "nudf_nb_emit": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [c_void_p, ctypes.c_int64] + [c_void_p] * 5),
     "nudf_sb_mark": (ctypes.c_int, [c_void_p, ctypes.c_int32] + [c_void_p] * 3),

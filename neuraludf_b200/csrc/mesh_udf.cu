@@ -26,6 +26,7 @@
 // Threshold meshing (nudf_iso_*) runs stages 4-5 on v = fl32(f - level) instead of the pseudo-signed udf (the corner rules
 // UdfCorners / IsoCorners), with its own active-cell test and fp64 vertices; tests/proto/iso_mc.py restates it.
 #include <algorithm>
+#include <type_traits>
 
 #include "../../include/nudf.h"
 #include "common.cuh"
@@ -219,13 +220,14 @@ struct UdfCorners {             // MeshUDF: the udf with the cell's pseudo-sign
   }
 };
 
+template <class A>
 struct IsoCorners {             // threshold meshing: v = fl32(f - level), faces wound from the > level side into the <= level side
-  const float* __restrict__ df;
+  A df;
   float level;
   static constexpr bool kDescent = true;
   __device__ __forceinline__ void operator()(const Dims& D, int64_t, int64_t g, float v[8]) const {
 #pragma unroll
-    for (int c = 0; c < 8; ++c) v[c] = __fsub_rn(df[g + D.coff(c)], level);
+    for (int c = 0; c < 8; ++c) v[c] = __fsub_rn(df(g + D.coff(c)), level);
   }
 };
 
@@ -457,10 +459,160 @@ __global__ void k_iso_active(const float* __restrict__ df, Dims D, float level, 
   }
 }
 
+// Active cells without a scan of every cell (nudf_iso_lat_cells_*): every active cell has a corner with v <= 0, which is
+// finite and therefore stored, so visiting the storage positions of the lattice (S below) with v <= 0 and testing the up
+// to 8 cells holding each finds them all.  A cell is emitted by its lowest corner with v <= 0 only (corners ascend with
+// the flat index), so once.  The test is k_iso_active's on the same corner values, so the set is nonzero(nudf_iso_active)
+// on any lattice whose reader gives those values -- +inf (unstored) and NaN corners included, with no Lipschitz condition.
+// Positions are taken in segments of NUDF_ISO_SEG, one thread each: the count pass writes each segment's cell count, the
+// emit pass writes the segment's cells from its offset in position order; the caller sorts.
+struct DenseSites {             // the flat array: position = flat index
+  DenseDf df;
+  int64_t n;
+  __device__ __forceinline__ float at(int64_t p) const { return df.p[p]; }
+  __device__ __forceinline__ bool point(const Dims& D, int64_t p, int64_t x[3]) const {
+#pragma unroll
+    for (int a = 0; a < 3; ++a) x[a] = D.coord(p, a);
+    return true;
+  }
+  // w[(a + 1) * 9 + (b + 1) * 3 + c + 1] = the value at x + (a, b, c) for the offsets inside the lattice (others unread)
+  __device__ __forceinline__ void around(const Dims& D, const int64_t x[3], const bool in[3][3], float w[27]) const {
+    const int64_t g = (x[0] * D.n1 + x[1]) * D.n2 + x[2];
+#pragma unroll
+    for (int t = 0; t < 27; ++t)
+      if (in[0][t / 9] && in[1][(t / 3) % 3] && in[2][t % 3])
+        w[t] = df.p[g + (t / 9 - 1) * D.n1 * D.n2 + ((t / 3) % 3 - 1) * D.n2 + (t % 3 - 1)];
+  }
+};
+
+struct BrickSites {             // the brick store: coarse positions, then brick slots (nudf_sb_flat's positions)
+  BrickDf st;
+  const int64_t* __restrict__ keys;
+  int64_t n;
+  __device__ __forceinline__ float at(int64_t p) const { return st.at(p); }
+  // the lattice point stored at p; false for a brick slot beyond N - 1 or of a point held in coarse
+  __device__ __forceinline__ bool point(const Dims&, int64_t p, int64_t x[3]) const {
+    const int64_t m3 = st.mc * st.mc * st.mc, N = st.N;
+    if (p < m3) {
+      x[0] = min((p / (st.mc * st.mc)) * st.c, N - 1);
+      x[1] = min(((p / st.mc) % st.mc) * st.c, N - 1);
+      x[2] = min((p % st.mc) * st.c, N - 1);
+      return true;
+    }
+    const int64_t q = p - m3, key = keys[q / kBrickPoints], l = q % kBrickPoints;
+    x[0] = (key / (st.nbk * st.nbk)) * kBrick + l / (kBrick * kBrick);
+    x[1] = ((key / st.nbk) % st.nbk) * kBrick + (l / kBrick) % kBrick;
+    x[2] = (key % st.nbk) * kBrick + l % kBrick;
+    return x[0] < N && x[1] < N && x[2] < N && !(st.coarse_of(x[0]) >= 0 && st.coarse_of(x[1]) >= 0 && st.coarse_of(x[2]) >= 0);
+  }
+  // as DenseSites::around, through BrickDf::position with the per-axis terms computed once
+  __device__ __forceinline__ void around(const Dims&, const int64_t x[3], const bool in[3][3], float w[27]) const {
+    int64_t co[3][3], bk[3][3], lo[3][3];
+#pragma unroll
+    for (int a = 0; a < 3; ++a)
+#pragma unroll
+      for (int o = 0; o < 3; ++o) {
+        const int64_t y = x[a] + o - 1;
+        co[a][o] = in[a][o] ? st.coarse_of(y) : -1;
+        bk[a][o] = y / kBrick;
+        lo[a][o] = y % kBrick;
+      }
+#pragma unroll
+    for (int t = 0; t < 27; ++t) {
+      const int u = t / 9, v = (t / 3) % 3, z = t % 3;
+      if (!(in[0][u] && in[1][v] && in[2][z])) continue;
+      int64_t p;
+      if (co[0][u] >= 0 && co[1][v] >= 0 && co[2][z] >= 0) {
+        p = (co[0][u] * st.mc + co[1][v]) * st.mc + co[2][z];
+      } else {
+        const int32_t slot = st.dir[(bk[0][u] * st.nbk + bk[1][v]) * st.nbk + bk[2][z]];
+        p = slot < 0 ? -1 : st.mc * st.mc * st.mc + (int64_t)slot * kBrickPoints + (lo[0][u] * kBrick + lo[1][v]) * kBrick + lo[2][z];
+      }
+      w[t] = st.at(p);
+    }
+  }
+};
+
+// counts the active cells position p owns (cells != NULL: writes them): the cells holding its lattice point of which it
+// is the lowest corner with v <= 0, tested as k_iso_active tests them on the values around the point
+template <class S>
+__device__ __forceinline__ int iso_owned_cells(const S& sites, const Dims& D, float level, int64_t p,
+                                               int64_t* __restrict__ cells) {
+  if (p >= sites.n || !(__fsub_rn(sites.at(p), level) <= 0.f)) return 0;
+  int64_t x[3];
+  if (!sites.point(D, p, x)) return 0;
+  const int64_t lim[3] = {D.n0, D.n1, D.n2};
+  bool in[3][3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a)
+#pragma unroll
+    for (int o = 0; o < 3; ++o) in[a][o] = x[a] + o - 1 >= 0 && x[a] + o - 1 < lim[a];
+  float w[27];
+  sites.around(D, x, in, w);
+  int n = 0;
+#pragma unroll
+  for (int q = 0; q < 8; ++q) {             // the cell whose corner q is the point: corner c at offset c - q per axis
+    const int dq[3] = {(q >> 2) & 1, (q >> 1) & 1, q & 1};
+    if (!(in[0][1 - dq[0]] && in[0][2 - dq[0]] && in[1][1 - dq[1]] && in[1][2 - dq[1]] && in[2][1 - dq[2]] &&
+          in[2][2 - dq[2]]))
+      continue;
+    bool pos = false, neg = false, nan = false, lower = false;
+#pragma unroll
+    for (int c = 0; c < 8; ++c) {
+      const int t = (((c >> 2) & 1) - dq[0] + 1) * 9 + (((c >> 1) & 1) - dq[1] + 1) * 3 + ((c & 1) - dq[2] + 1);
+      const float v = __fsub_rn(w[t], level);
+      pos |= v > 0.f;
+      neg |= v <= 0.f;
+      nan |= v != v;
+      lower |= c < q && v <= 0.f;
+    }
+    if (pos && neg && !nan && !lower) {
+      if (cells) cells[n] = ((x[0] - dq[0]) * D.n1 + x[1] - dq[1]) * D.n2 + x[2] - dq[2];
+      ++n;
+    }
+  }
+  return n;
+}
+
+constexpr int kIsoSeg = NUDF_ISO_SEG;
+
+// one block of kIsoSeg threads per segment; offsets NULL: counts[seg] = the segment's cells, else cells[offsets[seg] ...]
+template <class S>
+__global__ void __launch_bounds__(kIsoSeg) k_iso_cells(S sites, Dims D, float level, int64_t n_seg,
+                                                        int32_t* __restrict__ counts, const int64_t* __restrict__ offsets,
+                                                        int64_t* __restrict__ cells) {
+  __shared__ int32_t warp_sum[kIsoSeg / 32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int64_t seg = blockIdx.x; seg < n_seg; seg += gridDim.x) {
+    const int64_t p = seg * kIsoSeg + threadIdx.x;
+    const int n = iso_owned_cells(sites, D, level, p, (int64_t*)nullptr);
+    int incl = n;                           // inclusive scan over the block: warps, then the warp totals
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const int y = __shfl_up_sync(0xffffffffu, incl, d);
+      if (lane >= d) incl += y;
+    }
+    if (lane == 31) warp_sum[warp] = incl;
+    __syncthreads();
+    int before = 0, total = 0;
+#pragma unroll
+    for (int w = 0; w < kIsoSeg / 32; ++w) {
+      before += w < warp ? warp_sum[w] : 0;
+      total += warp_sum[w];
+    }
+    if (!offsets) {
+      if (threadIdx.x == 0) counts[seg] = total;
+    } else if (n) {                         // the same cells again, written in place
+      iso_owned_cells(sites, D, level, p, cells + offsets[seg] + before + incl - n);
+    }
+    __syncthreads();                        // warp_sum is reused by the next segment
+  }
+}
+
 // fp64 lattice-index coordinates of the point on the edge (lower corner gk, axis ax): t = v_a / (v_a - v_b) of the fp32 v
-__device__ __forceinline__ void iso_edge_point(const float* __restrict__ df, const Dims& D, float level, int64_t gk, int ax,
-                                               double x[3]) {
-  const double va = __fsub_rn(df[gk], level), vb = __fsub_rn(df[gk + D.stride(ax)], level);
+template <class A>
+__device__ __forceinline__ void iso_edge_point(const A& df, const Dims& D, float level, int64_t gk, int ax, double x[3]) {
+  const double va = __fsub_rn(df(gk), level), vb = __fsub_rn(df(gk + D.stride(ax)), level);
   const double tt = __ddiv_rn(va, __dsub_rn(va, vb));
   for (int k = 0; k < 3; ++k) {
     const double c = (double)D.coord(gk, k);
@@ -468,8 +620,9 @@ __device__ __forceinline__ void iso_edge_point(const float* __restrict__ df, con
   }
 }
 
-__global__ void k_iso_vertices(const float* __restrict__ df, Dims D, float level, const int64_t* __restrict__ cells,
-                               const int64_t* __restrict__ keys, int64_t n, double* __restrict__ verts) {
+template <class A>
+__device__ __forceinline__ void iso_vertices(const A& df, const Dims& D, float level, const int64_t* __restrict__ cells,
+                                             const int64_t* __restrict__ keys, int64_t n, double* __restrict__ verts) {
   const int64_t centre0 = 3 * D.n0 * D.n1 * D.n2;
   for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < n; t += (int64_t)gridDim.x * blockDim.x) {
     const int64_t key = keys[t];
@@ -479,7 +632,7 @@ __global__ void k_iso_vertices(const float* __restrict__ df, Dims D, float level
     } else {                   // centre of a loop: the mean of its edge points, summed in canonical loop order
       const int64_t c = (key - centre0) >> 2, g = cells[c];
       int8_t cl[12];
-      const int len = centre_loop(IsoCorners{df, level}, D, c, g, (int)((key - centre0) & 3), cl);
+      const int len = centre_loop(IsoCorners<A>{df, level}, D, c, g, (int)((key - centre0) & 3), cl);
       double s[3] = {0.0, 0.0, 0.0}, y[3];
       for (int i = 0; i < len; ++i) {
         const int e = cl[i];
@@ -490,6 +643,18 @@ __global__ void k_iso_vertices(const float* __restrict__ df, Dims D, float level
     }
     for (int k = 0; k < 3; ++k) verts[t * 3 + k] = x[k];
   }
+}
+
+template <class A>
+__global__ void k_iso_vertices(A df, Dims D, float level, const int64_t* __restrict__ cells, const int64_t* __restrict__ keys,
+                               int64_t n, double* __restrict__ verts) {
+  iso_vertices(df, D, level, cells, keys, n, verts);
+}
+
+// the flat array as a restrict-qualified parameter: its loads take the read-only path, as before the reader template
+__global__ void k_iso_vertices_dense(const float* __restrict__ df, Dims D, float level, const int64_t* __restrict__ cells,
+                                     const int64_t* __restrict__ keys, int64_t n, double* __restrict__ verts) {
+  iso_vertices(DenseDf{df}, D, level, cells, keys, n, verts);
 }
 
 static inline unsigned grid_for(int64_t n) { return (unsigned)std::min<int64_t>(std::max<int64_t>(cdiv(n, 256), 1), 65535ll * 8); }
@@ -626,36 +791,107 @@ int nudf_iso_active(const float* df, int32_t n0, int32_t n1, int32_t n2, float l
   return 0;
 }
 
+// the threshold stages on a lattice descriptor; the nudf_iso_* entry points taking a flat array are their dense form
+template <class F>
+static int with_iso_lattice(const nudf_lattice* lat, float level, F&& launch) {
+  ISO_LEVEL_OK();
+  return with_lattice(lat, [&](auto df) { return launch(df, dims(*lat)); });
+}
+
+static inline nudf_lattice dense_lattice(const float* df, int32_t n0, int32_t n1, int32_t n2) {
+  return nudf_lattice{n0, n1, n2, df, nullptr};
+}
+
+static int iso_cells(const nudf_lattice* lat, float level, int64_t n_seg, int32_t* counts, const int64_t* offsets,
+                     int64_t* cells, void* stream) {
+  return with_iso_lattice(lat, level, [&](auto df, Dims D) {
+    NUDF_REQUIRE(offsets ? (cells != nullptr) : (counts != nullptr), "null pointer");
+    int64_t n_pos = D.n0 * D.n1 * D.n2;
+    if (lat->store) {
+      NUDF_REQUIRE(lat->store->n_bricks == 0 || lat->store->keys, "null brick keys");
+      n_pos = (int64_t)lat->store->mc * lat->store->mc * lat->store->mc + lat->store->n_bricks * kBrickPoints;
+    }
+    NUDF_REQUIRE(n_seg == cdiv(n_pos, (int64_t)kIsoSeg), "n_seg must be ceil(storage positions / NUDF_ISO_SEG)");
+    const unsigned grid = (unsigned)std::min<int64_t>(std::max<int64_t>(n_seg, 1), 65535ll * 8);
+    if constexpr (std::is_same<decltype(df), DenseDf>::value)
+      k_iso_cells<<<grid, kIsoSeg, 0, (cudaStream_t)stream>>>(DenseSites{df, n_pos}, D, level, n_seg, counts, offsets,
+                                                                cells);
+    else
+      k_iso_cells<<<grid, kIsoSeg, 0, (cudaStream_t)stream>>>(BrickSites{df, lat->store->keys, n_pos}, D, level, n_seg,
+                                                                counts, offsets, cells);
+    NUDF_LAUNCH_OK();
+    return 0;
+  });
+}
+
+int nudf_iso_lat_cells_count(const nudf_lattice* lat, float level, int64_t n_seg, int32_t* counts, void* stream) {
+  return iso_cells(lat, level, n_seg, counts, nullptr, nullptr, stream);
+}
+
+int nudf_iso_lat_cells_emit(const nudf_lattice* lat, float level, int64_t n_seg, const int64_t* offsets, int64_t* cells,
+                            void* stream) {
+  NUDF_REQUIRE(offsets, "null pointer");
+  return iso_cells(lat, level, n_seg, nullptr, offsets, cells, stream);
+}
+
+int nudf_iso_lat_count(const nudf_lattice* lat, float level, const int64_t* cells, int64_t n_cells, int32_t* counts,
+                       void* stream) {
+  return with_iso_lattice(lat, level, [&](auto df, Dims D) {
+    NUDF_REQUIRE(cells && counts && n_cells >= 0, "null pointer or negative count");
+    if (n_cells == 0) return 0;
+    k_count<<<grid_for(n_cells), 128, 0, (cudaStream_t)stream>>>(IsoCorners<decltype(df)>{df, level}, D, cells, n_cells,
+                                                                  counts);
+    NUDF_LAUNCH_OK();
+    return 0;
+  });
+}
+
+int nudf_iso_lat_emit(const nudf_lattice* lat, float level, const int64_t* cells, int64_t n_cells, const int64_t* offsets,
+                      int64_t* keys, void* stream) {
+  return with_iso_lattice(lat, level, [&](auto df, Dims D) {
+    NUDF_REQUIRE(cells && offsets && keys && n_cells >= 0, "null pointer or negative count");
+    if (n_cells == 0) return 0;
+    k_emit<<<grid_for(n_cells), 128, 0, (cudaStream_t)stream>>>(IsoCorners<decltype(df)>{df, level}, D, cells, n_cells,
+                                                                 offsets, keys);
+    NUDF_LAUNCH_OK();
+    return 0;
+  });
+}
+
+int nudf_iso_lat_vertices(const nudf_lattice* lat, float level, const int64_t* cells, int64_t n_cells, const int64_t* keys,
+                          int64_t n_keys, double* verts, void* stream) {
+  return with_iso_lattice(lat, level, [&](auto df, Dims D) {
+    NUDF_REQUIRE(cells && keys && verts && n_cells >= 0 && n_keys >= 0, "null pointer or negative count");
+    if (n_keys == 0) return 0;
+    if constexpr (std::is_same<decltype(df), DenseDf>::value)
+      k_iso_vertices_dense<<<grid_for(n_keys), 128, 0, (cudaStream_t)stream>>>(df.p, D, level, cells, keys, n_keys, verts);
+    else
+      k_iso_vertices<<<grid_for(n_keys), 128, 0, (cudaStream_t)stream>>>(df, D, level, cells, keys, n_keys, verts);
+    NUDF_LAUNCH_OK();
+    return 0;
+  });
+}
+
 int nudf_iso_count(const float* df, int32_t n0, int32_t n1, int32_t n2, float level, const int64_t* cells, int64_t n_cells,
                    int32_t* counts, void* stream) {
   MC_DIMS_OK();
-  ISO_LEVEL_OK();
-  NUDF_REQUIRE(df && cells && counts && n_cells >= 0, "null pointer or negative count");
-  if (n_cells == 0) return 0;
-  k_count<<<grid_for(n_cells), 128, 0, (cudaStream_t)stream>>>(IsoCorners{df, level}, dims(n0, n1, n2), cells, n_cells, counts);
-  NUDF_LAUNCH_OK();
-  return 0;
+  NUDF_REQUIRE(df, "null pointer");
+  const nudf_lattice lat = dense_lattice(df, n0, n1, n2);
+  return nudf_iso_lat_count(&lat, level, cells, n_cells, counts, stream);
 }
 
 int nudf_iso_emit(const float* df, int32_t n0, int32_t n1, int32_t n2, float level, const int64_t* cells, int64_t n_cells,
                   const int64_t* offsets, int64_t* keys, void* stream) {
   MC_DIMS_OK();
-  ISO_LEVEL_OK();
-  NUDF_REQUIRE(df && cells && offsets && keys && n_cells >= 0, "null pointer or negative count");
-  if (n_cells == 0) return 0;
-  k_emit<<<grid_for(n_cells), 128, 0, (cudaStream_t)stream>>>(IsoCorners{df, level}, dims(n0, n1, n2), cells, n_cells, offsets,
-                                                               keys);
-  NUDF_LAUNCH_OK();
-  return 0;
+  NUDF_REQUIRE(df, "null pointer");
+  const nudf_lattice lat = dense_lattice(df, n0, n1, n2);
+  return nudf_iso_lat_emit(&lat, level, cells, n_cells, offsets, keys, stream);
 }
 
 int nudf_iso_vertices(const float* df, int32_t n0, int32_t n1, int32_t n2, float level, const int64_t* cells, int64_t n_cells,
                       const int64_t* keys, int64_t n_keys, double* verts, void* stream) {
   MC_DIMS_OK();
-  ISO_LEVEL_OK();
-  NUDF_REQUIRE(df && cells && keys && verts && n_cells >= 0 && n_keys >= 0, "null pointer or negative count");
-  if (n_keys == 0) return 0;
-  k_iso_vertices<<<grid_for(n_keys), 128, 0, (cudaStream_t)stream>>>(df, dims(n0, n1, n2), level, cells, keys, n_keys, verts);
-  NUDF_LAUNCH_OK();
-  return 0;
+  NUDF_REQUIRE(df, "null pointer");
+  const nudf_lattice lat = dense_lattice(df, n0, n1, n2);
+  return nudf_iso_lat_vertices(&lat, level, cells, n_cells, keys, n_keys, verts, stream);
 }

@@ -99,7 +99,8 @@ def get_mesh_udf_fast(func, func_grad, samples=None, indices=None, N_MC=128, gra
     The N_MC^3 lattice on [-1,1]^3 holds func's values (batches of 2^20 points), negative values set to 0; the normals are
     -normalize(func_grad(x)[:, 0]) where the value is below 2 voxels.  The lattice is dense, or narrow-band (grid.udf_band)
     with NUDF_BAND_MESH=1 in the environment: the same mesh when func is 2-Lipschitz and gives a point the same bits in any
-    batch (udf_band warns when the lattice shows a steeper slope).  Then the MC, the vertex filter (func at every vertex in
+    batch (udf_band warns when the lattice shows a steeper slope); with NUDF_BAND_MESH=sparse that band is held
+    block-sparse (grid.udf_band_sparse, its values clamped as the dense lattice's are): the band mesh, with no N^3 array.  Then the MC, the vertex filter (func at every vertex in
     one call) and mesh_post.postprocess(smooth_borders).
 
     Raises RuntimeError when the MC finds no surface (the reference's MC does), and IndexError when the post-processed mesh
@@ -112,7 +113,7 @@ def get_mesh_udf_fast(func, func_grad, samples=None, indices=None, N_MC=128, gra
         raise NotImplementedError("get_mesh_udf_fast: re-evaluation from a passed-back `samples` is not served on the device; "
                                   "pass samples=None for a full evaluation")
     N = int(N_MC)
-    lattice = "band" if os.environ.get("NUDF_BAND_MESH") == "1" else "dense"
+    lattice = {"1": "band", "sparse": "sparse"}.get(os.environ.get("NUDF_BAND_MESH"), "dense")
     with torch.no_grad():
         v64, f, minfo = mesh._mesh_post(CallerField(func, func_grad), N, lattice, dist_threshold_ratio, smooth_borders,
                                         max_batch=LATTICE_BATCH)

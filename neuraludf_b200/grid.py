@@ -12,7 +12,8 @@ Lipschitz bound cannot rule out udf < 2 voxels (kernels in csrc/mesh_band.cu).  
 lattice of validate_mesh (any box, torch.linspace coordinates): it evaluates every point a threshold mesh at `level` can
 read.  `udf_band_sparse` runs udf_band's levels into a block-sparse store (SparseBand: a coarse dense array plus 8^3
 bricks, csrc/mesh_sparse.cu) instead of an N^3 array, and `near_surface_cells_sparse` selects the band from it: what
-mesh.udf_mesh_sparse meshes at 2048^3."""
+mesh.udf_mesh_sparse meshes at 2048^3.  `iso_band_sparse` runs iso_band's levels into the same store: what
+mesh.iso_mesh_sparse meshes."""
 import ctypes
 import math
 import warnings
@@ -163,8 +164,8 @@ def band_block_test(df, N, s, parent=None, parent_s=0, lipschitz=2.0, tau=None, 
     out = torch.empty(nb ** 3, dtype=torch.uint8, device=device) if flags else None
     slope = torch.zeros(1, dtype=torch.int32, device=device)
     tau = 2.0 * (2.0 / (N - 1)) if tau is None else tau
-    check(_lib.lib().nudf_nb_block_test(lat, s, ptr(parent), parent_s, _coords(N, axes, spacing, pad), float(lipschitz),
-                                        float(tau), ptr(out), ptr(slope), _lib.stream_ptr()), "nudf_nb_block_test")
+    check(_lib.lib().nudf_nb_lat_block_test(lat, s, ptr(parent), parent_s, _coords(N, axes, spacing, pad), float(lipschitz),
+                                            float(tau), ptr(out), ptr(slope), _lib.stream_ptr()), "nudf_nb_lat_block_test")
     return out, float(slope.view(torch.float32))
 
 
@@ -444,21 +445,8 @@ def iso_cull(level, lipschitz, h, e):
     return tau, pad
 
 
-@torch.no_grad()
-def iso_band(query, bound_min, bound_max, resolution, level, lipschitz=2.0, strides=None, max_batch=1 << 21, device=None):
-    """Narrow-band threshold lattice, coarse to fine: (df [R^3] fp32 flat, +inf where never evaluated; info).
-
-    The lattice is extract_geometry's: R = `resolution` points per axis on the box [bound_min, bound_max], coordinates from
-    axis_tables (the dense sweep's torch.linspace tables, read by the kernels, so the points are that sweep's bit for bit),
-    flat index (i R + j) R + k.  The level is rounded to fp32 once (mesh.iso_marching_cubes_index's rule); a non-finite
-    level raises ValueError.  The levels run as udf_band's, with the block test of csrc/mesh_band.cu's table rule: a block
-    is culled when min(corner value) - L r >= tau, r half its diagonal in table coordinates, tau = level + L D (iso_cull).
-    If `query` is `lipschitz`-Lipschitz at the lattice points and gives a point the same bits in any batch, df equals the
-    dense lattice bit for bit wherever that is below tau, every +inf stands for a value >= tau, and the threshold marching
-    cubes of df at `level` (mesh.iso_mesh_band) is the dense one exactly (the argument is beside the kernels).
-    `query`: any callable points [P,3] fp32 -> [P] or [P,1].  info: udf_band's keys, with the same RuntimeWarning when
-    max_edge_slope exceeds `lipschitz`, plus tau (the threshold compared with, slack included), pad and spacing (the largest
-    step per axis)."""
+def _iso_setup(level, resolution, lipschitz, strides, bound_min, bound_max, device):
+    """iso_band's checks, tables and block-test constants: (level, N, lipschitz, strides, device, axes, h, tau, pad)"""
     from neuraludf_b200.mesh import _iso_level
     level = _iso_level(level)
     N = int(resolution)
@@ -474,12 +462,56 @@ def iso_band(query, bound_min, bound_max, resolution, level, lipschitz=2.0, stri
         raise ValueError("the lattice tables must be float32 (torch's default dtype is %s)" % torch.get_default_dtype())
     h, e = table_spacing(axes)
     tau, pad = iso_cull(level, lipschitz, h, e)
+    return level, N, lipschitz, strides, device, axes, h, tau, pad
+
+
+@torch.no_grad()
+def iso_band(query, bound_min, bound_max, resolution, level, lipschitz=2.0, strides=None, max_batch=1 << 21, device=None):
+    """Narrow-band threshold lattice, coarse to fine: (df [R^3] fp32 flat, +inf where never evaluated; info).
+
+    The lattice is extract_geometry's: R = `resolution` points per axis on the box [bound_min, bound_max], coordinates from
+    axis_tables (the dense sweep's torch.linspace tables, read by the kernels, so the points are that sweep's bit for bit),
+    flat index (i R + j) R + k.  The level is rounded to fp32 once (mesh.iso_marching_cubes_index's rule); a non-finite
+    level raises ValueError.  The levels run as udf_band's, with the block test of csrc/mesh_band.cu's table rule: a block
+    is culled when min(corner value) - L r >= tau, r half its diagonal in table coordinates, tau = level + L D (iso_cull).
+    If `query` is `lipschitz`-Lipschitz at the lattice points and gives a point the same bits in any batch, df equals the
+    dense lattice bit for bit wherever that is below tau, every +inf stands for a value >= tau, and the threshold marching
+    cubes of df at `level` (mesh.iso_mesh_band) is the dense one exactly (the argument is beside the kernels).
+    `query`: any callable points [P,3] fp32 -> [P] or [P,1].  info: udf_band's keys, with the same RuntimeWarning when
+    max_edge_slope exceeds `lipschitz`, plus tau (the threshold compared with, slack included), pad and spacing (the largest
+    step per axis)."""
+    level, N, lipschitz, strides, device, axes, h, tau, pad = _iso_setup(level, resolution, lipschitz, strides, bound_min,
+                                                                         bound_max, device)
     lattice = _DenseLattice(torch.full((N ** 3,), float("inf"), device=device), N)
     info = _coarse_to_fine(lattice, lambda pts: query(pts).detach().reshape(-1).float(), N, strides, lipschitz, tau,
                            max_batch, axes=axes, spacing=h, pad=pad)
     info.update(tau=tau, pad=pad, spacing=h)
     _warn_slope(info, lipschitz, "iso_band", "a threshold mesh may miss cells")
     return lattice.df, info
+
+
+@torch.no_grad()
+def iso_band_sparse(query, bound_min, bound_max, resolution, level, lipschitz=2.0, strides=None, max_batch=1 << 21,
+                    device=None):
+    """iso_band's lattice without an R^3 array: (SparseBand, info).
+
+    The checks, tables, block test (the table rule, reading the store), levels and RuntimeWarning are iso_band's; the store
+    and its brick allocation are udf_band_sparse's (the points of strides >= c in the coarse array, the finer ones in the
+    bricks meeting a kept stride-c block), and each level is emitted and evaluated in chunks of about max_batch points.  If
+    `query` gives a point the same bits in any batch, SparseBand.values equals iso_band's df at every lattice point, +inf
+    included, whatever the field (DESIGN.md section 1); mesh.iso_marching_cubes_sparse meshes it.  info: iso_band's keys,
+    plus coarse_stride, bricks and bytes as udf_band_sparse reports them."""
+    level, N, lipschitz, strides, device, axes, h, tau, pad = _iso_setup(level, resolution, lipschitz, strides, bound_min,
+                                                                         bound_max, device)
+    c = sparse_coarse_stride(strides)
+    band = SparseBand(N, c, device)
+    info = _coarse_to_fine(band, lambda pts: query(pts).detach().reshape(-1).float(), N, strides, lipschitz, tau, max_batch,
+                           chunk=max_batch, axes=axes, spacing=h, pad=pad)
+    band.check_stored()
+    info.update(tau=tau, pad=pad, spacing=h, coarse_stride=c, bricks=band.n_bricks,
+                bytes=dict(band.nbytes(), flags=max([(-(-(N - 1) // s)) ** 3 for s in strides[:-1]], default=0)))
+    _warn_slope(info, lipschitz, "iso_band_sparse", "a threshold mesh may miss cells")
+    return band, info
 
 
 @torch.no_grad()

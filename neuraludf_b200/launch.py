@@ -12,7 +12,9 @@ NUDF_BAND_MESH=1, `validate_mesh`'s `extract_geometry` (when PyMCubes cannot be 
 (grid.iso_band: the same mesh when the UDF is 2-Lipschitz and batch-invariant); without it the whole lattice is queried.
 With NUDF_DEVICE_MESH=1, `extract_mesh` (the runner's get_mesh_udf_fast) is bound to neuraludf_b200.extract_mesh: the
 lattice, MC, post-processing and gradient branch of extract_udf_mesh on the device, with no N^3 host array (NUDF_BAND_MESH=1
-then evaluates its lattice narrow-band too); without it the runner's own extract_mesh.py runs.
+then evaluates its lattice narrow-band too); without it the runner's own extract_mesh.py runs.  NUDF_BAND_MESH=sparse
+holds either band block-sparse (grid.iso_band_sparse / udf_band_sparse): the same meshes with no N^3 device array either,
+for resolutions up to 2048.
 """
 import importlib
 import importlib.machinery

@@ -9,7 +9,8 @@ for the reference's `custom_mc._marching_cubes_lewiner.udf_mc_lewiner`, served t
 csrc/mesh_udf.cu (stages and deviations documented there); tests/proto/udf_mc.py is their NumPy restatement.
 `iso_marching_cubes_index` / `iso_marching_cubes` are threshold marching cubes on the same kernels (the runner's
 validate_mesh without PyMCubes; `python -m neuraludf_b200.mesh --threshold T`), restated in tests/proto/iso_mc.py;
-`iso_mesh_band` is the same with the lattice evaluated narrow-band (grid.iso_band; `--threshold T --band`).
+`iso_mesh_band` is the same with the lattice evaluated narrow-band (grid.iso_band; `--threshold T --band`), and
+`iso_mesh_sparse` the same again with the band held block-sparse (grid.iso_band_sparse; `--threshold T --band --sparse`).
 `udf_mesh_sparse` is `udf_mesh_band` on the block-sparse band (grid.udf_band_sparse, `marching_cubes_sparse`): the same
 mesh with no N^3 array, for lattices up to 2048^3 (`--sparse`).
 """
@@ -150,28 +151,86 @@ def iso_marching_cubes_index(df, dims, level):
     flags = torch.empty(df.numel(), dtype=torch.uint8, device=dev)
     check(L.nudf_iso_active(ptr(df), n0, n1, n2, level, ptr(flags), st), "nudf_iso_active")
     cells = torch.nonzero(flags).reshape(-1).contiguous()
+    del flags
+    lat = _lib.Lattice(n0, n1, n2, df.data_ptr(), None)
+    return _iso_stages(ctypes.byref(lat), cells, level, dev)
+
+
+def _iso_stages(lat, cells, level, dev):
+    """the threshold MC stages after the active cells (sorted `cells`) on the lattice descriptor `lat` (a flat array or a
+    brick store): iso_marching_cubes_index's returns"""
+    L = _lib.lib()
+    st = _lib.stream_ptr()
     n = cells.numel()
     empty = (torch.zeros(0, 3, dtype=torch.float64, device=dev), torch.zeros(0, 3, dtype=torch.int64, device=dev))
     info = {"active": cells, "face_keys": empty[1], "vertex_keys": torch.zeros(0, dtype=torch.int64, device=dev)}
     if n == 0:
         return empty[0], empty[1], info
     counts = torch.empty(n, dtype=torch.int32, device=dev)
-    check(L.nudf_iso_count(ptr(df), n0, n1, n2, level, ptr(cells), n, ptr(counts), st), "nudf_iso_count")
+    check(L.nudf_iso_lat_count(lat, level, ptr(cells), n, ptr(counts), st), "nudf_iso_lat_count")
     csum = torch.cumsum(counts, 0, dtype=torch.int64)
     n_faces = int(csum[-1])
     offsets = (csum - counts).contiguous()
+    del counts, csum
     keys = torch.empty(3 * n_faces, dtype=torch.int64, device=dev)
-    check(L.nudf_iso_emit(ptr(df), n0, n1, n2, level, ptr(cells), n, ptr(offsets), ptr(keys), st), "nudf_iso_emit")
+    check(L.nudf_iso_lat_emit(lat, level, ptr(cells), n, ptr(offsets), ptr(keys), st), "nudf_iso_lat_emit")
+    del offsets
     info["face_keys"] = keys.reshape(-1, 3)
     if n_faces == 0:
         return empty[0], empty[1], info
     ukeys, inv = torch.unique(keys, sorted=True, return_inverse=True)
     ukeys = ukeys.contiguous()
     verts = torch.empty(ukeys.numel(), 3, dtype=torch.float64, device=dev)
-    check(L.nudf_iso_vertices(ptr(df), n0, n1, n2, level, ptr(cells), n, ptr(ukeys), ukeys.numel(), ptr(verts), st),
-          "nudf_iso_vertices")
+    check(L.nudf_iso_lat_vertices(lat, level, ptr(cells), n, ptr(ukeys), ukeys.numel(), ptr(verts), st),
+          "nudf_iso_lat_vertices")
     info["vertex_keys"] = ukeys
     return verts, inv.reshape(-1, 3).to(torch.int64), info
+
+
+def _iso_cells(lat, n_positions, level, dev):
+    """sorted active cells of the lattice descriptor `lat` at the fp32 `level` from its n_positions storage positions
+    (nudf_iso_lat_cells_*: no scan of every cell)"""
+    L = _lib.lib()
+    st = _lib.stream_ptr()
+    n_seg = -(-n_positions // _lib.ISO_SEG)
+    counts = torch.empty(n_seg, dtype=torch.int32, device=dev)
+    check(L.nudf_iso_lat_cells_count(lat, level, n_seg, ptr(counts), st), "nudf_iso_lat_cells_count")
+    csum = torch.cumsum(counts, 0, dtype=torch.int64)
+    total = int(csum[-1]) if n_seg else 0
+    offsets = (csum - counts).contiguous()
+    del counts, csum
+    cells = torch.empty(total, dtype=torch.int64, device=dev)
+    if total:
+        check(L.nudf_iso_lat_cells_emit(lat, level, n_seg, ptr(offsets), ptr(cells), st), "nudf_iso_lat_cells_emit")
+    del offsets
+    return torch.sort(cells).values
+
+
+@torch.no_grad()
+def iso_active_cells(lattice, level, dims=None):
+    """The sorted active cells of threshold meshing at `level` (rounded to fp32), found from the lattice's stored points
+    with no scan of every cell: a grid.SparseBand, or an fp32 CUDA array of shape `dims`.  They equal
+    iso_marching_cubes_index's info["active"] (nonzero of nudf_iso_active) of the same values, for any field."""
+    level = _iso_level(level)
+    if isinstance(lattice, torch.Tensor):
+        n0, n1, n2 = (int(d) for d in dims)
+        df = lattice.reshape(-1)
+        if df.dtype != torch.float32 or df.device.type != "cuda" or df.numel() != n0 * n1 * n2:
+            raise ValueError("df must be a float32 CUDA array of %d values" % (n0 * n1 * n2))
+        df = df.contiguous()
+        lat = _lib.Lattice(n0, n1, n2, df.data_ptr(), None)
+        return _iso_cells(ctypes.byref(lat), df.numel(), level, df.device)
+    return _iso_cells(lattice.lattice(), lattice.mc ** 3 + lattice.n_bricks * _lib.BRICK ** 3, level, lattice.device)
+
+
+@torch.no_grad()
+def iso_marching_cubes_sparse(band, level):
+    """iso_marching_cubes_index on the R^3 lattice of a grid.SparseBand (grid.iso_band_sparse), every value read through
+    the brick store: the same (fp64 verts [V,3] in lattice-index units, int64 faces [F,3], info) as on the array the store
+    reads as, with no array of R^3 elements.  The active cells come from the stored points (iso_active_cells)."""
+    level = _iso_level(level)
+    cells = iso_active_cells(band, level)
+    return _iso_stages(band.lattice(), cells, level, band.device)
 
 
 @torch.no_grad()
@@ -191,6 +250,22 @@ def iso_mesh_band(query, bound_min, bound_max, resolution, level, lipschitz=2.0,
     df, binfo = grid.iso_band(query, bound_min, bound_max, R, level, lipschitz=lipschitz, strides=strides,
                               max_batch=max_batch, device=device)
     verts, faces, info = iso_marching_cubes_index(df, (R, R, R), level)
+    info["band"] = binfo
+    return verts, faces, info
+
+
+@torch.no_grad()
+def iso_mesh_sparse(query, bound_min, bound_max, resolution, level, lipschitz=2.0, strides=None, max_batch=1 << 21,
+                    device=None):
+    """`iso_mesh_band` on the block-sparse band (grid.iso_band_sparse, iso_marching_cubes_sparse): the same (fp64 verts,
+    int64 faces, info with info["band"]), with no array of R^3 elements, for lattices up to 2048^3.
+
+    The store reads iso_band's df at every lattice point whatever the field, and the active cells, faces and vertices are
+    those of that df, so the mesh is iso_mesh_band's bit for bit; it is the dense one under iso_mesh_band's conditions."""
+    from neuraludf_b200 import grid
+    band, binfo = grid.iso_band_sparse(query, bound_min, bound_max, resolution, level, lipschitz=lipschitz,
+                                       strides=strides, max_batch=max_batch, device=device)
+    verts, faces, info = iso_marching_cubes_sparse(band, level)
     info["band"] = binfo
     return verts, faces, info
 
@@ -265,13 +340,15 @@ def _udf_mc(udf_network, N, lattice, lipschitz=2.0, strides=None, max_batch=1 <<
     """The raw MeshUDF MC of the N^3 lattice evaluated `lattice`: "dense" (grid.udf_grid of the slab [lo, hi)), "band"
     (grid.udf_band) or "sparse" (grid.udf_band_sparse): (verts [V,3] fp32 in the slab's lattice-index units, faces [F,3]
     int64).  Negative lattice values are set to 0 (extract_mesh.py:196; a UDF network gives none) after the normals'
-    selection, which reads them unchanged either way (< 2 voxels).  The lattice is released on return.  mark(stage) is
+    selection, which reads them unchanged either way (< 2 voxels); on the sparse lattice in the coarse array and bricks.  The lattice is released on return.  mark(stage) is
     called after the lattice, the normals and the MC."""
     from neuraludf_b200 import grid
     if lattice == "sparse":
         band, _ = grid.udf_band_sparse(udf_network, N, lipschitz=lipschitz, strides=strides, max_batch=max_batch)
         mark("lattice")
         idx, normals = grid.near_surface_cells_sparse(udf_network, band, max_batch=max(max_batch // 2, 1))
+        band.coarse.masked_fill_(band.coarse < 0, 0.0)              # the clamp below, on what the store holds
+        band.bricks.masked_fill_(band.bricks < 0, 0.0)
         mark("normals")
         verts, faces, _ = marching_cubes_sparse(band, normals, idx)
         mark("mc")
@@ -515,16 +592,16 @@ def main(argv=None):
     ap.add_argument("--scale", type=float, default=1.0, help="the conf's udf_network.scale")
     ap.add_argument("--dense", action="store_true", help="evaluate the whole lattice (udf_mesh) instead of the narrow band")
     ap.add_argument("--sparse", action="store_true",
-                    help="hold the narrow band block-sparse (udf_mesh_sparse): the same mesh with no N^3 array, for "
-                         "--resolution up to 2048")
+                    help="hold the narrow band block-sparse (udf_mesh_sparse, or iso_mesh_sparse with --threshold "
+                         "--band): the same mesh with no N^3 array, for --resolution up to 2048")
     ap.add_argument("--postprocess", action="store_true",
                     help="apply the runner's post-processing (merge, duplicate and degenerate faces, hole filling, border "
                          "smoothing, the final merge after --cameras): the mesh Runner.extract_udf_mesh writes; the runner "
                          "passes --dist_threshold_ratio 5")
     ap.add_argument("--out", required=True, help="output PLY")
     a = ap.parse_args(argv)
-    if a.sparse and (a.dense or a.threshold is not None):
-        ap.error("--sparse cannot be combined with %s" % ("--dense" if a.dense else "--threshold"))
+    if a.sparse and (a.dense or (a.threshold is not None and not a.band)):
+        ap.error("--sparse cannot be combined with %s" % ("--dense" if a.dense else "--threshold without --band"))
     if a.band and a.threshold is None:
         ap.error("--band needs --threshold (the MeshUDF lattice is evaluated narrow-band without it)")
     if a.threshold is not None:
@@ -543,8 +620,8 @@ def main(argv=None):
         from neuraludf_b200.models.udf_renderer_blending import box_vertices, extract_geometry
         bmin, bmax, sm = threshold_box(a.cameras)
         bmin, bmax = torch.tensor(bmin, dtype=torch.float32), torch.tensor(bmax, dtype=torch.float32)
-        if a.band:                                # extract_geometry's device path with NUDF_BAND_MESH=1
-            v, faces, _ = iso_mesh_band(lambda pts: net.udf_values(pts), bmin, bmax, a.resolution, a.threshold,
+        if a.band:                                # extract_geometry's device path with NUDF_BAND_MESH=1 (or =sparse)
+            v, faces, _ = (iso_mesh_sparse if a.sparse else iso_mesh_band)(lambda pts: net.udf_values(pts), bmin, bmax, a.resolution, a.threshold,
                                         lipschitz=a.lipschitz, device=torch.device("cuda"))
             v, faces = box_vertices(v.cpu().numpy(), a.resolution, bmin, bmax), faces.cpu().numpy()
         else:

@@ -71,7 +71,8 @@ def extract_geometry(bound_min, bound_max, resolution, threshold, query_func, de
     project's vertex numbering and ambiguous-cell triangulation); the vertices then take the reference's mapping
     (box_vertices).  With NUDF_BAND_MESH=1 in the environment (and no PyMCubes) the lattice is evaluated narrow-band
     (mesh.iso_mesh_band, Lipschitz bound 2): the same mesh when query_func is 2-Lipschitz and gives a point the same bits
-    in any batch."""
+    in any batch.  NUDF_BAND_MESH=sparse holds that band block-sparse (mesh.iso_mesh_sparse): the band mesh bit for bit,
+    with no resolution^3 array."""
     try:
         import mcubes
     except ImportError:
@@ -80,10 +81,11 @@ def extract_geometry(bound_min, bound_max, resolution, threshold, query_func, de
         u = extract_fields(bound_min, bound_max, resolution, query_func, device)
         vertices, triangles = mcubes.marching_cubes(u, threshold)
     else:
-        from ..mesh import iso_marching_cubes_index, iso_mesh_band
+        from ..mesh import iso_marching_cubes_index, iso_mesh_band, iso_mesh_sparse
+        band = {"1": iso_mesh_band, "sparse": iso_mesh_sparse}.get(os.environ.get("NUDF_BAND_MESH"))
         with torch.no_grad():
-            if os.environ.get("NUDF_BAND_MESH") == "1":
-                v, f, _ = iso_mesh_band(query_func, bound_min, bound_max, resolution, threshold, device=device)
+            if band is not None:
+                v, f, _ = band(query_func, bound_min, bound_max, resolution, threshold, device=device)
             else:
                 u = _grid_query_device(bound_min, bound_max, resolution, query_func, device, 0)
                 v, f, _ = iso_marching_cubes_index(u, u.shape, threshold)
