@@ -546,6 +546,28 @@ int nudf_sb_gather(const nudf_brick_store* st, const int64_t* idx, int64_t n, fl
 int nudf_sb_flat(const nudf_brick_store* st, const int64_t* pos, int64_t n, int64_t* out, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * Surface point clouds (neuraludf_b200/cloud.py drives the steps; DESIGN.md section 1 states the algorithm)
+ * ------------------------------------------------------------------------------------------------------------
+ * p, out: fp32 [n,3]; u fp32 [n]; g fp32 [n,3]; all DEVICE.  Every fp32 operation is rounded once in the stated order,
+ * with no contraction.  The points are taken in n_seg = ceil(n / NUDF_UC_SEG) segments: the count pass writes
+ * counts[seg] = the segment's survivors, the emit pass writes them to out[offsets[seg] ...] in point order (offsets: an
+ * exclusive scan of the counts, plus any base), so that the survivors of consecutive calls can share one output. */
+#define NUDF_UC_SEG 256
+/* projection step: q = p - (u / n) g with n = sqrt((gx gx + gy gy) + gz gz); survives when u and g are finite, n != 0 and
+ * q lies in [-1,1]^3 (the survivor is q) */
+int nudf_uc_step_count(const float* p, const float* u, const float* g, int64_t n, int32_t* counts, void* stream);
+int nudf_uc_step_emit(const float* p, const float* u, const float* g, int64_t n, const int64_t* offsets, float* out,
+                      void* stream);
+/* filter: p survives when u < thr */
+int nudf_uc_filter_count(const float* p, const float* u, int64_t n, float thr, int32_t* counts, void* stream);
+int nudf_uc_filter_emit(const float* p, const float* u, int64_t n, float thr, const int64_t* offsets, float* out,
+                        void* stream);
+/* out[i] (i < m < 2^32) = pool[hash(seed, round, i, 0) mod n_pool] + ((b_a 2^-24 - 1/2) voxel)_a, b_a = hash(seed, round, i,
+ * 1 + a) >> 8; hash(s, r, i, k) = mix(mix(s + 0x9e3779b9 (4 r + k)) ^ i) mod 2^32, mix the lowbias32 mixer (udf_cloud.cu) */
+int nudf_uc_resample(const float* pool, int64_t n_pool, int64_t m, uint32_t seed, int32_t round, float voxel, float* out,
+                     void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------
  * Mesh post-processing (neuraludf_b200/mesh_post.py drives the steps; sorting, unique and compaction in torch)
  * ------------------------------------------------------------------------------------------------------------
  * verts: fp64 [V,3]; faces and edges: int64 rows.  All fp64 arithmetic is correctly rounded per operation with no

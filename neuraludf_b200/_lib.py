@@ -81,6 +81,7 @@ class BrickStore(ctypes.Structure):
 
 BRICK = 8   # NUDF_BRICK
 ISO_SEG = 256   # NUDF_ISO_SEG
+UC_SEG = 256    # NUDF_UC_SEG
 
 
 class Lattice(ctypes.Structure):
@@ -241,6 +242,12 @@ _SIGNATURES = {
     "nudf_sb_store": (ctypes.c_int, [c_void_p] * 3 + [ctypes.c_int64] + [c_void_p] * 2),
     "nudf_sb_gather": (ctypes.c_int, [c_void_p] * 2 + [ctypes.c_int64] + [c_void_p] * 2),
     "nudf_sb_flat": (ctypes.c_int, [c_void_p] * 2 + [ctypes.c_int64] + [c_void_p] * 2),
+    "nudf_uc_step_count": (ctypes.c_int, [c_void_p] * 3 + [ctypes.c_int64] + [c_void_p] * 2),
+    "nudf_uc_step_emit": (ctypes.c_int, [c_void_p] * 3 + [ctypes.c_int64] + [c_void_p] * 3),
+    "nudf_uc_filter_count": (ctypes.c_int, [c_void_p] * 2 + [ctypes.c_int64, ctypes.c_float] + [c_void_p] * 2),
+    "nudf_uc_filter_emit": (ctypes.c_int, [c_void_p] * 2 + [ctypes.c_int64, ctypes.c_float] + [c_void_p] * 3),
+    "nudf_uc_resample": (ctypes.c_int, [c_void_p, ctypes.c_int64, ctypes.c_int64, ctypes.c_uint32, ctypes.c_int32,
+                                        ctypes.c_float, c_void_p, c_void_p]),
     "nudf_mp_faces": (ctypes.c_int, [c_void_p, ctypes.c_int64, c_void_p, ctypes.c_int64] + [c_void_p] * 6),
     "nudf_mp_hole_count": (ctypes.c_int, [c_void_p, ctypes.c_int64, c_void_p, c_void_p, ctypes.c_int64, c_void_p, c_void_p]),
     "nudf_mp_hole_emit": (ctypes.c_int, [c_void_p] * 3 + [ctypes.c_int64, c_void_p, c_void_p, ctypes.c_int64]

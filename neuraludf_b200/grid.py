@@ -11,8 +11,8 @@ out of scope).  `udf_band` is the coarse-to-fine alternative to the dense sweep:
 Lipschitz bound cannot rule out udf < 2 voxels (kernels in csrc/mesh_band.cu).  `iso_band` does the same for the threshold
 lattice of validate_mesh (any box, torch.linspace coordinates): it evaluates every point a threshold mesh at `level` can
 read.  `udf_band_sparse` runs udf_band's levels into a block-sparse store (SparseBand: a coarse dense array plus 8^3
-bricks, csrc/mesh_sparse.cu) instead of an N^3 array, and `near_surface_cells_sparse` selects the band from it: what
-mesh.udf_mesh_sparse meshes at 2048^3.  `iso_band_sparse` runs iso_band's levels into the same store: what
+bricks, csrc/mesh_sparse.cu) instead of an N^3 array, and `near_surface_cells_sparse` selects the band from it
+(`near_surface_indices_sparse`, also the seeds of cloud.udf_point_cloud): what mesh.udf_mesh_sparse meshes at 2048^3.  `iso_band_sparse` runs iso_band's levels into the same store: what
 mesh.iso_mesh_sparse meshes."""
 import ctypes
 import math
@@ -398,17 +398,23 @@ def udf_band_sparse(udf_network, N, lipschitz=2.0, strides=None, max_batch=1 << 
 
 
 @torch.no_grad()
-def near_surface_cells_sparse(udf_network, band, max_batch=1 << 20, dist_voxels=2.0):
-    """near_surface_cells on a SparseBand: (sorted flat lattice indices [M] int64, unit vectors towards the surface [M,3])
-    of the points with udf < dist_voxels * voxel, the same comparison as near_surface_cells' (fp32 values against the
-    threshold), over the coarse array and the bricks only.  Equal to near_surface_cells on udf_band's df when band equals
-    it (udf_band_sparse)."""
+def near_surface_indices_sparse(band, dist_voxels=2.0):
+    """sorted flat lattice indices [M] int64 of the points of a SparseBand with udf < dist_voxels * voxel, the same
+    comparison as near_surface_cells' (fp32 values against the threshold), over the coarse array and the bricks only: the
+    selection of near_surface_cells_sparse and the seeds of cloud.udf_point_cloud"""
     voxel = 2.0 / (band.N - 1)
     thr = dist_voxels * voxel
     pos = torch.cat([torch.nonzero(band.coarse < thr).reshape(-1),
                      torch.nonzero(band.bricks < thr).reshape(-1) + band.coarse.numel()])
-    idx = torch.sort(band.flat_index(pos.contiguous())).values
-    del pos
+    return torch.sort(band.flat_index(pos.contiguous())).values
+
+
+@torch.no_grad()
+def near_surface_cells_sparse(udf_network, band, max_batch=1 << 20, dist_voxels=2.0):
+    """near_surface_cells on a SparseBand: (sorted flat lattice indices [M] int64, unit vectors towards the surface [M,3])
+    of the points near_surface_indices_sparse selects.  Equal to near_surface_cells on udf_band's df when band equals it
+    (udf_band_sparse)."""
+    idx = near_surface_indices_sparse(band, dist_voxels)
     return idx, _surface_normals(udf_network, band.N, idx, max_batch)
 
 

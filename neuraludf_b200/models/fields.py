@@ -129,6 +129,11 @@ class UDFNetwork(nn.Module):
         """udf [P] only, no autograd, no saved activations (importance sampling, grid extraction)."""
         return ops.udf_value(self._handle, x.reshape(-1, 3))
 
+    def value_gradient(self, x):
+        """(udf [P], d udf/d x [P,3]) from ONE fused evaluation without the feature output and without autograd (surface
+        projection, cloud.udf_point_cloud): the bits of value_and_gradient's udf column and gradient."""
+        return ops.udf_value_gradient(self._handle, x.reshape(-1, 3))
+
     def gradient(self, x):
         if x.is_leaf and x.dtype.is_floating_point:
             x.requires_grad_(True)          # side effect of the reference (fields.py:220); the value is not used

@@ -267,6 +267,21 @@ def udf_value(handle, pts):
     return udf
 
 
+def udf_value_gradient(handle, pts):
+    """(udf [P], d udf/d x [P,3]) without autograd: one nudf_udf_forward_split with no feature output (the feature layer is
+    skipped), the udf and gradient bits of udf_forward's"""
+    handle.refresh()
+    pts = _f32c(pts)
+    _require_cuda(pts)
+    P = pts.shape[0]
+    udf = torch.empty(P, dtype=torch.float32, device=pts.device)
+    grad = torch.empty(P, 3, dtype=torch.float32, device=pts.device)
+    ctx = _udf_ctx(handle, P, True, pts.device)
+    L.check(L.lib().nudf_udf_forward_split(ctypes.byref(handle.desc), L.ptr(handle.wfold), L.ptr(pts), P, L.ptr(udf), None, 0,
+                                           L.ptr(grad), L.ptr(ctx), L.stream_ptr()), "nudf_udf_forward_split")
+    return udf, grad
+
+
 # ---------------------------------------------------------------------------------------------------------------
 # colour network
 # ---------------------------------------------------------------------------------------------------------------
