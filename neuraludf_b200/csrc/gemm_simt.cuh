@@ -259,41 +259,69 @@ struct EpiSplitStore {
   NUDF_EPI_CALL
 };
 
-// epi(row, col, sum over z of ws[z][row][col .. col + 3])   (ws slices are row-major [M x N])
+// epi(row, col, sum over z of ws[z][row][col .. col + 3])   (ws slices are row-major [M x N]).  Each sum runs in split
+// order.  The grid is small (one thread per 4 columns: 4096 threads for a 128 x 128 gradient) and a thread's sum is a
+// chain over all the splits, so the loads of SPLITK_UNROLL splits are issued before their adds: with a load or two in
+// flight per thread the kernel waited on memory latency, not bandwidth.  Small blocks spread the grid over more SMs.
+constexpr int SPLITK_UNROLL = 16, SPLITK_THREADS = 64;
+// ws[col .. col + nv - 1] and zeros beyond: one 16-byte load where the four columns are whole and aligned
+__device__ __forceinline__ float4 splitk_load4(const float* __restrict__ p, int nv, bool vec) {
+  if (vec) return __ldg(reinterpret_cast<const float4*>(p));
+  float4 r = make_float4(0.f, 0.f, 0.f, 0.f);
+  if (nv > 0) r.x = __ldg(p);
+  if (nv > 1) r.y = __ldg(p + 1);
+  if (nv > 2) r.z = __ldg(p + 2);
+  if (nv > 3) r.w = __ldg(p + 3);
+  return r;
+}
 template <class Epi>
-__global__ void splitk_reduce_kernel(const float* __restrict__ ws, int64_t slice, int splits, int64_t M, int N, Epi epi) {
+__global__ void __launch_bounds__(SPLITK_THREADS) splitk_reduce_kernel(const float* __restrict__ ws, int64_t slice, int splits, int64_t M, int N, Epi epi) {
   const int ncq = (N + 3) / 4;
   const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   const int64_t row = idx / ncq;
   if (row >= M) return;
   const int col = (int)(idx - row * ncq) * 4;
   const int nv = N - col < 4 ? N - col : 4;
+  const float* p = ws + row * N + col;
+  const bool vec = nv == 4 && (N & 3) == 0 && (slice & 3) == 0 && aligned16(ws);
   float x[4] = {0.f, 0.f, 0.f, 0.f};
-  for (int z = 0; z < splits; ++z) {
-    const float* p = ws + z * slice + row * N + col;
+  auto add = [&](const float4& v) { x[0] += v.x; x[1] += v.y; x[2] += v.z; x[3] += v.w; };
+  int z = 0;
+  for (; z + SPLITK_UNROLL <= splits; z += SPLITK_UNROLL) {
+    float4 v[SPLITK_UNROLL];
 #pragma unroll
-    for (int j = 0; j < 4; ++j)
-      if (j < nv) x[j] += p[j];
+    for (int u = 0; u < SPLITK_UNROLL; ++u) v[u] = splitk_load4(p + (z + u) * slice, nv, vec);
+#pragma unroll
+    for (int u = 0; u < SPLITK_UNROLL; ++u) add(v[u]);
   }
+  for (; z < splits; ++z) add(splitk_load4(p + z * slice, nv, vec));
   epi(row, col, x, nv);
 }
-// out[i] += sum over z of ws[z * n + i]
-static __global__ void vec_reduce_kernel(const float* __restrict__ ws, int splits, int64_t n, float* __restrict__ out) {
+// out[i] += sum over z of ws[z * n + i], in split order, SPLITK_UNROLL loads in flight as in splitk_reduce_kernel
+static __global__ void __launch_bounds__(SPLITK_THREADS) vec_reduce_kernel(const float* __restrict__ ws, int splits, int64_t n, float* __restrict__ out) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   float t = 0.f;
-  for (int z = 0; z < splits; ++z) t += ws[z * n + i];
+  int z = 0;
+  for (; z + SPLITK_UNROLL <= splits; z += SPLITK_UNROLL) {
+    float v[SPLITK_UNROLL];
+#pragma unroll
+    for (int u = 0; u < SPLITK_UNROLL; ++u) v[u] = __ldg(ws + (z + u) * n + i);
+#pragma unroll
+    for (int u = 0; u < SPLITK_UNROLL; ++u) t += v[u];
+  }
+  for (; z < splits; ++z) t += ws[z * n + i];
   out[i] += t;
 }
 template <class Epi>
 static inline int splitk_reduce(const float* ws, int splits, int64_t M, int N, const Epi& epi, cudaStream_t st) {
   const int64_t n = M * ((N + 3) / 4);
-  splitk_reduce_kernel<Epi><<<(unsigned)cdiv(n, 256), 256, 0, st>>>(ws, M * N, splits, M, N, epi);
+  splitk_reduce_kernel<Epi><<<(unsigned)cdiv(n, SPLITK_THREADS), SPLITK_THREADS, 0, st>>>(ws, M * N, splits, M, N, epi);
   NUDF_LAUNCH_OK();
   return 0;
 }
 static inline int vec_reduce(const float* ws, int splits, int64_t n, float* out, cudaStream_t st) {
-  vec_reduce_kernel<<<(unsigned)cdiv(n, 256), 256, 0, st>>>(ws, splits, n, out);
+  vec_reduce_kernel<<<(unsigned)cdiv(n, SPLITK_THREADS), SPLITK_THREADS, 0, st>>>(ws, splits, n, out);
   NUDF_LAUNCH_OK();
   return 0;
 }

@@ -8,8 +8,8 @@
 //   The accumulators go through shared memory to the fused epilogue functor (4 consecutive columns of a row per call).
 // * gemm_w3_tma_kernel, 3-plane layers: persistent, a producer warpgroup feeding two consumer warpgroups through
 //   mbarriers, the epilogue applied from the accumulator fragments.
-// * gemm_tn_kernel, weight gradients: a ring of fp32 slices of both operands split into MN-major planes, split-K over
-//   the points.
+// * gemm_tn_kernel, weight gradients: a producer warpgroup splitting a ring of fp32 slices of both operands into
+//   MN-major planes for two consumer warpgroups through mbarriers, split-K over the points.
 // Every activation operand has a row stride of whole 16-byte units and a 16-byte-aligned base (check_tma_operand).
 #pragma once
 #include <cuda.h>
@@ -38,9 +38,13 @@ __host__ __device__ inline uint32_t sw128(uint32_t row, uint32_t k) {
 }
 
 // gemm_tn_kernel: slices of TN_PS points, fp32 operand blocks as they lie in HBM ([point][128 columns]) in a
-// TN_RING-deep ring, and a double-buffered stage of bf16 planes (hi, lo of A, then of B)
+// TN_LAND-deep landing ring, split into a TN_STAGES-deep ring of bf16 plane stages (hi, lo of A, then of B)
 constexpr int TN_PS = 32;
-constexpr int TN_RING = 4;
+constexpr int TN_LAND = 4;
+constexpr int TN_STAGES = 3;
+constexpr int TN_THREADS = 384;                              // a producer and two consumer warpgroups
+constexpr int TN_PRODUCER_REGS = 104, TN_CONSUMER_REGS = 200;
+static_assert(TN_PRODUCER_REGS + 2 * TN_CONSUMER_REGS <= 65536 / 128, "register file of one SM");
 constexpr uint32_t TN_F32_OPND = TN_PS * BM * 4;            // 16 KB: one operand's [32 x 128] fp32 block
 constexpr uint32_t TN_F32_STAGE = 2 * TN_F32_OPND;          // A, then B
 constexpr uint32_t TN_PLANE = BM * TN_PS * 2;               // 8 KB: one bf16 plane of one operand
@@ -128,9 +132,10 @@ static __global__ void tc_prep_weights_kernel(const float* __restrict__ W, int64
 
 // ---- PTX wrappers --------------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ uint8_t* align1024(uint8_t* p) {
-  return reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(p) + 1023) & ~(uintptr_t)1023);
-}
+// p (the dynamic shared array) rounded up to 1024 bytes by an offset: rounding the pointer through an integer would
+// lose its address space, and every access through the result would compile to a generic load or store with a 64-bit
+// address instead of LDS / STS
+__device__ __forceinline__ uint8_t* align1024(uint8_t* p) { return p + ((1024u - (smem_u32(p) & 1023u)) & 1023u); }
 
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
@@ -190,6 +195,8 @@ __device__ __forceinline__ uint64_t make_desc_mn(uint32_t smem_addr) {
 }
 // the threads of one warpgroup (named barrier 1; 0 is __syncthreads)
 __device__ __forceinline__ void wg_bar_sync() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
+// the two consumer warpgroups of gemm_tn_kernel (named barrier 2)
+__device__ __forceinline__ void tn_consumer_bar_sync() { asm volatile("bar.sync 2, 256;" ::: "memory"); }
 template <uint32_t R> __device__ __forceinline__ void reg_dealloc() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 template <uint32_t R> __device__ __forceinline__ void reg_alloc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
@@ -692,112 +699,146 @@ gemm_w3_tma_kernel(const float* __restrict__ A, int64_t M, int N, int K, const u
 // column's sum has a fixed order: per k-quarter partials (points 8q + 2kq, 8q + 2kq + 1 of each 64 points, pairs added
 // first, in point order), then (q0 + q1) + (q2 + q3).
 //
-// The operands reach shared memory as they lie in HBM.  One thread issues a 2-D TMA copy per operand and slice (a
-// [TN_PS points x 128 columns] fp32 box, 16 KB; columns past M / N and points past K arrive as zeros) into a TN_RING-deep
-// ring on an mbarrier, and refills a stage as soon as the barrier after its split has passed: up to TN_RING - 1 slices
-// are in flight per CTA beyond the one being split, in no registers.  While the wgmma group of slice i runs, all threads
-// split slice i + 1 into the free MN-major plane stage (warps 0-3 A, warps 4-7 B; warp w takes k-quarter kq = w & 3 of
-// each 8 points, lane l columns 4l..4l+3), and the wgmma reads both operands with its transpose flags set.  Points of the
-// last slice past the chunk end (the next chunk's) are split as zeros.
+// The operands reach shared memory as they lie in HBM, and three warpgroups share the work with no CTA barrier in the
+// main loop:
+// * Producer (warpgroup 0, TN_PRODUCER_REGS registers).  One thread issues a 2-D TMA copy per operand and slice (a
+//   [TN_PS points x 128 columns] fp32 box, 16 KB; columns past M / N and points past K arrive as zeros) into a
+//   TN_LAND-deep landing ring on one mbarrier per stage.  Once the consumers have released a plane stage ("empty"), the
+//   warpgroup splits the next landed slice into it as MN-major hi / lo planes: warp w takes k-quarter w of each 8 points
+//   of A, then of B, lane l columns 4l..4l+3; points past the chunk end (the next chunk's) are split as zeros.  Each
+//   thread fences its plane stores for the async proxy and arrives on the stage's "full" barrier (128 arrivals).  The
+//   landing stage is refilled with slice i + TN_LAND only after a warpgroup barrier: the refill is an async-proxy write
+//   over it, and every thread's reads of it must have returned first (a barrier after the fence; see gemm_w3_tma_kernel).
+// * Two consumers (warpgroups 1 and 2, 64 rows of the tile each).  Per slice: wait "full", issue mma_slice_mn (transpose
+//   flags set) on one accumulator chain across the split's slices, then wait until only that group is in flight and
+//   release the stage of the slice before it ("empty", 256 arrivals).
+// Epilogue: one barrier over all 384 threads, after which every copy has landed and been split and every wgmma has
+// completed; the consumers pass their accumulators through the landing ring to tile_epilogue, and the producer reduces
+// its column-sum partials (written past the accumulator tile in the landing ring).
 // ---------------------------------------------------------------------------------------------------------------
 template <class Epi>
-__global__ void __launch_bounds__(THREADS, 1)
+__global__ void __launch_bounds__(TN_THREADS, 1)
 gemm_tn_kernel(int M, int N, int64_t K, int64_t k_chunk, Epi epi, float* __restrict__ colsum, float* __restrict__ cs_ws,
                const __grid_constant__ TnMaps maps) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = align1024(smem_raw);
-  const int tid = threadIdx.x, wg = tid >> 7, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, wg = tid >> 7, lane = tid & 31;
   const int m0 = blockIdx.x * BM;
   const int n0 = blockIdx.y * BN;
   const int64_t kb = (int64_t)blockIdx.z * k_chunk;
   const int64_t ke = (kb + k_chunk < K) ? kb + k_chunk : K;
   const bool do_csum = colsum != nullptr && blockIdx.y == 0;
-  float csum[4] = {0.f, 0.f, 0.f, 0.f};
   if (ke <= kb) return;
-  float acc[64];
-#pragma unroll
-  for (int q = 0; q < 64; ++q) acc[q] = 0.f;
-  uint8_t* ring = smem;
-  uint8_t* planes = smem + TN_RING * TN_F32_STAGE;
-  float* cs_part = reinterpret_cast<float*>(planes + 2 * TN_PLANE_STAGE);   // [4 k-quarters][128 columns]
-  uint64_t* full = reinterpret_cast<uint64_t*>(cs_part + 4 * BM);
+  uint8_t* land = smem;
+  uint8_t* planes = smem + TN_LAND * TN_F32_STAGE;
+  float* acc_s = reinterpret_cast<float*>(land);                               // after the main loop
+  float* cs_part = acc_s + BM * acc_ld(BN);                                    // [4 k-quarters][128 columns]
+  uint64_t* landed = reinterpret_cast<uint64_t*>(planes + TN_STAGES * TN_PLANE_STAGE);
+  uint64_t* full = landed + TN_LAND;
+  uint64_t* empty = full + TN_STAGES;
   const int n_sl = (int)((ke - kb + TN_PS - 1) / TN_PS);
-  const int opnd = warp >> 2, kq = warp & 3;
 
-  auto issue = [&](int i) {                               // one thread: slice i into ring stage i % TN_RING
-    const int r = i % TN_RING;
+  auto issue = [&](int i) {                               // one thread: slice i into landing stage i % TN_LAND
+    const int r = i % TN_LAND;
     const int k0 = (int)(kb + (int64_t)i * TN_PS);
-    uint8_t* st = ring + r * TN_F32_STAGE;
-    mbar_arrive_expect_tx(&full[r], TN_F32_STAGE);
-    tma_load_2d(st, &maps.a, m0, k0, &full[r]);
-    tma_load_2d(st + TN_F32_OPND, &maps.b, n0, k0, &full[r]);
-  };
-  // slice i from the ring into the plane stage dst.  Shared-memory traffic without bank conflicts: a warp's float4
-  // reads cover one point's 512 contiguous bytes, and each half-warp's 8-byte plane stores cover all 8 16-byte chunks
-  // of one 128-byte swizzled row (64 columns of one point), i.e. all 32 banks once.
-  auto split = [&](int i, uint8_t* dst) {
-    const int r = i % TN_RING;
-    mbar_wait(&full[r], (uint32_t)((i / TN_RING) & 1));
-    const float* f = reinterpret_cast<const float*>(ring + r * TN_F32_STAGE + opnd * TN_F32_OPND) + 4 * lane;
-    uint8_t* hi = dst + opnd * 2 * TN_PLANE;
-    const int64_t k0 = kb + (int64_t)i * TN_PS;
-#pragma unroll
-    for (int q = 0; q < TN_PS / 8; ++q) {
-      float4 v[2];
-#pragma unroll
-      for (int kk = 0; kk < 2; ++kk) {
-        const int p = 8 * q + 2 * kq + kk;
-        v[kk] = k0 + p < ke ? *reinterpret_cast<const float4*>(f + p * BM) : make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-      if (opnd == 0 && do_csum) {
-        csum[0] += v[0].x + v[1].x; csum[1] += v[0].y + v[1].y;
-        csum[2] += v[0].z + v[1].z; csum[3] += v[0].w + v[1].w;
-      }
-#pragma unroll
-      for (int kk = 0; kk < 2; ++kk) {
-        const float x[4] = {v[kk].x, v[kk].y, v[kk].z, v[kk].w};
-        uint2 pl[2];
-        split4<2>(x, pl);
-        const uint32_t off = sw128_mn(4u * lane, (uint32_t)(8 * q + 2 * kq + kk));
-        *reinterpret_cast<uint2*>(hi + off) = pl[0];
-        *reinterpret_cast<uint2*>(hi + TN_PLANE + off) = pl[1];
-      }
-    }
+    uint8_t* st = land + r * TN_F32_STAGE;
+    mbar_arrive_expect_tx(&landed[r], TN_F32_STAGE);
+    tma_load_2d(st, &maps.a, m0, k0, &landed[r]);
+    tma_load_2d(st + TN_F32_OPND, &maps.b, n0, k0, &landed[r]);
   };
   if (tid == 0) {
-    for (int r = 0; r < TN_RING; ++r) mbar_init(&full[r], 1);
+    for (int r = 0; r < TN_LAND; ++r) mbar_init(&landed[r], 1);
+    for (int s = 0; s < TN_STAGES; ++s) {
+      mbar_init(&full[s], 128);
+      mbar_init(&empty[s], 256);
+    }
     fence_barrier_init();
-    for (int i = 0; i < TN_RING && i < n_sl; ++i) issue(i);
+    for (int i = 0; i < TN_LAND && i < n_sl; ++i) issue(i);
   }
   __syncthreads();
-  split(0, planes);
-  fence_proxy_async();
-  __syncthreads();
-  if (tid == 0 && TN_RING < n_sl) issue(TN_RING);         // slice 0's ring stage is split
-  for (int i = 0; i < n_sl; ++i) {
-    const int s = i & 1;
-    const uint32_t st = smem_u32(planes + s * TN_PLANE_STAGE);
-    wg_fence();
-    mma_slice_mn(acc, st + wg * 4096u, st + 2 * TN_PLANE, i == 0);
-    wg_commit();
-    if (i + 1 < n_sl) split(i + 1, planes + (s ^ 1) * TN_PLANE_STAGE);   // released by the wait + barrier of i - 1
-    wg_wait_all();
-    fence_proxy_async();
-    __syncthreads();
-    if (tid == 0 && i + 1 + TN_RING < n_sl) issue(i + 1 + TN_RING);     // slice i + 1's ring stage is split
-  }
-  if (do_csum && opnd == 0)
+
+  if (wg == 0) {
+    reg_dealloc<TN_PRODUCER_REGS>();
+    const int kq = tid >> 5;
+    float csum[4] = {0.f, 0.f, 0.f, 0.f};
+    for (int i = 0; i < n_sl; ++i) {
+      const int r = i % TN_LAND, s = i % TN_STAGES;
+      uint8_t* st = planes + s * TN_PLANE_STAGE;
+      mbar_wait(&empty[s], ((i / TN_STAGES) & 1) ^ 1);
+      mbar_wait(&landed[r], (i / TN_LAND) & 1);
+      const int64_t left = ke - (kb + (int64_t)i * TN_PS);
+      const int np = left < TN_PS ? (int)left : TN_PS;     // points of this slice inside the chunk
+      const float* f = reinterpret_cast<const float*>(land + r * TN_F32_STAGE) + 4 * lane;
+      // Shared-memory traffic without bank conflicts: a warp's float4 reads cover one point's 512 contiguous bytes, and
+      // each half-warp's 8-byte plane stores cover all 8 16-byte chunks of one 128-byte swizzled row (64 columns of one
+      // point), i.e. all 32 banks once.  All 16 reads of a thread are in flight together: the wgmma operand fetches keep
+      // shared memory busy, and with fewer reads in flight the split, not the tensor core, set the pace.
+      float4 v[2][TN_PS / 8][2];
 #pragma unroll
-    for (int j = 0; j < 4; ++j) cs_part[kq * BM + 4 * lane + j] = csum[j];
-  float* acc_s = reinterpret_cast<float*>(smem);            // the ring: every copy has landed
-  acc_to_smem<BN>(acc, acc_s, wg, tid & 127);
-  __syncthreads();
-  if (do_csum && tid < BM && m0 + tid < M) {
-    const float c = (cs_part[tid] + cs_part[BM + tid]) + (cs_part[2 * BM + tid] + cs_part[3 * BM + tid]);
-    if (cs_ws != nullptr) cs_ws[(int64_t)blockIdx.z * M + m0 + tid] = c;
-    else colsum[m0 + tid] += c;
+      for (int opnd = 0; opnd < 2; ++opnd)
+#pragma unroll
+        for (int q = 0; q < TN_PS / 8; ++q)
+#pragma unroll
+          for (int kk = 0; kk < 2; ++kk) {
+            const int p = 8 * q + 2 * kq + kk;
+            v[opnd][q][kk] = p < np ? *reinterpret_cast<const float4*>(f + opnd * (TN_F32_OPND / 4) + p * BM) : make_float4(0.f, 0.f, 0.f, 0.f);
+          }
+      if (do_csum)
+#pragma unroll
+        for (int q = 0; q < TN_PS / 8; ++q) {
+          csum[0] += v[0][q][0].x + v[0][q][1].x; csum[1] += v[0][q][0].y + v[0][q][1].y;
+          csum[2] += v[0][q][0].z + v[0][q][1].z; csum[3] += v[0][q][0].w + v[0][q][1].w;
+        }
+#pragma unroll
+      for (int opnd = 0; opnd < 2; ++opnd)
+#pragma unroll
+        for (int q = 0; q < TN_PS / 8; ++q)
+#pragma unroll
+          for (int kk = 0; kk < 2; ++kk) {
+            const float x[4] = {v[opnd][q][kk].x, v[opnd][q][kk].y, v[opnd][q][kk].z, v[opnd][q][kk].w};
+            uint2 pl[2];
+            split4<2>(x, pl);
+            const uint32_t off = sw128_mn(4u * lane, (uint32_t)(8 * q + 2 * kq + kk));
+            *reinterpret_cast<uint2*>(st + opnd * 2 * TN_PLANE + off) = pl[0];
+            *reinterpret_cast<uint2*>(st + opnd * 2 * TN_PLANE + TN_PLANE + off) = pl[1];
+          }
+      fence_proxy_async();
+      mbar_arrive(&full[s]);
+      wg_bar_sync();                                      // every read of landing stage r has returned
+      if (tid == 0 && i + TN_LAND < n_sl) issue(i + TN_LAND);
+    }
+    if (do_csum)                                          // the landing ring is free: the last barrier above passed
+#pragma unroll
+      for (int j = 0; j < 4; ++j) cs_part[kq * BM + 4 * lane + j] = csum[j];
+    __syncthreads();
+    if (do_csum && m0 + tid < M) {
+      const float c = (cs_part[tid] + cs_part[BM + tid]) + (cs_part[2 * BM + tid] + cs_part[3 * BM + tid]);
+      if (cs_ws != nullptr) cs_ws[(int64_t)blockIdx.z * M + m0 + tid] = c;
+      else colsum[m0 + tid] += c;
+    }
+  } else {
+    reg_alloc<TN_CONSUMER_REGS>();
+    const int cw = wg - 1;
+    float acc[64];
+#pragma unroll
+    for (int q = 0; q < 64; ++q) acc[q] = 0.f;
+    for (int i = 0; i < n_sl; ++i) {
+      const int s = i % TN_STAGES;
+      mbar_wait(&full[s], (i / TN_STAGES) & 1);
+      const uint32_t st = smem_u32(planes + s * TN_PLANE_STAGE);
+      wg_fence();
+      mma_slice_mn(acc, st + cw * 4096u, st + 2 * TN_PLANE, i == 0);
+      wg_commit();
+      wg_wait_but_one();
+      if (i > 0) mbar_arrive(&empty[(i - 1) % TN_STAGES]);   // the group that read slice i - 1 has completed
+    }
+    wg_wait_all();
+    fence_operand(acc);
+    __syncthreads();                                      // the producer is done with the landing ring
+    acc_to_smem<BN>(acc, acc_s, cw, tid & 127);
+    tn_consumer_bar_sync();
+    tile_epilogue<BN>(acc_s, m0, M, n0, N, epi, tid - 128);
   }
-  tile_epilogue<BN>(acc_s, m0, M, n0, N, epi, tid);
 }
 
 static inline int sm_count() {
@@ -922,23 +963,25 @@ static inline int64_t tn_k_chunk(int M, int N, int64_t K) {
   return round_up(cdiv(K, splits), BK);
 }
 
-// the fp32 ring, 2 plane stages, the k-quarter column-sum partials and one mbarrier per ring stage
-constexpr size_t TN_RING_SMEM = (size_t)TN_RING * TN_F32_STAGE + 2 * TN_PLANE_STAGE + 4 * BM * sizeof(float) + TN_RING * sizeof(uint64_t) + 1024;
-static_assert(BM * acc_ld(BN) * sizeof(float) <= (size_t)TN_RING * TN_F32_STAGE, "accumulator tile in the ring");
-static_assert(TN_RING_SMEM <= 227 * 1024, "one CTA per SM");
+// the landing ring, the plane stages and an mbarrier per landing stage plus two per plane stage; the accumulator tile
+// and the column-sum partials reuse the landing ring
+constexpr size_t TN_SMEM = (size_t)TN_LAND * TN_F32_STAGE + (size_t)TN_STAGES * TN_PLANE_STAGE +
+                           (TN_LAND + 2 * TN_STAGES) * sizeof(uint64_t) + 1024;
+static_assert((BM * acc_ld(BN) + 4 * BM) * sizeof(float) <= (size_t)TN_LAND * TN_F32_STAGE, "accumulator tile and column sums in the landing ring");
+static_assert(TN_SMEM <= 227 * 1024, "one CTA per SM");
 
 template <class Epi>
 static inline int gemm_tn_launch(dim3 grid, const float* A, int64_t lda, const float* B, int64_t ldb, int M, int N, int64_t K,
                                  int64_t k_chunk, const Epi& epi, float* colsum, float* cs_ws, cudaStream_t st) {
   static bool attr_set = false;   // per template instantiation
   if (!attr_set) {
-    NUDF_CUDA_OK(cudaFuncSetAttribute(gemm_tn_kernel<Epi>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TN_RING_SMEM));
+    NUDF_CUDA_OK(cudaFuncSetAttribute(gemm_tn_kernel<Epi>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TN_SMEM));
     attr_set = true;
   }
   TnMaps maps{};
   if (int rc = tensor_map_2d(&maps.a, A, lda, M, K, BM, TN_PS)) return rc;
   if (int rc = tensor_map_2d(&maps.b, B, ldb, N, K, BN, TN_PS)) return rc;
-  gemm_tn_kernel<Epi><<<grid, THREADS, TN_RING_SMEM, st>>>(M, N, K, k_chunk, epi, colsum, cs_ws, maps);
+  gemm_tn_kernel<Epi><<<grid, TN_THREADS, TN_SMEM, st>>>(M, N, K, k_chunk, epi, colsum, cs_ws, maps);
   NUDF_LAUNCH_OK();
   return 0;
 }
