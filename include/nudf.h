@@ -568,6 +568,48 @@ int nudf_uc_resample(const float* pool, int64_t n_pool, int64_t m, uint32_t seed
                      void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * Camera visibility, orientation and colour of surface points (neuraludf_b200/paint.py drives the rounds; DESIGN.md
+ * section 1 states the algorithm)
+ * ------------------------------------------------------------------------------------------------------------
+ * p, n: fp32 [m,3] points and unit normal lines; mats fp32 [V,12], the row-major 3x4 pixel projections K w2c; centres fp32
+ * [V,3]; images fp32 [V,H,W,3]; all DEVICE.  Every fp32 operation is rounded once in the stated order, with no
+ * contraction: dot(a, b) = (a0 b0 + a1 b1) + a2 b2; the pixel of p is (x0 / x2, x1 / x2), x_r = dot(P_r, p) + P_r3; the
+ * direction to camera k is v = d / L, d = c_k - p, L = sqrt(dot(d, d)).  A pair (i, k) is the ray q(t) = p_i + t v; pairs
+ * are held as idx, cam int32 [A], t fp32 [A] and q fp32 [A,3] (the point where the caller evaluates the udf), and are
+ * compacted as the point clouds' survivors (NUDF_PT_SEG segments; count pass, then emit pass from the offsets). */
+#define NUDF_PT_SEG 256
+#define NUDF_PT_MAX_VIEWS 64
+#define NUDF_PT_MAX_CAND 8
+/* out = g / sqrt(dot(g, g)), 0 where that norm is 0 or not finite */
+int nudf_pt_normals(const float* g, int64_t m, float* out, void* stream);
+/* cand int32 [m,K] (m < 2^31, K <= NUDF_PT_MAX_CAND, V <= NUDF_PT_MAX_VIEWS): the cameras p lands in front of (x2 > 0)
+ * and inside [0,W-1] x [0,H-1], with |dot(n, v)| >= cos_min, by |dot(n, v)| descending, ties to the lower index; -1 pads */
+int nudf_pt_rank(const float* p, const float* n, int64_t m, const float* mats, const float* centres, int32_t V, int32_t H,
+                 int32_t W, float cos_min, int32_t K, int32_t* cand, void* stream);
+/* round r's pairs: every i with view[i] < 0 and k = cand[i,r] >= 0, in point order, at t0 = t_start / |dot(n, v)| */
+int nudf_pt_start_count(const float* p, const float* n, const int32_t* cand, int32_t K, int32_t r, const int32_t* view,
+                        int64_t m, const float* centres, float t_start, int32_t* counts, void* stream);
+int nudf_pt_start_emit(const float* p, const float* n, const int32_t* cand, int32_t K, int32_t r, const int32_t* view,
+                       int64_t m, const float* centres, float t_start, const int64_t* offsets, int32_t* out_idx,
+                       int32_t* out_cam, float* out_t, float* out_q, void* stream);
+/* one trace step with u fp32 [n], the udf at the pairs' q: a pair is occluded (dropped) unless u >= hit; else t += u and
+ * q = p + t v, and it is visible (dropped; the emit pass sets view[idx] = cam) when dot(q, q) > 1 or t >= L; the others
+ * stay active and are emitted in order */
+int nudf_pt_trace_count(const float* p, const float* centres, const int32_t* idx, const int32_t* cam, const float* t,
+                        const float* u, int64_t n, float hit, int32_t* counts, void* stream);
+int nudf_pt_trace_emit(const float* p, const float* centres, const int32_t* idx, const int32_t* cam, const float* t,
+                       const float* u, int64_t n, float hit, const int64_t* offsets, int32_t* view, int32_t* out_idx,
+                       int32_t* out_cam, float* out_t, float* out_q, void* stream);
+/* out = -n where view >= 0 and dot(n, v_view) < 0, else n (view values in [-1, V)) */
+int nudf_pt_orient(const float* p, const float* n, const int32_t* view, int64_t m, const float* centres, float* out,
+                   void* stream);
+/* out fp32 [m,3]: the bilinear sample of images[view] at p's pixel (u, w), pixel centres on the integers: x0 = floor(u),
+ * a = u - x0, x1 = min(x0 + 1, W - 1) (rows alike, b); top = c00 + a (c01 - c00), bottom = c10 + a (c11 - c10),
+ * out = top + b (bottom - top); 0 where view < 0 or p does not land in front and inside the view */
+int nudf_pt_gather(const float* p, const int32_t* view, int64_t m, const float* mats, const float* images, int32_t V,
+                   int32_t H, int32_t W, float* out, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------
  * Mesh post-processing (neuraludf_b200/mesh_post.py drives the steps; sorting, unique and compaction in torch)
  * ------------------------------------------------------------------------------------------------------------
  * verts: fp64 [V,3]; faces and edges: int64 rows.  All fp64 arithmetic is correctly rounded per operation with no

@@ -82,6 +82,8 @@ class BrickStore(ctypes.Structure):
 BRICK = 8   # NUDF_BRICK
 ISO_SEG = 256   # NUDF_ISO_SEG
 UC_SEG = 256    # NUDF_UC_SEG
+PT_SEG = 256    # NUDF_PT_SEG
+PT_MAX_VIEWS, PT_MAX_CAND = 64, 8      # NUDF_PT_MAX_VIEWS, NUDF_PT_MAX_CAND
 
 
 class Lattice(ctypes.Structure):
@@ -248,6 +250,18 @@ _SIGNATURES = {
     "nudf_uc_filter_emit": (ctypes.c_int, [c_void_p] * 2 + [ctypes.c_int64, ctypes.c_float] + [c_void_p] * 3),
     "nudf_uc_resample": (ctypes.c_int, [c_void_p, ctypes.c_int64, ctypes.c_int64, ctypes.c_uint32, ctypes.c_int32,
                                         ctypes.c_float, c_void_p, c_void_p]),
+    "nudf_pt_normals": (ctypes.c_int, [c_void_p, ctypes.c_int64, c_void_p, c_void_p]),
+    "nudf_pt_rank": (ctypes.c_int, [c_void_p, c_void_p, ctypes.c_int64, c_void_p, c_void_p] + [ctypes.c_int32] * 3
+                     + [ctypes.c_float, ctypes.c_int32, c_void_p, c_void_p]),
+    "nudf_pt_start_count": (ctypes.c_int, [c_void_p] * 3 + [ctypes.c_int32] * 2 + [c_void_p, ctypes.c_int64, c_void_p,
+                                                                                  ctypes.c_float, c_void_p, c_void_p]),
+    "nudf_pt_start_emit": (ctypes.c_int, [c_void_p] * 3 + [ctypes.c_int32] * 2 + [c_void_p, ctypes.c_int64, c_void_p,
+                                                                                 ctypes.c_float] + [c_void_p] * 6),
+    "nudf_pt_trace_count": (ctypes.c_int, [c_void_p] * 6 + [ctypes.c_int64, ctypes.c_float, c_void_p, c_void_p]),
+    "nudf_pt_trace_emit": (ctypes.c_int, [c_void_p] * 6 + [ctypes.c_int64, ctypes.c_float] + [c_void_p] * 7),
+    "nudf_pt_orient": (ctypes.c_int, [c_void_p] * 3 + [ctypes.c_int64] + [c_void_p] * 3),
+    "nudf_pt_gather": (ctypes.c_int, [c_void_p] * 2 + [ctypes.c_int64] + [c_void_p] * 2 + [ctypes.c_int32] * 3
+                       + [c_void_p] * 2),
     "nudf_mp_faces": (ctypes.c_int, [c_void_p, ctypes.c_int64, c_void_p, ctypes.c_int64] + [c_void_p] * 6),
     "nudf_mp_hole_count": (ctypes.c_int, [c_void_p, ctypes.c_int64, c_void_p, c_void_p, ctypes.c_int64, c_void_p, c_void_p]),
     "nudf_mp_hole_emit": (ctypes.c_int, [c_void_p] * 3 + [ctypes.c_int64, c_void_p, c_void_p, ctypes.c_int64]

@@ -190,6 +190,7 @@ def main(argv=None):
     import numpy as np
     from neuraludf_b200.evaluate import write_ply_points
     from neuraludf_b200.mesh import udf_network_from_state
+    from neuraludf_b200 import paint
     ap = argparse.ArgumentParser(prog="python -m neuraludf_b200.cloud",
                                  description="A dense point cloud on the zero level set of the UDF network of a runner "
                                              "checkpoint: narrow-band seeds projected along the gradient (udf_point_cloud).")
@@ -202,19 +203,23 @@ def main(argv=None):
     ap.add_argument("--seed", type=int, default=0, help="seed of the densify rounds' jitter")
     ap.add_argument("--scale", type=float, default=1.0, help="the conf's udf_network.scale")
     ap.add_argument("--cameras", default=None, help="cameras_sphere.npz: map the cloud to world space with its scale_mat_0")
+    paint.add_cli_args(ap)
     ap.add_argument("--out", required=True, help="output PLY")
     a = ap.parse_args(argv)
+    if (a.normals or a.colors) and a.scan_dir is None:
+        ap.error("--normals and --colors need --scan_dir")
     if not torch.cuda.is_available():
         raise SystemExit("point clouds are computed on a CUDA device")
     ck = torch.load(a.ckpt, map_location="cpu", weights_only=True)
     net = udf_network_from_state(ck["udf_network_fine"] if "udf_network_fine" in ck else ck, a.scale).cuda()
     info = {}
-    v = udf_point_cloud(net, a.resolution, a.points, a.steps, a.dist_threshold_ratio, seed=a.seed,
-                        info=info).double().cpu().numpy()
+    pts = udf_point_cloud(net, a.resolution, a.points, a.steps, a.dist_threshold_ratio, seed=a.seed, info=info)
+    normals, colors = paint.cli_paint(a, ck, net, pts, a.resolution) if a.scan_dir is not None else (None, None)
+    v = pts.double().cpu().numpy()
     if a.cameras is not None:                     # as the mesh CLI: the dataset's fp32 scale_mat_0
         sm = np.load(a.cameras)["scale_mat_0"].astype(np.float32)
-        v = v * sm[0, 0] + sm[:3, 3][None]
-    write_ply_points(a.out, v)
+        v = v * sm[0, 0] + sm[:3, 3][None]        # a uniform scale and a shift: the normals are unchanged
+    write_ply_points(a.out, v, colors=colors, normals=normals if a.normals else None)
     print("%s: %d points (%d seeds, %d after filtering, %d densify rounds)" % (a.out, v.shape[0], info["seeds"],
                                                                               info["filtered"], info["rounds_used"]))
     return v

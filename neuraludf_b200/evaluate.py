@@ -420,18 +420,31 @@ def read_ply(path):
     return verts, faces
 
 
-def write_ply_points(path, points, colors=None, ascii=False):
-    """A point cloud as PLY: double x / y / z and, with colors in [0,1], uchar red / green / blue (round(255 c))."""
+def _vertex_colors(colors, n):
+    """uchar round(255 c) of colours in [0,1], one row per vertex"""
+    c = np.asarray(torch.as_tensor(colors).detach().cpu().numpy(), dtype=np.float64).reshape(-1, 3)
+    if len(c) != n:
+        raise ValueError("colors must have one row per point")
+    return np.clip(np.round(c * 255.0), 0, 255).astype(np.uint8)
+
+
+def write_ply_points(path, points, colors=None, ascii=False, normals=None):
+    """A point cloud as PLY: double x / y / z, with normals float nx / ny / nz, and with colors in [0,1] uchar red / green /
+    blue (round(255 c))."""
     pts = np.ascontiguousarray(torch.as_tensor(points).detach().cpu().numpy(), dtype=np.float64).reshape(-1, 3)
     head = ["ply", "format %s 1.0" % ("ascii" if ascii else "binary_little_endian"), "element vertex %d" % len(pts),
             "property double x", "property double y", "property double z"]
     fields = [("x", "<f8"), ("y", "<f8"), ("z", "<f8")]
+    nrm = None
+    if normals is not None:
+        nrm = np.asarray(torch.as_tensor(normals).detach().cpu().numpy(), dtype=np.float32).reshape(-1, 3)
+        if len(nrm) != len(pts):
+            raise ValueError("normals must have one row per point")
+        head += ["property float nx", "property float ny", "property float nz"]
+        fields += [("nx", "<f4"), ("ny", "<f4"), ("nz", "<f4")]
     rgb = None
     if colors is not None:
-        c = np.asarray(torch.as_tensor(colors).detach().cpu().numpy(), dtype=np.float64).reshape(-1, 3)
-        if len(c) != len(pts):
-            raise ValueError("colors must have one row per point")
-        rgb = np.clip(np.round(c * 255.0), 0, 255).astype(np.uint8)
+        rgb = _vertex_colors(colors, len(pts))
         head += ["property uchar red", "property uchar green", "property uchar blue"]
         fields += [("red", "u1"), ("green", "u1"), ("blue", "u1")]
     head.append("end_header")
@@ -439,24 +452,35 @@ def write_ply_points(path, points, colors=None, ascii=False):
         f.write(("\n".join(head) + "\n").encode("ascii"))
         if ascii:
             for i in range(len(pts)):
-                row = ["%r" % float(x) for x in pts[i]] + ([str(int(x)) for x in rgb[i]] if rgb is not None else [])
+                row = (["%r" % float(x) for x in pts[i]] + (["%r" % float(x) for x in nrm[i]] if nrm is not None else [])
+                       + ([str(int(x)) for x in rgb[i]] if rgb is not None else []))
                 f.write((" ".join(row) + "\n").encode("ascii"))
         else:
             a = np.empty(len(pts), dtype=np.dtype(fields))
             a["x"], a["y"], a["z"] = pts[:, 0], pts[:, 1], pts[:, 2]
+            if nrm is not None:
+                a["nx"], a["ny"], a["nz"] = nrm[:, 0], nrm[:, 1], nrm[:, 2]
             if rgb is not None:
                 a["red"], a["green"], a["blue"] = rgb[:, 0], rgb[:, 1], rgb[:, 2]
             f.write(a.tobytes())
 
 
-def write_ply_mesh(path, verts, faces):
-    """A triangle mesh as binary little-endian PLY: double x / y / z and faces as `list uchar int vertex_indices`."""
+def write_ply_mesh(path, verts, faces, colors=None):
+    """A triangle mesh as binary little-endian PLY: double x / y / z, with colors in [0,1] uchar vertex red / green / blue
+    (round(255 c)), and faces as `list uchar int vertex_indices`."""
     v = np.ascontiguousarray(torch.as_tensor(verts).detach().cpu().numpy(), dtype="<f8").reshape(-1, 3)
     f = np.asarray(torch.as_tensor(faces).detach().cpu().numpy()).reshape(-1, 3)
     if f.size and (f.min() < 0 or f.max() >= len(v)):
         raise ValueError("face index out of range")
     head = ["ply", "format binary_little_endian 1.0", "element vertex %d" % len(v), "property double x", "property double y",
-            "property double z", "element face %d" % len(f), "property list uchar int vertex_indices", "end_header"]
+            "property double z"]
+    if colors is not None:
+        rgb = _vertex_colors(colors, len(v))
+        head += ["property uchar red", "property uchar green", "property uchar blue"]
+        a = np.empty(len(v), dtype=[("x", "<f8", (3,)), ("rgb", "u1", (3,))])
+        a["x"], a["rgb"] = v, rgb
+        v = a
+    head += ["element face %d" % len(f), "property list uchar int vertex_indices", "end_header"]
     fd = np.empty(len(f), dtype=[("n", "u1"), ("i", "<i4", (3,))])
     fd["n"], fd["i"] = 3, f
     with open(path, "wb") as fh:

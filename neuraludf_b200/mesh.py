@@ -568,9 +568,21 @@ def threshold_box(cameras=None):
     return lo[:3, 0].astype(np.float32), hi[:3, 0].astype(np.float32), sm
 
 
+def _paint(a, ck, net, verts, faces):
+    """the vertex colours of the CLI's --colors (None without), verts in the network's frame"""
+    if not a.colors:
+        return None
+    from neuraludf_b200 import paint
+    dev = torch.device("cuda")
+    v = torch.as_tensor(np.asarray(verts.cpu() if torch.is_tensor(verts) else verts), dtype=torch.float64).to(dev)
+    f = torch.as_tensor(np.asarray(faces.cpu() if torch.is_tensor(faces) else faces), dtype=torch.int64).to(dev)
+    return paint.cli_paint(a, ck, net, v, a.resolution, faces=f)[1]
+
+
 def main(argv=None):
     """python -m neuraludf_b200.mesh: a runner checkpoint's UDF network -> PLY mesh (see INTEGRATION.md)"""
     import argparse
+    from neuraludf_b200 import paint
     from neuraludf_b200.evaluate import write_ply_mesh
     ap = argparse.ArgumentParser(prog="python -m neuraludf_b200.mesh",
                                  description="Mesh the UDF network of a runner checkpoint: the mesh as udf_mesh makes it, with "
@@ -598,8 +610,11 @@ def main(argv=None):
                     help="apply the runner's post-processing (merge, duplicate and degenerate faces, hole filling, border "
                          "smoothing, the final merge after --cameras): the mesh Runner.extract_udf_mesh writes; the runner "
                          "passes --dist_threshold_ratio 5")
+    paint.add_cli_args(ap, normals=False)
     ap.add_argument("--out", required=True, help="output PLY")
     a = ap.parse_args(argv)
+    if a.colors and a.scan_dir is None:
+        ap.error("--colors needs --scan_dir")
     if a.sparse and (a.dense or (a.threshold is not None and not a.band)):
         ap.error("--sparse cannot be combined with %s" % ("--dense" if a.dense else "--threshold without --band"))
     if a.band and a.threshold is None:
@@ -627,9 +642,10 @@ def main(argv=None):
         else:
             v, faces = extract_geometry(bmin, bmax, a.resolution, a.threshold, lambda pts: net.udf_values(pts),
                                         torch.device("cuda"))
+        colors = _paint(a, ck, net, v, faces)
         if sm is not None:
             v = v * sm[0, 0] + sm[:3, 3][None]
-        write_ply_mesh(a.out, v, faces)
+        write_ply_mesh(a.out, v, faces, colors=colors)
         print("%s: %d vertices, %d faces" % (a.out, v.shape[0], faces.shape[0]))
         return v, np.asarray(faces)
     if a.postprocess:
@@ -645,7 +661,11 @@ def main(argv=None):
         from neuraludf_b200.mesh_post import export_merge
         vt, faces = export_merge(torch.from_numpy(v).to(verts.device), faces)
         v = vt.cpu().numpy()
-    write_ply_mesh(a.out, v, faces)
+        if a.cameras is not None and a.colors:    # the merged mesh back in the network's frame, for its colours
+            verts = (vt - torch.from_numpy(sm[:3, 3]).double().to(vt.device)) / float(sm[0, 0])
+        else:
+            verts = vt
+    write_ply_mesh(a.out, v, faces, colors=_paint(a, ck, net, verts, faces))
     print("%s: %d vertices, %d faces" % (a.out, v.shape[0], faces.shape[0]))
     return v, faces.cpu().numpy()
 

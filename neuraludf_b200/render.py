@@ -359,15 +359,10 @@ def load_checkpoint(path):
         return torch.load(path, map_location="cpu", weights_only=True)
 
 
-def networks_from_checkpoint(ck, device):
-    """UDF, colour, NeRF++, variance and beta networks of a runner checkpoint (exp_runner_blending.py:484-495), their
-    shapes read off the weights: the UDF network as mesh.udf_network_from_state; colour lin_base0 [d_hidden, 3 + d_feature],
-    lin0 [d_hidden, d_hidden + 6 + 6 multires_view], last main layer [3 + blending views, d_hidden]; NeRF pts_linears.0
-    [W, 4 + 8 multires], a layer after a skip [W, W + 4 + 8 multires], views_linears.0 [W/2, W + 3 + 6 multires_view]."""
-    from neuraludf_b200.mesh import udf_network_from_state
+def color_network_from_state(cs):
+    """A ResidualRenderingNetwork holding the state dict `cs` (the runner's `color_network_fine`), its shape read off the
+    weights as networks_from_checkpoint describes"""
     from neuraludf_b200.models import fields as F
-    udf = udf_network_from_state(ck["udf_network_fine"])
-    cs = ck["color_network_fine"]
     n_lin = 0
     while "lin%d.weight_v" % n_lin in cs:
         n_lin += 1
@@ -378,6 +373,18 @@ def networks_from_checkpoint(ck, device):
                                      squeeze_out=True,
                                      blending_cand_views=int(cs["lin%d.weight_v" % (n_lin - 1)].shape[0]) - 3)
     col.load_state_dict(cs)
+    return col
+
+
+def networks_from_checkpoint(ck, device):
+    """UDF, colour, NeRF++, variance and beta networks of a runner checkpoint (exp_runner_blending.py:484-495), their
+    shapes read off the weights: the UDF network as mesh.udf_network_from_state; colour lin_base0 [d_hidden, 3 + d_feature],
+    lin0 [d_hidden, d_hidden + 6 + 6 multires_view], last main layer [3 + blending views, d_hidden]; NeRF pts_linears.0
+    [W, 4 + 8 multires], a layer after a skip [W, W + 4 + 8 multires], views_linears.0 [W/2, W + 3 + 6 multires_view]."""
+    from neuraludf_b200.mesh import udf_network_from_state
+    from neuraludf_b200.models import fields as F
+    udf = udf_network_from_state(ck["udf_network_fine"])
+    col = color_network_from_state(ck["color_network_fine"])
     ns = ck["nerf"]
     D = 0
     while "pts_linears.%d.weight" % D in ns:
