@@ -8,6 +8,11 @@ the flat buffer and autograd adopts those views as `.grad` -- no pack / unpack c
 region's all-reduce is issued asynchronously as soon as its backward kernels have been enqueued (the colour network's
 gradients travel while the ~4 ms UDF backward still runs); `allreduce_mean()` reduces what is left and waits.
 Parameters without a sink (the scalar heads) are packed into a small tail of the same buffer.
+
+The kernels OVERWRITE their targets, so a backward invocation may only write the region when the region holds nothing
+autograd still has to add to.  Otherwise (the network appears twice in one backward, two backward passes are accumulated,
+or zero_grad(set_to_none=False) kept the `.grad` views) it writes fresh tensors and autograd adds them to what is there;
+`allreduce_mean()` copies any gradient that does not live in its slot into it before reducing.
 """
 import torch
 import torch.distributed as dist
@@ -28,21 +33,33 @@ def shard_rays(rays_o, rays_d, *more, rank=None, world=None):
     return tuple(t[lo:hi] for t in (rays_o, rays_d) + more)
 
 
+class _Reduced:
+    """the collective handle of a region already reduced synchronously (every backend but NCCL): nothing to wait for"""
+
+    @staticmethod
+    def wait():
+        return True
+
+
 class _Region:
     """Contiguous slice [lo, hi) of the flat buffer holding all gradients of one kernel-backed network."""
 
     def __init__(self, bucket, lo):
         self.bucket, self.lo, self.hi = bucket, lo, lo
         self.offsets = {}            # id(param) -> (offset, shape)
-        self.work = None
-        self.written = False
-        self.first = None
+        self.params = []
+        self.work = None             # the region's collective once ready() issued it (overlap at world > 1)
+        self.task = None             # the autograd graph task (one backward call) whose kernels last wrote the region
 
     def add(self, p):
-        if self.first is None:
-            self.first = p
+        self.params.append(p)
         self.offsets[id(p)] = (self.hi, tuple(p.shape))
         self.hi += p.numel()
+
+    def holds(self, p):
+        """True if p.grad is the slot of p (the tensor view() hands out, adopted by autograd)"""
+        flat = self.bucket.flat
+        return p.grad is not None and p.grad.data_ptr() == flat.data_ptr() + self.offsets[id(p)][0] * flat.element_size()
 
     def block(self, params):
         """one contiguous view covering `params` (which were added consecutively), e.g. all biases of a network"""
@@ -56,22 +73,24 @@ class _Region:
         return self.bucket.flat.narrow(0, off, p.numel()).view(shape)
 
     def begin(self):
-        """True if this backward invocation may write the region.  A second invocation in the same step (the network
-        appears twice in the graph) must use fresh tensors instead: autograd then accumulates them into the views."""
-        if self.written and self.work is None and self.first.grad is None:
-            self.written = False         # the gradients were cleared (zero_grad(set_to_none=True)): a new step has begun
-        if not self.written:
-            return True
+        """True if this backward invocation may write the region (its kernels overwrite it).  False when autograd has
+        something to add the invocation's gradients to: the region was already written in this backward call (the
+        network appears twice in the graph), or a parameter still holds a `.grad` (backward passes accumulated before
+        allreduce_mean(), or zero_grad(set_to_none=False)), which may be a view of the region.  The invocation then
+        writes fresh tensors and autograd sums them."""
         if self.work is not None:
-            raise RuntimeError("GradBucket(overlap=True): a kernel-backed network ran backward twice in one step after its "
-                               "gradients were already handed to the collective; construct the bucket with overlap=False")
-        return False
+            raise RuntimeError("GradBucket(overlap=True): a kernel-backed network ran backward again after its gradients "
+                               "were handed to the collective (it appears twice in one backward, or backward passes are "
+                               "accumulated before allreduce_mean()); construct the bucket with overlap=False")
+        if self.task == torch._C._current_graph_task_id():
+            return False
+        return all(p.grad is None for p in self.params)
 
     def ready(self):
         """called by the backward wrapper once every kernel writing this region has been enqueued"""
-        self.written = True
+        self.task = torch._C._current_graph_task_id()
         b = self.bucket
-        if b.overlap and b.world() > 1 and self.work is None:
+        if b.overlap and b.world() > 1:
             self.work = b._reduce(b.flat.narrow(0, self.lo, self.hi - self.lo), async_op=True)
 
 
@@ -114,12 +133,12 @@ class GradBucket:
         return dist.get_world_size(self.group) if dist.is_available() and dist.is_initialized() else 1
 
     def _reduce(self, t, async_op=False):
-        """mean over ranks, in place"""
+        """mean over ranks, in place; with async_op a handle to wait() on (other backends than NCCL reduce at once)"""
         if dist.get_backend(self.group) == "nccl":
             return dist.all_reduce(t, op=dist.ReduceOp.AVG, group=self.group, async_op=async_op)
-        w = dist.all_reduce(t, op=dist.ReduceOp.SUM, group=self.group, async_op=False)
+        dist.all_reduce(t, op=dist.ReduceOp.SUM, group=self.group, async_op=False)
         t.mul_(1.0 / self.world())
-        return w
+        return _Reduced() if async_op else None
 
     def allreduce_replayed(self):
         """All-reduce after a CUDA-graph REPLAY of forward + backward: the kernels have written every region of the flat
@@ -145,41 +164,46 @@ class GradBucket:
             off += n
 
     def allreduce_mean(self, group=None):
+        """Afterwards every sinked parameter's `.grad` is its slot of `flat` (at world 1: every one that has a gradient)."""
         if group is not None:
             self.group = group
-        if self.world() == 1:
-            for r in self.regions:
-                r.work, r.written = None, False
-            return
-        # regions whose backward never ran this step (e.g. a network outside the graph) hold stale data: zero them
+        world = self.world()
         for r in self.regions:
-            if not r.written:
-                self.flat.narrow(0, r.lo, r.hi - r.lo).zero_()
-        off = self.loose_lo
-        for p in self.loose:
-            n = p.numel()
-            if p.grad is None:
-                self.flat.narrow(0, off, n).zero_()
-            else:
-                self.flat.narrow(0, off, n).copy_(p.grad.reshape(-1))
-            off += n
-        pending = [r for r in self.regions if r.work is None]
-        works = [r.work for r in self.regions if r.work is not None]
-        if not works:
-            self._reduce(self.flat)                              # nothing in flight: one collective for everything
-        else:
-            for r in pending:
-                self._reduce(self.flat.narrow(0, r.lo, r.hi - r.lo))
-            if self.loose:
-                self._reduce(self.flat.narrow(0, self.loose_lo, self.flat.numel() - self.loose_lo))
-            for w in works:
-                if w is not None:
+            if r.work is not None:
+                continue                             # in the collective already: the gradients are the slots
+            for p in r.params:
+                if p.grad is None:
+                    if world > 1:
+                        r.view(p).zero_()            # e.g. a network outside this step's graph: it adds zero to the mean
+                elif not r.holds(p):
+                    r.view(p).copy_(p.grad)          # summed by autograd from fresh tensors (see _Region.begin)
+        if world > 1:
+            off = self.loose_lo
+            for p in self.loose:
+                n = p.numel()
+                if p.grad is None:
+                    self.flat.narrow(0, off, n).zero_()
+                else:
+                    self.flat.narrow(0, off, n).copy_(p.grad.reshape(-1))
+                off += n
+            works = [r.work for r in self.regions if r.work is not None]
+            if not works:
+                self._reduce(self.flat)                          # nothing in flight: one collective for everything
+            else:                                                # each element enters one collective
+                for r in self.regions:
+                    if r.work is None:
+                        self._reduce(self.flat.narrow(0, r.lo, r.hi - r.lo))
+                if self.loose:
+                    self._reduce(self.flat.narrow(0, self.loose_lo, self.flat.numel() - self.loose_lo))
+                for w in works:
                     w.wait()
         for r in self.regions:
-            for p in self.params:
-                if id(p) in r.offsets and p.grad is None:
+            for p in r.params:
+                if (p.grad is not None or world > 1) and not r.holds(p):
                     p.grad = r.view(p)
-            r.work, r.written = None, False
+            r.work, r.task = None, None
+        if world == 1:
+            return
         off = self.loose_lo
         for p in self.loose:
             n = p.numel()
