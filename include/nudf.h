@@ -269,11 +269,32 @@ int nudf_render_composite_backward(const nudf_render_cfg* cfg, const float* head
                                    float* sc_bar, float* bg_alpha_bar, float* bg_color_bar, float* scalar_bar,
                                    void* stream);
 
+/* The three compositing entry points above under a chosen sdf2alpha rule (:292-325).  Arguments as above plus
+ *   alpha_rule  0 = 'numerical' (:308-320; exactly the entry points above, same bits),
+ *               1 = 'theorical' (:321-323): alpha = 1 - exp(-relu(|iter_cos| inv_s (1 - sigmoid(sdf inv_s))) dist).
+ * The backward pass is the adjoint of the forward pass under the same rule. */
+int nudf_render_composite_forward_rule(const nudf_render_cfg* cfg, const float* heads, const float* rays_d, const float* pts,
+                                       const float* mid_z, const float* dists, const float* udf, int64_t ld_udf,
+                                       const float* grads, const float* sampled_color_base, const float* sampled_color,
+                                       const float* bg_alpha, const float* bg_color, const nudf_render_out* out,
+                                       int32_t alpha_rule, void* stream);
+int nudf_render_view_forward_rule(const nudf_render_cfg* cfg, const float* heads, const float* rays_d, const float* pts,
+                                  const float* mid_z, const float* dists, const float* udf, int64_t ld_udf, const float* grads,
+                                  const float* sampled_color, const float* c_pix, const float* bg_alpha, const float* bg_color,
+                                  const float* rot, const nudf_view_out* out, int32_t alpha_rule, void* stream);
+int nudf_render_composite_backward_rule(const nudf_render_cfg* cfg, const float* heads, const float* rays_d, const float* pts,
+                                        const float* mid_z, const float* dists, const float* udf, int64_t ld_udf,
+                                        const float* grads, const float* sampled_color_base, const float* sampled_color,
+                                        const float* bg_alpha, const float* bg_color, const nudf_render_bar* bar,
+                                        float* udf_bar, float* grads_bar, float* scb_bar, float* sc_bar, float* bg_alpha_bar,
+                                        float* bg_color_bar, float* scalar_bar, int32_t alpha_rule, void* stream);
+
 /* ------------------------------------------------------------------------------------------------------------
  * hierarchical sampling  (reference: models/udf_renderer_blending.py:66-104, 197-290, 723-755, 834-866)
  * ------------------------------------------------------------------------------------------------------------ */
 /* One up-sampling round: new_z[N,m] (and optionally the searchsorted indices inds[N,m], int64) from z[N,n], udf[N,n].
- * mode 0 = up_sample_unbias (:197-272), 1 = up_sample_no_occ_aware (:834-866).  Scans are accumulated in fp64 and
+ * mode 0 = up_sample_unbias (:197-272), 1 = up_sample_no_occ_aware (:834-866), 2 = up_sample_unbias with the
+ * 'theorical' sdf2alpha (:321-323) in place of the 'numerical' one.  Scans are accumulated in fp64 and
  * rounded to fp32 per element, like torch's CPU cumsum/cumprod, so that indices are reproducible.
  * u_lin: DEVICE float[m] = torch.linspace(0.5/m, 1-0.5/m, m) (:76), supplied by the caller so that its rounding is
  * exactly torch's.  status: DEVICE int or NULL, see NUDF_STATUS_NONFINITE_SAMPLES. */

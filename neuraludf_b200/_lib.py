@@ -180,6 +180,12 @@ _SIGNATURES = {
     "nudf_render_composite_forward": (ctypes.c_int, [c_void_p] * 2 + [c_void_p] * 5 + [ctypes.c_int64] + [c_void_p] * 7),
     "nudf_render_view_forward": (ctypes.c_int, [c_void_p] * 2 + [c_void_p] * 5 + [ctypes.c_int64] + [c_void_p] * 8),
     "nudf_render_composite_backward": (ctypes.c_int, [c_void_p] * 2 + [c_void_p] * 5 + [ctypes.c_int64] + [c_void_p] * 14),
+    "nudf_render_composite_forward_rule": (ctypes.c_int, [c_void_p] * 2 + [c_void_p] * 5 + [ctypes.c_int64] + [c_void_p] * 6
+                                           + [ctypes.c_int32, c_void_p]),
+    "nudf_render_view_forward_rule": (ctypes.c_int, [c_void_p] * 2 + [c_void_p] * 5 + [ctypes.c_int64] + [c_void_p] * 7
+                                      + [ctypes.c_int32, c_void_p]),
+    "nudf_render_composite_backward_rule": (ctypes.c_int, [c_void_p] * 2 + [c_void_p] * 5 + [ctypes.c_int64]
+                                            + [c_void_p] * 13 + [ctypes.c_int32, c_void_p]),
     "nudf_up_sample": (ctypes.c_int, [ctypes.c_int32, c_void_p, c_void_p, c_void_p, c_void_p, ctypes.c_int32,
                                       ctypes.c_int32, ctypes.c_int32, ctypes.c_float, ctypes.c_float, ctypes.c_float,
                                       ctypes.c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),

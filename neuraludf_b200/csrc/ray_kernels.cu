@@ -104,7 +104,9 @@ struct RayIn {
   const float* grads; const float* scb; const float* sc; const float* bg_alpha; const float* bg_color;
 };
 
-// Steps shared by forward and backward: fills tc, q, t, P, ap, am, alpha, T for ray r.
+// Steps shared by forward and backward: fills tc, q, t, P, ap, am, alpha, T for ray r.  RULE is the alpha rule
+// (AlphaRule, raymath.cuh) of pass 3.
+template <int RULE>
 __device__ __forceinline__ void ray_forward_state(const nudf_render_cfg& cfg, const RayIn& in, int r, int lane, RaySmem sm) {
   const int S = cfg.n_samples, O = cfg.n_outside, SO = S + O;
   const int64_t base = (int64_t)r * S;
@@ -147,8 +149,8 @@ __device__ __forceinline__ void ray_forward_state(const nudf_render_cfg& cfg, co
       float u = in.udf[(base + i) * in.ld_udf];
       float dist = in.dists[base + i];
       float ic = iter_cos_forward(sm.tc[i], cfg.has_cos_anneal, cfg.cos_anneal_ratio);
-      float ap = neus_alpha_forward(u, ic, dist, inv_s);
-      float am = neus_alpha_forward(-u, ic, dist, inv_s);
+      float ap = alpha_forward<RULE>(u, ic, dist, inv_s);
+      float am = alpha_forward<RULE>(-u, ic, dist, inv_s);
       float vis = clampf_(sm.P[i], 0.0f, 1.0f);
       sm.ap[i] = ap; sm.am[i] = am;
       a = ap * vis + am * (1.0f - vis);
@@ -284,6 +286,7 @@ struct CoreExtra {
   }
 };
 
+template <int RULE>
 __global__ void __launch_bounds__(RK_WARPS * 32)
 composite_forward_kernel(nudf_render_cfg cfg, RayIn in, nudf_render_out out) {
   extern __shared__ float smem[];
@@ -292,7 +295,7 @@ composite_forward_kernel(nudf_render_cfg cfg, RayIn in, nudf_render_out out) {
   if (r >= cfg.n_rays) return;
   const int S = cfg.n_samples, O = cfg.n_outside, SO = S + O;
   RaySmem sm = carve(smem + (size_t)warp * RK_ARRAYS * SO, SO, RK_ARRAYS);
-  ray_forward_state(cfg, in, r, lane, sm);
+  ray_forward_state<RULE>(cfg, in, r, lane, sm);
 
   CoreExtra ex(cfg, in, out, sm, r);
   const RaySums s = ray_composite(cfg, in, r, lane, sm, ex);
@@ -362,6 +365,7 @@ struct ViewArgs {
   nudf_view_out out;
 };
 
+template <int RULE>
 __global__ void __launch_bounds__(RK_WARPS * 32)
 view_forward_kernel(nudf_render_cfg cfg, RayIn in, ViewArgs va) {
   extern __shared__ float smem[];
@@ -370,7 +374,7 @@ view_forward_kernel(nudf_render_cfg cfg, RayIn in, ViewArgs va) {
   if (r >= cfg.n_rays) return;
   const int S = cfg.n_samples, O = cfg.n_outside, SO = S + O;
   RaySmem sm = carve(smem + (size_t)warp * RK_ARRAYS * SO, SO, RK_ARRAYS);
-  ray_forward_state(cfg, in, r, lane, sm);
+  ray_forward_state<RULE>(cfg, in, r, lane, sm);
 
   ViewExtra ex(in, va.c_pix, (int64_t)r * SO, O > 0);
   const RaySums s = ray_composite(cfg, in, r, lane, sm, ex);
@@ -400,6 +404,7 @@ struct RayBar {
   const float* ray_sums;  // [N,5] upstream gradient of the per-ray regulariser sums
 };
 
+template <int RULE>
 __global__ void __launch_bounds__(RK_WARPS * 32)
 composite_backward_kernel(nudf_render_cfg cfg, RayIn in, RayBar bar, RayBwdOut out) {
   extern __shared__ float smem[];
@@ -408,7 +413,7 @@ composite_backward_kernel(nudf_render_cfg cfg, RayIn in, RayBar bar, RayBwdOut o
   if (r >= cfg.n_rays) return;
   const int S = cfg.n_samples, O = cfg.n_outside, SO = S + O;
   RaySmem sm = carve(smem + (size_t)warp * RK_ARRAYS * SO, SO, RK_ARRAYS);
-  ray_forward_state(cfg, in, r, lane, sm);
+  ray_forward_state<RULE>(cfg, in, r, lane, sm);
 
   const int64_t base = (int64_t)r * S;
   const float d[3] = {in.rays_d[r * 3 + 0], in.rays_d[r * 3 + 1], in.rays_d[r * 3 + 2]};
@@ -519,8 +524,8 @@ composite_backward_kernel(nudf_render_cfg cfg, RayIn in, RayBar bar, RayBwdOut o
     float ap_bar = ab * vis, am_bar = ab * (1.0f - vis);
     float ic = iter_cos_forward(tc, cfg.has_cos_anneal, cfg.cos_anneal_ratio);
     float sdf_b1, ic_b1, s_b1, sdf_b2, ic_b2, s_b2;
-    neus_alpha_backward(u, ic, dist, inv_s, ap_bar, &sdf_b1, &ic_b1, &s_b1);
-    neus_alpha_backward(-u, ic, dist, inv_s, am_bar, &sdf_b2, &ic_b2, &s_b2);
+    alpha_backward<RULE>(u, ic, dist, inv_s, ap_bar, &sdf_b1, &ic_b1, &s_b1);
+    alpha_backward<RULE>(-u, ic, dist, inv_s, am_bar, &sdf_b2, &ic_b2, &s_b2);
     float u_bar = sdf_b1 - sdf_b2;
     s_bar += s_b1 + s_b2;
     float tc_bar = (ic_b1 + ic_b2) * iter_cos_dtc(tc, cfg.has_cos_anneal, cfg.cos_anneal_ratio);
@@ -595,27 +600,81 @@ static int check_cfg(const nudf_render_cfg* cfg, const float* bg_alpha, const fl
   return 0;
 }
 
-int nudf_render_composite_forward(const nudf_render_cfg* cfg, const float* heads, const float* rays_d, const float* pts, const float* mid_z,
-                                  const float* dists, const float* udf, int64_t ld_udf, const float* grads,
-                                  const float* sampled_color_base, const float* sampled_color, const float* bg_alpha,
-                                  const float* bg_color, const nudf_render_out* out, void* stream) {
-  if (int rc = check_cfg(cfg, bg_alpha, bg_color)) return rc;
-  NUDF_REQUIRE(heads && rays_d && pts && mid_z && dists && udf && grads && sampled_color_base && sampled_color && out, "null pointer");
-  if (cfg->n_rays <= 0) return 0;
-  RayIn in{heads, rays_d, pts, mid_z, dists, udf, ld_udf, grads, sampled_color_base, sampled_color, bg_alpha, bg_color};
+}  // extern "C"
+
+namespace {
+
+// Launchers shared by the entry points with and without an alpha rule: one kernel instantiation per rule.
+template <int RULE>
+int composite_forward_launch(const nudf_render_cfg* cfg, const RayIn& in, const nudf_render_out* out, cudaStream_t st) {
   size_t smem = (size_t)RK_WARPS * RK_ARRAYS * (cfg->n_samples + cfg->n_outside) * sizeof(float);
   if (smem > 48 * 1024)
-    NUDF_CUDA_OK(cudaFuncSetAttribute(composite_forward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  LaunchTimer lt_(FAM_RAY, (cudaStream_t)stream);
-  composite_forward_kernel<<<(unsigned)cdiv(cfg->n_rays, RK_WARPS), RK_WARPS * 32, smem, (cudaStream_t)stream>>>(*cfg, in, *out);
+    NUDF_CUDA_OK(cudaFuncSetAttribute(composite_forward_kernel<RULE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  LaunchTimer lt_(FAM_RAY, st);
+  composite_forward_kernel<RULE><<<(unsigned)cdiv(cfg->n_rays, RK_WARPS), RK_WARPS * 32, smem, st>>>(*cfg, in, *out);
   NUDF_LAUNCH_OK();
   return 0;
 }
 
-int nudf_render_view_forward(const nudf_render_cfg* cfg, const float* heads, const float* rays_d, const float* pts,
-                             const float* mid_z, const float* dists, const float* udf, int64_t ld_udf, const float* grads,
-                             const float* sampled_color, const float* c_pix, const float* bg_alpha, const float* bg_color,
-                             const float* rot, const nudf_view_out* out, void* stream) {
+template <int RULE>
+int view_forward_launch(const nudf_render_cfg* cfg, const RayIn& in, const ViewArgs& va, cudaStream_t st) {
+  size_t smem = (size_t)RK_WARPS * RK_ARRAYS * (cfg->n_samples + cfg->n_outside) * sizeof(float);
+  if (smem > 48 * 1024)
+    NUDF_CUDA_OK(cudaFuncSetAttribute(view_forward_kernel<RULE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  LaunchTimer lt_(FAM_RAY, st);
+  view_forward_kernel<RULE><<<(unsigned)cdiv(cfg->n_rays, RK_WARPS), RK_WARPS * 32, smem, st>>>(*cfg, in, va);
+  NUDF_LAUNCH_OK();
+  return 0;
+}
+
+template <int RULE>
+int composite_backward_launch(const nudf_render_cfg* cfg, const RayIn& in, const RayBar& rb, const RayBwdOut& ob,
+                              cudaStream_t st) {
+  size_t smem = (size_t)RK_WARPS * RK_ARRAYS * (cfg->n_samples + cfg->n_outside) * sizeof(float);
+  if (smem > 48 * 1024)
+    NUDF_CUDA_OK(cudaFuncSetAttribute(composite_backward_kernel<RULE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  LaunchTimer lt_(FAM_RAY, st);
+  composite_backward_kernel<RULE><<<(unsigned)cdiv(cfg->n_rays, RK_WARPS), RK_WARPS * 32, smem, st>>>(*cfg, in, rb, ob);
+  NUDF_LAUNCH_OK();
+  return 0;
+}
+
+int check_rule(int32_t alpha_rule) {
+  NUDF_REQUIRE(alpha_rule == ALPHA_NUMERICAL || alpha_rule == ALPHA_THEORICAL, "alpha_rule must be 0 (numerical) or 1 (theorical)");
+  return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int nudf_render_composite_forward_rule(const nudf_render_cfg* cfg, const float* heads, const float* rays_d, const float* pts,
+                                       const float* mid_z, const float* dists, const float* udf, int64_t ld_udf,
+                                       const float* grads, const float* sampled_color_base, const float* sampled_color,
+                                       const float* bg_alpha, const float* bg_color, const nudf_render_out* out,
+                                       int32_t alpha_rule, void* stream) {
+  if (int rc = check_rule(alpha_rule)) return rc;
+  if (int rc = check_cfg(cfg, bg_alpha, bg_color)) return rc;
+  NUDF_REQUIRE(heads && rays_d && pts && mid_z && dists && udf && grads && sampled_color_base && sampled_color && out, "null pointer");
+  if (cfg->n_rays <= 0) return 0;
+  RayIn in{heads, rays_d, pts, mid_z, dists, udf, ld_udf, grads, sampled_color_base, sampled_color, bg_alpha, bg_color};
+  return alpha_rule == ALPHA_THEORICAL ? composite_forward_launch<ALPHA_THEORICAL>(cfg, in, out, (cudaStream_t)stream)
+                                       : composite_forward_launch<ALPHA_NUMERICAL>(cfg, in, out, (cudaStream_t)stream);
+}
+
+int nudf_render_composite_forward(const nudf_render_cfg* cfg, const float* heads, const float* rays_d, const float* pts, const float* mid_z,
+                                  const float* dists, const float* udf, int64_t ld_udf, const float* grads,
+                                  const float* sampled_color_base, const float* sampled_color, const float* bg_alpha,
+                                  const float* bg_color, const nudf_render_out* out, void* stream) {
+  return nudf_render_composite_forward_rule(cfg, heads, rays_d, pts, mid_z, dists, udf, ld_udf, grads, sampled_color_base,
+                                            sampled_color, bg_alpha, bg_color, out, ALPHA_NUMERICAL, stream);
+}
+
+int nudf_render_view_forward_rule(const nudf_render_cfg* cfg, const float* heads, const float* rays_d, const float* pts,
+                                  const float* mid_z, const float* dists, const float* udf, int64_t ld_udf, const float* grads,
+                                  const float* sampled_color, const float* c_pix, const float* bg_alpha, const float* bg_color,
+                                  const float* rot, const nudf_view_out* out, int32_t alpha_rule, void* stream) {
+  if (int rc = check_rule(alpha_rule)) return rc;
   if (int rc = check_cfg(cfg, bg_alpha, bg_color)) return rc;
   NUDF_REQUIRE(heads && rays_d && pts && mid_z && dists && udf && grads && sampled_color && rot && out, "null pointer");
   if (cfg->n_rays <= 0) return 0;
@@ -624,21 +683,25 @@ int nudf_render_view_forward(const nudf_render_cfg* cfg, const float* heads, con
   va.c_pix = c_pix;
   for (int k = 0; k < 9; ++k) va.rot[k] = rot[k];
   va.out = *out;
-  size_t smem = (size_t)RK_WARPS * RK_ARRAYS * (cfg->n_samples + cfg->n_outside) * sizeof(float);
-  if (smem > 48 * 1024)
-    NUDF_CUDA_OK(cudaFuncSetAttribute(view_forward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  LaunchTimer lt_(FAM_RAY, (cudaStream_t)stream);
-  view_forward_kernel<<<(unsigned)cdiv(cfg->n_rays, RK_WARPS), RK_WARPS * 32, smem, (cudaStream_t)stream>>>(*cfg, in, va);
-  NUDF_LAUNCH_OK();
-  return 0;
+  return alpha_rule == ALPHA_THEORICAL ? view_forward_launch<ALPHA_THEORICAL>(cfg, in, va, (cudaStream_t)stream)
+                                       : view_forward_launch<ALPHA_NUMERICAL>(cfg, in, va, (cudaStream_t)stream);
 }
 
-int nudf_render_composite_backward(const nudf_render_cfg* cfg, const float* heads, const float* rays_d, const float* pts, const float* mid_z,
-                                   const float* dists, const float* udf, int64_t ld_udf, const float* grads,
-                                   const float* sampled_color_base, const float* sampled_color, const float* bg_alpha,
-                                   const float* bg_color, const nudf_render_bar* bar,
-                                   float* udf_bar, float* grads_bar, float* scb_bar, float* sc_bar, float* bg_alpha_bar,
-                                   float* bg_color_bar, float* scalar_bar, void* stream) {
+int nudf_render_view_forward(const nudf_render_cfg* cfg, const float* heads, const float* rays_d, const float* pts,
+                             const float* mid_z, const float* dists, const float* udf, int64_t ld_udf, const float* grads,
+                             const float* sampled_color, const float* c_pix, const float* bg_alpha, const float* bg_color,
+                             const float* rot, const nudf_view_out* out, void* stream) {
+  return nudf_render_view_forward_rule(cfg, heads, rays_d, pts, mid_z, dists, udf, ld_udf, grads, sampled_color, c_pix,
+                                       bg_alpha, bg_color, rot, out, ALPHA_NUMERICAL, stream);
+}
+
+int nudf_render_composite_backward_rule(const nudf_render_cfg* cfg, const float* heads, const float* rays_d, const float* pts,
+                                        const float* mid_z, const float* dists, const float* udf, int64_t ld_udf,
+                                        const float* grads, const float* sampled_color_base, const float* sampled_color,
+                                        const float* bg_alpha, const float* bg_color, const nudf_render_bar* bar,
+                                        float* udf_bar, float* grads_bar, float* scb_bar, float* sc_bar, float* bg_alpha_bar,
+                                        float* bg_color_bar, float* scalar_bar, int32_t alpha_rule, void* stream) {
+  if (int rc = check_rule(alpha_rule)) return rc;
   if (int rc = check_cfg(cfg, bg_alpha, bg_color)) return rc;
   NUDF_REQUIRE(heads && rays_d && pts && mid_z && dists && udf && grads && sampled_color_base && sampled_color && bar, "null pointer");
   NUDF_REQUIRE(udf_bar && grads_bar && scb_bar && sc_bar, "null output pointer");
@@ -650,13 +713,19 @@ int nudf_render_composite_backward(const nudf_render_cfg* cfg, const float* head
   rb.weights = bar->weights;
   rb.ray_sums = bar->ray_sums;
   RayBwdOut ob{udf_bar, grads_bar, scb_bar, sc_bar, bg_alpha_bar, bg_color_bar, scalar_bar};
-  size_t smem = (size_t)RK_WARPS * RK_ARRAYS * (cfg->n_samples + cfg->n_outside) * sizeof(float);
-  if (smem > 48 * 1024)
-    NUDF_CUDA_OK(cudaFuncSetAttribute(composite_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  LaunchTimer lt_(FAM_RAY, (cudaStream_t)stream);
-  composite_backward_kernel<<<(unsigned)cdiv(cfg->n_rays, RK_WARPS), RK_WARPS * 32, smem, (cudaStream_t)stream>>>(*cfg, in, rb, ob);
-  NUDF_LAUNCH_OK();
-  return 0;
+  return alpha_rule == ALPHA_THEORICAL ? composite_backward_launch<ALPHA_THEORICAL>(cfg, in, rb, ob, (cudaStream_t)stream)
+                                       : composite_backward_launch<ALPHA_NUMERICAL>(cfg, in, rb, ob, (cudaStream_t)stream);
+}
+
+int nudf_render_composite_backward(const nudf_render_cfg* cfg, const float* heads, const float* rays_d, const float* pts, const float* mid_z,
+                                   const float* dists, const float* udf, int64_t ld_udf, const float* grads,
+                                   const float* sampled_color_base, const float* sampled_color, const float* bg_alpha,
+                                   const float* bg_color, const nudf_render_bar* bar,
+                                   float* udf_bar, float* grads_bar, float* scb_bar, float* sc_bar, float* bg_alpha_bar,
+                                   float* bg_color_bar, float* scalar_bar, void* stream) {
+  return nudf_render_composite_backward_rule(cfg, heads, rays_d, pts, mid_z, dists, udf, ld_udf, grads, sampled_color_base,
+                                             sampled_color, bg_alpha, bg_color, bar, udf_bar, grads_bar, scb_bar, sc_bar,
+                                             bg_alpha_bar, bg_color_bar, scalar_bar, ALPHA_NUMERICAL, stream);
 }
 
 }  // extern "C"

@@ -78,6 +78,47 @@ NUDF_HD void neus_alpha_backward(float sdf, float ic, float dist, float s, float
   *ic_bar = (nxt_bar - prv_bar) * dist * 0.5f;
 }
 
+// ---- NeuS density alpha, 'theorical' branch (:321-323) -----------------------------------------------------------
+// raw = |ic| * s * (1 - sigmoid(sdf * s)) ;  alpha = 1 - exp(-relu(raw) * dist).  No clip.  1 - sigmoid is formed as
+// written (sigmoid, then the subtraction), so that it is exactly 0 where the reference's is.
+NUDF_HD float theorical_alpha_forward(float sdf, float ic, float dist, float s) {
+  float m = 1.0f - sigmoidf_(sdf * s);
+  float raw = fabsf(ic) * s * m;
+  return 1.0f - expf(-fmaxf(raw, 0.0f) * dist);
+}
+// d/d(sdf, ic, s) with torch's conventions at the edges: d|ic|/d ic = sign(ic) (0 at 0), relu'(0) = 0
+NUDF_HD void theorical_alpha_backward(float sdf, float ic, float dist, float s, float a_bar, float* sdf_bar, float* ic_bar,
+                                      float* s_bar) {
+  float sg = sigmoidf_(sdf * s);
+  float m = 1.0f - sg;
+  float A = fabsf(ic);
+  float As = A * s;
+  float raw = As * m;
+  float rr = fmaxf(raw, 0.0f);
+  float raw_bar = raw > 0.0f ? a_bar * expf(-rr * dist) * dist : 0.0f;
+  float x_bar = -(raw_bar * As) * (sg * (1.0f - sg));   // through m = 1 - sigmoid(x), x = sdf * s
+  float As_bar = raw_bar * m;
+  float A_bar = As_bar * s;
+  *sdf_bar = x_bar * s;
+  *s_bar = As_bar * A + x_bar * sdf;
+  *ic_bar = ic > 0.0f ? A_bar : (ic < 0.0f ? -A_bar : 0.0f);
+}
+
+// The alpha rule as a compile-time choice (sdf2alpha_type): the kernels are instantiated once per rule, so neither
+// pays a per-sample branch.  Rule 0 is 'numerical', rule 1 'theorical'.
+enum AlphaRule : int { ALPHA_NUMERICAL = 0, ALPHA_THEORICAL = 1 };
+template <int RULE>
+NUDF_HD float alpha_forward(float sdf, float ic, float dist, float s) {
+  if constexpr (RULE == ALPHA_THEORICAL) return theorical_alpha_forward(sdf, ic, dist, s);
+  else return neus_alpha_forward(sdf, ic, dist, s);
+}
+template <int RULE>
+NUDF_HD void alpha_backward(float sdf, float ic, float dist, float s, float a_bar, float* sdf_bar, float* ic_bar,
+                            float* s_bar) {
+  if constexpr (RULE == ALPHA_THEORICAL) theorical_alpha_backward(sdf, ic, dist, s, a_bar, sdf_bar, ic_bar, s_bar);
+  else neus_alpha_backward(sdf, ic, dist, s, a_bar, sdf_bar, ic_bar, s_bar);
+}
+
 // ---- gradient-derived quantities (:370-388) ----------------------------------------------------------------------
 struct GradQ { float gmag, tc, cosn, flip; };
 NUDF_HD GradQ grad_quantities(const float g[3], const float d[3], int use_norm) {

@@ -89,7 +89,9 @@ __device__ __forceinline__ void sample_pdf_warp(const float* bins, const float* 
   }
 }
 
-// mode 0: up_sample_unbias ; mode 1: up_sample_no_occ_aware
+// mode 0: up_sample_unbias ; mode 1: up_sample_no_occ_aware.  RULE is the alpha rule (AlphaRule, raymath.cuh) of the
+// unbias branch's sdf2alpha calls (:256-257); the no-occ-aware branch has none.
+template <int RULE>
 __global__ void __launch_bounds__(SP_WARPS * 32)
 up_sample_kernel(int mode, const float* __restrict__ rays_o, const float* __restrict__ rays_d, const float* __restrict__ z,
                  const float* __restrict__ udf, int n_rays, int n, int m, float sample_dist, float inv_s, float beta,
@@ -149,8 +151,8 @@ up_sample_kernel(int mode, const float* __restrict__ rays_o, const float* __rest
       float cv = clampf_(fminf(prevc, cosj), -1e3f, 0.0f) * inside;
       float mid_udf = __fmul_rn(__fadd_rn(su[j], su[j + 1]), 0.5f);
       float dist = __fsub_rn(sz[j + 1], sz[j]);
-      float ap = neus_alpha_forward(mid_udf, cv, dist, inv_s);
-      float am = neus_alpha_forward(-mid_udf, cv, dist, inv_s);
+      float ap = alpha_forward<RULE>(mid_udf, cv, dist, inv_s);
+      float am = alpha_forward<RULE>(-mid_udf, cv, dist, inv_s);
       float sg = vis[j];
       float a = ap * sg + am * (1.0f - sg);
       alp[j] = a;
@@ -218,16 +220,19 @@ extern "C" {
 int nudf_up_sample(int32_t mode, const float* rays_o, const float* rays_d, const float* z, const float* udf, int32_t n_rays,
                    int32_t n, int32_t m, float sample_dist, float inv_s, float beta, float gamma, const float* u_lin,
                    float* new_z, int64_t* inds, int32_t* status, void* stream) {
-  NUDF_REQUIRE(mode == 0 || mode == 1, "mode must be 0 or 1");
+  NUDF_REQUIRE(mode == 0 || mode == 1 || mode == 2, "mode must be 0, 1 or 2");
   NUDF_REQUIRE(rays_o && rays_d && z && udf && new_z && u_lin, "null pointer");
   NUDF_REQUIRE(n >= 2 && m >= 1, "need n >= 2, m >= 1");
   if (n_rays <= 0) return 0;
   size_t smem = (size_t)SP_WARPS * 8 * n * sizeof(float);
   NUDF_REQUIRE(smem <= 200 * 1024, "too many samples per ray");
+  // mode 2 is mode 0's up_sample_unbias under the 'theorical' alpha
+  const bool theorical = mode == 2;
+  auto kernel = theorical ? up_sample_kernel<ALPHA_THEORICAL> : up_sample_kernel<ALPHA_NUMERICAL>;
   if (smem > 48 * 1024)
-    NUDF_CUDA_OK(cudaFuncSetAttribute(up_sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  up_sample_kernel<<<(unsigned)cdiv(n_rays, SP_WARPS), SP_WARPS * 32, smem, (cudaStream_t)stream>>>(
-      mode, rays_o, rays_d, z, udf, n_rays, n, m, sample_dist, inv_s, beta, gamma, u_lin, new_z, inds, status);
+    NUDF_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  kernel<<<(unsigned)cdiv(n_rays, SP_WARPS), SP_WARPS * 32, smem, (cudaStream_t)stream>>>(
+      theorical ? 0 : mode, rays_o, rays_d, z, udf, n_rays, n, m, sample_dist, inv_s, beta, gamma, u_lin, new_z, inds, status);
   NUDF_LAUNCH_OK();
   return 0;
 }

@@ -11,6 +11,10 @@ Differences that are deliberate (DESIGN.md "boundary"):
   * `render()` evaluates the NeRF++ background only on the n_outside samples render_core consumes (:493-501);
   * per-sample outputs (`gradients`, `alpha*`, ...) are returned detached -- the trainer only uses them after
     .detach() or for logging (exp_runner_blending.py:309-371, 641-668); `weights` is differentiable.
+Both sdf2alpha rules of the reference (:292-325) run on the device: 'numerical' (the default, every shipped conf) and
+'theorical' (alpha = 1 - exp(-relu(|cos| inv_s (1 - sigmoid(udf inv_s))) dist), :321-323).  The rule is a compile-time
+choice of the sampling and compositing kernels; it decides the importance samples of up_sample_unbias and every alpha,
+weight and colour of render_core, and their gradients.
 Pixel / patch blending (fine-tuning stage, :431-480): one fused CUDA kernel per pass (csrc/blend.cu: projection, bilinear
 gathers of pixel and homography-warped patch colours, masked-softmax fusion over views), composited with the
 differentiable ray weights of the CUDA compositing kernel; patch_projector.py / fields.color_blend keep the op-by-op form,
@@ -113,9 +117,9 @@ class UDFRendererBlending:
     def __init__(self, nerf, udf_network, deviation_network, color_network, beta_network, n_samples, n_importance,
                  n_outside, up_sample_steps, perturb, sdf2alpha_type='numerical', upsampling_type='classical',
                  sparse_scale_factor=25000, h_patch_size=3, use_norm_grad_for_cosine=False):
-        if sdf2alpha_type != 'numerical':
-            raise NotImplementedError("sdf2alpha_type %r: only 'numerical' (all shipped confs) is implemented" %
-                                      (sdf2alpha_type,))
+        if sdf2alpha_type not in ops.ALPHA_RULES:
+            raise NotImplementedError("sdf2alpha_type %r: only 'numerical' (all shipped confs) and 'theorical' are "
+                                      "implemented" % (sdf2alpha_type,))
         if upsampling_type not in ('classical', 'mix'):
             raise ValueError("upsampling_type must be 'classical' or 'mix'")
         self.nerf = nerf
@@ -129,6 +133,7 @@ class UDFRendererBlending:
         self.perturb = perturb
         self.up_sample_steps = up_sample_steps
         self.sdf2alpha_type = sdf2alpha_type
+        self.alpha_rule = ops.alpha_rule(sdf2alpha_type)
         self.upsampling_type = upsampling_type
         self.sparse_scale_factor = sparse_scale_factor
         self.h_patch_size = h_patch_size
@@ -150,6 +155,9 @@ class UDFRendererBlending:
             iter_cos = -(F.relu(-true_cos * 0.5 + 0.5) * (1.0 - cos_anneal_ratio) + F.relu(-true_cos) * cos_anneal_ratio)
         else:
             iter_cos = true_cos
+        if self.sdf2alpha_type == 'theorical':
+            raw = iter_cos.abs() * inv_s * (1 - torch.sigmoid(sdf * inv_s))
+            return 1.0 - torch.exp(-F.relu(raw) * dists)
         nxt = sdf + iter_cos * dists * 0.5
         prv = sdf - iter_cos * dists * 0.5
         cp, cn = torch.sigmoid(prv * inv_s), torch.sigmoid(nxt * inv_s)
@@ -160,7 +168,7 @@ class UDFRendererBlending:
     # ------------------------------------------------------------------------------------------------------------
     def up_sample_unbias(self, rays_o, rays_d, z_vals, udf, sample_dist, n_importance, inv_s, beta, gamma, debug=False):
         return ops.up_sample(0, rays_o, rays_d, z_vals, udf.reshape(z_vals.shape), sample_dist, n_importance, inv_s, beta,
-                             float(gamma))
+                             float(gamma), alpha_rule=self.alpha_rule)
 
     def up_sample_no_occ_aware(self, rays_o, rays_d, z_vals, udf, sample_dist, n_importance, inv_s, beta, gamma):
         return ops.up_sample(1, rays_o, rays_d, z_vals, udf.reshape(z_vals.shape), sample_dist, n_importance, inv_s, beta,
@@ -258,7 +266,7 @@ class UDFRendererBlending:
         if background_alpha is not None:
             n_outside = background_alpha.shape[1] - n_samples
         cfg = ops._make_cfg(batch_size, n_samples, n_outside, sample_dist, cos_anneal_ratio, flip_saturation,
-                            self.sparse_scale_factor, self.use_norm_grad_for_cosine, background_rgb)
+                            self.sparse_scale_factor, self.use_norm_grad_for_cosine, background_rgb, self.alpha_rule)
         comp = ops.composite(udf, gradients, sampled_color_base, sampled_color,
                              background_alpha if n_outside > 0 else None,
                              background_sampled_color if n_outside > 0 else None, heads,

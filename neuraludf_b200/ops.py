@@ -540,8 +540,24 @@ DIAG_KEYS = ["gradient_mag", "true_cos", "vis_prob", "alpha", "alpha_plus", "alp
              "inside_sphere"]
 
 
-def _make_cfg(N, S, O, sample_dist, cos_anneal_ratio, flip_saturation, sparse_scale_factor, use_norm, background_rgb):
+ALPHA_RULES = {"numerical": 0, "theorical": 1}   # sdf2alpha_type -> the kernels' alpha_rule
+
+
+def alpha_rule(sdf2alpha_type):
+    """The kernels' alpha_rule for an sdf2alpha_type string; ValueError for any other string."""
+    if sdf2alpha_type not in ALPHA_RULES:
+        raise ValueError("sdf2alpha_type %r: expected one of %s" % (sdf2alpha_type, sorted(ALPHA_RULES)))
+    return ALPHA_RULES[sdf2alpha_type]
+
+
+def _make_cfg(N, S, O, sample_dist, cos_anneal_ratio, flip_saturation, sparse_scale_factor, use_norm, background_rgb,
+              alpha_rule=0):
+    """The compositing kernels' nudf_render_cfg.  alpha_rule (0 numerical, 1 theorical) is not part of the struct: it rides
+    along as a Python attribute and composite / view_composite hand it to the *_rule entry points."""
+    if alpha_rule not in (0, 1):
+        raise ValueError("alpha_rule must be 0 (numerical) or 1 (theorical), got %r" % (alpha_rule,))
     cfg = L.RenderCfg()
+    cfg.alpha_rule = int(alpha_rule)
     cfg.n_rays, cfg.n_samples, cfg.n_outside = N, S, O
     cfg.sample_dist = float(sample_dist)
     cfg.has_cos_anneal = 0 if cos_anneal_ratio is None else 1
@@ -589,6 +605,11 @@ def _check_composite_rows(N, S, O, **ts):
                 name, tuple(t.shape), r, " of %d" % w if w > 1 else "", N, S, O))
 
 
+def _cfg_rule(cfg):
+    """alpha_rule of a cfg from _make_cfg (0, numerical, for a bare nudf_render_cfg)"""
+    return getattr(cfg, "alpha_rule", 0)
+
+
 class _CompositeFunction(torch.autograd.Function):
     """differentiable inputs: udf [P] / [P,1] / [N,S], grads [P,3], scb [P,3], sc [P,3], bg_alpha [N,S+O],
     bg_color [N,S+O,3], heads [3]"""
@@ -618,10 +639,11 @@ class _CompositeFunction(torch.autograd.Function):
         for k in L.RENDER_OUT_FIELDS:
             setattr(ro, k, outs[k].data_ptr() if k in outs else None)
         ro.status = status_word(dev).data_ptr()
-        L.check(lib.nudf_render_composite_forward(ctypes.byref(cfg), L.ptr(heads), L.ptr(rays_d), L.ptr(pts), L.ptr(mid),
-                                                  L.ptr(dists), L.ptr(udf), ld_udf, L.ptr(grads), L.ptr(scb), L.ptr(sc),
-                                                  L.ptr(bg_alpha), L.ptr(bg_color), ctypes.byref(ro), L.stream_ptr()),
-                "nudf_render_composite_forward")
+        L.check(lib.nudf_render_composite_forward_rule(ctypes.byref(cfg), L.ptr(heads), L.ptr(rays_d), L.ptr(pts), L.ptr(mid),
+                                                       L.ptr(dists), L.ptr(udf), ld_udf, L.ptr(grads), L.ptr(scb), L.ptr(sc),
+                                                       L.ptr(bg_alpha), L.ptr(bg_color), ctypes.byref(ro), _cfg_rule(cfg),
+                                                       L.stream_ptr()),
+                "nudf_render_composite_forward_rule")
         ctx.cfg, ctx.geom, ctx.ld_udf, ctx.udf_shape = cfg, geom, ld_udf, udf_shape
         ctx.has_bg = bg_alpha is not None
         ctx.save_for_backward(udf, grads, scb, sc, bg_alpha, bg_color, heads)
@@ -655,12 +677,13 @@ class _CompositeFunction(torch.autograd.Function):
         if bgc_bar is not None:
             bgc_bar[:, :S].zero_()
         scal = f(N, 3)
-        L.check(lib.nudf_render_composite_backward(ctypes.byref(cfg), L.ptr(heads), L.ptr(rays_d), L.ptr(pts), L.ptr(mid),
-                                                   L.ptr(dists), L.ptr(udf), ctx.ld_udf, L.ptr(grads), L.ptr(scb),
-                                                   L.ptr(sc), L.ptr(bg_alpha), L.ptr(bg_color), ctypes.byref(bar),
-                                                   L.ptr(udf_bar), L.ptr(grads_bar), L.ptr(scb_bar), L.ptr(sc_bar),
-                                                   L.ptr(bga_bar), L.ptr(bgc_bar), L.ptr(scal), L.stream_ptr()),
-                "nudf_render_composite_backward")
+        L.check(lib.nudf_render_composite_backward_rule(ctypes.byref(cfg), L.ptr(heads), L.ptr(rays_d), L.ptr(pts),
+                                                        L.ptr(mid), L.ptr(dists), L.ptr(udf), ctx.ld_udf, L.ptr(grads),
+                                                        L.ptr(scb), L.ptr(sc), L.ptr(bg_alpha), L.ptr(bg_color),
+                                                        ctypes.byref(bar), L.ptr(udf_bar), L.ptr(grads_bar), L.ptr(scb_bar),
+                                                        L.ptr(sc_bar), L.ptr(bga_bar), L.ptr(bgc_bar), L.ptr(scal),
+                                                        _cfg_rule(cfg), L.stream_ptr()),
+                "nudf_render_composite_backward_rule")
         # in the caller's shape: [P] (possibly a strided view), [P, 1] or [N, S]
         return (udf_bar.reshape(ctx.udf_shape), grads_bar, scb_bar, sc_bar, bga_bar, bgc_bar, scal.sum(dim=0),
                 None, None, None)
@@ -737,7 +760,11 @@ def _u_lin(m, device):
     return _U_CACHE[key]
 
 
-def up_sample(mode, rays_o, rays_d, z, udf, sample_dist, m, inv_s, beta, gamma, return_inds=False):
+def up_sample(mode, rays_o, rays_d, z, udf, sample_dist, m, inv_s, beta, gamma, return_inds=False, alpha_rule=0):
+    """One nudf_up_sample round.  mode 0 up_sample_unbias, 1 up_sample_no_occ_aware, 2 up_sample_unbias under the
+    'theorical' alpha; alpha_rule=1 turns mode 0 into mode 2 (mode 1 has no alpha to choose)."""
+    if mode == 0 and alpha_rule == 1:
+        mode = 2
     lib = L.lib()
     rays_o, rays_d, z, udf = _f32c(rays_o), _f32c(rays_d), _f32c(z), _f32c(udf)
     _require_cuda(rays_o, rays_d, z, udf)
@@ -821,7 +848,7 @@ def nerf_forward_into(desc, wimg, pts, dirs, samples_per_ray, sigma, rgb, ctx):
 
 
 def view_composite(cfg, heads, rays_d, pts, mid, dists, udf, grads, sc, c_pix, bg_alpha, bg_color, rot, outs):
-    """nudf_render_view_forward: outs maps color / color_pixel / depth / normal / weight_sum to [N, .] tensors (views
+    """nudf_render_view_forward_rule under the cfg's alpha_rule: outs maps color / color_pixel / depth / normal / weight_sum to [N, .] tensors (views
     into the image buffers are fine) or None; rot is a host 3x3 (nested sequence or array)."""
     lib = L.lib()
     ro = L.ViewOut()
@@ -829,9 +856,10 @@ def view_composite(cfg, heads, rays_d, pts, mid, dists, udf, grads, sc, c_pix, b
         t = outs.get(k)
         setattr(ro, k, None if t is None else t.data_ptr())
     r9 = (ctypes.c_float * 9)(*[float(v) for row in rot for v in row])
-    L.check(lib.nudf_render_view_forward(ctypes.byref(cfg), L.ptr(heads), L.ptr(rays_d), L.ptr(pts), L.ptr(mid), L.ptr(dists),
-                                         L.ptr(udf), 1, L.ptr(grads), L.ptr(sc), L.ptr(c_pix), L.ptr(bg_alpha),
-                                         L.ptr(bg_color), r9, ctypes.byref(ro), L.stream_ptr()), "nudf_render_view_forward")
+    L.check(lib.nudf_render_view_forward_rule(ctypes.byref(cfg), L.ptr(heads), L.ptr(rays_d), L.ptr(pts), L.ptr(mid),
+                                              L.ptr(dists), L.ptr(udf), 1, L.ptr(grads), L.ptr(sc), L.ptr(c_pix),
+                                              L.ptr(bg_alpha), L.ptr(bg_color), r9, ctypes.byref(ro), _cfg_rule(cfg),
+                                              L.stream_ptr()), "nudf_render_view_forward_rule")
 
 
 def blend_forward_into(cfg, pts, proj, hom, px, imgs, logits, c_pix, c_pat, m_pat):

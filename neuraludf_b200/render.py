@@ -143,7 +143,7 @@ def render_view(renderer, rays_o, rays_d, near, far, *, color_maps=None, w2cs=No
         gamma = float(renderer.beta_network.get_gamma().clip(1e-6, 1e6))
     heads = _heads(renderer, dev)
     cfg_args = (sample_dist, cos_anneal_ratio, 0.0, renderer.sparse_scale_factor, renderer.use_norm_grad_for_cosine,
-                background_rgb)
+                background_rgb, renderer.alpha_rule)
     rot = np.eye(3) if rot is None else np.asarray(rot, dtype=np.float64).reshape(3, 3)
 
     proj = imgs = None
@@ -429,6 +429,8 @@ def main(argv=None):
     ap.add_argument("--up_sample_steps", type=int, default=5)
     ap.add_argument("--n_outside", type=int, default=32)
     ap.add_argument("--upsampling_type", default="classical", choices=("classical", "mix"))
+    ap.add_argument("--sdf2alpha_type", default="numerical", choices=("numerical", "theorical"),
+                    help="the conf's sdf2alpha_type (a checkpoint does not record it)")
     ap.add_argument("--use_norm_grad_for_cosine", action="store_true")
     ap.add_argument("--workspace_gib", type=float, default=DEFAULT_WORKSPACE_BYTES / 2 ** 30)
     ap.add_argument("--out_dir", required=True)
@@ -442,7 +444,8 @@ def main(argv=None):
     udf, col, nerf, var, beta = networks_from_checkpoint(ck, dev)
     ren = UDFRendererBlending(nerf, udf, var, col, beta, n_samples=a.n_samples, n_importance=a.n_importance,
                               n_outside=a.n_outside, up_sample_steps=a.up_sample_steps, perturb=a.perturb,
-                              upsampling_type=a.upsampling_type, use_norm_grad_for_cosine=a.use_norm_grad_for_cosine)
+                              sdf2alpha_type=a.sdf2alpha_type, upsampling_type=a.upsampling_type,
+                              use_norm_grad_for_cosine=a.use_norm_grad_for_cosine)
     it = int(ck.get("iter_step", 0))
     ratio = a.cos_anneal_ratio
     if ratio is None:                                      # Runner.get_cos_anneal_ratio (exp_runner_blending.py:193-197)
