@@ -20,7 +20,7 @@ extern "C" {
 #endif
 
 #define NUDF_MAX_LAYERS 16
-#define NUDF_ABI_VERSION 5
+#define NUDF_ABI_VERSION 6
 /* bits of the device-side status word (nudf_render_out.status, `status` of the sampling entry points): set by the kernels,
  * never cleared by the library; the caller reads it at a host synchronisation point of its choice */
 #define NUDF_STATUS_NONFINITE_SAMPLES 1   /* sample_pdf / up_sample produced a non-finite sample position (:97-101, 265-269) */
@@ -199,6 +199,9 @@ typedef struct nudf_render_cfg {
   float sparse_scale_factor;/* :553 */
   int32_t use_norm_grad_for_cosine; /* :380-383 */
   int32_t has_background_rgb; float background_rgb[3]; /* :527-528 */
+  int32_t alpha_rule;       /* sdf2alpha (:292-325): 0 = 'numerical' (:308-320), 1 = 'theorical' (:321-323):
+                             * alpha = 1 - exp(-relu(|iter_cos| inv_s (1 - sigmoid(sdf inv_s))) dist).  The backward pass
+                             * is the adjoint of the forward pass under the same rule.  Any other value is refused. */
 } nudf_render_cfg;
 
 /* pts[N*S,3], mid_z[N,S], dists[N,S] <- rays and z_vals (:352-362) */
@@ -268,26 +271,6 @@ int nudf_render_composite_backward(const nudf_render_cfg* cfg, const float* head
                                    float* udf_bar, float* grads_bar, float* scb_bar,
                                    float* sc_bar, float* bg_alpha_bar, float* bg_color_bar, float* scalar_bar,
                                    void* stream);
-
-/* The three compositing entry points above under a chosen sdf2alpha rule (:292-325).  Arguments as above plus
- *   alpha_rule  0 = 'numerical' (:308-320; exactly the entry points above, same bits),
- *               1 = 'theorical' (:321-323): alpha = 1 - exp(-relu(|iter_cos| inv_s (1 - sigmoid(sdf inv_s))) dist).
- * The backward pass is the adjoint of the forward pass under the same rule. */
-int nudf_render_composite_forward_rule(const nudf_render_cfg* cfg, const float* heads, const float* rays_d, const float* pts,
-                                       const float* mid_z, const float* dists, const float* udf, int64_t ld_udf,
-                                       const float* grads, const float* sampled_color_base, const float* sampled_color,
-                                       const float* bg_alpha, const float* bg_color, const nudf_render_out* out,
-                                       int32_t alpha_rule, void* stream);
-int nudf_render_view_forward_rule(const nudf_render_cfg* cfg, const float* heads, const float* rays_d, const float* pts,
-                                  const float* mid_z, const float* dists, const float* udf, int64_t ld_udf, const float* grads,
-                                  const float* sampled_color, const float* c_pix, const float* bg_alpha, const float* bg_color,
-                                  const float* rot, const nudf_view_out* out, int32_t alpha_rule, void* stream);
-int nudf_render_composite_backward_rule(const nudf_render_cfg* cfg, const float* heads, const float* rays_d, const float* pts,
-                                        const float* mid_z, const float* dists, const float* udf, int64_t ld_udf,
-                                        const float* grads, const float* sampled_color_base, const float* sampled_color,
-                                        const float* bg_alpha, const float* bg_color, const nudf_render_bar* bar,
-                                        float* udf_bar, float* grads_bar, float* scb_bar, float* sc_bar, float* bg_alpha_bar,
-                                        float* bg_color_bar, float* scalar_bar, int32_t alpha_rule, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * hierarchical sampling  (reference: models/udf_renderer_blending.py:66-104, 197-290, 723-755, 834-866)
@@ -403,38 +386,33 @@ int nudf_mc_vertices(const nudf_lattice* lat, const int64_t* cells, int64_t n_ce
  * Threshold marching cubes (replaces PyMCubes' marching_cubes in the runner's validate_mesh; neuraludf_b200/mesh.py's
  * iso_marching_cubes_index drives the stages).  The MeshUDF construction above on the corner values v = fl32(f - level)
  * (corner positive when v > 0), with no pseudo-signs and no polarity; the lattice is read in place, never shifted.
- * df: DEVICE fp32 lattice [n0, n1, n2]; level must be finite.  Faces are wound so that their normals (right-hand rule)
- * point from the > level side into the <= level side.  All buffers are caller-provided; nothing is allocated.
+ * Every stage reads the lattice `lat` (the flat array or a brick store, as nudf_mc_*); level must be finite.  Faces are
+ * wound so that their normals (right-hand rule) point from the > level side into the <= level side.  All buffers are
+ * caller-provided; nothing is allocated.
  * ------------------------------------------------------------------------------------------------------------ */
-/* flags[g] (g < n0 * n1 * n2) = 1 when the cell with lower corner g has a corner with v > 0, one with v <= 0 and none NaN */
-int nudf_iso_active(const float* df, int32_t n0, int32_t n1, int32_t n2, float level, uint8_t* flags, void* stream);
+/* flags[g] (g < n0 * n1 * n2) = 1 when the cell with lower corner g has a corner with v > 0, one with v <= 0 and none NaN.
+ * A df lattice only: a store is refused (nudf_iso_cells_* find the active cells of either form) */
+int nudf_iso_active(const nudf_lattice* lat, float level, uint8_t* flags, void* stream);
+/* The active cells without a scan of every cell: the storage positions (df: the flat indices; a store: coarse, then the
+ * brick slots, as nudf_sb_flat numbers them) are taken in n_seg = ceil(positions / NUDF_ISO_SEG) segments.  Each position
+ * holding a lattice point with v <= 0 emits the active cells (as nudf_iso_active defines them) of which it is the lowest
+ * corner with v <= 0: counts[seg] = the segment's cells; cells[offsets[seg] ...] = them, in position order (offsets =
+ * exclusive scan of the counts).  Sorted, they are nonzero(nudf_iso_active) of the lattice's values, with no condition on
+ * the field: every active cell has a corner with v <= 0, which is finite and so stored. */
+#define NUDF_ISO_SEG 256
+int nudf_iso_cells_count(const nudf_lattice* lat, float level, int64_t n_seg, int32_t* counts, void* stream);
+int nudf_iso_cells_emit(const nudf_lattice* lat, float level, int64_t n_seg, const int64_t* offsets, int64_t* cells,
+                        void* stream);
 /* triangles per cell (<= 12), as nudf_mc_count */
-int nudf_iso_count(const float* df, int32_t n0, int32_t n1, int32_t n2, float level, const int64_t* cells, int64_t n_cells,
-                   int32_t* counts, void* stream);
+int nudf_iso_count(const nudf_lattice* lat, float level, const int64_t* cells, int64_t n_cells, int32_t* counts,
+                   void* stream);
 /* vertex keys of the triangles, as nudf_mc_emit: 3 * corner + axis, then 3 * n0 * n1 * n2 + 4 * t + l for loop centres */
-int nudf_iso_emit(const float* df, int32_t n0, int32_t n1, int32_t n2, float level, const int64_t* cells, int64_t n_cells,
-                  const int64_t* offsets, int64_t* keys, void* stream);
+int nudf_iso_emit(const nudf_lattice* lat, float level, const int64_t* cells, int64_t n_cells, const int64_t* offsets,
+                  int64_t* keys, void* stream);
 /* verts[n_keys, 3] fp64 lattice-index coordinates: edge points at t = v_a / (v_a - v_b) from the lower corner (fp64 from the
  * fp32 v, no contraction), loop centres at the mean of their loop's edge points summed in loop order */
-int nudf_iso_vertices(const float* df, int32_t n0, int32_t n1, int32_t n2, float level, const int64_t* cells, int64_t n_cells,
-                      const int64_t* keys, int64_t n_keys, double* verts, void* stream);
-/* The same stages on a nudf_lattice (the flat array or a brick store; the nudf_iso_* above are their df form, the same
- * kernels).  The active cells without a scan of every cell: the storage positions (df: the flat indices; a store: coarse,
- * then the brick slots, as nudf_sb_flat numbers them) are taken in n_seg = ceil(positions / NUDF_ISO_SEG) segments.  Each
- * position holding a lattice point with v <= 0 emits the active cells (as nudf_iso_active defines them) of which it is the
- * lowest corner with v <= 0: counts[seg] = the segment's cells; cells[offsets[seg] ...] = them, in position order
- * (offsets = exclusive scan of the counts).  Sorted, they are nonzero(nudf_iso_active) of the lattice's values, with no
- * condition on the field: every active cell has a corner with v <= 0, which is finite and so stored. */
-#define NUDF_ISO_SEG 256
-int nudf_iso_lat_cells_count(const nudf_lattice* lat, float level, int64_t n_seg, int32_t* counts, void* stream);
-int nudf_iso_lat_cells_emit(const nudf_lattice* lat, float level, int64_t n_seg, const int64_t* offsets, int64_t* cells,
-                            void* stream);
-int nudf_iso_lat_count(const nudf_lattice* lat, float level, const int64_t* cells, int64_t n_cells, int32_t* counts,
-                       void* stream);
-int nudf_iso_lat_emit(const nudf_lattice* lat, float level, const int64_t* cells, int64_t n_cells, const int64_t* offsets,
-                      int64_t* keys, void* stream);
-int nudf_iso_lat_vertices(const nudf_lattice* lat, float level, const int64_t* cells, int64_t n_cells, const int64_t* keys,
-                          int64_t n_keys, double* verts, void* stream);
+int nudf_iso_vertices(const nudf_lattice* lat, float level, const int64_t* cells, int64_t n_cells, const int64_t* keys,
+                      int64_t n_keys, double* verts, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Point-cloud evaluation (the DTU / DeepFashion3D Chamfer protocols; neuraludf_b200/evaluate.py drives the stages)
@@ -511,22 +489,18 @@ typedef struct nudf_band_coords {
 } nudf_band_coords;
 /* idx / pts [m^3] (m = ceil((N - 1) / s) + 1): the stride-s lattice in (x, y, z) lexicographic order */
 int nudf_nb_sublattice(int32_t n, int32_t s, const nudf_band_coords* co, int64_t* idx, float* pts, void* stream);
-/* flags[nb^3] (may be NULL) = 1 for the kept blocks of stride s on the cubic lattice `lat` (N = n0 = n1 = n2): candidates
+/* flags[nb^3] (may be NULL) = 1 for the kept blocks of stride s on the cubic lattice `lat` (N = n0 = n1 = n2; the flat
+ * array or a brick store, with either coordinate form): candidates
  * (every block when parent_flags is NULL, else the blocks inside a kept block of stride parent_s) with a NaN corner or
  * min(corner df) - lipschitz r < tau in fp64, r = half the box diagonal.  Cube: r in voxels, with slack
- * (r + 1e-6 relative + 1e-6, tau + 1e-6 relative) against rounding; edge slopes |du| / (e_a voxel).  Table (a df lattice
- * only): r from the block's table-coordinate box (fp64, |ax[hi] - ax[lo]| per axis), enlarged by 1e-6 relative plus pad,
+ * (r + 1e-6 relative + 1e-6, tau + 1e-6 relative) against rounding; edge slopes |du| / (e_a voxel).  Table: r from the
+ * block's table-coordinate box (fp64, |ax[hi] - ax[lo]| per axis), enlarged by 1e-6 relative plus pad,
  * and tau used as given (the caller's slack included); edge slopes |du| / (e_a h_a).  Candidates' corners must have been
  * evaluated.  max_slope (DEVICE uint32[1], fp32 bits, zeroed by the caller) is raised to the largest |du| / (edge length)
  * over the candidates' box edges with finite ends */
 int nudf_nb_block_test(const nudf_lattice* lat, int32_t s, const uint8_t* parent_flags, int32_t parent_s,
                        const nudf_band_coords* co, double lipschitz, double tau, uint8_t* flags, uint32_t* max_slope,
                        void* stream);
-/* nudf_nb_block_test on any lattice with either coordinate form: the table form on a brick store too
- * (grid.iso_band_sparse), the same test on the same corner values */
-int nudf_nb_lat_block_test(const nudf_lattice* lat, int32_t s, const uint8_t* parent_flags, int32_t parent_s,
-                           const nudf_band_coords* co, double lipschitz, double tau, uint8_t* flags, uint32_t* max_slope,
-                           void* stream);
 /* counts[i] = the points block kept[i] of stride s emits: the stride-t lattice (t divides s) in its closed box, less the
  * stride-s lattice, less the points that a lower-numbered kept block (flags) also holds.  kept: ascending block numbers */
 int nudf_nb_count(const uint8_t* flags, int32_t n, int32_t s, int32_t t, const int64_t* kept, int64_t n_kept,

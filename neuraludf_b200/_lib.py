@@ -43,7 +43,8 @@ class RenderCfg(ctypes.Structure):
                 ("sample_dist", ctypes.c_float), ("cos_anneal_ratio", ctypes.c_float),
                 ("has_cos_anneal", ctypes.c_int32), ("flip_saturation", ctypes.c_float),
                 ("sparse_scale_factor", ctypes.c_float), ("use_norm_grad_for_cosine", ctypes.c_int32),
-                ("has_background_rgb", ctypes.c_int32), ("background_rgb", ctypes.c_float * 3)]
+                ("has_background_rgb", ctypes.c_int32), ("background_rgb", ctypes.c_float * 3),
+                ("alpha_rule", ctypes.c_int32)]
 
 
 RENDER_OUT_FIELDS = ["color_base", "color", "depth", "normals", "weights", "weight_sum", "weight_sum_fg_bg",
@@ -180,12 +181,6 @@ _SIGNATURES = {
     "nudf_render_composite_forward": (ctypes.c_int, [c_void_p] * 2 + [c_void_p] * 5 + [ctypes.c_int64] + [c_void_p] * 7),
     "nudf_render_view_forward": (ctypes.c_int, [c_void_p] * 2 + [c_void_p] * 5 + [ctypes.c_int64] + [c_void_p] * 8),
     "nudf_render_composite_backward": (ctypes.c_int, [c_void_p] * 2 + [c_void_p] * 5 + [ctypes.c_int64] + [c_void_p] * 14),
-    "nudf_render_composite_forward_rule": (ctypes.c_int, [c_void_p] * 2 + [c_void_p] * 5 + [ctypes.c_int64] + [c_void_p] * 6
-                                           + [ctypes.c_int32, c_void_p]),
-    "nudf_render_view_forward_rule": (ctypes.c_int, [c_void_p] * 2 + [c_void_p] * 5 + [ctypes.c_int64] + [c_void_p] * 7
-                                      + [ctypes.c_int32, c_void_p]),
-    "nudf_render_composite_backward_rule": (ctypes.c_int, [c_void_p] * 2 + [c_void_p] * 5 + [ctypes.c_int64]
-                                            + [c_void_p] * 13 + [ctypes.c_int32, c_void_p]),
     "nudf_up_sample": (ctypes.c_int, [ctypes.c_int32, c_void_p, c_void_p, c_void_p, c_void_p, ctypes.c_int32,
                                       ctypes.c_int32, ctypes.c_int32, ctypes.c_float, ctypes.c_float, ctypes.c_float,
                                       ctypes.c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
@@ -206,13 +201,6 @@ _SIGNATURES = {
     "nudf_mc_count": (ctypes.c_int, [c_void_p] * 2 + [ctypes.c_int64] + [c_void_p] * 3),
     "nudf_mc_emit": (ctypes.c_int, [c_void_p] * 2 + [ctypes.c_int64] + [c_void_p] * 4),
     "nudf_mc_vertices": (ctypes.c_int, [c_void_p] * 2 + [ctypes.c_int64] + [c_void_p] * 2 + [ctypes.c_int64] + [c_void_p] * 2),
-    "nudf_iso_active": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [ctypes.c_float, c_void_p, c_void_p]),
-    "nudf_iso_count": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [ctypes.c_float, c_void_p, ctypes.c_int64, c_void_p,
-                                                                          c_void_p]),
-    "nudf_iso_emit": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [ctypes.c_float, c_void_p, ctypes.c_int64]
-                      + [c_void_p] * 3),
-    "nudf_iso_vertices": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [ctypes.c_float, c_void_p, ctypes.c_int64,
-                                                                             c_void_p, ctypes.c_int64, c_void_p, c_void_p]),
     "nudf_pc_sample_count": (ctypes.c_int, [c_void_p, ctypes.c_int64, c_void_p, ctypes.c_int64, ctypes.c_double, c_void_p,
                                             c_void_p]),
     "nudf_pc_sample_emit": (ctypes.c_int, [c_void_p, ctypes.c_int64, c_void_p, ctypes.c_int64, ctypes.c_double, c_void_p,
@@ -233,17 +221,16 @@ _SIGNATURES = {
                        + [c_void_p] * 2),
     "nudf_cl_vote": (ctypes.c_int, [c_void_p, ctypes.c_int64, c_void_p, ctypes.c_int32, c_void_p] + [ctypes.c_int32] * 3
                      + [c_void_p] * 2),
-    "nudf_iso_lat_cells_count": (ctypes.c_int, [c_void_p, ctypes.c_float, ctypes.c_int64, c_void_p, c_void_p]),
-    "nudf_iso_lat_cells_emit": (ctypes.c_int, [c_void_p, ctypes.c_float, ctypes.c_int64] + [c_void_p] * 3),
-    "nudf_iso_lat_count": (ctypes.c_int, [c_void_p, ctypes.c_float, c_void_p, ctypes.c_int64, c_void_p, c_void_p]),
-    "nudf_iso_lat_emit": (ctypes.c_int, [c_void_p, ctypes.c_float, c_void_p, ctypes.c_int64] + [c_void_p] * 3),
-    "nudf_iso_lat_vertices": (ctypes.c_int, [c_void_p, ctypes.c_float, c_void_p, ctypes.c_int64, c_void_p, ctypes.c_int64,
-                                             c_void_p, c_void_p]),
+    "nudf_iso_active": (ctypes.c_int, [c_void_p, ctypes.c_float, c_void_p, c_void_p]),
+    "nudf_iso_cells_count": (ctypes.c_int, [c_void_p, ctypes.c_float, ctypes.c_int64, c_void_p, c_void_p]),
+    "nudf_iso_cells_emit": (ctypes.c_int, [c_void_p, ctypes.c_float, ctypes.c_int64] + [c_void_p] * 3),
+    "nudf_iso_count": (ctypes.c_int, [c_void_p, ctypes.c_float, c_void_p, ctypes.c_int64, c_void_p, c_void_p]),
+    "nudf_iso_emit": (ctypes.c_int, [c_void_p, ctypes.c_float, c_void_p, ctypes.c_int64] + [c_void_p] * 3),
+    "nudf_iso_vertices": (ctypes.c_int, [c_void_p, ctypes.c_float, c_void_p, ctypes.c_int64, c_void_p, ctypes.c_int64,
+                                         c_void_p, c_void_p]),
     "nudf_nb_sublattice": (ctypes.c_int, [ctypes.c_int32] * 2 + [c_void_p] * 4),
     "nudf_nb_block_test": (ctypes.c_int, [c_void_p, ctypes.c_int32, c_void_p, ctypes.c_int32, c_void_p] + [ctypes.c_double] * 2
                            + [c_void_p] * 3),
-    "nudf_nb_lat_block_test": (ctypes.c_int, [c_void_p, ctypes.c_int32, c_void_p, ctypes.c_int32, c_void_p]
-                               + [ctypes.c_double] * 2 + [c_void_p] * 3),
     "nudf_nb_count": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [c_void_p, ctypes.c_int64] + [c_void_p] * 2),
     "nudf_nb_emit": (ctypes.c_int, [c_void_p] + [ctypes.c_int32] * 3 + [c_void_p, ctypes.c_int64] + [c_void_p] * 5),
     "nudf_sb_mark": (ctypes.c_int, [c_void_p, ctypes.c_int32] + [c_void_p] * 3),
@@ -299,7 +286,7 @@ def lib():
             fn = getattr(L, name)
             fn.restype = res
             fn.argtypes = args
-        if L.nudf_abi_version() != 5:
+        if L.nudf_abi_version() != 6:
             raise RuntimeError("libnudf.so ABI version mismatch")
         _lib = L
     return _lib

@@ -264,9 +264,10 @@ int nudf_nb_sublattice(int32_t n, int32_t s, const nudf_band_coords* co, int64_t
 }
 
 // every reader with either spacing rule: the table rule on a brick store keeps the blocks it keeps on the dense band
-static int block_test(const nudf_lattice* lat, int32_t s, const uint8_t* parent_flags, int32_t parent_s,
-                      const nudf_band_coords* co, double lipschitz, double tau, uint8_t* flags, uint32_t* max_slope,
-                      void* stream) {
+int nudf_nb_block_test(const nudf_lattice* lat, int32_t s, const uint8_t* parent_flags, int32_t parent_s,
+                       const nudf_band_coords* co, double lipschitz, double tau, uint8_t* flags, uint32_t* max_slope,
+                       void* stream) {
+  if (check_coords(co)) return -1;
   return with_lattice(lat, [&](auto df) {
     NUDF_REQUIRE(max_slope, "null pointer");
     NUDF_REQUIRE(lat->n0 == lat->n1 && lat->n1 == lat->n2, "the band lattice must be cubic");
@@ -285,22 +286,6 @@ static int block_test(const nudf_lattice* lat, int32_t s, const uint8_t* parent_
     if (is_table(*co)) return launch(TableSpacing{{co->ax[0], co->ax[1], co->ax[2]}, {co->h[0], co->h[1], co->h[2]}, co->pad});
     return launch(CubeSpacing{co->voxel});
   });
-}
-
-int nudf_nb_block_test(const nudf_lattice* lat, int32_t s, const uint8_t* parent_flags, int32_t parent_s,
-                       const nudf_band_coords* co, double lipschitz, double tau, uint8_t* flags, uint32_t* max_slope,
-                       void* stream) {
-  // this entry point's contract: the table form on a dense lattice only (nudf_nb_lat_block_test reads a store too)
-  if (check_coords(co)) return -1;
-  NUDF_REQUIRE(!(is_table(*co) && lat && lat->store), "the table coordinates need a dense lattice");
-  return block_test(lat, s, parent_flags, parent_s, co, lipschitz, tau, flags, max_slope, stream);
-}
-
-int nudf_nb_lat_block_test(const nudf_lattice* lat, int32_t s, const uint8_t* parent_flags, int32_t parent_s,
-                           const nudf_band_coords* co, double lipschitz, double tau, uint8_t* flags, uint32_t* max_slope,
-                           void* stream) {
-  if (check_coords(co)) return -1;
-  return block_test(lat, s, parent_flags, parent_s, co, lipschitz, tau, flags, max_slope, stream);
 }
 
 int nudf_nb_count(const uint8_t* flags, int32_t n, int32_t s, int32_t t, const int64_t* kept, int64_t n_kept,

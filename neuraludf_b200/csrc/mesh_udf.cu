@@ -459,7 +459,7 @@ __global__ void k_iso_active(const float* __restrict__ df, Dims D, float level, 
   }
 }
 
-// Active cells without a scan of every cell (nudf_iso_lat_cells_*): every active cell has a corner with v <= 0, which is
+// Active cells without a scan of every cell (nudf_iso_cells_*): every active cell has a corner with v <= 0, which is
 // finite and therefore stored, so visiting the storage positions of the lattice (S below) with v <= 0 and testing the up
 // to 8 cells holding each finds them all.  A cell is emitted by its lowest corner with v <= 0 only (corners ascend with
 // the flat index), so once.  The test is k_iso_active's on the same corner values, so the set is nonzero(nudf_iso_active)
@@ -658,7 +658,6 @@ __global__ void k_iso_vertices_dense(const float* __restrict__ df, Dims D, float
 }
 
 static inline unsigned grid_for(int64_t n) { return (unsigned)std::min<int64_t>(std::max<int64_t>(cdiv(n, 256), 1), 65535ll * 8); }
-static inline Dims dims(int32_t n0, int32_t n1, int32_t n2) { return Dims{n0, n1, n2}; }
 static inline Dims dims(const nudf_lattice& l) { return Dims{l.n0, l.n1, l.n2}; }
 
 }  // namespace mc
@@ -666,8 +665,6 @@ static inline Dims dims(const nudf_lattice& l) { return Dims{l.n0, l.n1, l.n2}; 
 
 using namespace nudf;
 using namespace nudf::mc;
-
-#define MC_DIMS_OK() NUDF_REQUIRE(n0 >= 2 && n1 >= 2 && n2 >= 2, "lattice dimensions must be at least 2")
 
 int nudf_mc_active(const nudf_lattice* lat, const int64_t* cand, int64_t n_cand, float avg_t, float max_t, uint8_t* flags,
                    void* stream) {
@@ -781,25 +778,23 @@ int nudf_mc_vertices(const nudf_lattice* lat, const int64_t* cells, int64_t n_ce
 
 #define ISO_LEVEL_OK() NUDF_REQUIRE(level == level && level - level == 0.f, "level must be finite")
 
-int nudf_iso_active(const float* df, int32_t n0, int32_t n1, int32_t n2, float level, uint8_t* flags, void* stream) {
-  MC_DIMS_OK();
-  ISO_LEVEL_OK();
-  NUDF_REQUIRE(df && flags, "null pointer");
-  const int64_t n = (int64_t)n0 * n1 * n2;
-  k_iso_active<<<grid_for(n), 256, 0, (cudaStream_t)stream>>>(df, dims(n0, n1, n2), level, n, flags);
-  NUDF_LAUNCH_OK();
-  return 0;
-}
-
-// the threshold stages on a lattice descriptor; the nudf_iso_* entry points taking a flat array are their dense form
+// the threshold stages on a lattice descriptor
 template <class F>
 static int with_iso_lattice(const nudf_lattice* lat, float level, F&& launch) {
   ISO_LEVEL_OK();
   return with_lattice(lat, [&](auto df) { return launch(df, dims(*lat)); });
 }
 
-static inline nudf_lattice dense_lattice(const float* df, int32_t n0, int32_t n1, int32_t n2) {
-  return nudf_lattice{n0, n1, n2, df, nullptr};
+// every cell of a df lattice; the raw restrict pointer keeps k_iso_active's loads on the read-only path
+int nudf_iso_active(const nudf_lattice* lat, float level, uint8_t* flags, void* stream) {
+  return with_iso_lattice(lat, level, [&](auto, Dims D) {
+    NUDF_REQUIRE(lat->df, "nudf_iso_active reads a df lattice only (nudf_iso_cells_* read a store)");
+    NUDF_REQUIRE(flags, "null pointer");
+    const int64_t n = D.n0 * D.n1 * D.n2;
+    k_iso_active<<<grid_for(n), 256, 0, (cudaStream_t)stream>>>(lat->df, D, level, n, flags);
+    NUDF_LAUNCH_OK();
+    return 0;
+  });
 }
 
 static int iso_cells(const nudf_lattice* lat, float level, int64_t n_seg, int32_t* counts, const int64_t* offsets,
@@ -824,18 +819,18 @@ static int iso_cells(const nudf_lattice* lat, float level, int64_t n_seg, int32_
   });
 }
 
-int nudf_iso_lat_cells_count(const nudf_lattice* lat, float level, int64_t n_seg, int32_t* counts, void* stream) {
+int nudf_iso_cells_count(const nudf_lattice* lat, float level, int64_t n_seg, int32_t* counts, void* stream) {
   return iso_cells(lat, level, n_seg, counts, nullptr, nullptr, stream);
 }
 
-int nudf_iso_lat_cells_emit(const nudf_lattice* lat, float level, int64_t n_seg, const int64_t* offsets, int64_t* cells,
-                            void* stream) {
+int nudf_iso_cells_emit(const nudf_lattice* lat, float level, int64_t n_seg, const int64_t* offsets, int64_t* cells,
+                        void* stream) {
   NUDF_REQUIRE(offsets, "null pointer");
   return iso_cells(lat, level, n_seg, nullptr, offsets, cells, stream);
 }
 
-int nudf_iso_lat_count(const nudf_lattice* lat, float level, const int64_t* cells, int64_t n_cells, int32_t* counts,
-                       void* stream) {
+int nudf_iso_count(const nudf_lattice* lat, float level, const int64_t* cells, int64_t n_cells, int32_t* counts,
+                   void* stream) {
   return with_iso_lattice(lat, level, [&](auto df, Dims D) {
     NUDF_REQUIRE(cells && counts && n_cells >= 0, "null pointer or negative count");
     if (n_cells == 0) return 0;
@@ -846,8 +841,8 @@ int nudf_iso_lat_count(const nudf_lattice* lat, float level, const int64_t* cell
   });
 }
 
-int nudf_iso_lat_emit(const nudf_lattice* lat, float level, const int64_t* cells, int64_t n_cells, const int64_t* offsets,
-                      int64_t* keys, void* stream) {
+int nudf_iso_emit(const nudf_lattice* lat, float level, const int64_t* cells, int64_t n_cells, const int64_t* offsets,
+                  int64_t* keys, void* stream) {
   return with_iso_lattice(lat, level, [&](auto df, Dims D) {
     NUDF_REQUIRE(cells && offsets && keys && n_cells >= 0, "null pointer or negative count");
     if (n_cells == 0) return 0;
@@ -858,8 +853,8 @@ int nudf_iso_lat_emit(const nudf_lattice* lat, float level, const int64_t* cells
   });
 }
 
-int nudf_iso_lat_vertices(const nudf_lattice* lat, float level, const int64_t* cells, int64_t n_cells, const int64_t* keys,
-                          int64_t n_keys, double* verts, void* stream) {
+int nudf_iso_vertices(const nudf_lattice* lat, float level, const int64_t* cells, int64_t n_cells, const int64_t* keys,
+                      int64_t n_keys, double* verts, void* stream) {
   return with_iso_lattice(lat, level, [&](auto df, Dims D) {
     NUDF_REQUIRE(cells && keys && verts && n_cells >= 0 && n_keys >= 0, "null pointer or negative count");
     if (n_keys == 0) return 0;
@@ -870,28 +865,4 @@ int nudf_iso_lat_vertices(const nudf_lattice* lat, float level, const int64_t* c
     NUDF_LAUNCH_OK();
     return 0;
   });
-}
-
-int nudf_iso_count(const float* df, int32_t n0, int32_t n1, int32_t n2, float level, const int64_t* cells, int64_t n_cells,
-                   int32_t* counts, void* stream) {
-  MC_DIMS_OK();
-  NUDF_REQUIRE(df, "null pointer");
-  const nudf_lattice lat = dense_lattice(df, n0, n1, n2);
-  return nudf_iso_lat_count(&lat, level, cells, n_cells, counts, stream);
-}
-
-int nudf_iso_emit(const float* df, int32_t n0, int32_t n1, int32_t n2, float level, const int64_t* cells, int64_t n_cells,
-                  const int64_t* offsets, int64_t* keys, void* stream) {
-  MC_DIMS_OK();
-  NUDF_REQUIRE(df, "null pointer");
-  const nudf_lattice lat = dense_lattice(df, n0, n1, n2);
-  return nudf_iso_lat_emit(&lat, level, cells, n_cells, offsets, keys, stream);
-}
-
-int nudf_iso_vertices(const float* df, int32_t n0, int32_t n1, int32_t n2, float level, const int64_t* cells, int64_t n_cells,
-                      const int64_t* keys, int64_t n_keys, double* verts, void* stream) {
-  MC_DIMS_OK();
-  NUDF_REQUIRE(df, "null pointer");
-  const nudf_lattice lat = dense_lattice(df, n0, n1, n2);
-  return nudf_iso_lat_vertices(&lat, level, cells, n_cells, keys, n_keys, verts, stream);
 }

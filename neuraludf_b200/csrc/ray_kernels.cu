@@ -174,11 +174,10 @@ __device__ __forceinline__ void ray_forward_state(const nudf_render_cfg& cfg, co
   __syncwarp();
 }
 
-__device__ __forceinline__ RaySmem carve(float* base, int SO, int n_arrays_check) {
+__device__ __forceinline__ RaySmem carve(float* base, int SO) {
   RaySmem sm;
   sm.tc = base; sm.t = base + SO; sm.q = base + 2 * SO; sm.P = base + 3 * SO; sm.ap = base + 4 * SO;
   sm.am = base + 5 * SO; sm.alpha = base + 6 * SO; sm.T = base + 7 * SO; sm.wbar = base + 8 * SO; sm.abar = base + 9 * SO;
-  (void)n_arrays_check;
   return sm;
 }
 constexpr int RK_ARRAYS = 10;
@@ -294,7 +293,7 @@ composite_forward_kernel(nudf_render_cfg cfg, RayIn in, nudf_render_out out) {
   const int r = blockIdx.x * RK_WARPS + warp;
   if (r >= cfg.n_rays) return;
   const int S = cfg.n_samples, O = cfg.n_outside, SO = S + O;
-  RaySmem sm = carve(smem + (size_t)warp * RK_ARRAYS * SO, SO, RK_ARRAYS);
+  RaySmem sm = carve(smem + (size_t)warp * RK_ARRAYS * SO, SO);
   ray_forward_state<RULE>(cfg, in, r, lane, sm);
 
   CoreExtra ex(cfg, in, out, sm, r);
@@ -373,7 +372,7 @@ view_forward_kernel(nudf_render_cfg cfg, RayIn in, ViewArgs va) {
   const int r = blockIdx.x * RK_WARPS + warp;
   if (r >= cfg.n_rays) return;
   const int S = cfg.n_samples, O = cfg.n_outside, SO = S + O;
-  RaySmem sm = carve(smem + (size_t)warp * RK_ARRAYS * SO, SO, RK_ARRAYS);
+  RaySmem sm = carve(smem + (size_t)warp * RK_ARRAYS * SO, SO);
   ray_forward_state<RULE>(cfg, in, r, lane, sm);
 
   ViewExtra ex(in, va.c_pix, (int64_t)r * SO, O > 0);
@@ -412,7 +411,7 @@ composite_backward_kernel(nudf_render_cfg cfg, RayIn in, RayBar bar, RayBwdOut o
   const int r = blockIdx.x * RK_WARPS + warp;
   if (r >= cfg.n_rays) return;
   const int S = cfg.n_samples, O = cfg.n_outside, SO = S + O;
-  RaySmem sm = carve(smem + (size_t)warp * RK_ARRAYS * SO, SO, RK_ARRAYS);
+  RaySmem sm = carve(smem + (size_t)warp * RK_ARRAYS * SO, SO);
   ray_forward_state<RULE>(cfg, in, r, lane, sm);
 
   const int64_t base = (int64_t)r * S;
@@ -591,56 +590,37 @@ int nudf_outside_points(const float* rays_o, const float* rays_d, const float* z
   return 0;
 }
 
-static int check_cfg(const nudf_render_cfg* cfg, const float* bg_alpha, const float* bg_color) {
-  NUDF_REQUIRE(cfg != nullptr, "null cfg");
-  NUDF_REQUIRE(cfg->n_samples > 0 && cfg->n_outside >= 0, "bad sample counts");
-  NUDF_REQUIRE(cfg->n_outside == 0 || (bg_alpha && bg_color), "n_outside > 0 needs bg_alpha / bg_color");
-  size_t smem = (size_t)RK_WARPS * RK_ARRAYS * (cfg->n_samples + cfg->n_outside) * sizeof(float);
-  NUDF_REQUIRE(smem <= 200 * 1024, "too many samples per ray for the compositing kernel (max ~1280)");
-  return 0;
-}
-
 }  // extern "C"
 
 namespace {
 
-// Launchers shared by the entry points with and without an alpha rule: one kernel instantiation per rule.
-template <int RULE>
-int composite_forward_launch(const nudf_render_cfg* cfg, const RayIn& in, const nudf_render_out* out, cudaStream_t st) {
-  size_t smem = (size_t)RK_WARPS * RK_ARRAYS * (cfg->n_samples + cfg->n_outside) * sizeof(float);
-  if (smem > 48 * 1024)
-    NUDF_CUDA_OK(cudaFuncSetAttribute(composite_forward_kernel<RULE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  LaunchTimer lt_(FAM_RAY, st);
-  composite_forward_kernel<RULE><<<(unsigned)cdiv(cfg->n_rays, RK_WARPS), RK_WARPS * 32, smem, st>>>(*cfg, in, *out);
-  NUDF_LAUNCH_OK();
+// dynamic shared memory of a ray kernel: RK_ARRAYS per-sample arrays per warp
+size_t ray_smem(const nudf_render_cfg& cfg) {
+  return (size_t)RK_WARPS * RK_ARRAYS * (cfg.n_samples + cfg.n_outside) * sizeof(float);
+}
+
+// The alpha rule is checked first, so that a bad rule is refused before any pointer is looked at.
+int check_cfg(const nudf_render_cfg* cfg, const float* bg_alpha, const float* bg_color) {
+  NUDF_REQUIRE(cfg != nullptr, "null cfg");
+  NUDF_REQUIRE(cfg->alpha_rule == ALPHA_NUMERICAL || cfg->alpha_rule == ALPHA_THEORICAL,
+               "alpha_rule must be 0 (numerical) or 1 (theorical)");
+  NUDF_REQUIRE(cfg->n_samples > 0 && cfg->n_outside >= 0, "bad sample counts");
+  NUDF_REQUIRE(cfg->n_outside == 0 || (bg_alpha && bg_color), "n_outside > 0 needs bg_alpha / bg_color");
+  NUDF_REQUIRE(ray_smem(*cfg) <= 200 * 1024, "too many samples per ray for the compositing kernel (max ~1280)");
   return 0;
 }
 
-template <int RULE>
-int view_forward_launch(const nudf_render_cfg* cfg, const RayIn& in, const ViewArgs& va, cudaStream_t st) {
-  size_t smem = (size_t)RK_WARPS * RK_ARRAYS * (cfg->n_samples + cfg->n_outside) * sizeof(float);
+// Launches the instantiation of a ray kernel for the cfg's alpha rule, one warp per ray.
+template <class... A>
+int launch_rays(void (*numerical)(nudf_render_cfg, RayIn, A...), void (*theorical)(nudf_render_cfg, RayIn, A...),
+                const nudf_render_cfg* cfg, const RayIn& in, cudaStream_t st, const A&... args) {
+  const auto kernel = cfg->alpha_rule == ALPHA_THEORICAL ? theorical : numerical;
+  const size_t smem = ray_smem(*cfg);
   if (smem > 48 * 1024)
-    NUDF_CUDA_OK(cudaFuncSetAttribute(view_forward_kernel<RULE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    NUDF_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   LaunchTimer lt_(FAM_RAY, st);
-  view_forward_kernel<RULE><<<(unsigned)cdiv(cfg->n_rays, RK_WARPS), RK_WARPS * 32, smem, st>>>(*cfg, in, va);
+  kernel<<<(unsigned)cdiv(cfg->n_rays, RK_WARPS), RK_WARPS * 32, smem, st>>>(*cfg, in, args...);
   NUDF_LAUNCH_OK();
-  return 0;
-}
-
-template <int RULE>
-int composite_backward_launch(const nudf_render_cfg* cfg, const RayIn& in, const RayBar& rb, const RayBwdOut& ob,
-                              cudaStream_t st) {
-  size_t smem = (size_t)RK_WARPS * RK_ARRAYS * (cfg->n_samples + cfg->n_outside) * sizeof(float);
-  if (smem > 48 * 1024)
-    NUDF_CUDA_OK(cudaFuncSetAttribute(composite_backward_kernel<RULE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  LaunchTimer lt_(FAM_RAY, st);
-  composite_backward_kernel<RULE><<<(unsigned)cdiv(cfg->n_rays, RK_WARPS), RK_WARPS * 32, smem, st>>>(*cfg, in, rb, ob);
-  NUDF_LAUNCH_OK();
-  return 0;
-}
-
-int check_rule(int32_t alpha_rule) {
-  NUDF_REQUIRE(alpha_rule == ALPHA_NUMERICAL || alpha_rule == ALPHA_THEORICAL, "alpha_rule must be 0 (numerical) or 1 (theorical)");
   return 0;
 }
 
@@ -648,33 +628,22 @@ int check_rule(int32_t alpha_rule) {
 
 extern "C" {
 
-int nudf_render_composite_forward_rule(const nudf_render_cfg* cfg, const float* heads, const float* rays_d, const float* pts,
-                                       const float* mid_z, const float* dists, const float* udf, int64_t ld_udf,
-                                       const float* grads, const float* sampled_color_base, const float* sampled_color,
-                                       const float* bg_alpha, const float* bg_color, const nudf_render_out* out,
-                                       int32_t alpha_rule, void* stream) {
-  if (int rc = check_rule(alpha_rule)) return rc;
+int nudf_render_composite_forward(const nudf_render_cfg* cfg, const float* heads, const float* rays_d, const float* pts,
+                                  const float* mid_z, const float* dists, const float* udf, int64_t ld_udf,
+                                  const float* grads, const float* sampled_color_base, const float* sampled_color,
+                                  const float* bg_alpha, const float* bg_color, const nudf_render_out* out, void* stream) {
   if (int rc = check_cfg(cfg, bg_alpha, bg_color)) return rc;
   NUDF_REQUIRE(heads && rays_d && pts && mid_z && dists && udf && grads && sampled_color_base && sampled_color && out, "null pointer");
   if (cfg->n_rays <= 0) return 0;
   RayIn in{heads, rays_d, pts, mid_z, dists, udf, ld_udf, grads, sampled_color_base, sampled_color, bg_alpha, bg_color};
-  return alpha_rule == ALPHA_THEORICAL ? composite_forward_launch<ALPHA_THEORICAL>(cfg, in, out, (cudaStream_t)stream)
-                                       : composite_forward_launch<ALPHA_NUMERICAL>(cfg, in, out, (cudaStream_t)stream);
+  return launch_rays(composite_forward_kernel<ALPHA_NUMERICAL>, composite_forward_kernel<ALPHA_THEORICAL>, cfg, in,
+                     (cudaStream_t)stream, *out);
 }
 
-int nudf_render_composite_forward(const nudf_render_cfg* cfg, const float* heads, const float* rays_d, const float* pts, const float* mid_z,
-                                  const float* dists, const float* udf, int64_t ld_udf, const float* grads,
-                                  const float* sampled_color_base, const float* sampled_color, const float* bg_alpha,
-                                  const float* bg_color, const nudf_render_out* out, void* stream) {
-  return nudf_render_composite_forward_rule(cfg, heads, rays_d, pts, mid_z, dists, udf, ld_udf, grads, sampled_color_base,
-                                            sampled_color, bg_alpha, bg_color, out, ALPHA_NUMERICAL, stream);
-}
-
-int nudf_render_view_forward_rule(const nudf_render_cfg* cfg, const float* heads, const float* rays_d, const float* pts,
-                                  const float* mid_z, const float* dists, const float* udf, int64_t ld_udf, const float* grads,
-                                  const float* sampled_color, const float* c_pix, const float* bg_alpha, const float* bg_color,
-                                  const float* rot, const nudf_view_out* out, int32_t alpha_rule, void* stream) {
-  if (int rc = check_rule(alpha_rule)) return rc;
+int nudf_render_view_forward(const nudf_render_cfg* cfg, const float* heads, const float* rays_d, const float* pts,
+                             const float* mid_z, const float* dists, const float* udf, int64_t ld_udf, const float* grads,
+                             const float* sampled_color, const float* c_pix, const float* bg_alpha, const float* bg_color,
+                             const float* rot, const nudf_view_out* out, void* stream) {
   if (int rc = check_cfg(cfg, bg_alpha, bg_color)) return rc;
   NUDF_REQUIRE(heads && rays_d && pts && mid_z && dists && udf && grads && sampled_color && rot && out, "null pointer");
   if (cfg->n_rays <= 0) return 0;
@@ -683,25 +652,16 @@ int nudf_render_view_forward_rule(const nudf_render_cfg* cfg, const float* heads
   va.c_pix = c_pix;
   for (int k = 0; k < 9; ++k) va.rot[k] = rot[k];
   va.out = *out;
-  return alpha_rule == ALPHA_THEORICAL ? view_forward_launch<ALPHA_THEORICAL>(cfg, in, va, (cudaStream_t)stream)
-                                       : view_forward_launch<ALPHA_NUMERICAL>(cfg, in, va, (cudaStream_t)stream);
+  return launch_rays(view_forward_kernel<ALPHA_NUMERICAL>, view_forward_kernel<ALPHA_THEORICAL>, cfg, in,
+                     (cudaStream_t)stream, va);
 }
 
-int nudf_render_view_forward(const nudf_render_cfg* cfg, const float* heads, const float* rays_d, const float* pts,
-                             const float* mid_z, const float* dists, const float* udf, int64_t ld_udf, const float* grads,
-                             const float* sampled_color, const float* c_pix, const float* bg_alpha, const float* bg_color,
-                             const float* rot, const nudf_view_out* out, void* stream) {
-  return nudf_render_view_forward_rule(cfg, heads, rays_d, pts, mid_z, dists, udf, ld_udf, grads, sampled_color, c_pix,
-                                       bg_alpha, bg_color, rot, out, ALPHA_NUMERICAL, stream);
-}
-
-int nudf_render_composite_backward_rule(const nudf_render_cfg* cfg, const float* heads, const float* rays_d, const float* pts,
-                                        const float* mid_z, const float* dists, const float* udf, int64_t ld_udf,
-                                        const float* grads, const float* sampled_color_base, const float* sampled_color,
-                                        const float* bg_alpha, const float* bg_color, const nudf_render_bar* bar,
-                                        float* udf_bar, float* grads_bar, float* scb_bar, float* sc_bar, float* bg_alpha_bar,
-                                        float* bg_color_bar, float* scalar_bar, int32_t alpha_rule, void* stream) {
-  if (int rc = check_rule(alpha_rule)) return rc;
+int nudf_render_composite_backward(const nudf_render_cfg* cfg, const float* heads, const float* rays_d, const float* pts,
+                                   const float* mid_z, const float* dists, const float* udf, int64_t ld_udf,
+                                   const float* grads, const float* sampled_color_base, const float* sampled_color,
+                                   const float* bg_alpha, const float* bg_color, const nudf_render_bar* bar,
+                                   float* udf_bar, float* grads_bar, float* scb_bar, float* sc_bar, float* bg_alpha_bar,
+                                   float* bg_color_bar, float* scalar_bar, void* stream) {
   if (int rc = check_cfg(cfg, bg_alpha, bg_color)) return rc;
   NUDF_REQUIRE(heads && rays_d && pts && mid_z && dists && udf && grads && sampled_color_base && sampled_color && bar, "null pointer");
   NUDF_REQUIRE(udf_bar && grads_bar && scb_bar && sc_bar, "null output pointer");
@@ -713,19 +673,8 @@ int nudf_render_composite_backward_rule(const nudf_render_cfg* cfg, const float*
   rb.weights = bar->weights;
   rb.ray_sums = bar->ray_sums;
   RayBwdOut ob{udf_bar, grads_bar, scb_bar, sc_bar, bg_alpha_bar, bg_color_bar, scalar_bar};
-  return alpha_rule == ALPHA_THEORICAL ? composite_backward_launch<ALPHA_THEORICAL>(cfg, in, rb, ob, (cudaStream_t)stream)
-                                       : composite_backward_launch<ALPHA_NUMERICAL>(cfg, in, rb, ob, (cudaStream_t)stream);
-}
-
-int nudf_render_composite_backward(const nudf_render_cfg* cfg, const float* heads, const float* rays_d, const float* pts, const float* mid_z,
-                                   const float* dists, const float* udf, int64_t ld_udf, const float* grads,
-                                   const float* sampled_color_base, const float* sampled_color, const float* bg_alpha,
-                                   const float* bg_color, const nudf_render_bar* bar,
-                                   float* udf_bar, float* grads_bar, float* scb_bar, float* sc_bar, float* bg_alpha_bar,
-                                   float* bg_color_bar, float* scalar_bar, void* stream) {
-  return nudf_render_composite_backward_rule(cfg, heads, rays_d, pts, mid_z, dists, udf, ld_udf, grads, sampled_color_base,
-                                             sampled_color, bg_alpha, bg_color, bar, udf_bar, grads_bar, scb_bar, sc_bar,
-                                             bg_alpha_bar, bg_color_bar, scalar_bar, ALPHA_NUMERICAL, stream);
+  return launch_rays(composite_backward_kernel<ALPHA_NUMERICAL>, composite_backward_kernel<ALPHA_THEORICAL>, cfg, in,
+                     (cudaStream_t)stream, rb, ob);
 }
 
 }  // extern "C"

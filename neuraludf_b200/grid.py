@@ -164,8 +164,8 @@ def band_block_test(df, N, s, parent=None, parent_s=0, lipschitz=2.0, tau=None, 
     out = torch.empty(nb ** 3, dtype=torch.uint8, device=device) if flags else None
     slope = torch.zeros(1, dtype=torch.int32, device=device)
     tau = 2.0 * (2.0 / (N - 1)) if tau is None else tau
-    check(_lib.lib().nudf_nb_lat_block_test(lat, s, ptr(parent), parent_s, _coords(N, axes, spacing, pad), float(lipschitz),
-                                            float(tau), ptr(out), ptr(slope), _lib.stream_ptr()), "nudf_nb_lat_block_test")
+    check(_lib.lib().nudf_nb_block_test(lat, s, ptr(parent), parent_s, _coords(N, axes, spacing, pad), float(lipschitz),
+                                        float(tau), ptr(out), ptr(slope), _lib.stream_ptr()), "nudf_nb_block_test")
     return out, float(slope.view(torch.float32))
 
 

@@ -148,12 +148,12 @@ def iso_marching_cubes_index(df, dims, level):
     df = df.contiguous()
     if df.numel() != n0 * n1 * n2:
         raise ValueError("df has %d values, dims %s need %d" % (df.numel(), (n0, n1, n2), n0 * n1 * n2))
+    lat = ctypes.byref(_lib.Lattice(n0, n1, n2, df.data_ptr(), None))
     flags = torch.empty(df.numel(), dtype=torch.uint8, device=dev)
-    check(L.nudf_iso_active(ptr(df), n0, n1, n2, level, ptr(flags), st), "nudf_iso_active")
+    check(L.nudf_iso_active(lat, level, ptr(flags), st), "nudf_iso_active")
     cells = torch.nonzero(flags).reshape(-1).contiguous()
     del flags
-    lat = _lib.Lattice(n0, n1, n2, df.data_ptr(), None)
-    return _iso_stages(ctypes.byref(lat), cells, level, dev)
+    return _iso_stages(lat, cells, level, dev)
 
 
 def _iso_stages(lat, cells, level, dev):
@@ -167,13 +167,13 @@ def _iso_stages(lat, cells, level, dev):
     if n == 0:
         return empty[0], empty[1], info
     counts = torch.empty(n, dtype=torch.int32, device=dev)
-    check(L.nudf_iso_lat_count(lat, level, ptr(cells), n, ptr(counts), st), "nudf_iso_lat_count")
+    check(L.nudf_iso_count(lat, level, ptr(cells), n, ptr(counts), st), "nudf_iso_count")
     csum = torch.cumsum(counts, 0, dtype=torch.int64)
     n_faces = int(csum[-1])
     offsets = (csum - counts).contiguous()
     del counts, csum
     keys = torch.empty(3 * n_faces, dtype=torch.int64, device=dev)
-    check(L.nudf_iso_lat_emit(lat, level, ptr(cells), n, ptr(offsets), ptr(keys), st), "nudf_iso_lat_emit")
+    check(L.nudf_iso_emit(lat, level, ptr(cells), n, ptr(offsets), ptr(keys), st), "nudf_iso_emit")
     del offsets
     info["face_keys"] = keys.reshape(-1, 3)
     if n_faces == 0:
@@ -181,27 +181,27 @@ def _iso_stages(lat, cells, level, dev):
     ukeys, inv = torch.unique(keys, sorted=True, return_inverse=True)
     ukeys = ukeys.contiguous()
     verts = torch.empty(ukeys.numel(), 3, dtype=torch.float64, device=dev)
-    check(L.nudf_iso_lat_vertices(lat, level, ptr(cells), n, ptr(ukeys), ukeys.numel(), ptr(verts), st),
-          "nudf_iso_lat_vertices")
+    check(L.nudf_iso_vertices(lat, level, ptr(cells), n, ptr(ukeys), ukeys.numel(), ptr(verts), st),
+          "nudf_iso_vertices")
     info["vertex_keys"] = ukeys
     return verts, inv.reshape(-1, 3).to(torch.int64), info
 
 
 def _iso_cells(lat, n_positions, level, dev):
     """sorted active cells of the lattice descriptor `lat` at the fp32 `level` from its n_positions storage positions
-    (nudf_iso_lat_cells_*: no scan of every cell)"""
+    (nudf_iso_cells_*: no scan of every cell)"""
     L = _lib.lib()
     st = _lib.stream_ptr()
     n_seg = -(-n_positions // _lib.ISO_SEG)
     counts = torch.empty(n_seg, dtype=torch.int32, device=dev)
-    check(L.nudf_iso_lat_cells_count(lat, level, n_seg, ptr(counts), st), "nudf_iso_lat_cells_count")
+    check(L.nudf_iso_cells_count(lat, level, n_seg, ptr(counts), st), "nudf_iso_cells_count")
     csum = torch.cumsum(counts, 0, dtype=torch.int64)
     total = int(csum[-1]) if n_seg else 0
     offsets = (csum - counts).contiguous()
     del counts, csum
     cells = torch.empty(total, dtype=torch.int64, device=dev)
     if total:
-        check(L.nudf_iso_lat_cells_emit(lat, level, n_seg, ptr(offsets), ptr(cells), st), "nudf_iso_lat_cells_emit")
+        check(L.nudf_iso_cells_emit(lat, level, n_seg, ptr(offsets), ptr(cells), st), "nudf_iso_cells_emit")
     del offsets
     return torch.sort(cells).values
 

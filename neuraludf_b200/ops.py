@@ -552,8 +552,7 @@ def alpha_rule(sdf2alpha_type):
 
 def _make_cfg(N, S, O, sample_dist, cos_anneal_ratio, flip_saturation, sparse_scale_factor, use_norm, background_rgb,
               alpha_rule=0):
-    """The compositing kernels' nudf_render_cfg.  alpha_rule (0 numerical, 1 theorical) is not part of the struct: it rides
-    along as a Python attribute and composite / view_composite hand it to the *_rule entry points."""
+    """The compositing kernels' nudf_render_cfg; alpha_rule: 0 numerical, 1 theorical."""
     if alpha_rule not in (0, 1):
         raise ValueError("alpha_rule must be 0 (numerical) or 1 (theorical), got %r" % (alpha_rule,))
     cfg = L.RenderCfg()
@@ -605,11 +604,6 @@ def _check_composite_rows(N, S, O, **ts):
                 name, tuple(t.shape), r, " of %d" % w if w > 1 else "", N, S, O))
 
 
-def _cfg_rule(cfg):
-    """alpha_rule of a cfg from _make_cfg (0, numerical, for a bare nudf_render_cfg)"""
-    return getattr(cfg, "alpha_rule", 0)
-
-
 class _CompositeFunction(torch.autograd.Function):
     """differentiable inputs: udf [P] / [P,1] / [N,S], grads [P,3], scb [P,3], sc [P,3], bg_alpha [N,S+O],
     bg_color [N,S+O,3], heads [3]"""
@@ -639,11 +633,10 @@ class _CompositeFunction(torch.autograd.Function):
         for k in L.RENDER_OUT_FIELDS:
             setattr(ro, k, outs[k].data_ptr() if k in outs else None)
         ro.status = status_word(dev).data_ptr()
-        L.check(lib.nudf_render_composite_forward_rule(ctypes.byref(cfg), L.ptr(heads), L.ptr(rays_d), L.ptr(pts), L.ptr(mid),
-                                                       L.ptr(dists), L.ptr(udf), ld_udf, L.ptr(grads), L.ptr(scb), L.ptr(sc),
-                                                       L.ptr(bg_alpha), L.ptr(bg_color), ctypes.byref(ro), _cfg_rule(cfg),
-                                                       L.stream_ptr()),
-                "nudf_render_composite_forward_rule")
+        L.check(lib.nudf_render_composite_forward(ctypes.byref(cfg), L.ptr(heads), L.ptr(rays_d), L.ptr(pts), L.ptr(mid),
+                                                  L.ptr(dists), L.ptr(udf), ld_udf, L.ptr(grads), L.ptr(scb), L.ptr(sc),
+                                                  L.ptr(bg_alpha), L.ptr(bg_color), ctypes.byref(ro), L.stream_ptr()),
+                "nudf_render_composite_forward")
         ctx.cfg, ctx.geom, ctx.ld_udf, ctx.udf_shape = cfg, geom, ld_udf, udf_shape
         ctx.has_bg = bg_alpha is not None
         ctx.save_for_backward(udf, grads, scb, sc, bg_alpha, bg_color, heads)
@@ -677,13 +670,12 @@ class _CompositeFunction(torch.autograd.Function):
         if bgc_bar is not None:
             bgc_bar[:, :S].zero_()
         scal = f(N, 3)
-        L.check(lib.nudf_render_composite_backward_rule(ctypes.byref(cfg), L.ptr(heads), L.ptr(rays_d), L.ptr(pts),
-                                                        L.ptr(mid), L.ptr(dists), L.ptr(udf), ctx.ld_udf, L.ptr(grads),
-                                                        L.ptr(scb), L.ptr(sc), L.ptr(bg_alpha), L.ptr(bg_color),
-                                                        ctypes.byref(bar), L.ptr(udf_bar), L.ptr(grads_bar), L.ptr(scb_bar),
-                                                        L.ptr(sc_bar), L.ptr(bga_bar), L.ptr(bgc_bar), L.ptr(scal),
-                                                        _cfg_rule(cfg), L.stream_ptr()),
-                "nudf_render_composite_backward_rule")
+        L.check(lib.nudf_render_composite_backward(ctypes.byref(cfg), L.ptr(heads), L.ptr(rays_d), L.ptr(pts),
+                                                   L.ptr(mid), L.ptr(dists), L.ptr(udf), ctx.ld_udf, L.ptr(grads),
+                                                   L.ptr(scb), L.ptr(sc), L.ptr(bg_alpha), L.ptr(bg_color),
+                                                   ctypes.byref(bar), L.ptr(udf_bar), L.ptr(grads_bar), L.ptr(scb_bar),
+                                                   L.ptr(sc_bar), L.ptr(bga_bar), L.ptr(bgc_bar), L.ptr(scal), L.stream_ptr()),
+                "nudf_render_composite_backward")
         # in the caller's shape: [P] (possibly a strided view), [P, 1] or [N, S]
         return (udf_bar.reshape(ctx.udf_shape), grads_bar, scb_bar, sc_bar, bga_bar, bgc_bar, scal.sum(dim=0),
                 None, None, None)
@@ -848,7 +840,7 @@ def nerf_forward_into(desc, wimg, pts, dirs, samples_per_ray, sigma, rgb, ctx):
 
 
 def view_composite(cfg, heads, rays_d, pts, mid, dists, udf, grads, sc, c_pix, bg_alpha, bg_color, rot, outs):
-    """nudf_render_view_forward_rule under the cfg's alpha_rule: outs maps color / color_pixel / depth / normal / weight_sum to [N, .] tensors (views
+    """nudf_render_view_forward: outs maps color / color_pixel / depth / normal / weight_sum to [N, .] tensors (views
     into the image buffers are fine) or None; rot is a host 3x3 (nested sequence or array)."""
     lib = L.lib()
     ro = L.ViewOut()
@@ -856,10 +848,10 @@ def view_composite(cfg, heads, rays_d, pts, mid, dists, udf, grads, sc, c_pix, b
         t = outs.get(k)
         setattr(ro, k, None if t is None else t.data_ptr())
     r9 = (ctypes.c_float * 9)(*[float(v) for row in rot for v in row])
-    L.check(lib.nudf_render_view_forward_rule(ctypes.byref(cfg), L.ptr(heads), L.ptr(rays_d), L.ptr(pts), L.ptr(mid),
-                                              L.ptr(dists), L.ptr(udf), 1, L.ptr(grads), L.ptr(sc), L.ptr(c_pix),
-                                              L.ptr(bg_alpha), L.ptr(bg_color), r9, ctypes.byref(ro), _cfg_rule(cfg),
-                                              L.stream_ptr()), "nudf_render_view_forward_rule")
+    L.check(lib.nudf_render_view_forward(ctypes.byref(cfg), L.ptr(heads), L.ptr(rays_d), L.ptr(pts), L.ptr(mid),
+                                         L.ptr(dists), L.ptr(udf), 1, L.ptr(grads), L.ptr(sc), L.ptr(c_pix),
+                                         L.ptr(bg_alpha), L.ptr(bg_color), r9, ctypes.byref(ro), L.stream_ptr()),
+            "nudf_render_view_forward")
 
 
 def blend_forward_into(cfg, pts, proj, hom, px, imgs, logits, c_pix, c_pat, m_pat):

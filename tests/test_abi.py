@@ -24,7 +24,7 @@ def test_library_exports_the_declared_abi():
     for name in declared:
         assert hasattr(L, name), "libnudf.so does not export %s" % name
     assert sorted(_lib.exported_symbols()) == declared, "python binding and include/nudf.h disagree"
-    assert L.nudf_abi_version() == 5
+    assert L.nudf_abi_version() == 6
 
 
 def test_descriptor_validation_runs_without_gpu():
@@ -67,14 +67,31 @@ def test_lattice_descriptor_validation_runs_without_gpu():
                       (_lib.Lattice(4, 4, 5, None, ctypes.pointer(store)), b"the store's n")):
         assert L.nudf_mc_links(ctypes.byref(lat), None, 0, None, None, None) == -1
         assert what in L.nudf_last_error()
-    tables = _lib.BandCoords(0.0, (ctypes.c_void_p * 3)(1, 1, 1))
     lat = _lib.Lattice(4, 4, 4, None, ctypes.pointer(store))
-    assert L.nudf_nb_block_test(ctypes.byref(lat), 1, None, 0, ctypes.byref(tables), 2.0, 0.1, None, 1, None) == -1
-    assert b"dense lattice" in L.nudf_last_error()
+    assert L.nudf_iso_active(ctypes.byref(lat), 0.0, 1, None) == -1
+    assert b"df lattice" in L.nudf_last_error()
     lat = _lib.Lattice(4, 4, 5, 1, None)
     assert L.nudf_nb_block_test(ctypes.byref(lat), 1, None, 0, ctypes.byref(_lib.BandCoords(0.5)), 2.0, 0.1, None, 1,
                                 None) == -1
     assert b"cubic" in L.nudf_last_error()
+
+
+def test_render_cfg_alpha_rule_validation_runs_without_gpu():
+    from neuraludf_b200 import _lib
+    import ctypes
+    L = _lib.lib()
+    cfg = _lib.RenderCfg()
+    cfg.n_rays, cfg.n_samples = 4, 64
+    calls = (lambda: L.nudf_render_composite_forward(ctypes.byref(cfg), *[None] * 6, 1, *[None] * 7),
+             lambda: L.nudf_render_view_forward(ctypes.byref(cfg), *[None] * 6, 1, *[None] * 8),
+             lambda: L.nudf_render_composite_backward(ctypes.byref(cfg), *[None] * 6, 1, *[None] * 14))
+    for call in calls:
+        cfg.alpha_rule = 2
+        assert call() == -1
+        assert b"alpha_rule" in L.nudf_last_error()
+        cfg.alpha_rule = 1       # a valid rule gets as far as the pointers
+        assert call() == -1
+        assert b"null pointer" in L.nudf_last_error()
 
 
 @pytest.mark.skipif(torch.cuda.is_available(), reason="checks the no-GPU behaviour")

@@ -1,6 +1,6 @@
 """Block-sparse narrow-band threshold meshing (grid.iso_band_sparse, mesh.iso_marching_cubes_sparse / iso_mesh_sparse,
 the BrickDf instantiations of the table block test and of the threshold MC, and the active-cell enumeration
-nudf_iso_lat_cells_*): the store against iso_band's df bit for bit, the mesh against iso_mesh_band bit for bit on the C5
+nudf_iso_cells_*): the store against iso_band's df bit for bit, the mesh against iso_mesh_band bit for bit on the C5
 network on three boxes, on a steep field and with a small batch; the enumeration on dense lattices against
 nudf_iso_active; the runner's NUDF_BAND_MESH=sparse switch; the 1024^3 memory bound; the 2048^3 CLI."""
 import os

@@ -1,7 +1,7 @@
 """The 'theorical' sdf2alpha rule on the device (reference models/udf_renderer_blending.py:321-323): nudf_up_sample mode 2,
 the compositing forward / backward and the view renderer under alpha_rule 1, against the UNMODIFIED reference's outputs
-(tests/golden/theorical_outputs.*.npz) and the oracle's fp64 autograd, with the bounds of SURVEY.md 8(c); the numerical
-rule through the new entry points keeps the old entry points' bits; and the unmodified runner trains under the rule."""
+(tests/golden/theorical_outputs.*.npz) and the oracle's fp64 autograd, with the bounds of SURVEY.md 8(c); the view renderer
+keeps the compositing forward's bits under either rule; and the unmodified runner trains under the rule."""
 import ctypes
 import glob
 import math
@@ -321,12 +321,12 @@ def _composite_args(S=96, Oo=16, seed=5):
     return N, S, Oo, float(c["dists"][0, -1]), args, geom
 
 
-def _raw_calls(rule_entry, N, S, Oo, sd, a, geom, rule):
-    """every forward output and backward output of one entry-point pair (old: rule None; new: alpha_rule = rule)"""
+def _forward_and_view(N, S, Oo, sd, a, geom, rule):
+    """every output of the compositing forward and of the view renderer on the same inputs under alpha_rule = rule"""
     from neuraludf_b200 import _lib as L
     from neuraludf_b200 import ops
     lib = L.lib()
-    cfg = ops._make_cfg(N, S, Oo, sd, 0.35, 0.4, 300.0, False, torch.tensor([0.2, 0.5, 0.9]))
+    cfg = ops._make_cfg(N, S, Oo, sd, 0.35, 0.4, 300.0, False, torch.tensor([0.2, 0.5, 0.9]), rule)
     rays_d, pts, mid, dists = geom
     f = lambda *shape: torch.full(shape, float("nan"), device=DEV)
     outs = {"color_base": f(N, 3), "color": f(N, 3), "depth": f(N, 1), "normals": f(N, 3), "weights": f(N, S + Oo),
@@ -338,63 +338,32 @@ def _raw_calls(rule_entry, N, S, Oo, sd, a, geom, rule):
     for k in L.RENDER_OUT_FIELDS:
         setattr(ro, k, outs[k].data_ptr() if k in outs else None)
     ro.status = None
-    common = (ctypes.byref(cfg), L.ptr(a["heads"]), L.ptr(rays_d), L.ptr(pts), L.ptr(mid), L.ptr(dists), L.ptr(a["udf"]), 1,
-              L.ptr(a["grads"]), L.ptr(a["scb"]), L.ptr(a["sc"]), L.ptr(a["bga"]), L.ptr(a["bgc"]))
-    if rule_entry:
-        L.check(lib.nudf_render_composite_forward_rule(*common, ctypes.byref(ro), rule, None), "fwd_rule")
-    else:
-        L.check(lib.nudf_render_composite_forward(*common, ctypes.byref(ro), None), "fwd")
-    gen = torch.Generator(device=DEV).manual_seed(3)
-    bar_t = {k: torch.randn(outs[k].shape, generator=gen, device=DEV) for k in
-             ("color_base", "color", "depth", "weight_sum", "weight_sum_fg_bg", "ray_sums", "weights")}
-    bar = L.RenderBar()
-    for k, t in bar_t.items():
-        setattr(bar, k, t.data_ptr())
-    P = N * S
-    bw = {"udf_bar": f(P), "grads_bar": f(P, 3), "scb_bar": f(P, 3), "sc_bar": f(P, 3), "bga_bar": f(N, S + Oo),
-          "bgc_bar": f(N, S + Oo, 3), "scal": f(N, 3)}
-    bargs = common + (ctypes.byref(bar),) + tuple(L.ptr(bw[k]) for k in ("udf_bar", "grads_bar", "scb_bar", "sc_bar",
-                                                                       "bga_bar", "bgc_bar", "scal"))
-    if rule_entry:
-        L.check(lib.nudf_render_composite_backward_rule(*bargs, rule, None), "bwd_rule")
-    else:
-        L.check(lib.nudf_render_composite_backward(*bargs, None), "bwd")
-    # view forward
+    L.check(lib.nudf_render_composite_forward(ctypes.byref(cfg), L.ptr(a["heads"]), L.ptr(rays_d), L.ptr(pts), L.ptr(mid),
+                                              L.ptr(dists), L.ptr(a["udf"]), 1, L.ptr(a["grads"]), L.ptr(a["scb"]),
+                                              L.ptr(a["sc"]), L.ptr(a["bga"]), L.ptr(a["bgc"]), ctypes.byref(ro), None), "fwd")
     vo = {k: f(N, 3 if k in ("color", "color_pixel", "normal") else 1) for k in L.VIEW_OUT_FIELDS}
     ro2 = L.ViewOut()
     for k in L.VIEW_OUT_FIELDS:
         setattr(ro2, k, vo[k].data_ptr())
     r9 = (ctypes.c_float * 9)(1, 0, 0, 0, 1, 0, 0, 0, 1)
-    vargs = (ctypes.byref(cfg), L.ptr(a["heads"]), L.ptr(rays_d), L.ptr(pts), L.ptr(mid), L.ptr(dists), L.ptr(a["udf"]), 1,
-             L.ptr(a["grads"]), L.ptr(a["sc"]), L.ptr(a["sc"]), L.ptr(a["bga"]), L.ptr(a["bgc"]), r9, ctypes.byref(ro2))
-    if rule_entry:
-        L.check(lib.nudf_render_view_forward_rule(*vargs, rule, None), "view_rule")
-    else:
-        L.check(lib.nudf_render_view_forward(*vargs, None), "view")
+    L.check(lib.nudf_render_view_forward(ctypes.byref(cfg), L.ptr(a["heads"]), L.ptr(rays_d), L.ptr(pts), L.ptr(mid),
+                                         L.ptr(dists), L.ptr(a["udf"]), 1, L.ptr(a["grads"]), L.ptr(a["sc"]), L.ptr(a["sc"]),
+                                         L.ptr(a["bga"]), L.ptr(a["bgc"]), r9, ctypes.byref(ro2), None), "view")
     torch.cuda.synchronize()
     res = {"fwd." + k: v for k, v in outs.items()}
-    res.update({"bwd." + k: v for k, v in bw.items()})
     res.update({"view." + k: v for k, v in vo.items()})
     return res
 
 
-def test_numerical_rule_through_new_entry_points_keeps_bits():
+def test_view_forward_matches_forward_under_both_rules():
     if not torch.cuda.is_available():
         pytest.skip("no CUDA device")
     N, S, Oo, sd, a, geom = _composite_args()
-    old = _raw_calls(False, N, S, Oo, sd, a, geom, None)
-    new = _raw_calls(True, N, S, Oo, sd, a, geom, 0)
-    th_ = _raw_calls(True, N, S, Oo, sd, a, geom, 1)
-    for k in old:
-        if k == "bwd.bgc_bar":
-            old[k][:, :S].zero_(); new[k][:, :S].zero_(); th_[k][:, :S].zero_()   # columns < S are left unwritten
-        assert torch.equal(old[k], new[k]), k
-    assert not torch.equal(old["fwd.alpha"], th_["fwd.alpha"])
-    assert torch.equal(th_["view.color"], th_["fwd.color"]) and torch.equal(th_["view.depth"], th_["fwd.depth"])
-    from neuraludf_b200 import _lib as L
-    assert L.lib().nudf_render_composite_forward_rule(None, None, None, None, None, None, None, 1, None, None, None, None,
-                                                      None, None, 2, None) != 0
-    assert b"alpha_rule" in L.lib().nudf_last_error()
+    num = _forward_and_view(N, S, Oo, sd, a, geom, 0)
+    th_ = _forward_and_view(N, S, Oo, sd, a, geom, 1)
+    assert not torch.equal(num["fwd.alpha"], th_["fwd.alpha"])
+    for r in (num, th_):
+        assert torch.equal(r["view.color"], r["fwd.color"]) and torch.equal(r["view.depth"], r["fwd.depth"])
 
 
 def test_non_finite_results_raise_under_the_rule():

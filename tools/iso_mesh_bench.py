@@ -33,31 +33,33 @@ def _gpu_info():
 
 def _stages(df, N, level):
     """iso_marching_cubes_index's stages, each bracketed by CUDA events: (ms per stage, active cells, vertices, faces)"""
+    import ctypes
     import torch
     from neuraludf_b200 import _lib
     from neuraludf_b200._lib import check, ptr
     L, st = _lib.lib(), _lib.stream_ptr()
+    lat = ctypes.byref(_lib.Lattice(N, N, N, df.data_ptr(), None))
     ev = [torch.cuda.Event(enable_timing=True) for _ in range(6)]
     ev[0].record()
     flags = torch.empty(df.numel(), dtype=torch.uint8, device=df.device)
-    check(L.nudf_iso_active(ptr(df), N, N, N, level, ptr(flags), st), "nudf_iso_active")
+    check(L.nudf_iso_active(lat, level, ptr(flags), st), "nudf_iso_active")
     cells = torch.nonzero(flags).reshape(-1).contiguous()
     n = cells.numel()
     ev[1].record()
     counts = torch.empty(n, dtype=torch.int32, device=df.device)
-    check(L.nudf_iso_count(ptr(df), N, N, N, level, ptr(cells), n, ptr(counts), st), "nudf_iso_count")
+    check(L.nudf_iso_count(lat, level, ptr(cells), n, ptr(counts), st), "nudf_iso_count")
     csum = torch.cumsum(counts, 0, dtype=torch.int64)
     n_faces = int(csum[-1]) if n else 0
     offsets = (csum - counts).contiguous()
     ev[2].record()
     keys = torch.empty(3 * n_faces, dtype=torch.int64, device=df.device)
-    check(L.nudf_iso_emit(ptr(df), N, N, N, level, ptr(cells), n, ptr(offsets), ptr(keys), st), "nudf_iso_emit")
+    check(L.nudf_iso_emit(lat, level, ptr(cells), n, ptr(offsets), ptr(keys), st), "nudf_iso_emit")
     ev[3].record()
     ukeys, inv = torch.unique(keys, sorted=True, return_inverse=True)
     ukeys = ukeys.contiguous()
     ev[4].record()
     verts = torch.empty(ukeys.numel(), 3, dtype=torch.float64, device=df.device)
-    check(L.nudf_iso_vertices(ptr(df), N, N, N, level, ptr(cells), n, ptr(ukeys), ukeys.numel(), ptr(verts), st),
+    check(L.nudf_iso_vertices(lat, level, ptr(cells), n, ptr(ukeys), ukeys.numel(), ptr(verts), st),
           "nudf_iso_vertices")
     ev[5].record()
     torch.cuda.synchronize()

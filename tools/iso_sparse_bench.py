@@ -61,20 +61,20 @@ def _stages(band, level):
     mark()
     n = cells.numel()
     counts = torch.empty(n, dtype=torch.int32, device=dev)
-    check(L.nudf_iso_lat_count(lat, level, ptr(cells), n, ptr(counts), st), "nudf_iso_lat_count")
+    check(L.nudf_iso_count(lat, level, ptr(cells), n, ptr(counts), st), "nudf_iso_count")
     csum = torch.cumsum(counts, 0, dtype=torch.int64)
     offsets = (csum - counts).contiguous()
     n_faces = int(csum[-1])
     mark()
     keys = torch.empty(3 * n_faces, dtype=torch.int64, device=dev)
-    check(L.nudf_iso_lat_emit(lat, level, ptr(cells), n, ptr(offsets), ptr(keys), st), "nudf_iso_lat_emit")
+    check(L.nudf_iso_emit(lat, level, ptr(cells), n, ptr(offsets), ptr(keys), st), "nudf_iso_emit")
     mark()
     ukeys, inv = torch.unique(keys, sorted=True, return_inverse=True)
     ukeys = ukeys.contiguous()
     mark()
     verts = torch.empty(ukeys.numel(), 3, dtype=torch.float64, device=dev)
-    check(L.nudf_iso_lat_vertices(lat, level, ptr(cells), n, ptr(ukeys), ukeys.numel(), ptr(verts), st),
-          "nudf_iso_lat_vertices")
+    check(L.nudf_iso_vertices(lat, level, ptr(cells), n, ptr(ukeys), ukeys.numel(), ptr(verts), st),
+          "nudf_iso_vertices")
     mark()
     torch.cuda.synchronize()
     names = ("enumerate", "count", "emit", "weld", "vertices")
