@@ -25,6 +25,12 @@ extern "C" {
  * never cleared by the library; the caller reads it at a host synchronisation point of its choice */
 #define NUDF_STATUS_NONFINITE_SAMPLES 1   /* sample_pdf / up_sample produced a non-finite sample position (:97-101, 265-269) */
 #define NUDF_STATUS_NONFINITE_RENDER 2    /* compositing produced a non-finite per-ray result (:543-544) */
+/* Stable compaction (nudf_iso_cells_*, nudf_uc_step_* / _filter_*, nudf_pt_start_* / _trace_*): the n items of a call are
+ * taken in n_seg = ceil(n / NUDF_COMPACT_SEG) segments.  The count pass writes counts[seg] (int32 [n_seg]), the outputs of
+ * the segment's items; the emit pass makes the same decisions again and writes those outputs from offsets[seg] (int64
+ * [n_seg]: an exclusive scan of the counts, plus any base the caller adds) on, in item order, so that the outputs of
+ * consecutive calls can share one buffer. */
+#define NUDF_COMPACT_SEG 256
 
 int nudf_abi_version(void);
 const char* nudf_last_error(void);
@@ -393,13 +399,12 @@ int nudf_mc_vertices(const nudf_lattice* lat, const int64_t* cells, int64_t n_ce
 /* flags[g] (g < n0 * n1 * n2) = 1 when the cell with lower corner g has a corner with v > 0, one with v <= 0 and none NaN.
  * A df lattice only: a store is refused (nudf_iso_cells_* find the active cells of either form) */
 int nudf_iso_active(const nudf_lattice* lat, float level, uint8_t* flags, void* stream);
-/* The active cells without a scan of every cell: the storage positions (df: the flat indices; a store: coarse, then the
- * brick slots, as nudf_sb_flat numbers them) are taken in n_seg = ceil(positions / NUDF_ISO_SEG) segments.  Each position
- * holding a lattice point with v <= 0 emits the active cells (as nudf_iso_active defines them) of which it is the lowest
- * corner with v <= 0: counts[seg] = the segment's cells; cells[offsets[seg] ...] = them, in position order (offsets =
- * exclusive scan of the counts).  Sorted, they are nonzero(nudf_iso_active) of the lattice's values, with no condition on
- * the field: every active cell has a corner with v <= 0, which is finite and so stored. */
-#define NUDF_ISO_SEG 256
+/* The active cells without a scan of every cell, a stable compaction (NUDF_COMPACT_SEG) whose items are the storage
+ * positions (df: the flat indices; a store: coarse, then the brick slots, as nudf_sb_flat numbers them); n_seg must be
+ * ceil(positions / NUDF_COMPACT_SEG).  Each position holding a lattice point with v <= 0 emits the active cells (as
+ * nudf_iso_active defines them) of which it is the lowest corner with v <= 0: counts[seg] = the segment's cells;
+ * cells[offsets[seg] ...] = them, in position order.  Sorted, they are nonzero(nudf_iso_active) of the lattice's values,
+ * with no condition on the field: every active cell has a corner with v <= 0, which is finite and so stored. */
 int nudf_iso_cells_count(const nudf_lattice* lat, float level, int64_t n_seg, int32_t* counts, void* stream);
 int nudf_iso_cells_emit(const nudf_lattice* lat, float level, int64_t n_seg, const int64_t* offsets, int64_t* cells,
                         void* stream);
@@ -544,10 +549,8 @@ int nudf_sb_flat(const nudf_brick_store* st, const int64_t* pos, int64_t n, int6
  * Surface point clouds (neuraludf_b200/cloud.py drives the steps; DESIGN.md section 1 states the algorithm)
  * ------------------------------------------------------------------------------------------------------------
  * p, out: fp32 [n,3]; u fp32 [n]; g fp32 [n,3]; all DEVICE.  Every fp32 operation is rounded once in the stated order,
- * with no contraction.  The points are taken in n_seg = ceil(n / NUDF_UC_SEG) segments: the count pass writes
- * counts[seg] = the segment's survivors, the emit pass writes them to out[offsets[seg] ...] in point order (offsets: an
- * exclusive scan of the counts, plus any base), so that the survivors of consecutive calls can share one output. */
-#define NUDF_UC_SEG 256
+ * with no contraction.  The step and the filter are stable compactions of the points (NUDF_COMPACT_SEG): the count pass
+ * writes counts[seg] = the segment's survivors, the emit pass writes them to out[offsets[seg] ...] in point order. */
 /* projection step: q = p - (u / n) g with n = sqrt((gx gx + gy gy) + gz gz); survives when u and g are finite, n != 0 and
  * q lies in [-1,1]^3 (the survivor is q) */
 int nudf_uc_step_count(const float* p, const float* u, const float* g, int64_t n, int32_t* counts, void* stream);
@@ -571,8 +574,7 @@ int nudf_uc_resample(const float* pool, int64_t n_pool, int64_t m, uint32_t seed
  * contraction: dot(a, b) = (a0 b0 + a1 b1) + a2 b2; the pixel of p is (x0 / x2, x1 / x2), x_r = dot(P_r, p) + P_r3; the
  * direction to camera k is v = d / L, d = c_k - p, L = sqrt(dot(d, d)).  A pair (i, k) is the ray q(t) = p_i + t v; pairs
  * are held as idx, cam int32 [A], t fp32 [A] and q fp32 [A,3] (the point where the caller evaluates the udf), and are
- * compacted as the point clouds' survivors (NUDF_PT_SEG segments; count pass, then emit pass from the offsets). */
-#define NUDF_PT_SEG 256
+ * compacted by stable compactions (NUDF_COMPACT_SEG; count pass, then emit pass from the offsets). */
 #define NUDF_PT_MAX_VIEWS 64
 #define NUDF_PT_MAX_CAND 8
 /* out = g / sqrt(dot(g, g)), 0 where that norm is 0 or not finite */

@@ -81,9 +81,7 @@ class BrickStore(ctypes.Structure):
 
 
 BRICK = 8   # NUDF_BRICK
-ISO_SEG = 256   # NUDF_ISO_SEG
-UC_SEG = 256    # NUDF_UC_SEG
-PT_SEG = 256    # NUDF_PT_SEG
+COMPACT_SEG = 256   # NUDF_COMPACT_SEG
 PT_MAX_VIEWS, PT_MAX_CAND = 64, 8      # NUDF_PT_MAX_VIEWS, NUDF_PT_MAX_CAND
 
 
@@ -306,3 +304,27 @@ def ptr(t):
 def stream_ptr():
     import torch
     return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+
+def seg_counts(n, device):
+    """the counts buffer of a stable compaction (include/nudf.h) over n items: int32 [ceil(n / NUDF_COMPACT_SEG)]"""
+    import torch
+    return torch.empty(-(-n // COMPACT_SEG), dtype=torch.int32, device=device)
+
+
+def compact_batches(n, max_batch, device, batch):
+    """Runs a stable compaction over n items in batches of max_batch and returns its output count.  batch(lo, hi) readies
+    items [lo, hi) and returns launch(counts, offsets=None), which runs the count pass into counts when offsets is None
+    and else the emit pass from offsets.  Each batch's outputs follow the previous batches' from a running base kept on
+    the device, so that the output count is the only host read."""
+    import torch
+    base = torch.zeros(1, dtype=torch.int64, device=device)
+    for lo in range(0, n, max_batch):
+        hi = min(lo + max_batch, n)
+        launch = batch(lo, hi)
+        counts = seg_counts(hi - lo, device)
+        launch(counts)
+        csum = torch.cumsum(counts, 0, dtype=torch.int64)
+        launch(counts, base + (csum - counts))
+        base += csum[-1]
+    return int(base.item())

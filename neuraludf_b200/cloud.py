@@ -37,20 +37,16 @@ def _launch_filter(p, u, thr, counts, offsets=None, out=None):
 
 
 def _compact(pts, max_batch, evaluate, launch):
-    """the survivors of pts [n,3] in order, in batches of max_batch: evaluate(batch) gives the extra arguments of
-    launch(batch, *args, counts, offsets, out).  The batches' survivors go to one buffer from a running offset kept on the
-    device, so that the survivor count is the only host read."""
+    """the survivors of pts [n,3] in order, in batches of max_batch (_lib.compact_batches): evaluate(batch) gives the extra
+    arguments of launch(batch, *args, counts, offsets, out)"""
     out = torch.empty_like(pts)
-    base = torch.zeros(1, dtype=torch.int64, device=pts.device)
-    for head in range(0, pts.shape[0], max_batch):
-        p = pts[head:head + max_batch]
+
+    def batch(lo, hi):
+        p = pts[lo:hi]
         args = evaluate(p)
-        counts = torch.empty(-(-p.shape[0] // _lib.UC_SEG), dtype=torch.int32, device=pts.device)
-        launch(p, *args, counts)
-        csum = torch.cumsum(counts, 0, dtype=torch.int64)
-        launch(p, *args, counts, base + (csum - counts), out)
-        base += csum[-1]
-    return out[:int(base.item())]
+        return lambda counts, offsets=None: launch(p, *args, counts, offsets, out)
+
+    return out[:_lib.compact_batches(pts.shape[0], max_batch, pts.device, batch)]
 
 
 def _points(t, what):

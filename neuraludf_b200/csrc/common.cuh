@@ -49,6 +49,8 @@ NUDF_HD float clampf_(float x, float lo, float hi) { return fminf(fmaxf(x, lo), 
 #include <cuda_runtime.h>
 #include <stdio.h>
 
+#include <algorithm>
+
 namespace nudf {
 
 void set_error(const char* fmt, ...);
@@ -113,6 +115,10 @@ float* split_workspace(cudaStream_t st);
 
 static inline int64_t cdiv(int64_t a, int64_t b) { return (a + b - 1) / b; }
 static inline int64_t round_up(int64_t a, int64_t b) { return cdiv(a, b) * b; }
+// the grid of a grid-stride launch over n items, per_block items a block: at least 1 block, at most 8 * 65535
+static inline unsigned grid_for(int64_t n, int per_block = 256) {
+  return (unsigned)std::min<int64_t>(std::max<int64_t>(cdiv(n, per_block), 1), 65535ll * 8);
+}
 // the ctx / scratch layouts of the networks: offsets in floats, every block starts 16-byte aligned
 struct Bump {
   int64_t off = 0;

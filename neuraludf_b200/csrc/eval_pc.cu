@@ -19,8 +19,6 @@
 //                         of AABBs (node i has children 2i+1, 2i+2; leaf l is node L-1+l); per query a depth-first
 //                         branch-and-bound seeded with max_dist, queries in Morton order for warp coherence.  The distance is
 //                         sqrt((dx^2 + dy^2) + dz^2) in fp64 as in the KD-tree; a query with no target below max_dist gets +inf.
-#include <algorithm>
-
 #include "../../include/nudf.h"
 #include "common.cuh"
 
@@ -301,10 +299,6 @@ __global__ void __launch_bounds__(128) k_nearest(const double* __restrict__ qs, 
     const double d = __dsqrt_rn(best);
     dist[q] = (found && d < max_dist) ? d : INFINITY;
   }
-}
-
-static inline unsigned grid_for(int64_t n, int per_block = 256) {
-  return (unsigned)std::min<int64_t>(std::max<int64_t>(cdiv(n, per_block), 1), 65535ll * 8);
 }
 
 }  // namespace pc

@@ -36,7 +36,6 @@
 // below tau and evaluated.  A cell with a culled corner has, for the same reason, every dense corner value above the level,
 // so it is inactive in both lattices.  The threshold marching cubes (nudf_iso_*) reads df only at the corners of active
 // cells, so it gives the same active cells, faces, vertex keys and fp64 vertices on both.
-#include <algorithm>
 #include <type_traits>
 
 #include "../../include/nudf.h"
@@ -223,10 +222,6 @@ __global__ void k_emit(const uint8_t* __restrict__ flags, Lat B, int64_t t, cons
     int64_t o = offsets[i];
     block_points(flags, B, t, kept[i], [&](int64_t x, int64_t y, int64_t z) { write_point(x, y, z, B.N, cr, idx, pts, o++); });
   }
-}
-
-static inline unsigned grid_for(int64_t n, int per_block = 256) {
-  return (unsigned)std::min<int64_t>(std::max<int64_t>(cdiv(n, per_block), 1), 65535ll * 8);
 }
 
 }  // namespace nb

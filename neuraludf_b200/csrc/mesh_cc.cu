@@ -14,8 +14,6 @@
 // thread meanwhile, and the pair retries from the new roots.  So when the hooking launch ends, the trees are exactly the
 // components, whatever the interleaving, and by the invariant each root is the smallest face of its tree: the labels are
 // deterministic and equal the smallest face index of each component.
-#include <algorithm>
-
 #include "../../include/nudf.h"
 #include "common.cuh"
 
@@ -71,10 +69,6 @@ __global__ void k_compress(int64_t* par, int64_t nf) {
     const int64_t r = find(par, i);
     *(volatile int64_t*)(par + i) = r;
   }
-}
-
-static inline unsigned grid_for(int64_t n, int per_block = 256) {
-  return (unsigned)std::min<int64_t>(std::max<int64_t>(cdiv(n, per_block), 1), 65535ll * 8);
 }
 
 }  // namespace cc

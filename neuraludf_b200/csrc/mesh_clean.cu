@@ -119,10 +119,6 @@ __global__ void __launch_bounds__(256) k_vote(const double* __restrict__ pts, in
   }
 }
 
-static inline unsigned grid_for(int64_t n, int per_block = 256) {
-  return (unsigned)std::min<int64_t>(std::max<int64_t>(cdiv(n, per_block), 1), 65535ll * 8);
-}
-
 }  // namespace cl
 }  // namespace nudf
 

@@ -10,8 +10,6 @@
 //                   trunc(fl(x + 1) / fl(voxel)) per axis with their six clamped neighbours, block-major.
 // Every operation is an explicit __d*_rn / __f*_rn: no contraction, so the device and NumPy give the same bits (acos aside:
 // CUDA's and the host libm's may differ in the last fp64 bit).
-#include <algorithm>
-
 #include "../../include/nudf.h"
 #include "common.cuh"
 
@@ -121,10 +119,6 @@ __global__ void k_refine(const float* __restrict__ verts, const float* __restric
     o[5 * nv] = flat(i, max(jm, (int64_t)0), k, n_mc);
     o[6 * nv] = flat(i, j, max(km, (int64_t)0), n_mc);
   }
-}
-
-static inline unsigned grid_for(int64_t n, int per_block = 256) {
-  return (unsigned)std::min<int64_t>(std::max<int64_t>(cdiv(n, per_block), 1), 65535ll * 8);
 }
 
 }  // namespace mg

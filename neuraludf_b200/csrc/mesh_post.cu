@@ -13,8 +13,6 @@
 //   smoothing       one Jacobi step over the border vertices: v + lambda (sum of neighbours / count - v), neighbours summed
 //                   in ascending index order; everything read from the previous step's buffer.
 // Every fp64 operation is an explicit __d*_rn: no contraction, so the device and NumPy give the same bits.
-#include <algorithm>
-
 #include "../../include/nudf.h"
 #include "common.cuh"
 
@@ -150,10 +148,6 @@ __global__ void k_smooth(const double* __restrict__ vin, double* __restrict__ vo
       vout[3 * b + d] = __dadd_rn(v, __dmul_rn(lambda, __dsub_rn(__ddiv_rn(s[d], cnt), v)));
     }
   }
-}
-
-static inline unsigned grid_for(int64_t n, int per_block = 256) {
-  return (unsigned)std::min<int64_t>(std::max<int64_t>(cdiv(n, per_block), 1), 65535ll * 8);
 }
 
 }  // namespace mp

@@ -2,8 +2,6 @@
 // df_access.cuh): brick allocation from the kept blocks of the coarse stride, value stores and reads by flat lattice index,
 // and the inverse map from storage positions to flat indices that the near-surface selection uses.
 // tests/proto/udf_sparse.py restates the layout and the level chain in NumPy.
-#include <algorithm>
-
 #include "../../include/nudf.h"
 #include "common.cuh"
 #include "df_access.cuh"
@@ -66,8 +64,6 @@ __global__ void k_flat(BrickDf st, const int64_t* __restrict__ keys, const int64
     out[t] = (i * st.N + j) * st.N + k;
   }
 }
-
-static inline unsigned grid_for(int64_t n) { return (unsigned)std::min<int64_t>(std::max<int64_t>(cdiv(n, 256), 1), 65535ll * 8); }
 
 }  // namespace sb
 }  // namespace nudf

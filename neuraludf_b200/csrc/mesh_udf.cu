@@ -25,11 +25,11 @@
 // load: both compute the same values from the same corner values.
 // Threshold meshing (nudf_iso_*) runs stages 4-5 on v = fl32(f - level) instead of the pseudo-signed udf (the corner rules
 // UdfCorners / IsoCorners), with its own active-cell test and fp64 vertices; tests/proto/iso_mc.py restates it.
-#include <algorithm>
 #include <type_traits>
 
 #include "../../include/nudf.h"
 #include "common.cuh"
+#include "compact.cuh"
 #include "df_access.cuh"
 
 namespace nudf {
@@ -464,8 +464,8 @@ __global__ void k_iso_active(const float* __restrict__ df, Dims D, float level, 
 // to 8 cells holding each finds them all.  A cell is emitted by its lowest corner with v <= 0 only (corners ascend with
 // the flat index), so once.  The test is k_iso_active's on the same corner values, so the set is nonzero(nudf_iso_active)
 // on any lattice whose reader gives those values -- +inf (unstored) and NaN corners included, with no Lipschitz condition.
-// Positions are taken in segments of NUDF_ISO_SEG, one thread each: the count pass writes each segment's cell count, the
-// emit pass writes the segment's cells from its offset in position order; the caller sorts.
+// The positions are the items of compact.cuh's stable compaction (IsoCells below), so the cells come in position order;
+// the caller sorts.
 struct DenseSites {             // the flat array: position = flat index
   DenseDf df;
   int64_t n;
@@ -574,40 +574,20 @@ __device__ __forceinline__ int iso_owned_cells(const S& sites, const Dims& D, fl
   return n;
 }
 
-constexpr int kIsoSeg = NUDF_ISO_SEG;
-
-// one block of kIsoSeg threads per segment; offsets NULL: counts[seg] = the segment's cells, else cells[offsets[seg] ...]
+// the compaction op of the sites S: the emit pass computes a position's cells again, written in place (no Item holds them)
 template <class S>
-__global__ void __launch_bounds__(kIsoSeg) k_iso_cells(S sites, Dims D, float level, int64_t n_seg,
-                                                        int32_t* __restrict__ counts, const int64_t* __restrict__ offsets,
-                                                        int64_t* __restrict__ cells) {
-  __shared__ int32_t warp_sum[kIsoSeg / 32];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (int64_t seg = blockIdx.x; seg < n_seg; seg += gridDim.x) {
-    const int64_t p = seg * kIsoSeg + threadIdx.x;
-    const int n = iso_owned_cells(sites, D, level, p, (int64_t*)nullptr);
-    int incl = n;                           // inclusive scan over the block: warps, then the warp totals
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const int y = __shfl_up_sync(0xffffffffu, incl, d);
-      if (lane >= d) incl += y;
-    }
-    if (lane == 31) warp_sum[warp] = incl;
-    __syncthreads();
-    int before = 0, total = 0;
-#pragma unroll
-    for (int w = 0; w < kIsoSeg / 32; ++w) {
-      before += w < warp ? warp_sum[w] : 0;
-      total += warp_sum[w];
-    }
-    if (!offsets) {
-      if (threadIdx.x == 0) counts[seg] = total;
-    } else if (n) {                         // the same cells again, written in place
-      iso_owned_cells(sites, D, level, p, cells + offsets[seg] + before + incl - n);
-    }
-    __syncthreads();                        // warp_sum is reused by the next segment
+struct IsoCells {
+  struct Item {};
+  S sites;
+  Dims D;
+  float level;
+  __device__ __forceinline__ int eval(int64_t p, Item&, bool) const {
+    return iso_owned_cells(sites, D, level, p, (int64_t*)nullptr);
   }
-}
+  __device__ __forceinline__ void store(int64_t* __restrict__ cells, int64_t j, int64_t p, const Item&) const {
+    iso_owned_cells(sites, D, level, p, cells + j);
+  }
+};
 
 // fp64 lattice-index coordinates of the point on the edge (lower corner gk, axis ax): t = v_a / (v_a - v_b) of the fp32 v
 template <class A>
@@ -657,7 +637,6 @@ __global__ void k_iso_vertices_dense(const float* __restrict__ df, Dims D, float
   iso_vertices(DenseDf{df}, D, level, cells, keys, n, verts);
 }
 
-static inline unsigned grid_for(int64_t n) { return (unsigned)std::min<int64_t>(std::max<int64_t>(cdiv(n, 256), 1), 65535ll * 8); }
 static inline Dims dims(const nudf_lattice& l) { return Dims{l.n0, l.n1, l.n2}; }
 
 }  // namespace mc
@@ -806,16 +785,13 @@ static int iso_cells(const nudf_lattice* lat, float level, int64_t n_seg, int32_
       NUDF_REQUIRE(lat->store->n_bricks == 0 || lat->store->keys, "null brick keys");
       n_pos = (int64_t)lat->store->mc * lat->store->mc * lat->store->mc + lat->store->n_bricks * kBrickPoints;
     }
-    NUDF_REQUIRE(n_seg == cdiv(n_pos, (int64_t)kIsoSeg), "n_seg must be ceil(storage positions / NUDF_ISO_SEG)");
-    const unsigned grid = (unsigned)std::min<int64_t>(std::max<int64_t>(n_seg, 1), 65535ll * 8);
+    NUDF_REQUIRE(n_seg == cdiv(n_pos, kSeg), "n_seg must be ceil(storage positions / NUDF_COMPACT_SEG)");
+    using Out = int64_t* __restrict__;
     if constexpr (std::is_same<decltype(df), DenseDf>::value)
-      k_iso_cells<<<grid, kIsoSeg, 0, (cudaStream_t)stream>>>(DenseSites{df, n_pos}, D, level, n_seg, counts, offsets,
-                                                                cells);
+      return seg_compact<Out>(IsoCells<DenseSites>{{df, n_pos}, D, level}, n_pos, counts, offsets, cells, stream);
     else
-      k_iso_cells<<<grid, kIsoSeg, 0, (cudaStream_t)stream>>>(BrickSites{df, lat->store->keys, n_pos}, D, level, n_seg,
-                                                                counts, offsets, cells);
-    NUDF_LAUNCH_OK();
-    return 0;
+      return seg_compact<Out>(IsoCells<BrickSites>{{df, lat->store->keys, n_pos}, D, level}, n_pos, counts, offsets,
+                              cells, stream);
   });
 }
 

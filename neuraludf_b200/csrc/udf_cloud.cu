@@ -1,33 +1,37 @@
 // Surface point clouds of a UDF (neuraludf_b200/cloud.py drives them; DESIGN.md section 1 states the algorithm): the
 // projection step p <- p - (u / |g|) g with its stable compaction, the final udf filter with the same compaction, and the
 // seeded jittered resampling of the kept points.  Every fp32 operation is rounded once in the stated order with no
-// contraction (__f*_rn), so that tests/proto/udf_cloud.py reproduces the kernels bit for bit from the same (u, g).
-//
-// Compaction: the points are taken in segments of NUDF_UC_SEG, one thread each.  The count pass writes each segment's
-// survivor count; the emit pass recomputes the same survivors and writes them from the segment's offset (an exclusive
-// scan of the counts, plus any base the caller adds), in point order.
-#include <algorithm>
-
+// contraction (__f*_rn), so that tests/proto/udf_cloud.py reproduces the kernels bit for bit from the same (u, g).  The
+// step and the filter are compact.cuh's stable compaction: a point is an item with at most one output.
 #include "../../include/nudf.h"
 #include "common.cuh"
+#include "compact.cuh"
 
 namespace nudf {
 namespace uc {
-
-constexpr int kSeg = NUDF_UC_SEG;
 
 __device__ __forceinline__ bool in_box(const float q[3]) {
   // written so that a NaN coordinate is outside
   return q[0] >= -1.f && q[0] <= 1.f && q[1] >= -1.f && q[1] <= 1.f && q[2] >= -1.f && q[2] <= 1.f;
 }
 
+// the output of the compactions: the survivor q at out[3 j .. 3 j + 2], out a restrict pointer so that the inputs are
+// read through the read-only path
+using Out = float* __restrict__;
+__device__ __forceinline__ void store_point(Out out, int64_t j, const float q[3]) {
+  out[3 * j] = q[0];
+  out[3 * j + 1] = q[1];
+  out[3 * j + 2] = q[2];
+}
+
 // step 2: n = sqrt((gx gx + gy gy) + gz gz), q = p - (u / n) g; a point survives when u and g are finite, n != 0 and q
 // lies in [-1,1]^3
 struct StepOp {
+  using Item = float[3];
   const float* p;
   const float* u;
   const float* g;
-  __device__ __forceinline__ bool operator()(int64_t t, float q[3]) const {
+  __device__ __forceinline__ int eval(int64_t t, Item& q, bool) const {
     const float ut = u[t], gx = g[3 * t], gy = g[3 * t + 1], gz = g[3 * t + 2];
     const float n = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(gx, gx), __fmul_rn(gy, gy)), __fmul_rn(gz, gz)));
     const float s = __fdiv_rn(ut, n);
@@ -36,56 +40,23 @@ struct StepOp {
     q[2] = __fsub_rn(p[3 * t + 2], __fmul_rn(s, gz));
     return isfinite(ut) && isfinite(gx) && isfinite(gy) && isfinite(gz) && n != 0.f && in_box(q);
   }
+  __device__ __forceinline__ void store(Out out, int64_t j, int64_t, const Item& q) const { store_point(out, j, q); }
 };
 
 // step 3: a point survives when u < thr (NaN does not)
 struct FilterOp {
+  using Item = float[3];
   const float* p;
   const float* u;
   float thr;
-  __device__ __forceinline__ bool operator()(int64_t t, float q[3]) const {
+  __device__ __forceinline__ int eval(int64_t t, Item& q, bool) const {
     q[0] = p[3 * t];
     q[1] = p[3 * t + 1];
     q[2] = p[3 * t + 2];
     return u[t] < thr;
   }
+  __device__ __forceinline__ void store(Out out, int64_t j, int64_t, const Item& q) const { store_point(out, j, q); }
 };
-
-// one block of kSeg threads per segment; offsets NULL: counts[seg] = the segment's survivors, else out[offsets[seg] ...]
-template <class Op>
-__global__ void __launch_bounds__(kSeg) k_compact(Op op, int64_t n, int64_t n_seg, int32_t* __restrict__ counts,
-                                                  const int64_t* __restrict__ offsets, float* __restrict__ out) {
-  __shared__ int32_t warp_sum[kSeg / 32];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (int64_t seg = blockIdx.x; seg < n_seg; seg += gridDim.x) {
-    const int64_t t = seg * kSeg + threadIdx.x;
-    float q[3];
-    const int keep = (t < n && op(t, q)) ? 1 : 0;
-    int incl = keep;                        // inclusive scan over the block: warps, then the warp totals
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const int y = __shfl_up_sync(0xffffffffu, incl, d);
-      if (lane >= d) incl += y;
-    }
-    if (lane == 31) warp_sum[warp] = incl;
-    __syncthreads();
-    int before = 0, total = 0;
-#pragma unroll
-    for (int w = 0; w < kSeg / 32; ++w) {
-      before += w < warp ? warp_sum[w] : 0;
-      total += warp_sum[w];
-    }
-    if (!offsets) {
-      if (threadIdx.x == 0) counts[seg] = total;
-    } else if (keep) {
-      const int64_t o = offsets[seg] + before + incl - 1;
-      out[3 * o] = q[0];
-      out[3 * o + 1] = q[1];
-      out[3 * o + 2] = q[2];
-    }
-    __syncthreads();                        // warp_sum is reused by the next segment
-  }
-}
 
 // lowbias32, a public-domain bijective 32-bit integer mixer (C. Wellons); all arithmetic mod 2^32
 __device__ __forceinline__ uint32_t mix32(uint32_t x) {
@@ -116,16 +87,6 @@ __global__ void k_resample(const float* __restrict__ pool, uint32_t n_pool, int6
   }
 }
 
-static inline unsigned grid_for(int64_t blocks) { return (unsigned)std::min<int64_t>(std::max<int64_t>(blocks, 1), 65535ll * 8); }
-
-template <class Op>
-static int compact(Op op, int64_t n, int32_t* counts, const int64_t* offsets, float* out, void* stream) {
-  const int64_t n_seg = cdiv(n, kSeg);
-  k_compact<<<grid_for(n_seg), kSeg, 0, (cudaStream_t)stream>>>(op, n, n_seg, counts, offsets, out);
-  NUDF_LAUNCH_OK();
-  return 0;
-}
-
 }  // namespace uc
 }  // namespace nudf
 
@@ -135,27 +96,27 @@ using namespace nudf::uc;
 int nudf_uc_step_count(const float* p, const float* u, const float* g, int64_t n, int32_t* counts, void* stream) {
   NUDF_REQUIRE(n >= 0 && (n == 0 || (p && u && g && counts)), "null pointer or negative count");
   if (n == 0) return 0;
-  return compact(StepOp{p, u, g}, n, counts, nullptr, nullptr, stream);
+  return seg_compact<Out>(StepOp{p, u, g}, n, counts, nullptr, nullptr, stream);
 }
 
 int nudf_uc_step_emit(const float* p, const float* u, const float* g, int64_t n, const int64_t* offsets, float* out,
                       void* stream) {
   NUDF_REQUIRE(n >= 0 && (n == 0 || (p && u && g && offsets && out)), "null pointer or negative count");
   if (n == 0) return 0;
-  return compact(StepOp{p, u, g}, n, nullptr, offsets, out, stream);
+  return seg_compact<Out>(StepOp{p, u, g}, n, nullptr, offsets, out, stream);
 }
 
 int nudf_uc_filter_count(const float* p, const float* u, int64_t n, float thr, int32_t* counts, void* stream) {
   NUDF_REQUIRE(n >= 0 && (n == 0 || (p && u && counts)), "null pointer or negative count");
   if (n == 0) return 0;
-  return compact(FilterOp{p, u, thr}, n, counts, nullptr, nullptr, stream);
+  return seg_compact<Out>(FilterOp{p, u, thr}, n, counts, nullptr, nullptr, stream);
 }
 
 int nudf_uc_filter_emit(const float* p, const float* u, int64_t n, float thr, const int64_t* offsets, float* out,
                         void* stream) {
   NUDF_REQUIRE(n >= 0 && (n == 0 || (p && u && offsets && out)), "null pointer or negative count");
   if (n == 0) return 0;
-  return compact(FilterOp{p, u, thr}, n, nullptr, offsets, out, stream);
+  return seg_compact<Out>(FilterOp{p, u, thr}, n, nullptr, offsets, out, stream);
 }
 
 int nudf_uc_resample(const float* pool, int64_t n_pool, int64_t m, uint32_t seed, int32_t round, float voxel, float* out,
@@ -165,8 +126,7 @@ int nudf_uc_resample(const float* pool, int64_t n_pool, int64_t m, uint32_t seed
   if (m == 0) return 0;
   NUDF_REQUIRE(n_pool >= 1 && n_pool <= 0xffffffffll, "the pool must hold 1 .. 2^32 - 1 points");
   NUDF_REQUIRE(pool && out, "null pointer");
-  k_resample<<<grid_for(cdiv(m, 256)), 256, 0, (cudaStream_t)stream>>>(pool, (uint32_t)n_pool, m, seed,
-                                                                        (uint32_t)round, voxel, out);
+  k_resample<<<grid_for(m), 256, 0, (cudaStream_t)stream>>>(pool, (uint32_t)n_pool, m, seed, (uint32_t)round, voxel, out);
   NUDF_LAUNCH_OK();
   return 0;
 }

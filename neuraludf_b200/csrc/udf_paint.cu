@@ -2,20 +2,15 @@
 // states the algorithm): unit normal lines from gradients, the ranking of candidate cameras, the sphere-traced visibility
 // of (point, camera) pairs with its stable compaction, the orientation of the normals towards the chosen camera and the
 // bilinear image gather.  Every fp32 operation is rounded once in the stated order with no contraction (__f*_rn), so that
-// tests/proto/udf_paint.py reproduces the kernels bit for bit from the same inputs and udf values.
-//
-// Compaction: as udf_cloud.cu's.  The pairs are taken in segments of NUDF_PT_SEG, one thread each; the count pass writes
-// each segment's active count, the emit pass recomputes the same pairs and writes the active ones from the segment's
-// offset, in order.
-#include <algorithm>
-
+// tests/proto/udf_paint.py reproduces the kernels bit for bit from the same inputs and udf values.  The round start and
+// the trace step are compact.cuh's stable compaction: a point or a pair is an item with at most one output pair.
 #include "../../include/nudf.h"
 #include "common.cuh"
+#include "compact.cuh"
 
 namespace nudf {
 namespace pt {
 
-constexpr int kSeg = NUDF_PT_SEG;
 constexpr int kMaxViews = NUDF_PT_MAX_VIEWS;
 constexpr int kMaxCand = NUDF_PT_MAX_CAND;
 
@@ -132,17 +127,32 @@ struct Pair {
   float t, q[3];
 };
 
+// the output of the compactions: pair j in the four arrays
+struct PairOut {
+  int32_t *idx, *cam;
+  float *t, *q;
+  __device__ __forceinline__ void put(int64_t j, const Pair& o) const {
+    idx[j] = o.idx;
+    cam[j] = o.cam;
+    t[j] = o.t;
+    q[3 * j] = o.q[0];
+    q[3 * j + 1] = o.q[1];
+    q[3 * j + 2] = o.q[2];
+  }
+};
+
 // round start: point i (unresolved, view[i] < 0) with candidate k = cand[i, r] >= 0 starts the pair (i, k) at
 // t0 = t_start / |n . v| and q = p + t0 v
 struct StartOp {
+  using Item = Pair;
   const float *p, *n, *centres;
   const int32_t *cand, *view;
   int K, r;
   float t_start;
-  __device__ __forceinline__ bool operator()(int64_t i, Pair& o, bool) const {
-    if (view[i] >= 0) return false;
+  __device__ __forceinline__ int eval(int64_t i, Pair& o, bool) const {
+    if (view[i] >= 0) return 0;
     const int k = cand[i * K + r];
-    if (k < 0) return false;
+    if (k < 0) return 0;
     float px, py, pz, nx, ny, nz, v[3];
     load3(p, i, px, py, pz);
     load3(n, i, nx, ny, nz);
@@ -150,21 +160,23 @@ struct StartOp {
     const float t = __fdiv_rn(t_start, fabsf(dot3(nx, ny, nz, v[0], v[1], v[2])));
     o = Pair{(int32_t)i, k, t, {__fadd_rn(px, __fmul_rn(t, v[0])), __fadd_rn(py, __fmul_rn(t, v[1])),
                                  __fadd_rn(pz, __fmul_rn(t, v[2]))}};
-    return true;
+    return 1;
   }
+  __device__ __forceinline__ void store(PairOut out, int64_t j, int64_t, const Pair& o) const { out.put(j, o); }
 };
 
 // trace step of pair a with the udf u[a] at its q: occluded (dropped) unless u >= hit; else t += u, q = p + t v, and the
 // pair is visible (dropped; the emit pass sets view[idx] = cam) when |q|^2 > 1 or t >= |c - p|, else it stays active
 struct StepOp {
+  using Item = Pair;
   const float *p, *centres;
   const int32_t *idx, *cam;
   const float *t, *u;
   float hit;
   int32_t* view;
-  __device__ __forceinline__ bool operator()(int64_t a, Pair& o, bool emit) const {
+  __device__ __forceinline__ int eval(int64_t a, Pair& o, bool emit) const {
     const float ua = u[a];
-    if (!(ua >= hit)) return false;
+    if (!(ua >= hit)) return 0;
     const int32_t i = idx[a], k = cam[a];
     float px, py, pz, v[3];
     load3(p, i, px, py, pz);
@@ -174,56 +186,12 @@ struct StepOp {
                         __fadd_rn(pz, __fmul_rn(tn, v[2]))}};
     if (dot3(o.q[0], o.q[1], o.q[2], o.q[0], o.q[1], o.q[2]) > 1.f || tn >= L) {
       if (emit) view[i] = k;
-      return false;
+      return 0;
     }
-    return true;
+    return 1;
   }
+  __device__ __forceinline__ void store(PairOut out, int64_t j, int64_t, const Pair& o) const { out.put(j, o); }
 };
-
-struct PairOut {
-  int32_t *idx, *cam;
-  float *t, *q;
-};
-
-// one block of kSeg threads per segment; offsets NULL: counts[seg] = the segment's active pairs, else they go to
-// out[offsets[seg] ...]
-template <class Op>
-__global__ void __launch_bounds__(kSeg) k_compact(Op op, int64_t n, int64_t n_seg, int32_t* __restrict__ counts,
-                                                  const int64_t* __restrict__ offsets, PairOut out) {
-  __shared__ int32_t warp_sum[kSeg / 32];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (int64_t seg = blockIdx.x; seg < n_seg; seg += gridDim.x) {
-    const int64_t a = seg * kSeg + threadIdx.x;
-    Pair o;
-    const int keep = (a < n && op(a, o, offsets != nullptr)) ? 1 : 0;
-    int incl = keep;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const int y = __shfl_up_sync(0xffffffffu, incl, d);
-      if (lane >= d) incl += y;
-    }
-    if (lane == 31) warp_sum[warp] = incl;
-    __syncthreads();
-    int before = 0, total = 0;
-#pragma unroll
-    for (int w = 0; w < kSeg / 32; ++w) {
-      before += w < warp ? warp_sum[w] : 0;
-      total += warp_sum[w];
-    }
-    if (!offsets) {
-      if (threadIdx.x == 0) counts[seg] = total;
-    } else if (keep) {
-      const int64_t j = offsets[seg] + before + incl - 1;
-      out.idx[j] = o.idx;
-      out.cam[j] = o.cam;
-      out.t[j] = o.t;
-      out.q[3 * j] = o.q[0];
-      out.q[3 * j + 1] = o.q[1];
-      out.q[3 * j + 2] = o.q[2];
-    }
-    __syncthreads();
-  }
-}
 
 // n turned to n . v > 0 towards its view's centre (v as towards()); unchanged where view < 0
 __global__ void k_orient(const float* __restrict__ p, const float* __restrict__ n, const int32_t* __restrict__ view,
@@ -278,16 +246,6 @@ __global__ void k_gather(const float* __restrict__ p, const int32_t* __restrict_
   }
 }
 
-static inline unsigned grid_for(int64_t blocks) { return (unsigned)std::min<int64_t>(std::max<int64_t>(blocks, 1), 65535ll * 8); }
-
-template <class Op>
-static int compact(Op op, int64_t n, int32_t* counts, const int64_t* offsets, PairOut out, void* stream) {
-  const int64_t n_seg = cdiv(n, kSeg);
-  k_compact<<<grid_for(n_seg), kSeg, 0, (cudaStream_t)stream>>>(op, n, n_seg, counts, offsets, out);
-  NUDF_LAUNCH_OK();
-  return 0;
-}
-
 }  // namespace pt
 }  // namespace nudf
 
@@ -299,7 +257,7 @@ using namespace nudf::pt;
 int nudf_pt_normals(const float* g, int64_t m, float* out, void* stream) {
   NUDF_REQUIRE(m >= 0 && (m == 0 || (g && out)), "null pointer or negative count");
   if (m == 0) return 0;
-  k_normals<<<grid_for(cdiv(m, 256)), 256, 0, (cudaStream_t)stream>>>(g, m, out);
+  k_normals<<<grid_for(m), 256, 0, (cudaStream_t)stream>>>(g, m, out);
   NUDF_LAUNCH_OK();
   return 0;
 }
@@ -312,7 +270,7 @@ int nudf_pt_rank(const float* p, const float* n, int64_t m, const float* mats, c
   NUDF_REQUIRE(m >= 0 && m <= INT32_MAX, "the point count must lie in [0, 2^31)");
   if (m == 0) return 0;
   NUDF_REQUIRE(p && n && cand && (V == 0 || (mats && centres)), "null pointer");
-  k_rank<<<grid_for(cdiv(m, 256)), 256, 0, (cudaStream_t)stream>>>(p, n, m, mats, centres, V, H, W, cos_min, K, cand);
+  k_rank<<<grid_for(m), 256, 0, (cudaStream_t)stream>>>(p, n, m, mats, centres, V, H, W, cos_min, K, cand);
   NUDF_LAUNCH_OK();
   return 0;
 }
@@ -323,7 +281,7 @@ int nudf_pt_start_count(const float* p, const float* n, const int32_t* cand, int
   NUDF_REQUIRE(m >= 0 && m <= INT32_MAX, "the point count must lie in [0, 2^31)");
   if (m == 0) return 0;
   NUDF_REQUIRE(p && n && cand && view && centres && counts, "null pointer");
-  return compact(StartOp{p, n, centres, cand, view, K, r, t_start}, m, counts, nullptr, PairOut{}, stream);
+  return seg_compact<PairOut>(StartOp{p, n, centres, cand, view, K, r, t_start}, m, counts, nullptr, PairOut{}, stream);
 }
 
 int nudf_pt_start_emit(const float* p, const float* n, const int32_t* cand, int32_t K, int32_t r, const int32_t* view,
@@ -333,7 +291,7 @@ int nudf_pt_start_emit(const float* p, const float* n, const int32_t* cand, int3
   NUDF_REQUIRE(m >= 0 && m <= INT32_MAX, "the point count must lie in [0, 2^31)");
   if (m == 0) return 0;
   NUDF_REQUIRE(p && n && cand && view && centres && offsets && out_idx && out_cam && out_t && out_q, "null pointer");
-  return compact(StartOp{p, n, centres, cand, view, K, r, t_start}, m, nullptr, offsets,
+  return seg_compact<PairOut>(StartOp{p, n, centres, cand, view, K, r, t_start}, m, nullptr, offsets,
                  PairOut{out_idx, out_cam, out_t, out_q}, stream);
 }
 
@@ -342,7 +300,7 @@ int nudf_pt_trace_count(const float* p, const float* centres, const int32_t* idx
   NUDF_REQUIRE(n >= 0, "negative count");
   if (n == 0) return 0;
   NUDF_REQUIRE(p && centres && idx && cam && t && u && counts, "null pointer");
-  return compact(StepOp{p, centres, idx, cam, t, u, hit, nullptr}, n, counts, nullptr, PairOut{}, stream);
+  return seg_compact<PairOut>(StepOp{p, centres, idx, cam, t, u, hit, nullptr}, n, counts, nullptr, PairOut{}, stream);
 }
 
 int nudf_pt_trace_emit(const float* p, const float* centres, const int32_t* idx, const int32_t* cam, const float* t,
@@ -352,7 +310,7 @@ int nudf_pt_trace_emit(const float* p, const float* centres, const int32_t* idx,
   if (n == 0) return 0;
   NUDF_REQUIRE(p && centres && idx && cam && t && u && offsets && view && out_idx && out_cam && out_t && out_q,
                "null pointer");
-  return compact(StepOp{p, centres, idx, cam, t, u, hit, view}, n, nullptr, offsets,
+  return seg_compact<PairOut>(StepOp{p, centres, idx, cam, t, u, hit, view}, n, nullptr, offsets,
                  PairOut{out_idx, out_cam, out_t, out_q}, stream);
 }
 
@@ -361,7 +319,7 @@ int nudf_pt_orient(const float* p, const float* n, const int32_t* view, int64_t 
   NUDF_REQUIRE(m >= 0, "negative count");
   if (m == 0) return 0;
   NUDF_REQUIRE(p && n && view && out, "null pointer");
-  k_orient<<<grid_for(cdiv(m, 256)), 256, 0, (cudaStream_t)stream>>>(p, n, view, m, centres, out);
+  k_orient<<<grid_for(m), 256, 0, (cudaStream_t)stream>>>(p, n, view, m, centres, out);
   NUDF_LAUNCH_OK();
   return 0;
 }
@@ -373,7 +331,7 @@ int nudf_pt_gather(const float* p, const int32_t* view, int64_t m, const float* 
   NUDF_REQUIRE(m >= 0, "negative count");
   if (m == 0) return 0;
   NUDF_REQUIRE(p && view && out && (V == 0 || (mats && images)), "null pointer");
-  k_gather<<<grid_for(cdiv(m, 256)), 256, 0, (cudaStream_t)stream>>>(p, view, m, mats, images, H, W, out);
+  k_gather<<<grid_for(m), 256, 0, (cudaStream_t)stream>>>(p, view, m, mats, images, H, W, out);
   NUDF_LAUNCH_OK();
   return 0;
 }

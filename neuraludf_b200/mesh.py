@@ -192,8 +192,8 @@ def _iso_cells(lat, n_positions, level, dev):
     (nudf_iso_cells_*: no scan of every cell)"""
     L = _lib.lib()
     st = _lib.stream_ptr()
-    n_seg = -(-n_positions // _lib.ISO_SEG)
-    counts = torch.empty(n_seg, dtype=torch.int32, device=dev)
+    counts = _lib.seg_counts(n_positions, dev)
+    n_seg = counts.numel()
     check(L.nudf_iso_cells_count(lat, level, n_seg, ptr(counts), st), "nudf_iso_cells_count")
     csum = torch.cumsum(counts, 0, dtype=torch.int64)
     total = int(csum[-1]) if n_seg else 0

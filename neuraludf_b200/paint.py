@@ -108,10 +108,6 @@ def _pairs(n, dev):
             torch.empty(n, dtype=torch.float32, device=dev), torch.empty(n, 3, dtype=torch.float32, device=dev))
 
 
-def _counts(n, dev):
-    return torch.empty(-(-n // _lib.PT_SEG), dtype=torch.int32, device=dev)
-
-
 def start_pairs(points, normals, cand, r, view, centres, t_start):
     """round r's pairs (idx, cam int32 [A], t fp32 [A], q fp32 [A,3]; nudf_pt_start_*): every point with view < 0 and
     k = cand[i, r] >= 0, in order, at t0 = fp32(t_start) / |n . v| and q = p + t0 v"""
@@ -120,7 +116,7 @@ def start_pairs(points, normals, cand, r, view, centres, t_start):
     args = (ptr(points), ptr(normals), ptr(cand), K, int(r), ptr(view), M, ptr(centres), float(t_start))
     if M == 0:
         return _pairs(0, dev)
-    counts = _counts(M, dev)
+    counts = _lib.seg_counts(M, dev)
     check(L.nudf_pt_start_count(*args, ptr(counts), st), "nudf_pt_start_count")
     csum = torch.cumsum(counts, 0, dtype=torch.int64)
     out = _pairs(int(csum[-1].item()), dev)
@@ -138,25 +134,26 @@ def trace_step(points, centres, pairs, u, hit, view):
 
 
 def _trace(points, centres, pairs, values, hit, view, max_batch):
-    """one trace step of every pair, the udf taken from values(q) over batches of max_batch; the batches' active pairs go
-    to one buffer from a running offset kept on the device, so that the active count is the only host read"""
+    """one trace step of every pair, the udf taken from values(q) over batches of max_batch (_lib.compact_batches)"""
     L, st, dev = _lib.lib(), _lib.stream_ptr(), points.device
-    A = pairs[0].shape[0]
-    out = _pairs(A, dev)
-    base = torch.zeros(1, dtype=torch.int64, device=dev)
-    for head in range(0, A, max_batch):
-        b = [a[head:head + max_batch] for a in pairs]
-        u = values(b[3]).reshape(-1).float().contiguous()
-        if u.shape[0] != b[0].shape[0]:
+    out = _pairs(pairs[0].shape[0], dev)
+
+    def batch(lo, hi):
+        idx, cam, t, q = (a[lo:hi] for a in pairs)
+        u = values(q).reshape(-1).float().contiguous()
+        if u.shape[0] != hi - lo:
             raise ValueError("u must hold one value per pair")
-        args = (ptr(points), ptr(centres), ptr(b[0]), ptr(b[1]), ptr(b[2]), ptr(u), b[0].shape[0], float(hit))
-        counts = _counts(b[0].shape[0], dev)
-        check(L.nudf_pt_trace_count(*args, ptr(counts), st), "nudf_pt_trace_count")
-        csum = torch.cumsum(counts, 0, dtype=torch.int64)
-        check(L.nudf_pt_trace_emit(*args, ptr(base + (csum - counts)), ptr(view), *(ptr(a) for a in out), st),
-              "nudf_pt_trace_emit")
-        base += csum[-1]
-    n = int(base.item())
+
+        def launch(counts, offsets=None):      # holds u until both passes are enqueued
+            args = (ptr(points), ptr(centres), ptr(idx), ptr(cam), ptr(t), ptr(u), hi - lo, float(hit))
+            if offsets is None:
+                check(L.nudf_pt_trace_count(*args, ptr(counts), st), "nudf_pt_trace_count")
+            else:
+                check(L.nudf_pt_trace_emit(*args, ptr(offsets), ptr(view), *(ptr(a) for a in out), st),
+                      "nudf_pt_trace_emit")
+        return launch
+
+    n = _lib.compact_batches(pairs[0].shape[0], max_batch, dev, batch)
     return tuple(a[:n] for a in out)
 
 

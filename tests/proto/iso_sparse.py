@@ -1,5 +1,5 @@
 """NumPy restatement of the block-sparse threshold lattice (grid.iso_band_sparse) and of the active-cell enumeration
-from storage positions (mesh.iso_active_cells, csrc/mesh_udf.cu k_iso_cells): iso_band's level chain
+from storage positions (mesh.iso_active_cells, csrc/mesh_udf.cu IsoCells): iso_band's level chain
 (tests/proto/iso_band.py) run on udf_sparse's store (tests/proto/udf_sparse.py), the table block test reading the store,
 and the cells found from the stored points with v <= 0, each emitted by its lowest such corner."""
 import numpy as np

@@ -27,6 +27,21 @@ def test_library_exports_the_declared_abi():
     assert L.nudf_abi_version() == 6
 
 
+def test_python_constants_match_the_header():
+    """every constant _lib mirrors equals include/nudf.h's #define (a smaller COMPACT_SEG would let the count pass write
+    past the counts buffer)"""
+    from neuraludf_b200 import _lib
+    txt = open(os.path.join(ROOT, "include", "nudf.h")).read()
+    header = {k: int(v) for k, v in re.findall(r"^#define NUDF_([A-Z0-9_]+)[ \t]+(-?\d+)\b", txt, flags=re.M)}
+    mirrors = {"COMPACT_SEG": _lib.COMPACT_SEG, "BRICK": _lib.BRICK, "PT_MAX_VIEWS": _lib.PT_MAX_VIEWS,
+               "PT_MAX_CAND": _lib.PT_MAX_CAND, "MAX_LAYERS": _lib.MAX_LAYERS,
+               "STATUS_NONFINITE_SAMPLES": _lib.STATUS_NONFINITE_SAMPLES,
+               "STATUS_NONFINITE_RENDER": _lib.STATUS_NONFINITE_RENDER}
+    mirrors.update(("PATCH_" + name.upper(), v) for name, v in _lib.PATCH_TYPES.items())
+    for name, v in mirrors.items():
+        assert header.get(name) == v, "_lib mirrors NUDF_%s as %r, include/nudf.h has %r" % (name, v, header.get(name))
+
+
 def test_descriptor_validation_runs_without_gpu():
     from neuraludf_b200 import _lib
     import ctypes

@@ -1,5 +1,5 @@
 """The block-sparse threshold lattice and the active-cell enumeration from storage positions (tests/proto/iso_sparse.py,
-the restatement of grid.iso_band_sparse and csrc/mesh_udf.cu's k_iso_cells): the store reads iso_band's df at every
+the restatement of grid.iso_band_sparse and csrc/mesh_udf.cu's IsoCells compaction): the store reads iso_band's df at every
 lattice point, and the enumeration gives nudf_iso_active's cells of that df -- on random, analytic and non-Lipschitz
 fields, NaN corners, values exactly at the level and levels nothing crosses, for small and odd sizes and several
 schedules.  Also the CLI's --threshold --band --sparse rules."""
